@@ -73,4 +73,16 @@ unsigned stage_slots(uint64_t n, const uint64_t* __restrict__ idx, uint64_t capa
   return bad ? 1u : 0u;
 }
 
+// flags words `stride` u32 apart (a column, or the flags of packed records): 1 when a 5-field schedule names a
+// zone id above `n_zones` — ids are process-local, and only registered ones have offsets on the device
+AM_SIMD_CLONES
+unsigned unknown_zones(uint64_t n, const uint32_t* __restrict__ flags, uint64_t stride, uint32_t n_zones) {
+  uint32_t bad = 0;
+  for (uint64_t k = 0; k < n; ++k) {
+    const uint32_t f = flags[k * stride];
+    bad |= (uint32_t)((f & AM_KIND_MASK) == AM_KIND_CRON_SPEC) & (uint32_t)((f >> AM_F_TZ_SHIFT) > n_zones);
+  }
+  return bad;
+}
+
 }  // namespace amsweep_host

@@ -44,6 +44,7 @@ unsigned stage_results(uint64_t n, const uint64_t* idx, const uint8_t* phase, co
                        uint32_t op_result_kind, uint64_t* ops);
 void widen_list(uint64_t n, uint64_t base, const uint32_t* idx32, const uint8_t* act8, uint64_t* idx64, uint32_t* act32);
 unsigned stage_slots(uint64_t n, const uint64_t* idx, uint64_t capacity, uint32_t arg0, uint32_t arg_step, uint64_t* ops);
+unsigned unknown_zones(uint64_t n, const uint32_t* flags, uint64_t stride, uint32_t n_zones);
 }  // namespace amsweep_host
 
 namespace {
@@ -442,8 +443,12 @@ int refresh_zones(am_sweep* h, int64_t T, cudaStream_t s) {
     return AM_OK;
   }
   const size_t bytes = (amsweep_tz::kMaxZones + 1) * sizeof(int32_t);
-  AM_CUDA(h, h->tz_off.reserve(bytes));
-  AM_CUDA(h, h->tz_table.reserve((amsweep_tz::kMaxZones + 1) * sizeof(TickWords)));
+  if (!h->tz_off.p) {  // allocated once, for every id a record can carry; entries of zones not registered stay zero
+    AM_CUDA(h, h->tz_off.reserve(bytes));
+    AM_CUDA(h, cudaMemsetAsync(h->tz_off.p, 0, h->tz_off.cap, s));
+    AM_CUDA(h, h->tz_table.reserve((amsweep_tz::kMaxZones + 1) * sizeof(TickWords)));
+    AM_CUDA(h, cudaMemsetAsync(h->tz_table.p, 0, h->tz_table.cap, s));
+  }
   AM_CUDA(h, h->tz_pin.reserve(bytes));
   if (!h->tz_copied) AM_CUDA(h, cudaEventCreateWithFlags(&h->tz_copied, cudaEventDisableTiming));
   if (h->tz_copy_pending) AM_CUDA(h, cudaEventSynchronize(h->tz_copied));  // the previous copy has left the pinned array
@@ -803,6 +808,7 @@ int am_sweep_set_seed(am_sweep_t* h, uint64_t seed) {
 int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_record_cols_t* cols) {
   if (!h || !cols || first + n > h->capacity || first + n < first) return AM_E_INVAL;
   if (n == 0) return AM_OK;
+  if (cols->flags && amsweep_host::unknown_zones(n, cols->flags, 1, (uint32_t)amsweep_tz::count())) return AM_E_INVAL;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
   AM_CUDA(h, cudaSetDevice(h->device));
@@ -822,6 +828,8 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
 int am_sweep_upsert(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_record_t* recs) {
   if (!h || (n && (!idx || !recs))) return AM_E_INVAL;
   if (n == 0) return AM_OK;
+  if (amsweep_host::unknown_zones(n, &recs[0].flags, sizeof(am_record_t) / sizeof(uint32_t), (uint32_t)amsweep_tz::count()))
+    return AM_E_INVAL;
   std::unique_lock<std::mutex> lk(h->mu);
   Staging* stp = nullptr;
   if (int rc = reserve_staging(h, lk, n, n, &stp)) return rc;
@@ -1023,7 +1031,9 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
   AM_CUDA(h, cudaSetDevice(h->device));
   int rc = order_on(h, h->stream);
   if (rc != AM_OK) return rc;
-  rc = drain_staged(h, h->stream, &unix_sec0);
+  // A blocked run publishes no tick's accumulators: its drain leaves posted results pending in the flags,
+  // and the block kernel applies them at its first tick (and counts them in that tick's row).
+  rc = drain_staged(h, h->stream, (mode & AM_SWEEP_BLOCKED) ? nullptr : &unix_sec0);
   if (rc != AM_OK) return rc;
   h->seed = seed;
   am_tick_stats_t* d_stats = nullptr;
@@ -1144,10 +1154,18 @@ int am_sweep_next_due(am_sweep_t* h, int64_t unix_sec, int64_t* next_out) {
   if (rc != AM_OK) return rc;
   *next_out = INT64_MAX;  // nothing will ever be due (empty shard, only tombstones / exhausted schedules)
   if (h->n_records == 0) return AM_OK;
+  // Zone-bound schedules fire on their zone's minute.  While every offset is a whole number of minutes up
+  // to the next UTC minute, that is not before the next UTC minute; an offset with seconds (local mean
+  // time, e.g. Africa/Monrovia -0:44:30 until 1972) moves the local minute anywhere: then T + 1.
+  rc = refresh_zones(h, unix_sec + 1, h->stream);
+  if (rc != AM_OK) return rc;
+  const int64_t next_minute = unix_sec + 60 - ((unix_sec % 60) + 60) % 60;
+  const int64_t zone_due = (h->tz_aligned && h->tz_hi >= next_minute) ? next_minute : unix_sec + 1;
   AM_CUDA(h, h->dev_in.reserve(8));
   AM_CUDA(h, h->pin_in.reserve(8));
   AM_CUDA(h, cudaMemsetAsync(h->dev_in.p, 0xFF, 8, h->stream));
-  AM_LAUNCH(next_due_kernel, h->sms * 8, 256, h->stream, h->cols, h->n_records, unix_sec, (unsigned long long*)h->dev_in.p);
+  AM_LAUNCH(next_due_kernel, h->sms * 8, 256, h->stream, h->cols, h->n_records, unix_sec, zone_due,
+            (unsigned long long*)h->dev_in.p);
   h->launches++;
   AM_CUDA(h, cudaGetLastError());
   AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, 8, cudaMemcpyDeviceToHost, h->stream));

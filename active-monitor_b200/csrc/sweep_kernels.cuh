@@ -893,8 +893,9 @@ __global__ void next_fire_kernel(DevCols c, uint32_t first, uint32_t n, int64_t 
 // (time.AfterFunc, hcc.go:751) or cron activation (hcc.go:262) — the 1 Hz ticker may sleep until
 // then.  Pending results, an unreported "Stopped" and parse errors (requeued after 1 s, hcc.go:204)
 // are due at once.  Grid-stride, one record per thread and step; lane -> warp (shuffles) -> global
-// atomicMin on a biased unsigned key.
-__global__ void next_due_kernel(DevCols c, uint64_t n, int64_t T, unsigned long long* out_biased) {
+// atomicMin on a biased unsigned key.  `zone_due`: a lower bound, > T, of the first activation of any
+// schedule bound to a named time zone (the launcher derives it from the zones' offsets).
+__global__ void next_due_kernel(DevCols c, uint64_t n, int64_t T, int64_t zone_due, unsigned long long* out_biased) {
   unsigned long long best = ~0ull;
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t f = c.flags[i];
@@ -908,7 +909,7 @@ __global__ void next_due_kernel(DevCols c, uint64_t n, int64_t T, unsigned long 
       const int64_t at = (int64_t)((uint64_t)c.finished_at[i] + (uint64_t)(int64_t)c.ras[i]);
       due = ((f & AM_F_TIMER_ARMED) && at > T + 1) ? at : T + 1;
     } else if (kind == AM_KIND_CRON_SPEC && (f >> AM_F_TZ_SHIFT) != 0) {
-      due = T + 60 - ((T % 60) + 60) % 60;  // zone-bound: not before the next whole minute (a safe lower bound)
+      due = zone_due;
     } else if (kind == AM_KIND_CRON_SPEC) {
       const int64_t nx = cron_next_utc(c.minute[i], c.hour[i], c.dom[i], c.month[i], c.dow[i], T);
       if (nx != kNoNextFire) due = nx;

@@ -250,7 +250,12 @@ void am_sweep_destroy(am_sweep_t*);
  * after (re)start (SURVEY §5 "failure detection / recovery").  The columns are
  * taken as they are: they must be values this library produced
  * (am_healthcheck_classify / am_sweep_read).  In particular
- * AM_F_REMEDY_OUTCOME_OK only has a meaning together with AM_F_REMEDY_PENDING. */
+ * AM_F_REMEDY_OUTCOME_OK only has a meaning together with AM_F_REMEDY_PENDING.
+ * The time zone of a 5-field schedule (flags bits 24..31) is an id of THIS process's
+ * registry (am_tz_lookup, handed out in order of first registration): records read
+ * in another process, or before a restart that registered zones in another order,
+ * must be re-classified.  A CRON_SPEC record naming an id that is not registered makes
+ * this call and am_sweep_upsert return AM_E_INVAL without loading anything. */
 int am_sweep_load_range(am_sweep_t*, uint64_t first, uint64_t n, const am_record_cols_t* cols);
 
 /* Reconcile of created/updated CRs (hcc.go:170-188): scatter n records to

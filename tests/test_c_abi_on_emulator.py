@@ -43,14 +43,14 @@ def test_emulated_library_exports_the_whole_abi(emu_lib):
 def test_gpu_parity_suite_through_the_c_abi_on_the_emulated_library(emu_lib):
     env = dict(os.environ, AMSWEEP_LIB=emu_lib)
     out = subprocess.run([sys.executable, "-m", "pytest", "tests/test_sweep_gpu.py", "tests/test_golden_fixtures.py",
-                          "tests/test_timezones.py",
+                          "tests/test_timezones.py", "tests/test_sweep_adversarial_gpu.py",
                           "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider", "-k", "not tick_device and not 10m"],
                          cwd=ROOT, env=env, capture_output=True, text=True, timeout=1800)
     tail = out.stdout[-3000:] + out.stderr[-2000:]
     assert out.returncode == 0, tail
     last = out.stdout.strip().splitlines()[-1]
     assert " passed" in last and "failed" not in last and "error" not in last, tail
-    assert int(last.split(" passed")[0].split()[-1]) >= 68, tail
+    assert int(last.split(" passed")[0].split()[-1]) >= 135, tail
 
 
 def test_reconciler_cpp_mirror_on_the_emulated_library(emu_lib):

@@ -9,22 +9,23 @@ import pytest
 from conftest import ROOT
 
 SRC = os.path.join(ROOT, "tests", "cpp", "test_reconciler.cpp")
-EXE = os.path.join(ROOT, "tests", "cpp", "test_reconciler.bin")
 LIBDIR = os.path.join(ROOT, "active-monitor_b200", "lib")
 
 
-def _build():
+def _build(tmp_path):
+    """links the mirror into the test's temporary directory: the repository tree may be read-only"""
+    exe = str(tmp_path / "test_reconciler.bin")
     subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), SRC,
-                    "-L", LIBDIR, "-lamsweep", f"-Wl,-rpath,{LIBDIR}", "-o", EXE], check=True)
+                    "-L", LIBDIR, "-lamsweep", f"-Wl,-rpath,{LIBDIR}", "-o", exe], check=True)
+    return exe
 
 
-def test_reconciler_mirror_compiles():
-    _build()
-    assert os.path.exists(EXE)
+def test_reconciler_mirror_compiles(tmp_path):
+    assert os.path.exists(_build(tmp_path))
 
 
 @pytest.mark.gpu
-def test_reconciler_mirror_behaves_like_the_reference_tests():
-    _build()
-    out = subprocess.run([EXE], capture_output=True, text=True, timeout=120)
+def test_reconciler_mirror_behaves_like_the_reference_tests(tmp_path):
+    exe = _build(tmp_path)
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0 and out.stdout.strip().endswith("ok"), out.stdout + out.stderr

@@ -1,108 +1,29 @@
-"""Adversarial populations for the sweep kernels on the CPU emulator (tests/emu) against the
-oracle: the values the generated BASELINE configs never reach — counters at INT32_MAX (wrap-around
-of SuccessCount++ etc.), intervals of INT32_MAX, finishedAt exactly at / one second around the due
-boundary or 2^40 away, remedy gates with limits and reset intervals at the i32 extremes, all-ones and
-empty cron masks, T at 0, -1, 2^31, +-2^40, +-2^54 — and, beyond what the library itself can
-produce, kinds 6/7, both PENDING bits at once, zero / negative intervals on interval kinds and
-negative counters.  Three consecutive ticks, all four kernel variants (open/closed loop x
-masks/no masks), bit-exact lists, statistics and columns.
-
-One combination is deliberately absent: AM_F_REMEDY_OUTCOME_OK without AM_F_REMEDY_PENDING.  It
-has no meaning (post_result sets the two together); the oracle would clear the stray bit, the
-kernel leaves a record with nothing pending untouched (include/amsweep.h, am_sweep_load_range)."""
-import importlib
+"""Adversarial populations (tests/adversarial.py) for the sweep kernels on the CPU emulator (tests/emu)
+against the oracle: counters and intervals at the i32 extremes, finishedAt on the due boundary, remedy
+gates at the extremes, schedules bound to named time zones, T at 0, -1, 2^31, +-2^40, +-2^54 — and,
+beyond what the library itself can produce, kinds 6/7, both PENDING bits at once, zero / negative
+intervals and negative counters.  Three consecutive ticks, all four kernel variants (open/closed loop
+x masks/no masks), bit-exact lists, statistics and columns.  The same cases run on the device in
+tests/test_sweep_adversarial_gpu.py."""
 import os
 import sys
 
-import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
 import emu_sweep  # noqa: E402
-import oracle_c  # noqa: E402
-
-am = importlib.import_module("active-monitor_b200")
-I32MIN, I32MAX = -(1<<31), (1<<31)-1
-
-def population(rng, n, T, in_domain=True):
-    c = am.alloc_columns(n)
-    for name in ("minute","hour","dom","month","dow"):
-        v = rng.integers(0, 1<<63, n, dtype=np.uint64) | (rng.integers(0,2,n,dtype=np.uint64) << np.uint64(63))
-        sparse = rng.integers(0,3,n) == 0
-        v[sparse] = (np.uint64(1) << rng.integers(0,62,n).astype(np.uint64))[sparse]
-        v[rng.integers(0,10,n)==0] = 0
-        v[rng.integers(0,10,n)==0] = np.uint64(0xFFFFFFFFFFFFFFFF)
-        c[name][:] = v
-    kind = rng.integers(0, 6 if in_domain else 8, n).astype(np.uint32)
-    flags = kind.copy()
-    flags |= (rng.integers(0,2,n).astype(np.uint32) << 3)          # HAS_REMEDY
-    ph = rng.integers(0, 3 if in_domain else 4, n)                   # none / ok / fail / (both)
-    flags |= np.where(ph==1, am.F_PENDING_OK, 0).astype(np.uint32)
-    flags |= np.where(ph==2, am.F_PENDING_FAIL, 0).astype(np.uint32)
-    flags |= np.where(ph==3, am.F_PENDING_OK|am.F_PENDING_FAIL, 0).astype(np.uint32)
-    rp = rng.integers(0,3,n)
-    flags |= np.where(rp==1, am.F_REMEDY_PENDING|am.F_REMEDY_OUTCOME_OK, 0).astype(np.uint32)
-    flags |= np.where(rp==2, am.F_REMEDY_PENDING, 0).astype(np.uint32)
-    flags |= np.where(rng.integers(0,20,n)==0, am.F_TOMBSTONE, 0).astype(np.uint32)
-    flags |= np.where(rng.integers(0,4,n)==0, am.F_STOPPED_REPORTED, 0).astype(np.uint32)
-    flags |= (rng.integers(0,256,n).astype(np.uint32) << 16)
-    c["flags"][:] = flags
-    pick = lambda opts: np.array(opts, dtype=np.int64)[rng.integers(0,len(opts),n)]
-    ras = pick([1,5,60,3600,I32MAX, 7, 86400] + ([] if in_domain else [0,-1,I32MIN]))
-    c["ras"][:] = ras.astype(np.int32)
-    fa_rel = pick([0,1,-1,59,60,61,3600,100000])
-    fa = T - ras + fa_rel
-    alt = pick([0, T, T+1, T-1, T+100, -(1<<40), (1<<40)])
-    use_alt = rng.integers(0,3,n)==0
-    fa = np.where(use_alt, alt, fa)
-    c["finished_at"][:] = fa
-    c["runs_limit"][:] = pick([0,1,2,5,-1,I32MAX,I32MIN]).astype(np.int32)
-    c["reset_interval"][:] = pick([0,60,300,-1,1,I32MAX,I32MIN]).astype(np.int32)
-    for name in ("success","failed"):
-        c[name][:] = pick([0,1,7,1000,I32MAX,I32MAX-1] + ([] if in_domain else [-1,I32MIN])).astype(np.int32)
-    rs = pick([0,1,2,3,I32MAX] + ([] if in_domain else [-1])).astype(np.int64)
-    rf = pick([0,1,2,3,I32MAX] + ([] if in_domain else [-5])).astype(np.int64)
-    c["remedy_success"][:] = rs.astype(np.int32)
-    c["remedy_failed"][:] = rf.astype(np.int32)
-    rt = np.where(rng.integers(0,4,n)==0, pick([0,1,2,6,-1,I32MAX]), rs+rf)
-    c["remedy_total"][:] = rt.astype(np.int64).astype(np.int32, casting="unsafe") if False else (rt & 0xFFFFFFFF).astype(np.uint32).view(np.int32)
-    rst = c["reset_interval"].astype(np.int64)
-    rfa = T - rst + pick([0,1,-1,5])
-    rfa = np.where(rng.integers(0,3,n)==0, pick([0,0,T,T+5,-(1<<40),(1<<40), T-(1<<34), T+(1<<34)]), rfa)
-    c["remedy_finished_at"][:] = rfa
-    return c
-
-def run(seed, n, T, mode, in_domain):
-    rng = np.random.default_rng(seed)
-    cols = population(rng, n, T, in_domain)
-    ocols = {k: v.copy() for k, v in cols.items()}
-    with emu_sweep.EmuSweep(n) as s:
-        s.load_range(0, cols)
-        s.set_seed(seed)
-        for k in range(3):
-            gi, ga, gs = s.tick(T + k, mode=mode)
-            wi, wa, ws = oracle_c.sweep(ocols, T + k, mode=mode & 1, seed=seed)
-            bad = None
-            if gs != ws: bad = ("stats", {f:(gs[f],ws[f]) for f in gs if gs[f]!=ws[f]})
-            elif not np.array_equal(gi, wi): bad = ("idx",)
-            elif not np.array_equal(ga, wa): bad = ("act",)
-            dev = s.read_range(0, n)
-            for name in am.COLUMN_NAMES:
-                if not np.array_equal(dev[name], ocols[name]):
-                    i = int(np.flatnonzero(dev[name] != ocols[name])[0])
-                    bad = bad or ("col", name, i, int(dev[name][i]), int(ocols[name][i]), {q:int(cols[q][i]) for q in cols})
-                    break
-            if bad:
-                return (seed, n, T, mode, k, bad)
-    return None
+from adversarial import TS, ZoneMap, product_lookup, run_single_ticks  # noqa: E402
 
 
-TS = [1789982100, 1789982101, 0, -1, 59, 60, 1 << 31, -(1 << 33), (1 << 40) + 420, -(1 << 40), 1 << 54, -(1 << 54)]
+@pytest.fixture(scope="module")
+def emu_zones():
+    # zone ids of the emulated library's own registry
+    return ZoneMap(product_lookup(emu_sweep.load()))
 
 
 @pytest.mark.parametrize("in_domain", [True, False], ids=["library-domain", "beyond-domain"])
 @pytest.mark.parametrize("seed", range(12))
-def test_adversarial_population(seed, in_domain):
+def test_adversarial_population(emu_zones, seed, in_domain):
     for mode in (0, 1, 2, 3):  # closed loop / full scan bits
-        bad = run(seed, 2500, TS[seed % len(TS)], mode, in_domain)
+        bad = run_single_ticks(emu_sweep.EmuSweep, emu_zones, seed, 2500, TS[seed % len(TS)], mode, in_domain)
         assert bad is None, bad

@@ -255,31 +255,71 @@ def test_run_ticks_streaming_matches_single_ticks(am, orc, gen):
             np.testing.assert_array_equal(dev[name], orac[name], err_msg=name)
 
 
-@pytest.mark.parametrize("config,closed,start,nt,block", [
-    (5, True, -30, 200, 0),      # config-2 mix (cron + intervals), closed loop, three minute boundaries
-    (22, False, -70, 150, 0),    # open loop, zone-bound schedules among the crons
-    (55, True, -75, 160, 7),     # remedy mix, closed loop, short blocks
-    (3, False, -10, 90, 0),      # open loop: posted results and remedy gates at the first tick, then unarmed checks every tick
-    (2, False, 45, 70, 64),      # open loop config 2
-    (5, True, -100, 300, 128),   # the longest blocks
-    (5, True, 0, 1, 0),          # a single tick
-])
-def test_run_ticks_blocked_equals_the_oracle_tick_by_tick(am, orc, gen, monkeypatch, config, closed, start, nt, block):
+def _post_results(am, sweeps, ocols, n, density, seed):
+    """Workflow phases and remedy phases posted by separate calls (the reference's two watch loops) on
+    every `step`-th slot of each handle; the oracle's columns get the same pending bits.  Every 23rd slot
+    stays at most an eighth of the records in staged results (the drain's sparse path,
+    apply_results_now_kernel); every second slot is the dense path (apply_result_ops_kernel)."""
+    rng = np.random.default_rng(seed)
+    slots = np.arange(int(rng.integers(0, 23)), n, 23 if density.startswith("sparse") else 2)
+    phase = rng.integers(1, 3, len(slots)).astype(np.uint8)
+    rphase = rng.integers(0, 3, len(slots)).astype(np.uint8)
+    for s in sweeps:
+        s.post_result(slots, phase)
+        s.post_result(slots, np.zeros_like(phase), rphase)
+    hc = np.uint32(am.F_PENDING_OK | am.F_PENDING_FAIL)
+    rm = np.uint32(am.F_REMEDY_PENDING | am.F_REMEDY_OUTCOME_OK)
+    f = ocols["flags"][slots]
+    f = (f & ~hc) | np.where(phase == am.PHASE_SUCCEEDED, am.F_PENDING_OK, am.F_PENDING_FAIL).astype(np.uint32)
+    rbits = np.where(rphase == am.PHASE_SUCCEEDED, rm, np.uint32(am.F_REMEDY_PENDING)).astype(np.uint32)
+    f = np.where(rphase != 0, (f & ~rm) | rbits, f)
+    ocols["flags"][slots] = f
+    return slots
+
+
+RUN_TICKS_CASES = [
+    (5, True, -30, 200, 0, None),      # config-2 mix (cron + intervals), closed loop, three minute boundaries
+    (22, False, -70, 150, 0, None),    # open loop, zone-bound schedules among the crons
+    (55, True, -75, 160, 7, None),     # remedy mix, closed loop, short blocks
+    (3, False, -10, 90, 0, None),      # open loop: posted results and remedy gates at the first tick, then unarmed checks every tick
+    (2, False, 45, 70, 64, None),      # open loop config 2
+    (5, True, -100, 300, 128, None),   # the longest blocks
+    (5, True, 0, 1, 0, None),          # a single tick
+    # results posted through the C-ABI just before the run: applied by the run's first tick
+    (3, False, 0, 3, 0, "sparse"),
+    (3, True, -10, 90, 7, "sparse"),
+    (55, False, -75, 160, 1, "sparse"),
+    (3, False, 0, 3, 0, "dense"),
+    (55, True, -10, 150, 128, "dense"),
+    (3, False, 0, 3, 0, "sparse-late"),  # AMSWEEP_EARLY_RESULTS=0: every result applied inside the sweep
+    (5, True, -30, 200, 96, "sparse-late"),
+]
+
+
+# (the cases without posted results keep the ids they had before the `posted` column existed)
+@pytest.mark.parametrize("config,closed,start,nt,block,posted", RUN_TICKS_CASES,
+                         ids=["-".join(str(v) for v in case if v is not None) for case in RUN_TICKS_CASES])
+def test_run_ticks_blocked_equals_the_oracle_tick_by_tick(am, orc, gen, monkeypatch, config, closed, start, nt, block, posted):
     """AM_SWEEP_BLOCKED: up to 64 ticks per pass over the columns, every record stepped from event to event
     in registers (sweep_block.cuh).  Per-tick statistics — counts, action counts, index checksums, result
     counters — and every column afterwards must equal the oracle's tick-by-tick evaluation, and the
-    library's own unblocked run."""
+    library's own unblocked run; so must the host tick that follows the run."""
     n, seed = 30_000, 9
     if block:
         monkeypatch.setenv("AMSWEEP_BLOCK_TICKS", str(block))
+    if posted == "sparse-late":
+        monkeypatch.setenv("AMSWEEP_EARLY_RESULTS", "0")
     prod, orac = _gen_pair(gen, am, orc, config, seed, n, T0)
     mode = am.SWEEP_CLOSED_LOOP if closed else 0
     with am.Sweep(capacity=n) as s, am.Sweep(capacity=n) as s1:
         s.load_range(0, prod)
         s1.load_range(0, prod)
+        if posted:
+            _post_results(am, (s, s1), orac, n, posted, seed)
         l0 = s.launch_count
         stats = s.run_ticks(T0 + start, nt, mode=mode | am.SWEEP_BLOCKED, seed=seed)
-        assert s.launch_count - l0 <= (nt + (block or 96) - 1) // (block or 96) + 2  # one launch per block (+ a zone-window split)
+        drain = 3 if posted else 0  # mark, apply, clear the staged results
+        assert s.launch_count - l0 <= (nt + (block or 96) - 1) // (block or 96) + 2 + drain  # one launch per block (+ a zone-window split)
         plain = s1.run_ticks(T0 + start, nt, mode=mode, seed=seed)
         emitted = 0
         for k in range(nt):
@@ -292,6 +332,81 @@ def test_run_ticks_blocked_equals_the_oracle_tick_by_tick(am, orc, gen, monkeypa
         dev = s.read_range(0, n)
         for name in am.COLUMN_NAMES:
             np.testing.assert_array_equal(dev[name], orac[name], err_msg=name)
+        # the next host tick continues from where the run left off, on both handles
+        T = T0 + start + nt
+        s.set_seed(seed)
+        s1.set_seed(seed)
+        want = orc.sweep(orac, T, mode=mode, seed=seed)
+        _assert_tick_equal(am, s.tick(T, mode=mode), want, s, orac, n, "tick after the blocked run")
+        got = s1.tick(T, mode=mode)
+        assert got[2] == want[2], "tick after the unblocked run"
+        np.testing.assert_array_equal(got[0], want[0])
+        np.testing.assert_array_equal(got[1], want[1])
+
+
+@pytest.mark.parametrize("consumer", ["tick", "tick_view", "tick_device", "next_due", "repeat_after_sec", "read"])
+@pytest.mark.parametrize("density", ["sparse", "dense", "sparse-late"])
+def test_posted_results_then_any_consumer_then_a_tick(am, orc, gen, monkeypatch, density, consumer):
+    """Results posted through the C-ABI (phases by separate calls, sparse / dense / sparse with the early
+    path off), then ONE call that drains them — a host tick, a tick view, a device tick, next_due,
+    repeat_after_sec or a read — then a host tick.  Both must equal the oracle.  (The runs of ticks as
+    consumers: test_run_ticks_blocked_equals_the_oracle_tick_by_tick.)"""
+    import ctypes as C
+    n, seed = 40_000, 3
+    if density == "sparse-late":
+        monkeypatch.setenv("AMSWEEP_EARLY_RESULTS", "0")
+    prod, orac = _gen_pair(gen, am, orc, 3, seed, n, T0)
+    T = T0
+    with am.Sweep(capacity=n) as s:
+        s.load_range(0, prod)
+        slots = _post_results(am, (s,), orac, n, density, seed)
+        ticked = consumer.startswith("tick")
+        if consumer == "tick":
+            _assert_tick_equal(am, s.tick(T), orc.sweep(orac, T), s, orac, n, "tick")
+        elif consumer == "tick_view":
+            vi, va, st = s.tick_view(T)
+            wi, wa, ws = orc.sweep(orac, T)
+            assert st == ws
+            np.testing.assert_array_equal(vi.astype(np.uint64), wi)
+            np.testing.assert_array_equal(va.astype(np.uint32), wa)
+        elif consumer == "tick_device":
+            import torch
+            dev = torch.device("cuda:0")
+            d_idx = torch.empty(n, dtype=torch.int32, device=dev)
+            d_act = torch.empty(n, dtype=torch.uint8, device=dev)
+            d_cnt = torch.zeros(1, dtype=torch.int32, device=dev)
+            d_st = torch.zeros(16, dtype=torch.int64, device=dev)
+            stream = torch.cuda.current_stream()
+            s.tick_device(T, 0, d_idx.data_ptr(), d_act.data_ptr(), n, d_cnt.data_ptr(), d_st.data_ptr(), stream.cuda_stream)
+            stream.synchronize()
+            wi, wa, ws = orc.sweep(orac, T)
+            cnt = int(d_cnt.item())
+            assert cnt == len(wi)
+            np.testing.assert_array_equal(d_idx[:cnt].cpu().numpy().astype(np.uint64), wi)
+            np.testing.assert_array_equal(d_act[:cnt].cpu().numpy().astype(np.uint32), wa)
+            assert dict(zip(am.abi.STAT_FIELDS, [int(v) & ((1 << 64) - 1) for v in d_st.cpu().tolist()])) == ws
+        elif consumer == "next_due":
+            assert s.next_due(T) == T + 1  # results are waiting
+        elif consumer == "repeat_after_sec":
+            got = s.repeat_after_sec(T, 0, n)
+            kind = prod["flags"] & 7
+            want = np.zeros(n, dtype=np.int64)
+            iv = (kind == am.KIND_INTERVAL) | (kind == am.KIND_CRON_EVERY)
+            want[iv] = prod["ras"][iv]
+            for i in np.flatnonzero(kind == am.KIND_CRON_SPEC):
+                c = orc.OrcCron(int(prod["minute"][i]), int(prod["hour"][i]), int(prod["dom"][i]),
+                                int(prod["month"][i]), int(prod["dow"][i]), 0, 1, int(prod["flags"][i] >> 24))
+                want[i] = orc.load().orc_cron_repeat_after_sec(C.byref(c), T)
+            np.testing.assert_array_equal(got, want)
+        elif consumer == "read":
+            dev = s.read(slots)
+            for name in am.COLUMN_NAMES:
+                np.testing.assert_array_equal(dev[name], orac[name][slots], err_msg=f"read: {name}")
+            dev = s.read_range(0, n)
+            for name in am.COLUMN_NAMES:
+                np.testing.assert_array_equal(dev[name], orac[name], err_msg=f"read_range: {name}")
+        T_next = T + 1 if ticked else T
+        _assert_tick_equal(am, s.tick(T_next), orc.sweep(orac, T_next), s, orac, n, f"tick after {consumer}")
 
 
 def test_tick_device_resident_outputs(am, orc, gen):
