@@ -130,6 +130,8 @@ struct am_sweep {
   DevCols cols{};
   void* col_ptr[16] = {};
   size_t col_elem[16] = {};
+  PackedMasks pk{};                // [cap_padded] each: the on-minute sweep's copy of the mask columns
+  uint32_t* seg_dirty = nullptr;   // [cap_padded / kRecPerWarp] segments a drain's state ops touched
   TickSet set[2];
   uint32_t parity = 0;
   int last_shard_parity = -1;
@@ -374,8 +376,12 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   AM_LAUNCH(mark_ops_kernel, G, B, s, h->marks, d_ops, (uint32_t)n);
   h->launches++;
   if (st->n_state) {
-    AM_LAUNCH_PDL(apply_state_ops_kernel, G, B, s, h->cols, h->marks, d_ops, d_recs, (uint32_t)n);
-    h->launches++;
+    AM_LAUNCH_PDL(apply_state_ops_kernel, G, B, s, h->cols, h->marks, d_ops, d_recs, (uint32_t)n, h->seg_dirty);
+    // upserts and removes may change kinds and masks: repack the segments they touched (every drain, so a
+    // later tick sees them whichever call drained)
+    AM_LAUNCH_PDL(pack_dirty_kernel, (unsigned)((n + kWarps - 1) / kWarps), kBlock, s, h->cols, h->pk, h->seg_dirty, d_ops,
+                  (uint32_t)n);
+    h->launches += 2;
   }
   // A tick's drain applies sparse results right away (apply_results_now_kernel: no second memory round trip
   // in the sweep, and the posted bits never pass through the flags as a separate step); a read's drain, or a
@@ -474,6 +480,7 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   }
   SweepParams p{};
   p.c = h->cols;
+  p.pk = h->pk;
   p.n_records = h->n_records;
   p.shard_base = h->shard_base;
   p.seed = h->seed;
@@ -696,6 +703,13 @@ int am_sweep_create(am_sweep_t** out, int device_id, uint64_t capacity, uint64_t
     }
     AM_LAUNCH(fill_u32_kernel, h->sms * 8, 256, h->stream, h->cols.flags, AM_F_TOMBSTONE, h->cap_padded);
     h->launches++;
+    // the packed masks: every slot is a tombstone, no segment has a cron record to pack
+    for (uint64_t** pc : {&h->pk.minute, &h->pk.hour, &h->pk.dom, &h->pk.month, &h->pk.dow}) {
+      AM_CUDA(h, cudaMalloc((void**)pc, h->cap_padded * 8));
+      AM_CUDA(h, cudaMemsetAsync(*pc, 0, h->cap_padded * 8, h->stream));
+    }
+    AM_CUDA(h, cudaMalloc((void**)&h->seg_dirty, h->cap_padded / kRecPerWarp * 4));
+    AM_CUDA(h, cudaMemsetAsync(h->seg_dirty, 0, h->cap_padded / kRecPerWarp * 4, h->stream));
     const size_t ntiles = h->cap_padded / kTile;
     const size_t ngroups = (ntiles + kGroupTiles - 1) / kGroupTiles;
     for (int b = 0; b < 2; ++b) {
@@ -741,6 +755,8 @@ void am_sweep_destroy(am_sweep_t* h) {
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();  // ticks may have been issued on caller streams
   for (int k = 0; k < 16; ++k) if (h->col_ptr[k]) cudaFree(h->col_ptr[k]);
+  for (uint64_t* pc : {h->pk.minute, h->pk.hour, h->pk.dom, h->pk.month, h->pk.dow}) if (pc) cudaFree(pc);
+  if (h->seg_dirty) cudaFree(h->seg_dirty);
   for (int b = 0; b < 2; ++b) {
     TickOut& t = h->set[b].out;
     if (t.bitmap) cudaFree(t.bitmap);
@@ -819,6 +835,14 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
     const void* src = *cols_member(cols, k);
     if (src) AM_CUDA(h, cudaMemcpyAsync(dst, src, n * kColElem[k], cudaMemcpyHostToDevice, h->stream));
     else AM_CUDA(h, cudaMemsetAsync(dst, 0, n * kColElem[k], h->stream));
+  }
+  {  // repack every segment that overlaps the range, the partial ones at either end included
+    const uint64_t seg0 = first / kRecPerWarp, seg1 = (first + n + kRecPerWarp - 1) / kRecPerWarp;
+    const uint64_t n_seg = seg1 - seg0;
+    AM_LAUNCH(pack_range_kernel, (unsigned)((n_seg + kWarps - 1) / kWarps), kBlock, h->stream, h->cols, h->pk,
+              (uint32_t)seg0, (uint32_t)n_seg);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
   }
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   if (first + n > h->n_records) h->n_records = first + n;

@@ -268,19 +268,40 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
     ras[h] = ld_stream(reinterpret_cast<const int2*>(p.c.ras + r0[h]));
     fa[h] = ld_stream(reinterpret_cast<const longlong2*>(p.c.finished_at + r0[h]));
   }
+  // The masks come from the packed copy (PackedMasks): only the segment's CRON_SPEC records have slots
+  // there, so the flags decide which slots exist.  A record's slot is its rank among the segment's cron
+  // records in record order: half 0's records (lanes' pairs 2L, 2L+1) before half 1's.  Lane L loads
+  // slots 2L, 2L+1 of each half that has any: ~0.4 of the mask bytes at the population's 40 % cron records.
+  uint32_t n_cron = 0, rank[2][2] = {{0, 0}, {0, 0}};
   if (MASKS) {
+    const bool c00 = (fl[0].x & AM_KIND_MASK) == AM_KIND_CRON_SPEC, c01 = (fl[0].y & AM_KIND_MASK) == AM_KIND_CRON_SPEC;
+    const bool c10 = (fl[1].x & AM_KIND_MASK) == AM_KIND_CRON_SPEC, c11 = (fl[1].y & AM_KIND_MASK) == AM_KIND_CRON_SPEC;
+    const unsigned b00 = __ballot_sync(kFull, c00), b01 = __ballot_sync(kFull, c01);
+    const unsigned b10 = __ballot_sync(kFull, c10), b11 = __ballot_sync(kFull, c11);
+    const unsigned lt = (1u << lane) - 1u;
+    const uint32_t n_half0 = (uint32_t)(__popc(b00) + __popc(b01));
+    n_cron = n_half0 + (uint32_t)(__popc(b10) + __popc(b11));
+    rank[0][0] = (uint32_t)(__popc(b00 & lt) + __popc(b01 & lt));
+    rank[0][1] = rank[0][0] + (uint32_t)c00;
+    rank[1][0] = n_half0 + (uint32_t)(__popc(b10 & lt) + __popc(b11 & lt));
+    rank[1][1] = rank[1][0] + (uint32_t)c10;
+    const uint32_t seg = tile_base + (uint32_t)(warp * kRecPerWarp);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      mi[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.minute + r0[h]));
-      hr[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.hour + r0[h]));
-      dm[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.dom + r0[h]));
-      mo[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.month + r0[h]));
-      dw[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.dow + r0[h]));
+      const uint32_t slot = (uint32_t)(h * 64 + lane * 2);
+      mi[h] = hr[h] = dm[h] = mo[h] = dw[h] = make_ulonglong2(0ull, 0ull);
+      if (slot < n_cron) {
+        mi[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.minute + seg + slot));
+        hr[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.hour + seg + slot));
+        dm[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.dom + seg + slot));
+        mo[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.month + seg + slot));
+        dw[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.dow + seg + slot));
+      }
     }
   }
 
   // Scheduling fence: a warp-level memory-ordering point.  ptxas may not sink the loads
-  // above across it, so all 16 are issued before any of the arithmetic below (without it
+  // above across it, so all of them are issued before any of the arithmetic below (without it
   // the second half's loads were delayed behind the first half's compute, at a large cost in bandwidth).
   __syncwarp();
 
@@ -292,6 +313,31 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
   // named time zones are rare: one vote per warp decides whether the per-record zone lookup exists at all
   const uint32_t fl_or = fl[0].x | fl[0].y | fl[1].x | fl[1].y;
   const bool warp_tz = MASKS && p.tz_table != nullptr && __any_sync(kFull, (fl_or >> AM_F_TZ_SHIFT) != 0);
+
+  // Every packed slot is matched in packed order; bit L of match[h][j] = slot h*64 + 2L + j fires.  A
+  // record then takes bit `rank` (its own slot) of these four ballots.
+  unsigned match[2][2] = {{0u, 0u}, {0u, 0u}};
+  if (MASKS) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const uint64_t miv = j ? mi[h].y : mi[h].x, hrv = j ? hr[h].y : hr[h].x;
+        const uint64_t dmv = j ? dm[h].y : dm[h].x, mov = j ? mo[h].y : mo[h].x;
+        const uint64_t dwv = j ? dw[h].y : dw[h].x;
+        bool m = cron_matches(w, miv, hrv, dmv, mov, dwv);
+        if (warp_tz) {  // warp-uniform: some record of this warp is bound to a named time zone
+          const uint32_t tz = (uint32_t)(hrv >> kPackTzShift) & 0xFFu;
+          // the zone's wall clock instead of UTC's — behind a real call: inlined, ptxas turned the zone
+          // lookup of all four slots into predicated instructions that EVERY warp issues (+24 LDG,
+          // +40 address IMADs per warp, a clearly slower 10 M-record tick with 0.6 % zone-bound records)
+          if (tz && (uint32_t)(h * 64 + lane * 2 + j) < n_cron)
+            m = cron_matches_in_zone(p.tz_table + tz, miv, hrv, dmv, mov, dwv);
+        }
+        match[h][j] = __ballot_sync(kFull, m);
+      }
+    }
+  }
 
   uint32_t act[2][2];
   uint32_t res_lane = 0;  // 4 x 8-bit counts of results applied by this lane
@@ -322,18 +368,10 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
       const bool armed = has_result || (f & AM_F_TIMER_ARMED) != 0;
       const bool due_iv = !((elapsed < (int64_t)rasv) & armed);
       bool due_cron = false;
-      if (MASKS) {
-        const uint64_t miv = j ? mi[h].y : mi[h].x, hrv = j ? hr[h].y : hr[h].x;
-        const uint64_t dmv = j ? dm[h].y : dm[h].x, mov = j ? mo[h].y : mo[h].x;
-        const uint64_t dwv = j ? dw[h].y : dw[h].x;
-        due_cron = cron_matches(w, miv, hrv, dmv, mov, dwv);
-        if (warp_tz) {  // warp-uniform: some record of this warp is bound to a named time zone
-          const uint32_t tz = f >> AM_F_TZ_SHIFT;
-          // the zone's wall clock instead of UTC's — behind a real call: inlined, ptxas turned the zone
-          // lookup of all four records into predicated instructions that EVERY warp issues (+24 LDG,
-          // +40 address IMADs per warp, a clearly slower 10 M-record tick with 0.6 % zone-bound records)
-          if (tz) due_cron = cron_matches_in_zone(p.tz_table + tz, miv, hrv, dmv, mov, dwv);
-        }
+      if (MASKS) {  // (for a record that is not CRON_SPEC the bit read here is another record's: unused)
+        const uint32_t r = rank[h][j];
+        const unsigned m = (r & 64u) ? ((r & 1u) ? match[1][1] : match[1][0]) : ((r & 1u) ? match[0][1] : match[0][0]);
+        due_cron = ((m >> ((r >> 1) & 31u)) & 1u) != 0;
       }
       const bool is_iv = ((0x14u >> kind) & 1u) != 0;  // INTERVAL or CRON_EVERY
       const bool due = live && (is_iv ? due_iv : (kind == AM_KIND_CRON_SPEC && due_cron));
@@ -953,9 +991,10 @@ __global__ void mark_ops_kernel(uint32_t* marks, const uint2* __restrict__ ops, 
   if (arg & AM_F_REMEDY_PENDING) atomicMax(&marks[3u * i + 2u], k + 1u);
 }
 
-// upserts (hcc.go:170-188 Reconcile) and removes (hcc.go:175-186)
+// upserts (hcc.go:170-188 Reconcile) and removes (hcc.go:175-186).  Both may change the slot's kind or
+// masks: its segment is marked for pack_dirty_kernel.
 __global__ void apply_state_ops_kernel(DevCols c, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops,
-                                       const am_record_t* __restrict__ recs, uint32_t n) {
+                                       const am_record_t* __restrict__ recs, uint32_t n, uint32_t* seg_dirty) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
@@ -963,6 +1002,7 @@ __global__ void apply_state_ops_kernel(DevCols c, const uint32_t* __restrict__ m
   const uint32_t i = op.x, arg = op.y;
   const uint32_t kind = arg & kOpKindMask;
   if (kind == kOpResult || marks[3u * i] != k + 1u) return;
+  seg_dirty[i / kRecPerWarp] = 1u;
   if (kind == kOpRemove) { c.flags[i] = AM_F_TOMBSTONE; return; }
   const am_record_t r = recs[arg & ~kOpKindMask];
   c.minute[i] = r.minute; c.hour[i] = r.hour; c.dom[i] = r.dom; c.month[i] = r.month; c.dow[i] = r.dow;
@@ -971,6 +1011,60 @@ __global__ void apply_state_ops_kernel(DevCols c, const uint32_t* __restrict__ m
   c.success[i] = r.success; c.failed[i] = r.failed; c.remedy_success[i] = r.remedy_success;
   c.remedy_failed[i] = r.remedy_failed; c.remedy_total[i] = r.remedy_total;
   c.remedy_finished_at[i] = r.remedy_finished_at;
+}
+
+// ---- the packed mask copy (PackedMasks) -----------------------------------
+// Repack segment `seg` with one warp: lane L looks at records 4L .. 4L+3 of the segment, an exclusive
+// prefix of the lanes' cron counts gives each cron record its slot.  (The sweep derives the same slots
+// from its own record-to-lane layout; the two are independent formulations of "rank in record order".)
+__device__ __forceinline__ void pack_segment(const DevCols& c, const PackedMasks& pk, uint32_t seg, int lane) {
+  const uint32_t first = seg * (uint32_t)kRecPerWarp + (uint32_t)lane * 4u;
+  const uint4 f4 = *reinterpret_cast<const uint4*>(c.flags + first);
+  const uint32_t f[4] = {f4.x, f4.y, f4.z, f4.w};
+  uint32_t mine = 0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) mine |= ((f[q] & AM_KIND_MASK) == AM_KIND_CRON_SPEC ? 1u : 0u) << q;
+  const uint32_t cnt = (uint32_t)__popc(mine);
+  uint32_t incl = cnt;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t up = __shfl_up_sync(kFull, incl, d);
+    if (lane >= d) incl += up;
+  }
+  uint32_t slot = seg * (uint32_t)kRecPerWarp + incl - cnt;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    if ((mine >> q) & 1u) {
+      const uint32_t i = first + (uint32_t)q;
+      const uint64_t tz = f[q] >> AM_F_TZ_SHIFT;
+      pk.minute[slot] = c.minute[i];
+      pk.hour[slot] = (c.hour[i] & ~(0xFFull << kPackTzShift)) | (tz << kPackTzShift);
+      pk.dom[slot] = c.dom[i];
+      pk.month[slot] = c.month[i];
+      pk.dow[slot] = c.dow[i];
+      ++slot;
+    }
+  }
+}
+static_assert(kRecPerWarp == 32 * 4, "pack_segment: four records per lane");
+
+// every segment of [seg0, seg0 + n_seg), one warp each (am_sweep_load_range)
+__global__ void pack_range_kernel(DevCols c, PackedMasks pk, uint32_t seg0, uint32_t n_seg) {
+  const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (w >= n_seg) return;  // warp-uniform
+  pack_segment(c, pk, seg0 + w, (int)(threadIdx.x & 31));
+}
+
+// After apply_state_ops_kernel: one warp per staged op.  The first warp that claims a segment marked
+// there repacks it, so the cost is one claim per op plus one repack per segment touched.
+__global__ void pack_dirty_kernel(DevCols c, PackedMasks pk, uint32_t* seg_dirty, const uint2* __restrict__ ops, uint32_t n) {
+  pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
+  const uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (k >= n) return;  // warp-uniform
+  const int lane = (int)(threadIdx.x & 31);
+  const uint32_t seg = ops[k].x / (uint32_t)kRecPerWarp;
+  const bool won = lane == 0 && atomicAnd(&seg_dirty[seg], 0u) != 0u;  // (an exchange with 0)
+  if (__ballot_sync(kFull, won)) pack_segment(c, pk, seg, lane);
 }
 
 // terminal phases observed by the watch loops (hcc.go:635/:662/:821/:836).  The winner of

@@ -71,6 +71,17 @@ struct DevCols {
   int64_t* remedy_finished_at;
 };
 
+// A copy of the five cron-mask columns that only the on-minute sweep reads.  A "segment" is the
+// kRecPerWarp records one warp of sweep_tick_kernel owns; slots 0 .. k-1 of a segment hold the masks
+// of its k CRON_SPEC records ((flags & AM_KIND_MASK) == AM_KIND_CRON_SPEC) in ascending record order,
+// the slots after them are unspecified.  The hour word carries the record's time-zone id in bits
+// 24..31 (the matcher tests bits 0..23 of it only).  Every write of the canonical masks or of the kind
+// bits repacks the segments it touched (pack_segment); nothing else reads the copy.
+struct PackedMasks {
+  uint64_t *minute, *hour, *dom, *month, *dow;
+};
+constexpr int kPackTzShift = 24;
+
 // What one tick of one shard leaves behind for the list rebuild (expand_kernel) and for the
 // NVLink exchange: the same four arrays whether they are the sweep's own buffers or the copy
 // a peer pushed into this GPU's exchange block.
@@ -84,6 +95,7 @@ struct TickOut {
 
 struct SweepParams {
   DevCols c;
+  PackedMasks pk;  // read by the MASKS variants instead of the five canonical mask columns
   uint64_t n_records;
   uint64_t shard_base;
   uint64_t seed;
