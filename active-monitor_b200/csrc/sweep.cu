@@ -130,7 +130,7 @@ struct am_sweep {
   DevCols cols{};
   void* col_ptr[16] = {};
   size_t col_elem[16] = {};
-  PackedMasks pk{};                // [cap_padded] each: the on-minute sweep's copy of the mask columns
+  MaskPlanes planes{};             // the on-minute sweep's copy of the mask columns as bit planes
   uint32_t* seg_dirty = nullptr;   // [cap_padded / kRecPerWarp] segments a drain's state ops touched
   TickSet set[2];
   uint32_t parity = 0;
@@ -377,10 +377,10 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   h->launches++;
   if (st->n_state) {
     AM_LAUNCH_PDL(apply_state_ops_kernel, G, B, s, h->cols, h->marks, d_ops, d_recs, (uint32_t)n, h->seg_dirty);
-    // upserts and removes may change kinds and masks: repack the segments they touched (every drain, so a
-    // later tick sees them whichever call drained)
-    AM_LAUNCH_PDL(pack_dirty_kernel, (unsigned)((n + kWarps - 1) / kWarps), kBlock, s, h->cols, h->pk, h->seg_dirty, d_ops,
-                  (uint32_t)n);
+    // upserts and removes may change kinds, zones and masks: rebuild the plane words of the segments they
+    // touched (every drain, so a later tick sees them whichever call drained)
+    AM_LAUNCH_PDL(build_planes_dirty_kernel, (unsigned)((n + kWarps - 1) / kWarps), kBlock, s, h->cols, h->planes,
+                  h->seg_dirty, d_ops, (uint32_t)n);
     h->launches += 2;
   }
   // A tick's drain applies sparse results right away (apply_results_now_kernel: no second memory round trip
@@ -480,7 +480,6 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   }
   SweepParams p{};
   p.c = h->cols;
-  p.pk = h->pk;
   p.n_records = h->n_records;
   p.shard_base = h->shard_base;
   p.seed = h->seed;
@@ -505,6 +504,16 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
                   h->tz_n);
     h->launches++;
     p.tz_table = (const TickWords*)h->tz_table.p;
+  }
+  if (masks) {  // the six planes of T's UTC fields
+    const CivilTime ct = civil_from_unix(T);
+    auto plane = [&](int k) { return (const uint32_t*)(h->planes.w + (size_t)k * h->planes.words); };
+    p.pl.minute = plane(kPlaneMinute + ct.min);
+    p.pl.hour = plane(kPlaneHour + ct.hour);
+    p.pl.dom = plane(kPlaneDom + ct.dom);
+    p.pl.month = plane(kPlaneMonth + ct.month);
+    p.pl.dow = plane(kPlaneDow + ct.dow);
+    p.pl.star = plane(kPlaneStar);
   }
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[0], s));
   const bool closed = (mode & AM_SWEEP_CLOSED_LOOP) != 0;
@@ -703,11 +712,10 @@ int am_sweep_create(am_sweep_t** out, int device_id, uint64_t capacity, uint64_t
     }
     AM_LAUNCH(fill_u32_kernel, h->sms * 8, 256, h->stream, h->cols.flags, AM_F_TOMBSTONE, h->cap_padded);
     h->launches++;
-    // the packed masks: every slot is a tombstone, no segment has a cron record to pack
-    for (uint64_t** pc : {&h->pk.minute, &h->pk.hour, &h->pk.dom, &h->pk.month, &h->pk.dow}) {
-      AM_CUDA(h, cudaMalloc((void**)pc, h->cap_padded * 8));
-      AM_CUDA(h, cudaMemsetAsync(*pc, 0, h->cap_padded * 8, h->stream));
-    }
+    // the mask planes: every slot is a tombstone, no record has a plane bit
+    h->planes.words = h->cap_padded / 32;
+    AM_CUDA(h, cudaMalloc((void**)&h->planes.w, kPlanes * h->planes.words * 4));
+    AM_CUDA(h, cudaMemsetAsync(h->planes.w, 0, kPlanes * h->planes.words * 4, h->stream));
     AM_CUDA(h, cudaMalloc((void**)&h->seg_dirty, h->cap_padded / kRecPerWarp * 4));
     AM_CUDA(h, cudaMemsetAsync(h->seg_dirty, 0, h->cap_padded / kRecPerWarp * 4, h->stream));
     const size_t ntiles = h->cap_padded / kTile;
@@ -755,7 +763,7 @@ void am_sweep_destroy(am_sweep_t* h) {
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();  // ticks may have been issued on caller streams
   for (int k = 0; k < 16; ++k) if (h->col_ptr[k]) cudaFree(h->col_ptr[k]);
-  for (uint64_t* pc : {h->pk.minute, h->pk.hour, h->pk.dom, h->pk.month, h->pk.dow}) if (pc) cudaFree(pc);
+  if (h->planes.w) cudaFree(h->planes.w);
   if (h->seg_dirty) cudaFree(h->seg_dirty);
   for (int b = 0; b < 2; ++b) {
     TickOut& t = h->set[b].out;
@@ -836,10 +844,10 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
     if (src) AM_CUDA(h, cudaMemcpyAsync(dst, src, n * kColElem[k], cudaMemcpyHostToDevice, h->stream));
     else AM_CUDA(h, cudaMemsetAsync(dst, 0, n * kColElem[k], h->stream));
   }
-  {  // repack every segment that overlaps the range, the partial ones at either end included
+  {  // rebuild the planes of every segment that overlaps the range, the partial ones at either end included
     const uint64_t seg0 = first / kRecPerWarp, seg1 = (first + n + kRecPerWarp - 1) / kRecPerWarp;
     const uint64_t n_seg = seg1 - seg0;
-    AM_LAUNCH(pack_range_kernel, (unsigned)((n_seg + kWarps - 1) / kWarps), kBlock, h->stream, h->cols, h->pk,
+    AM_LAUNCH(build_planes_range_kernel, (unsigned)((n_seg + kWarps - 1) / kWarps), kBlock, h->stream, h->cols, h->planes,
               (uint32_t)seg0, (uint32_t)n_seg);
     h->launches++;
     AM_CUDA(h, cudaGetLastError());

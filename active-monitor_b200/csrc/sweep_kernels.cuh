@@ -17,18 +17,20 @@
 //     1024 consecutive records, a warp owns 128 of them;
 //   * every warp-level load instruction is fully coalesced: lane L reads the
 //     16 B (two u64 records) or 8 B (two i32 records) at column + (w + 2L),
-//     twice per tile ("halves"), so 16 independent loads are in flight per
-//     lane before the first use (a __syncwarp() after them keeps ptxas from
-//     delaying half of them).  Staging the tile in shared memory instead —
+//     twice per tile ("halves"), plus one 16-B warp-uniform load per cron-mask
+//     bit plane, all in flight before the first use (a __syncwarp() after them
+//     keeps ptxas from delaying half of them).  Staging the tile in shared memory instead —
 //     per-lane cp.async, TMA bulk copies one-shot, and a persistent two-stage
 //     TMA pipeline — was built, verified and measured slower for this
 //     streaming, near-issue-bound kernel (DESIGN.md section 3);
 //   * the tick's broken-down time is computed once per tick as one-hot words
 //     and reaches every CTA through the kernel parameters (constant bank); a
 //     5-field schedule fires iff minute&M && hour&H && month&Mo && dayMatches
-//     (five ANDs, no loop);
+//     (five ANDs, no loop) — on the minute evaluated 32 records per word from
+//     the six bit planes (MaskPlanes) those words select;
 //   * remedy/counter columns are touched only by lanes whose record has a
-//     posted result (or is due, in closed-loop mode): 56 B/record otherwise;
+//     posted result (or is due, in closed-loop mode): 16 B/record otherwise, plus
+//     0.75 B of mask planes on the minute;
 //   * the emitted set leaves the kernel as a BITMAP (one bit per record: the four
 //     warp ballots the kernel takes anyway, interleaved into four 32-record words
 //     per warp, one 128-B line per tile) plus a per-tile list of EXCEPTIONS — the
@@ -231,12 +233,16 @@ __global__ void tz_words_kernel(const int32_t* __restrict__ tz_off, TickWords* _
 #ifndef AM_MIN_BLOCKS
 #define AM_MIN_BLOCKS 3
 #endif
-// MASKS = the five cron-field columns are read and matched.  Off the minute a
-// 5-field schedule cannot fire (ParseStandard pins Second to 1<<0), so the
-// launcher picks MASKS=false unless AM_SWEEP_FULL_SCAN is set: 40 of the 56
-// bytes per record and all of the mask arithmetic disappear at compile time.
+// MASKS = the cron masks are read (as the six bit planes T tests) and matched.  Off
+// the minute a 5-field schedule cannot fire (ParseStandard pins Second to 1<<0), so
+// the launcher picks MASKS=false unless AM_SWEEP_FULL_SCAN is set: the plane loads
+// and all of the mask arithmetic disappear at compile time.
+// Registers: the closed-loop on-minute variant runs at AM_MIN_BLOCKS CTAs per SM (80 registers) and loads
+// both halves' remedy state at once in its dense result path; the other three fit 64 registers without
+// spills at one more CTA per SM, one half at a time (the open-loop on-minute sweep measured faster so).
 template <bool CLOSED, bool MASKS>
-__global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1) sweep_tick_kernel(const SweepParams p) {
+__global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1)
+    sweep_tick_kernel(const SweepParams p) {
   // one row per warp, written unconditionally: no zero-initialisation, no shared
   // atomics, and therefore a single __syncthreads in the whole kernel
   __shared__ uint32_t s_warp_tot[kWarps], s_warp_exc[kWarps];
@@ -257,7 +263,6 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
   // ---- phase A: issue every schedule-column load of this lane up front ----
   // half h covers records r0(h) .. r0(h)+1, r0 = tile_base + warp*128 + h*64 + lane*2
   uint32_t r0[2];
-  ulonglong2 mi[2], hr[2], dm[2], mo[2], dw[2];
   longlong2 fa[2];
   int2 ras[2];
   uint2 fl[2];
@@ -268,36 +273,18 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
     ras[h] = ld_stream(reinterpret_cast<const int2*>(p.c.ras + r0[h]));
     fa[h] = ld_stream(reinterpret_cast<const longlong2*>(p.c.finished_at + r0[h]));
   }
-  // The masks come from the packed copy (PackedMasks): only the segment's CRON_SPEC records have slots
-  // there, so the flags decide which slots exist.  A record's slot is its rank among the segment's cron
-  // records in record order: half 0's records (lanes' pairs 2L, 2L+1) before half 1's.  Lane L loads
-  // slots 2L, 2L+1 of each half that has any: ~0.4 of the mask bytes at the population's 40 % cron records.
-  uint32_t n_cron = 0, rank[2][2] = {{0, 0}, {0, 0}};
+  // The masks come from the six bit planes T tests (MaskPlanes): the warp's 128 records are 4 words of
+  // each, one 16-B load per plane that every lane of the warp makes at the same address.  Nothing about
+  // them depends on the flags.
+  uint4 pmi, phr, pdm, pmo, pdw, pst;
   if (MASKS) {
-    const bool c00 = (fl[0].x & AM_KIND_MASK) == AM_KIND_CRON_SPEC, c01 = (fl[0].y & AM_KIND_MASK) == AM_KIND_CRON_SPEC;
-    const bool c10 = (fl[1].x & AM_KIND_MASK) == AM_KIND_CRON_SPEC, c11 = (fl[1].y & AM_KIND_MASK) == AM_KIND_CRON_SPEC;
-    const unsigned b00 = __ballot_sync(kFull, c00), b01 = __ballot_sync(kFull, c01);
-    const unsigned b10 = __ballot_sync(kFull, c10), b11 = __ballot_sync(kFull, c11);
-    const unsigned lt = (1u << lane) - 1u;
-    const uint32_t n_half0 = (uint32_t)(__popc(b00) + __popc(b01));
-    n_cron = n_half0 + (uint32_t)(__popc(b10) + __popc(b11));
-    rank[0][0] = (uint32_t)(__popc(b00 & lt) + __popc(b01 & lt));
-    rank[0][1] = rank[0][0] + (uint32_t)c00;
-    rank[1][0] = n_half0 + (uint32_t)(__popc(b10 & lt) + __popc(b11 & lt));
-    rank[1][1] = rank[1][0] + (uint32_t)c10;
-    const uint32_t seg = tile_base + (uint32_t)(warp * kRecPerWarp);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const uint32_t slot = (uint32_t)(h * 64 + lane * 2);
-      mi[h] = hr[h] = dm[h] = mo[h] = dw[h] = make_ulonglong2(0ull, 0ull);
-      if (slot < n_cron) {
-        mi[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.minute + seg + slot));
-        hr[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.hour + seg + slot));
-        dm[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.dom + seg + slot));
-        mo[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.month + seg + slot));
-        dw[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.pk.dow + seg + slot));
-      }
-    }
+    const uint32_t wq = (tile_base + (uint32_t)(warp * kRecPerWarp)) / 32u;
+    pmi = ld_stream(reinterpret_cast<const uint4*>(p.pl.minute + wq));
+    phr = ld_stream(reinterpret_cast<const uint4*>(p.pl.hour + wq));
+    pdm = ld_stream(reinterpret_cast<const uint4*>(p.pl.dom + wq));
+    pmo = ld_stream(reinterpret_cast<const uint4*>(p.pl.month + wq));
+    pdw = ld_stream(reinterpret_cast<const uint4*>(p.pl.dow + wq));
+    pst = ld_stream(reinterpret_cast<const uint4*>(p.pl.star + wq));
   }
 
   // Scheduling fence: a warp-level memory-ordering point.  ptxas may not sink the loads
@@ -314,27 +301,41 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
   const uint32_t fl_or = fl[0].x | fl[0].y | fl[1].x | fl[1].y;
   const bool warp_tz = MASKS && p.tz_table != nullptr && __any_sync(kFull, (fl_or >> AM_F_TZ_SHIFT) != 0);
 
-  // Every packed slot is matched in packed order; bit L of match[h][j] = slot h*64 + 2L + j fires.  A
-  // record then takes bit `rank` (its own slot) of these four ballots.
-  unsigned match[2][2] = {{0u, 0u}, {0u, 0u}};
+  // cron_matches for 32 records per word: sec0 & MIN[m] & HR[h] & MO[mo] & dayMatches, where dayMatches
+  // is DOM[d] & DOW[w] under the star bit S and DOM[d] | DOW[w] without it.  Word k of the segment holds
+  // its records 32k .. 32k+31: the lane's records of half h are bits (2L & 31) + j of word 2h + (L >> 4).
+  uint32_t cron_bits = 0;  // bit (2h+j): the record's 5-field schedule fires at T
   if (MASKS) {
+    const uint32_t gate = w.sec0 ? kFull : 0u;
+    auto word = [&](int k) {
+      const uint32_t mi = k == 0 ? pmi.x : k == 1 ? pmi.y : k == 2 ? pmi.z : pmi.w;
+      const uint32_t hr = k == 0 ? phr.x : k == 1 ? phr.y : k == 2 ? phr.z : phr.w;
+      const uint32_t dm = k == 0 ? pdm.x : k == 1 ? pdm.y : k == 2 ? pdm.z : pdm.w;
+      const uint32_t mo = k == 0 ? pmo.x : k == 1 ? pmo.y : k == 2 ? pmo.z : pmo.w;
+      const uint32_t dw = k == 0 ? pdw.x : k == 1 ? pdw.y : k == 2 ? pdw.z : pdw.w;
+      const uint32_t st = k == 0 ? pst.x : k == 1 ? pst.y : k == 2 ? pst.z : pst.w;
+      return gate & mi & hr & mo & ((st & dm & dw) | (~st & (dm | dw)));
+    };
+    const uint32_t sh = (uint32_t)(2 * lane) & 31u;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+    for (int h = 0; h < 2; ++h) cron_bits |= (((lane >> 4) ? word(2 * h + 1) : word(2 * h)) >> sh & 3u) << (2 * h);
+    if (warp_tz) {  // warp-uniform: some record of this warp is bound to a named time zone
 #pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const uint64_t miv = j ? mi[h].y : mi[h].x, hrv = j ? hr[h].y : hr[h].x;
-        const uint64_t dmv = j ? dm[h].y : dm[h].x, mov = j ? mo[h].y : mo[h].x;
-        const uint64_t dwv = j ? dw[h].y : dw[h].x;
-        bool m = cron_matches(w, miv, hrv, dmv, mov, dwv);
-        if (warp_tz) {  // warp-uniform: some record of this warp is bound to a named time zone
-          const uint32_t tz = (uint32_t)(hrv >> kPackTzShift) & 0xFFu;
-          // the zone's wall clock instead of UTC's — behind a real call: inlined, ptxas turned the zone
-          // lookup of all four slots into predicated instructions that EVERY warp issues (+24 LDG,
-          // +40 address IMADs per warp, a clearly slower 10 M-record tick with 0.6 % zone-bound records)
-          if (tz && (uint32_t)(h * 64 + lane * 2 + j) < n_cron)
-            m = cron_matches_in_zone(p.tz_table + tz, miv, hrv, dmv, mov, dwv);
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const uint32_t f = j ? fl[h].y : fl[h].x;
+          const uint32_t tz = f >> AM_F_TZ_SHIFT;
+          // zone-bound records have no plane bits: their canonical masks against the zone's wall clock,
+          // behind a real call (inlined, ptxas turned the zone lookup of all four records into predicated
+          // instructions that EVERY warp issues: a clearly slower 10 M-record tick with 0.6 % zone-bound records)
+          if (tz && (f & AM_KIND_MASK) == AM_KIND_CRON_SPEC) {
+            const uint32_t i = r0[h] + (uint32_t)j;
+            const bool m = cron_matches_in_zone(p.tz_table + tz, ld_stream(p.c.minute + i), ld_stream(p.c.hour + i),
+                                                ld_stream(p.c.dom + i), ld_stream(p.c.month + i), ld_stream(p.c.dow + i));
+            cron_bits |= (m ? 1u : 0u) << (2 * h + j);
+          }
         }
-        match[h][j] = __ballot_sync(kFull, m);
       }
     }
   }
@@ -367,12 +368,10 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
       // hcc.go:161) the reference submits whatever finishedAt says
       const bool armed = has_result || (f & AM_F_TIMER_ARMED) != 0;
       const bool due_iv = !((elapsed < (int64_t)rasv) & armed);
+      // (an if, not `MASKS && ...`: with the latter ptxas hoisted this loop's arithmetic above the
+      // __syncwarp fence in the MASKS=false variants and delayed the second half's loads behind it)
       bool due_cron = false;
-      if (MASKS) {  // (for a record that is not CRON_SPEC the bit read here is another record's: unused)
-        const uint32_t r = rank[h][j];
-        const unsigned m = (r & 64u) ? ((r & 1u) ? match[1][1] : match[1][0]) : ((r & 1u) ? match[0][1] : match[0][0]);
-        due_cron = ((m >> ((r >> 1) & 31u)) & 1u) != 0;
-      }
+      if (MASKS) due_cron = ((cron_bits >> (2 * h + j)) & 1u) != 0;
       const bool is_iv = ((0x14u >> kind) & 1u) != 0;  // INTERVAL or CRON_EVERY
       const bool due = live && (is_iv ? due_iv : (kind == AM_KIND_CRON_SPEC && due_cron));
       const bool stopped_now = live && kind == AM_KIND_STOPPED && !(f & AM_F_STOPPED_REPORTED);
@@ -418,7 +417,7 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
   //         its next needy record with scalar accesses — the loop runs once or twice
   //         instead of four predicated copies of the state machine.
   if (__popc(__ballot_sync(kFull, needy != 0)) >= 16) {
-    // both halves' loads first (sixteen more in flight per lane: the mask registers are dead by now),
+    // at 80 registers both halves' loads first (sixteen more in flight per lane),
     // then the state machines, then the stores — a half's stores would otherwise fence the other
     // half's loads behind them (the compiler cannot tell the columns apart)
     int2 lim[2], rst[2], sc[2], fc[2], rsc[2], rfc[2], rtc[2];
@@ -436,7 +435,7 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
         rfa[h] = ld_stream(reinterpret_cast<const longlong2*>(p.c.remedy_finished_at + r));
       }
     };
-    if (MASKS) {  // (the variants without the mask columns run at 64 registers: one half at a time there)
+    if (CLOSED && MASKS) {  // (the variants at 64 registers: one half at a time)
       load_half(0);
       load_half(1);
       __syncwarp();
@@ -444,7 +443,7 @@ __global__ void __launch_bounds__(kBlock, MASKS ? AM_MIN_BLOCKS : AM_MIN_BLOCKS 
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const uint32_t nb = (needy >> (2 * h)) & 3u;
-      if (!MASKS) load_half(h);
+      if (!(CLOSED && MASKS)) load_half(h);
       if (nb) {
         const uint32_t r = r0[h];
         int32_t ns[2] = {sc[h].x, sc[h].y}, nf[2] = {fc[h].x, fc[h].y};
@@ -992,7 +991,7 @@ __global__ void mark_ops_kernel(uint32_t* marks, const uint2* __restrict__ ops, 
 }
 
 // upserts (hcc.go:170-188 Reconcile) and removes (hcc.go:175-186).  Both may change the slot's kind or
-// masks: its segment is marked for pack_dirty_kernel.
+// masks: its segment is marked for build_planes_dirty_kernel.
 __global__ void apply_state_ops_kernel(DevCols c, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops,
                                        const am_record_t* __restrict__ recs, uint32_t n, uint32_t* seg_dirty) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
@@ -1013,58 +1012,60 @@ __global__ void apply_state_ops_kernel(DevCols c, const uint32_t* __restrict__ m
   c.remedy_finished_at[i] = r.remedy_finished_at;
 }
 
-// ---- the packed mask copy (PackedMasks) -----------------------------------
-// Repack segment `seg` with one warp: lane L looks at records 4L .. 4L+3 of the segment, an exclusive
-// prefix of the lanes' cron counts gives each cron record its slot.  (The sweep derives the same slots
-// from its own record-to-lane layout; the two are independent formulations of "rank in record order".)
-__device__ __forceinline__ void pack_segment(const DevCols& c, const PackedMasks& pk, uint32_t seg, int lane) {
-  const uint32_t first = seg * (uint32_t)kRecPerWarp + (uint32_t)lane * 4u;
-  const uint4 f4 = *reinterpret_cast<const uint4*>(c.flags + first);
-  const uint32_t f[4] = {f4.x, f4.y, f4.z, f4.w};
-  uint32_t mine = 0;
+// ---- the mask bit planes (MaskPlanes) --------------------------------------
+// bit v of a record's masks for plane P (the star plane: bit 63 of dom or dow)
+__device__ __forceinline__ bool plane_bit(int P, uint64_t mi, uint64_t hr, uint64_t dm, uint64_t mo, uint64_t dw) {
+  if (P < kPlaneHour) return (mi >> (P - kPlaneMinute)) & 1u;
+  if (P <= kPlaneDom) return (hr >> (P - kPlaneHour)) & 1u;
+  if (P <= kPlaneMonth) return (dm >> (P - kPlaneDom)) & 1u;
+  if (P < kPlaneDow) return (mo >> (P - kPlaneMonth)) & 1u;
+  if (P < kPlaneStar) return (dw >> (P - kPlaneDow)) & 1u;
+  return ((dm | dw) >> 63) != 0;
+}
+
+// Rebuild the plane words of segment `seg` with one warp, a 32-record quarter (one word per plane) at a
+// time: lane L reads record 32q + L of the segment, one ballot per plane gives the word, and lane L
+// stores planes L, L + 32, ...
+__device__ __forceinline__ void build_segment_planes(const DevCols& c, const MaskPlanes& pl, uint32_t seg, int lane) {
+  for (uint32_t q = 0; q < (uint32_t)kRecPerWarp / 32u; ++q) {
+    const uint32_t wq = seg * (uint32_t)(kRecPerWarp / 32) + q;
+    const uint32_t i = wq * 32u + (uint32_t)lane;
+    const uint32_t f = c.flags[i];
+    const bool on = (f & AM_KIND_MASK) == AM_KIND_CRON_SPEC && (f >> AM_F_TZ_SHIFT) == 0;
+    const uint64_t mi = c.minute[i], hr = c.hour[i], dm = c.dom[i], mo = c.month[i], dw = c.dow[i];
+    uint32_t mine[(kPlanes + 31) / 32] = {};
 #pragma unroll
-  for (int q = 0; q < 4; ++q) mine |= ((f[q] & AM_KIND_MASK) == AM_KIND_CRON_SPEC ? 1u : 0u) << q;
-  const uint32_t cnt = (uint32_t)__popc(mine);
-  uint32_t incl = cnt;
+    for (int P = 0; P < kPlanes; ++P) {
+      const uint32_t b = __ballot_sync(kFull, on && plane_bit(P, mi, hr, dm, mo, dw));
+      if ((P & 31) == lane) mine[P / 32] = b;
+    }
 #pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t up = __shfl_up_sync(kFull, incl, d);
-    if (lane >= d) incl += up;
-  }
-  uint32_t slot = seg * (uint32_t)kRecPerWarp + incl - cnt;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    if ((mine >> q) & 1u) {
-      const uint32_t i = first + (uint32_t)q;
-      const uint64_t tz = f[q] >> AM_F_TZ_SHIFT;
-      pk.minute[slot] = c.minute[i];
-      pk.hour[slot] = (c.hour[i] & ~(0xFFull << kPackTzShift)) | (tz << kPackTzShift);
-      pk.dom[slot] = c.dom[i];
-      pk.month[slot] = c.month[i];
-      pk.dow[slot] = c.dow[i];
-      ++slot;
+    for (int k = 0; k < (kPlanes + 31) / 32; ++k) {
+      const uint32_t P = (uint32_t)(32 * k + lane);
+      if (P < (uint32_t)kPlanes) pl.w[P * pl.words + wq] = mine[k];
     }
   }
 }
-static_assert(kRecPerWarp == 32 * 4, "pack_segment: four records per lane");
+static_assert(kRecPerWarp % 32 == 0, "build_segment_planes: whole plane words per segment");
 
 // every segment of [seg0, seg0 + n_seg), one warp each (am_sweep_load_range)
-__global__ void pack_range_kernel(DevCols c, PackedMasks pk, uint32_t seg0, uint32_t n_seg) {
+__global__ void build_planes_range_kernel(DevCols c, MaskPlanes pl, uint32_t seg0, uint32_t n_seg) {
   const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (w >= n_seg) return;  // warp-uniform
-  pack_segment(c, pk, seg0 + w, (int)(threadIdx.x & 31));
+  build_segment_planes(c, pl, seg0 + w, (int)(threadIdx.x & 31));
 }
 
 // After apply_state_ops_kernel: one warp per staged op.  The first warp that claims a segment marked
-// there repacks it, so the cost is one claim per op plus one repack per segment touched.
-__global__ void pack_dirty_kernel(DevCols c, PackedMasks pk, uint32_t* seg_dirty, const uint2* __restrict__ ops, uint32_t n) {
+// there rebuilds it, so the cost is one claim per op plus one rebuild per segment touched.
+__global__ void build_planes_dirty_kernel(DevCols c, MaskPlanes pl, uint32_t* seg_dirty, const uint2* __restrict__ ops,
+                                          uint32_t n) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (k >= n) return;  // warp-uniform
   const int lane = (int)(threadIdx.x & 31);
   const uint32_t seg = ops[k].x / (uint32_t)kRecPerWarp;
   const bool won = lane == 0 && atomicAnd(&seg_dirty[seg], 0u) != 0u;  // (an exchange with 0)
-  if (__ballot_sync(kFull, won)) pack_segment(c, pk, seg, lane);
+  if (__ballot_sync(kFull, won)) build_segment_planes(c, pl, seg, lane);
 }
 
 // terminal phases observed by the watch loops (hcc.go:635/:662/:821/:836).  The winner of

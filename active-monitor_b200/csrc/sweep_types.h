@@ -71,16 +71,31 @@ struct DevCols {
   int64_t* remedy_finished_at;
 };
 
-// A copy of the five cron-mask columns that only the on-minute sweep reads.  A "segment" is the
-// kRecPerWarp records one warp of sweep_tick_kernel owns; slots 0 .. k-1 of a segment hold the masks
-// of its k CRON_SPEC records ((flags & AM_KIND_MASK) == AM_KIND_CRON_SPEC) in ascending record order,
-// the slots after them are unspecified.  The hour word carries the record's time-zone id in bits
-// 24..31 (the matcher tests bits 0..23 of it only).  Every write of the canonical masks or of the kind
-// bits repacks the segments it touched (pack_segment); nothing else reads the copy.
-struct PackedMasks {
-  uint64_t *minute, *hour, *dom, *month, *dow;
+// The cron masks as the on-minute sweep reads them: one bit plane per value a field of the tick's
+// one-hot words can take (minute 0..59, hour 0..23, dom 1..31, month 1..12, dow 0..6) plus the robfig
+// star bit (bit 63 of dom OR bit 63 of dow), each a bitmap over the shard with one bit per record.
+// Bit r of plane P is bit v of the field's mask of record r, set only for CRON_SPEC records that are
+// not bound to a time zone (flags bits 24..31 zero); every other record is zero in every plane.  A
+// mask bit outside those ranges is never tested by cron_matches, so it has no plane.  Plane-major:
+// plane P is words [P * words, (P + 1) * words).  A "segment" is the kRecPerWarp records one warp of
+// sweep_tick_kernel owns (4 words of a plane); every write of the canonical masks or of the kind or
+// zone bits rebuilds the segments it touched (build_segment_planes); nothing else reads the planes.
+// Plane of value v of a field: kPlane<field> + v.
+constexpr int kPlaneMinute = 0;   // minute 0..59: planes 0..59
+constexpr int kPlaneHour = 60;    // hour 0..23: planes 60..83
+constexpr int kPlaneDom = 83;     // dom 1..31: planes 84..114
+constexpr int kPlaneMonth = 114;  // month 1..12: planes 115..126
+constexpr int kPlaneDow = 127;    // dow 0..6: planes 127..133
+constexpr int kPlaneStar = 134;
+constexpr int kPlanes = 135;
+struct MaskPlanes {
+  uint32_t* w;     // [kPlanes * words]
+  uint64_t words;  // per plane: cap_padded / 32
 };
-constexpr int kPackTzShift = 24;
+// The six planes one tick tests (T's UTC minute, hour, dom, month, dow, and the star plane)
+struct TickPlanes {
+  const uint32_t *minute, *hour, *dom, *month, *dow, *star;
+};
 
 // What one tick of one shard leaves behind for the list rebuild (expand_kernel) and for the
 // NVLink exchange: the same four arrays whether they are the sweep's own buffers or the copy
@@ -95,7 +110,7 @@ struct TickOut {
 
 struct SweepParams {
   DevCols c;
-  PackedMasks pk;  // read by the MASKS variants instead of the five canonical mask columns
+  TickPlanes pl;  // read by the MASKS variants instead of the five canonical mask columns
   uint64_t n_records;
   uint64_t shard_base;
   uint64_t seed;

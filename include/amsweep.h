@@ -379,9 +379,10 @@ int am_sweep_last_profile(am_sweep_t*, double* sweep_ms, double* rest_ms);
 uint64_t am_sweep_launch_count(const am_sweep_t*);
 /* Raw device pointer of a column (for zero-copy wrapping by torch / NCCL
  * plumbing); column ids follow am_record_cols_t member order, 0..15.
- * The five cron-mask columns (0..4) and the kind bits of the flags column
- * (AM_KIND_MASK) must not be written through this pointer: the on-minute sweep
- * reads a packed copy of the masks that only am_sweep_load_range, upserts and
+ * The five cron-mask columns (0..4) and the kind and zone-id bits of the flags
+ * column (AM_KIND_MASK, AM_F_TZ_MASK) must not be written through this
+ * pointer: the on-minute sweep reads the masks as bit planes (one bitmap over the
+ * shard per value a field can take) that only am_sweep_load_range, upserts and
  * removes keep up to date.  The other flag bits and the other columns may be. */
 void* am_sweep_column_ptr(am_sweep_t*, int column);
 int am_sweep_set_seed(am_sweep_t*, uint64_t seed);
