@@ -17,10 +17,11 @@
 //   posted result / carry bits  the first tick of the block
 //
 // and at an event tick evaluates EXACTLY what sweep_tick_kernel evaluates for that (record, tick) —
-// same ladder, same apply_result, same closed-loop outcome key — so the per-tick statistics and the
-// columns after the block are bit-identical to K single ticks (tests: run_ticks blocked == unblocked ==
-// oracle).  Work is O(events), not O(records x ticks); the columns are read and written once per K
-// ticks.  What it does NOT produce is the per-tick (index, action) lists: a run of ticks publishes
+// interval_due and is_interval_kind for the schedule ladder, result_step for the posted result and the
+// closed-loop completion, load_state / store_changed_state for the remedy and counter columns — so the
+// per-tick statistics and the columns after the block are bit-identical to K single ticks (tests:
+// run_ticks blocked == unblocked == oracle).  Work is O(events), not O(records x ticks); the columns are
+// read and written once per K ticks.  What it does NOT produce is the per-tick (index, action) lists: a run of ticks publishes
 // per-tick statistics (counts, action counts, index checksums — am_tick_stats_t), which is all
 // am_sweep_run_ticks ever returned to the host.  Reported separately from the K = 1 roofline number.
 #pragma once
@@ -94,7 +95,7 @@ __device__ __forceinline__ void block_record(const BlockParams& p, BlockStats& S
   const int32_t rasv = ld_stream(p.c.ras + i);
   int64_t fa = ld_stream(p.c.finished_at + i);
   const uint32_t kind = f & AM_KIND_MASK;
-  const bool is_iv = ((0x14u >> kind) & 1u) != 0;  // INTERVAL or CRON_EVERY
+  const bool is_iv = is_interval_kind(kind);
   const bool is_cron = kind == AM_KIND_CRON_SPEC;
   int32_t zoff = 0;
   uint64_t mi = 0, hr = 0, dm = 0, mo = 0, dw = 0;
@@ -107,12 +108,7 @@ __device__ __forceinline__ void block_record(const BlockParams& p, BlockStats& S
   // remedy / counter state: every due record needs it in closed loop, a posted result in open loop
   RecState s{};
   const bool with_state = CLOSED || (f & kPend) != 0;
-  if (with_state) {
-    s.limit = ld_stream(p.c.runs_limit + i); s.reset = ld_stream(p.c.reset_interval + i);
-    s.s = ld_stream(p.c.success + i); s.f = ld_stream(p.c.failed + i);
-    s.rs = ld_stream(p.c.remedy_success + i); s.rf = ld_stream(p.c.remedy_failed + i);
-    s.rt = ld_stream(p.c.remedy_total + i); s.rfa = ld_stream(p.c.remedy_finished_at + i);
-  }
+  if (with_state) load_state(p.c, i, s);
   const RecState s0 = s;
   const uint32_t f0 = f;
   const int64_t fa0 = fa;
@@ -132,12 +128,8 @@ __device__ __forceinline__ void block_record(const BlockParams& p, BlockStats& S
   while (t < K) {
     const int64_t T = p.T0 + t;
     // ---- exactly sweep_tick_kernel's decision for (record, T) ----
-    const bool has_result = (f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL)) != 0;
     const bool pending = (f & kPend) != 0;
-    const int64_t fa_eff = has_result ? T : fa;
-    const int64_t elapsed = (int64_t)((uint64_t)T - (uint64_t)fa_eff);
-    const bool armed = has_result || (f & AM_F_TIMER_ARMED) != 0;
-    const bool due_iv = !((elapsed < (int64_t)rasv) & armed);
+    const bool due_iv = interval_due(f, rasv, fa, T);
     bool due_cron = false;
     if (is_cron) {
       const TickWords w = tick_words_from_unix(T + (int64_t)zoff);
@@ -159,16 +151,7 @@ __device__ __forceinline__ void block_record(const BlockParams& p, BlockStats& S
     if (pending || (CLOSED && due)) {
       s.flags = f;
       s.fa = fa;
-      uint32_t a = apply_result(s, T, res);
-      if (CLOSED && due) {
-        const uint64_t key = outcome_key(p.seed, g, (uint64_t)T);
-        const uint32_t failp = (s.flags >> AM_F_FAILP_SHIFT) & 0xFFu;
-        const bool fail = (uint32_t)(key & 0xFF) < failp;
-        const bool rem_ok = (uint32_t)((key >> 8) & 0xFF) < 179u;
-        s.flags |= (fail ? AM_F_PENDING_FAIL : AM_F_PENDING_OK) | AM_F_REMEDY_PENDING | (rem_ok ? AM_F_REMEDY_OUTCOME_OK : 0u);
-        a |= apply_result(s, T, res);
-      }
-      act |= a;
+      act |= result_step<CLOSED>(s, T, due, p.seed, g, res);
       f = s.flags;
       fa = s.fa;
     }
@@ -199,14 +182,7 @@ __device__ __forceinline__ void block_record(const BlockParams& p, BlockStats& S
   // ---- write back what changed ----
   if (f != f0) st_stream(p.c.flags + i, f);
   if (fa != fa0) st_stream(p.c.finished_at + i, fa);
-  if (with_state) {
-    if (s.s != s0.s) st_stream(p.c.success + i, s.s);
-    if (s.f != s0.f) st_stream(p.c.failed + i, s.f);
-    if (s.rs != s0.rs) st_stream(p.c.remedy_success + i, s.rs);
-    if (s.rf != s0.rf) st_stream(p.c.remedy_failed + i, s.rf);
-    if (s.rt != s0.rt) st_stream(p.c.remedy_total + i, s.rt);
-    if (s.rfa != s0.rfa) st_stream(p.c.remedy_finished_at + i, s.rfa);
-  }
+  if (with_state) store_changed_state(p.c, i, s, s0);
 }
 
 template <bool CLOSED>
@@ -245,8 +221,7 @@ __global__ void __launch_bounds__(kBlockThreads, AM_BLOCK_MIN_CTAS) sweep_block_
       const int64_t fa = q == 0 ? a01.x : q == 1 ? a01.y : q == 2 ? a23.x : a23.y;
       const uint32_t loc = loc0 + (uint32_t)q;
       const uint32_t kind = f & AM_KIND_MASK;
-      const bool live = ((0x3Eu >> kind) & 1u) && !(f & AM_F_TOMBSTONE);
-      if (!live) continue;  // tombstones, NO_RESOURCE (hcc.go:227), host-fallback: never evaluated
+      if (!is_live(f)) continue;  // tombstones, NO_RESOURCE (hcc.go:227), host-fallback: never evaluated
       const bool first_tick = (f & (kPend | AM_F_CARRY_MASK)) != 0;  // a posted result / carried action: an event at tick 0
       const uint64_t g = p.shard_base + cta_base + loc;
       int64_t n_ev = 0;  // expected events in the block (an upper bound is fine: it only picks the list)

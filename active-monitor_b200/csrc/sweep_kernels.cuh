@@ -190,6 +190,67 @@ __device__ __forceinline__ uint32_t apply_result(RecState& r, int64_t T, uint32_
   return act;
 }
 
+// apply_result, and in the closed-loop harness (SURVEY §8d config 5) a record due at T then completes in
+// the same tick: the outcome keyed by (seed, global index, T) is posted and applied as well.
+template <bool CLOSED>
+__device__ __forceinline__ uint32_t result_step(RecState& r, int64_t T, bool due, uint64_t seed, uint64_t g, uint32_t& res) {
+  uint32_t act = apply_result(r, T, res);
+  if (CLOSED && due) {
+    const uint64_t k = outcome_key(seed, g, (uint64_t)T);
+    const uint32_t failp = (r.flags >> AM_F_FAILP_SHIFT) & 0xFFu;
+    const bool fail = (uint32_t)(k & 0xFF) < failp;
+    const bool rem_ok = (uint32_t)((k >> 8) & 0xFF) < 179u;
+    r.flags |= (fail ? AM_F_PENDING_FAIL : AM_F_PENDING_OK) | AM_F_REMEDY_PENDING | (rem_ok ? AM_F_REMEDY_OUTCOME_OK : 0u);
+    act |= apply_result(r, T, res);
+  }
+  return act;
+}
+
+// The eight remedy / counter columns of record i, streamed in (flags and finishedAt are the caller's) ...
+template <typename I>
+__device__ __forceinline__ void load_state(const DevCols& c, I i, RecState& r) {
+  r.limit = ld_stream(c.runs_limit + i); r.reset = ld_stream(c.reset_interval + i);
+  r.s = ld_stream(c.success + i); r.f = ld_stream(c.failed + i);
+  r.rs = ld_stream(c.remedy_success + i); r.rf = ld_stream(c.remedy_failed + i);
+  r.rt = ld_stream(c.remedy_total + i); r.rfa = ld_stream(c.remedy_finished_at + i);
+}
+// ... and those of them that r changed against r0, streamed out
+template <typename I>
+__device__ __forceinline__ void store_changed_state(const DevCols& c, I i, const RecState& r, const RecState& r0) {
+  if (r.s != r0.s) st_stream(c.success + i, r.s);
+  if (r.f != r0.f) st_stream(c.failed + i, r.f);
+  if (r.rs != r0.rs) st_stream(c.remedy_success + i, r.rs);
+  if (r.rf != r0.rf) st_stream(c.remedy_failed + i, r.rf);
+  if (r.rt != r0.rt) st_stream(c.remedy_total + i, r.rt);
+  if (r.rfa != r0.rfa) st_stream(c.remedy_finished_at + i, r.rfa);
+}
+
+// The lanes' result counts (four 8-bit counts each, as apply_result adds them) summed over the warp: lane
+// q < 4 gets counter q {ok, fail, remedy ok, remedy fail}.  Two redux over 16-bit halves; every lane calls it.
+__device__ __forceinline__ uint32_t warp_result_count(uint32_t res, int lane) {
+  uint32_t lo = 0, hi = 0;
+  if (__any_sync(kFull, res != 0)) {
+    lo = __reduce_add_sync(kFull, (res & 0xFFu) | ((res & 0xFF00u) << 8));           // ok | fail<<16
+    hi = __reduce_add_sync(kFull, ((res >> 16) & 0xFFu) | ((res >> 8) & 0xFF0000u));  // remedy ok | fail<<16
+  }
+  return ((lane < 2 ? lo : hi) >> ((lane & 1) * 16)) & 0xFFFFu;
+}
+
+// kinds 1..5 are evaluated; tombstones, NO_RESOURCE (hcc.go:227) and host-fallback are not
+__device__ __forceinline__ bool is_live(uint32_t f) { return ((0x3Eu >> (f & AM_KIND_MASK)) & 1u) && !(f & AM_F_TOMBSTONE); }
+// INTERVAL or CRON_EVERY: due by the repeat timer
+__device__ __forceinline__ bool is_interval_kind(uint32_t kind) { return ((0x14u >> kind) & 1u) != 0; }
+
+// The interval rule, not(hcc.go:264): "elapsed < RepeatAfterSec && timer != nil" skips.  A posted result
+// is applied first (step 1): finishedAt = T and the timer re-armed.  Without a timer (controller restart,
+// hcc.go:161) the reference submits whatever finishedAt says.
+__device__ __forceinline__ bool interval_due(uint32_t f, int32_t ras, int64_t fa, int64_t T) {
+  const bool has_result = (f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL)) != 0;
+  const int64_t elapsed = (int64_t)((uint64_t)T - (uint64_t)(has_result ? T : fa));
+  const bool armed = has_result || (f & AM_F_TIMER_ARMED) != 0;
+  return !((elapsed < (int64_t)ras) & armed);
+}
+
 // Action bits of apply_result <-> the carry bits of the flags word (AM_F_CARRY_MASK): RUN_REMEDY (0x02)
 // in bit 11, REMEDY_SKIP .. ANOMALY (0x10 .. 0x80) in bits 12 .. 15.
 __device__ __forceinline__ uint32_t carried_actions(uint32_t f) { return ((f >> 10) & AM_ACT_RUN_REMEDY) | ((f >> 8) & 0xF0u); }
@@ -237,9 +298,10 @@ __global__ void tz_words_kernel(const int32_t* __restrict__ tz_off, TickWords* _
 // the minute a 5-field schedule cannot fire (ParseStandard pins Second to 1<<0), so
 // the launcher picks MASKS=false unless AM_SWEEP_FULL_SCAN is set: the plane loads
 // and all of the mask arithmetic disappear at compile time.
-// Registers: the closed-loop on-minute variant runs at AM_MIN_BLOCKS CTAs per SM (80 registers) and loads
-// both halves' remedy state at once in its dense result path; the other three fit 64 registers without
-// spills at one more CTA per SM, one half at a time (the open-loop on-minute sweep measured faster so).
+// Registers: the closed-loop on-minute variant runs at AM_MIN_BLOCKS CTAs per SM (80 registers, 16 B of
+// spill stores) and loads both halves' remedy state at once in its dense result path; the other three run
+// at one more CTA per SM within 64 registers, one half at a time (the open-loop on-minute sweep measured
+// faster so): the open-loop ones in 59 and 60 without spills, the closed-loop off-minute one with 20 B.
 template <bool CLOSED, bool MASKS>
 __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1)
     sweep_tick_kernel(const SweepParams p) {
@@ -353,26 +415,18 @@ __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const uint32_t f = j ? fl[h].y : fl[h].x;
-      const int32_t rasv = j ? ras[h].y : ras[h].x;
       const int64_t fav = j ? fa[h].y : fa[h].x;
-      const uint32_t kind = f & AM_KIND_MASK;
-      // kinds 1..5 are evaluated; tombstones, NO_RESOURCE (hcc.go:227) and host-fallback are not
-      const bool live = ((0x3Eu >> kind) & 1u) && !(f & AM_F_TOMBSTONE);
-      const bool has_result = (f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL)) != 0;
+      const bool live = is_live(f);
       const bool pending = (f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING)) != 0;
-      // step 1 sets finishedAt = T before the due decision is taken
-      const int64_t fa_eff = has_result ? T : fav;
-      const int64_t elapsed = (int64_t)((uint64_t)T - (uint64_t)fa_eff);
-      // not(hcc.go:264): "elapsed < RepeatAfterSec && timer != nil" skips; a posted result re-arms
-      // the timer in this very tick (step 1 runs first), and without a timer (controller restart,
-      // hcc.go:161) the reference submits whatever finishedAt says
-      const bool armed = has_result || (f & AM_F_TIMER_ARMED) != 0;
-      const bool due_iv = !((elapsed < (int64_t)rasv) & armed);
       // (an if, not `MASKS && ...`: with the latter ptxas hoisted this loop's arithmetic above the
       // __syncwarp fence in the MASKS=false variants and delayed the second half's loads behind it)
       bool due_cron = false;
       if (MASKS) due_cron = ((cron_bits >> (2 * h + j)) & 1u) != 0;
-      const bool is_iv = ((0x14u >> kind) & 1u) != 0;  // INTERVAL or CRON_EVERY
+      const uint32_t kind = f & AM_KIND_MASK;
+      const bool due_iv = interval_due(f, j ? ras[h].y : ras[h].x, fav, T);
+      const bool is_iv = is_interval_kind(kind);
+      // (the rest of the ladder is written out here and in block_record: behind a function, ptxas turned
+      // these `live && ...` into branch-free code that spilled more in the closed-loop on-minute variant)
       const bool due = live && (is_iv ? due_iv : (kind == AM_KIND_CRON_SPEC && due_cron));
       const bool stopped_now = live && kind == AM_KIND_STOPPED && !(f & AM_F_STOPPED_REPORTED);
       act[h][j] = (due ? AM_ACT_SUBMIT_HC : 0u) | (stopped_now ? AM_ACT_STOPPED : 0u) |
@@ -455,17 +509,7 @@ __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM
           if ((nb >> j) & 1u) {
             RecState s{nfl[h][j], nfa[h][j], ns[j], nf[j], nrs[j], nrf[j], nrt[j], nrfa[j], limv[j], rstv[j]};
             uint32_t res = 0;
-            uint32_t a = apply_result(s, T, res);
-            if (CLOSED && ((due_bits >> (2 * h + j)) & 1u)) {
-              const uint64_t k = outcome_key(p.seed, p.shard_base + r + (uint32_t)j, (uint64_t)T);
-              const uint32_t failp = (s.flags >> AM_F_FAILP_SHIFT) & 0xFFu;
-              const bool fail = (uint32_t)(k & 0xFF) < failp;
-              const bool rem_ok = (uint32_t)((k >> 8) & 0xFF) < 179u;
-              s.flags |= (fail ? AM_F_PENDING_FAIL : AM_F_PENDING_OK) | AM_F_REMEDY_PENDING |
-                         (rem_ok ? AM_F_REMEDY_OUTCOME_OK : 0u);
-              a |= apply_result(s, T, res);
-            }
-            act[h][j] |= a;
+            act[h][j] |= result_step<CLOSED>(s, T, (due_bits >> (2 * h + j)) & 1u, p.seed, p.shard_base + r + (uint32_t)j, res);
             res_lane += res;
             nfl[h][j] = s.flags; nfa[h][j] = s.fa;
             ns[j] = s.s; nf[j] = s.f; nrs[j] = s.rs; nrf[j] = s.rf; nrt[j] = s.rt; nrfa[j] = s.rfa;
@@ -491,32 +535,15 @@ __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM
       const int b = __ffs(needy) - 1;
       needy &= needy - 1;
       const uint32_t i = r0[0] + (uint32_t)(64 * (b >> 1) + (b & 1));
-      const int32_t lim = ld_stream(p.c.runs_limit + i), rst = ld_stream(p.c.reset_interval + i);
-      const int32_t sc = ld_stream(p.c.success + i), fc = ld_stream(p.c.failed + i);
-      const int32_t rsc = ld_stream(p.c.remedy_success + i), rfc = ld_stream(p.c.remedy_failed + i);
-      const int32_t rtc = ld_stream(p.c.remedy_total + i);
-      const int64_t rfa = ld_stream(p.c.remedy_finished_at + i);
-      const uint32_t f0 = b == 0 ? nfl[0][0] : b == 1 ? nfl[0][1] : b == 2 ? nfl[1][0] : nfl[1][1];
-      const int64_t fa0 = b == 0 ? nfa[0][0] : b == 1 ? nfa[0][1] : b == 2 ? nfa[1][0] : nfa[1][1];
-      RecState s{f0, fa0, sc, fc, rsc, rfc, rtc, rfa, lim, rst};
+      RecState s;
+      load_state(p.c, i, s);
+      s.flags = b == 0 ? nfl[0][0] : b == 1 ? nfl[0][1] : b == 2 ? nfl[1][0] : nfl[1][1];
+      s.fa = b == 0 ? nfa[0][0] : b == 1 ? nfa[0][1] : b == 2 ? nfa[1][0] : nfa[1][1];
+      const RecState s0 = s;
       uint32_t res = 0;
-      uint32_t a = apply_result(s, T, res);
-      if (CLOSED && ((due_bits >> b) & 1u)) {
-        const uint64_t k = outcome_key(p.seed, p.shard_base + i, (uint64_t)T);
-        const uint32_t failp = (s.flags >> AM_F_FAILP_SHIFT) & 0xFFu;
-        const bool fail = (uint32_t)(k & 0xFF) < failp;
-        const bool rem_ok = (uint32_t)((k >> 8) & 0xFF) < 179u;
-        s.flags |= (fail ? AM_F_PENDING_FAIL : AM_F_PENDING_OK) | AM_F_REMEDY_PENDING |
-                   (rem_ok ? AM_F_REMEDY_OUTCOME_OK : 0u);
-        a |= apply_result(s, T, res);
-      }
+      const uint32_t a = result_step<CLOSED>(s, T, (due_bits >> b) & 1u, p.seed, p.shard_base + i, res);
       res_lane += res;  // per lane at most 4 records x 2 results per byte
-      if (s.s != sc) st_stream(p.c.success + i, s.s);
-      if (s.f != fc) st_stream(p.c.failed + i, s.f);
-      if (s.rs != rsc) st_stream(p.c.remedy_success + i, s.rs);
-      if (s.rf != rfc) st_stream(p.c.remedy_failed + i, s.rf);
-      if (s.rt != rtc) st_stream(p.c.remedy_total + i, s.rt);
-      if (s.rfa != rfa) st_stream(p.c.remedy_finished_at + i, s.rfa);
+      store_changed_state(p.c, i, s, s0);
       // (a record "Stopped" in this very tick already carries STOPPED_REPORTED and
       // finishedAt = T in nfl/nfa, and apply_result preserves both: the pause rule of
       // hcc.go:238-250 and a posted result commute)
@@ -558,16 +585,12 @@ __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM
   if (lane == 0) { s_warp_tot[warp] = warp_total; s_warp_exc[warp] = warp_exc; }
 
   // ---- results applied this tick (feeds metrics.MonitorSuccess/Error): lane ->
-  //      warp (two redux over 16-bit halves) -> per-warp shared row.  The action
-  //      statistics and index checksums are derived from the emitted entries
-  //      by expand_kernel, so records that emit nothing cost nothing here.
+  //      warp -> per-warp shared row.  The action statistics and index checksums are
+  //      derived from the emitted entries by expand_kernel, so records that emit
+  //      nothing cost nothing here.
   {
-    uint32_t lo = 0, hi = 0;
-    if (__any_sync(kFull, res_lane != 0)) {
-      lo = __reduce_add_sync(kFull, (res_lane & 0xFFu) | ((res_lane & 0xFF00u) << 8));           // ok | fail<<16
-      hi = __reduce_add_sync(kFull, ((res_lane >> 16) & 0xFFu) | ((res_lane >> 8) & 0xFF0000u));  // remedy ok | fail<<16
-    }
-    if (lane < 4) s_wres[warp][lane] = ((lane < 2 ? lo : hi) >> ((lane & 1) * 16)) & 0xFFFFu;
+    const uint32_t v = warp_result_count(res_lane, lane);
+    if (lane < 4) s_wres[warp][lane] = v;
   }
   __syncthreads();
 
@@ -937,7 +960,7 @@ __global__ void next_due_kernel(DevCols c, uint64_t n, int64_t T, int64_t zone_d
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t f = c.flags[i];
     const uint32_t kind = f & AM_KIND_MASK;
-    if ((f & AM_F_TOMBSTONE) || !((0x3Eu >> kind) & 1u)) continue;
+    if (!is_live(f)) continue;
     int64_t due = INT64_MAX;
     if ((f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING)) || kind == AM_KIND_PARSE_ERROR ||
         (kind == AM_KIND_STOPPED && !(f & AM_F_STOPPED_REPORTED))) {
@@ -1122,8 +1145,7 @@ __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__
       uint32_t f = c.flags[i];
       if (mine_hc) f = (f & ~kHcBits) | (arg & kHcBits);
       if (rm_valid) f = (f & ~kRemedyBits) | ((mine_rm ? arg : ops[rmw - 1u].y) & kRemedyBits);
-      const bool live = ((0x3Eu >> (f & AM_KIND_MASK)) & 1u) && !(f & AM_F_TOMBSTONE);
-      if (!live || !(f & kPend)) {
+      if (!is_live(f) || !(f & kPend)) {
         c.flags[i] = f;  // (a record the sweep does not evaluate keeps its posted result)
       } else {
         // Gather only what this result can touch (every column is its own 32-B sector of a random record):
@@ -1157,15 +1179,9 @@ __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__
     }
   }
   // results applied (metrics.MonitorSuccess / Error): warp -> global RED, as the sweep does per tile
-  if (__any_sync(kFull, res != 0)) {
-    const uint32_t lo = __reduce_add_sync(kFull, (res & 0xFFu) | ((res & 0xFF00u) << 8));
-    const uint32_t hi = __reduce_add_sync(kFull, ((res >> 16) & 0xFFu) | ((res >> 8) & 0xFF0000u));
-    const int lane = threadIdx.x & 31;
-    if (lane < 4) {
-      const uint32_t v = ((lane < 2 ? lo : hi) >> ((lane & 1) * 16)) & 0xFFFFu;
-      if (v) atomicAdd(&acc[10 + lane], (unsigned long long)v);
-    }
-  }
+  const int lane = threadIdx.x & 31;
+  const uint32_t v = warp_result_count(res, lane);
+  if (lane < 4 && v) atomicAdd(&acc[10 + lane], (unsigned long long)v);
 }
 
 __global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n) {
