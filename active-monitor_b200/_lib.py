@@ -35,7 +35,7 @@ F_TZ_SHIFT = 24
 ACT_SUBMIT_HC, ACT_RUN_REMEDY, ACT_STOPPED, ACT_PARSE_ERROR = 0x01, 0x02, 0x04, 0x08
 ACT_REMEDY_SKIP, ACT_RESET_ON_PASS, ACT_RESET_ON_INTERVAL, ACT_ANOMALY = 0x10, 0x20, 0x40, 0x80
 
-SWEEP_CLOSED_LOOP, SWEEP_FULL_SCAN, SWEEP_BLOCKED = 0x1, 0x2, 0x4
+SWEEP_CLOSED_LOOP, SWEEP_FULL_SCAN, SWEEP_BLOCKED, SWEEP_CATCH_UP = 0x1, 0x2, 0x4, 0x8
 PHASE_NONE, PHASE_SUCCEEDED, PHASE_FAILED = 0, 1, 2
 IPC_HANDLE_BYTES = 64
 

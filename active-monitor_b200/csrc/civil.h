@@ -94,6 +94,58 @@ AM_HD TickWords tick_words_from_unix(int64_t t) {
   return w;
 }
 
+// A catch-up tick (AM_SWEEP_CATCH_UP) asks whether a schedule fires at SOME second of a window.  The
+// minute starts of a window form a few calendar boxes: one day, a range of hours, a range of minutes (a
+// partial first hour, whole hours, a partial last hour).  A box is a TickWords whose hour and minute words
+// are range masks instead of one-hot ones, with sec0 = 1: inside a box the hour and the minute tests are
+// independent, so cron_matches against it is exactly "fires at some minute start of the box".
+constexpr int kWindowBoxes = 16;  // boxes per zone of one catch-up tick
+
+AM_HD int64_t floor_div(int64_t a, int64_t b) {
+  const int64_t q = a / b;
+  return q - ((a % b != 0) && ((a < 0) != (b < 0)));
+}
+AM_HD uint64_t bit_range(int32_t lo, int32_t hi) { return (2ull << hi) - (1ull << lo); }  // bits lo..hi, hi < 63
+
+// Append the boxes of the minute starts in the LOCAL seconds (lo, hi] to out[*n ..].  False (out and *n
+// then unspecified) when they would not fit in `cap` boxes.  At most three boxes per day the window touches.
+AM_HD bool window_boxes(int64_t lo, int64_t hi, TickWords* out, int* n, int cap) {
+  const int64_t m0 = floor_div(lo, 60) + 1, m1 = floor_div(hi, 60);  // minute numbers of the first and last start
+  if (m0 > m1) return true;
+  for (int64_t day = floor_div(m0, 1440); day <= floor_div(m1, 1440); ++day) {
+    const int32_t a = (int32_t)((m0 > day * 1440 ? m0 : day * 1440) - day * 1440);         // minute of the day
+    const int32_t b = (int32_t)((m1 < day * 1440 + 1439 ? m1 : day * 1440 + 1439) - day * 1440);
+    int64_t y;
+    int32_t mo, d;
+    civil_from_days(day, y, mo, d);
+    TickWords w;
+    w.dom = 1ull << d;
+    w.month = 1ull << mo;
+    w.dow = 1ull << weekday_from_days(day);
+    w.sec0 = 1;
+    w.pad = 0;
+    const int32_t ha = a / 60, hb = b / 60, ma = a % 60, mb = b % 60;
+    // rows: [hour, hour] x [minute lo, minute hi]; a partial first / last hour that is whole joins the middle
+    int32_t rows[3][4];
+    int nr = 0;
+    if (ha == hb) {
+      rows[nr][0] = ha; rows[nr][1] = ha; rows[nr][2] = ma; rows[nr][3] = mb; ++nr;
+    } else {
+      const int32_t full_lo = ma == 0 ? ha : ha + 1, full_hi = mb == 59 ? hb : hb - 1;
+      if (ma != 0) { rows[nr][0] = ha; rows[nr][1] = ha; rows[nr][2] = ma; rows[nr][3] = 59; ++nr; }
+      if (full_lo <= full_hi) { rows[nr][0] = full_lo; rows[nr][1] = full_hi; rows[nr][2] = 0; rows[nr][3] = 59; ++nr; }
+      if (mb != 59) { rows[nr][0] = hb; rows[nr][1] = hb; rows[nr][2] = 0; rows[nr][3] = mb; ++nr; }
+    }
+    for (int k = 0; k < nr; ++k) {
+      if (*n >= cap) return false;
+      w.hour = bit_range(rows[k][0], rows[k][1]);
+      w.minute = bit_range(rows[k][2], rows[k][3]);
+      out[(*n)++] = w;
+    }
+  }
+  return true;
+}
+
 #if defined(__CUDA_ARCH__)
 #define AM_CTZ64(x) (__ffsll((long long)(x)) - 1)
 #else

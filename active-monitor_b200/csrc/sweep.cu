@@ -169,6 +169,14 @@ struct am_sweep {
   PinnedBuf tz_pin;
   cudaEvent_t tz_copied = nullptr;
   bool tz_copy_pending = false;
+  // catch-up ticks (AM_SWEEP_CATCH_UP): the second of the previous tick, and the device table of a window's
+  // calendar boxes ([kMaxZones + 1][kWindowBoxes], allocated at the first catch-up tick that needs it)
+  bool has_prev = false;
+  int64_t prev_T = 0;
+  DevBuf win_boxes;
+  PinnedBuf win_pin;
+  cudaEvent_t win_copied = nullptr;
+  bool win_copy_pending = false;
   std::string last_error;
   uint64_t launches = 0;
   double last_ms = -1.0;
@@ -466,7 +474,58 @@ int refresh_zones(am_sweep* h, int64_t T, cudaStream_t s) {
   return AM_OK;
 }
 
-int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStream_t s) {
+// A catch-up tick's window (P, T] as calendar boxes per zone.  Computed before anything of the tick happens,
+// so that AM_E_RANGE leaves the handle as it was.  `any` false: the tick is a plain one (no previous tick,
+// T <= P, no bit, or no minute start in the window in any zone).
+struct WindowPlan {
+  std::vector<TickWords> boxes;  // [n_zones][kWindowBoxes]
+  uint32_t n_zones = 0;
+  bool any = false;
+};
+
+int plan_window(am_sweep* h, int64_t T, uint32_t mode, WindowPlan* w) {
+  w->any = false;
+  if (!(mode & AM_SWEEP_CATCH_UP) || !h->has_prev || T <= h->prev_T) return AM_OK;
+  if (T - h->prev_T > 86400) {
+    h->last_error = "AM_SWEEP_CATCH_UP: more than a day since the previous tick";
+    return AM_E_RANGE;
+  }
+  bool steady = false;
+  if (!amsweep_tz::window_boxes(h->prev_T, T, &w->boxes, &w->n_zones, &steady)) {
+    h->last_error = "AM_SWEEP_CATCH_UP: a time zone splits the window into too many calendar boxes";
+    return AM_E_RANGE;
+  }
+  // The ticker's normal cadence: T is the window's only minute start in every zone (T on the UTC minute, P at most a
+  // minute back, every offset whole minutes and unchanged in the window).  The plain on-minute tick at T is then the
+  // same tick, and reads the planes instead of the 40 B of canonical masks per record.
+  int64_t sec_of_min = T % 60;
+  if (sec_of_min < 0) sec_of_min += 60;
+  if (steady && sec_of_min == 0 && T - h->prev_T <= 60) return AM_OK;
+  for (const TickWords& b : w->boxes) w->any |= b.sec0 != 0;
+  return AM_OK;
+}
+
+// The window's boxes on the device, stream-ordered like refresh_zones: a sweep still reading the previous
+// window's table runs before this copy on `s` (every device operation of a handle is ordered).  Zones
+// registered after the plan keep zero entries (sec0 = 0): no box, not due.
+int upload_window(am_sweep* h, const WindowPlan& w, cudaStream_t s) {
+  const size_t full = (size_t)(amsweep_tz::kMaxZones + 1) * kWindowBoxes * sizeof(TickWords);
+  if (!h->win_boxes.p) {
+    AM_CUDA(h, h->win_boxes.reserve(full));
+    AM_CUDA(h, cudaMemsetAsync(h->win_boxes.p, 0, h->win_boxes.cap, s));
+  }
+  AM_CUDA(h, h->win_pin.reserve(full));  // full size at once: the pinned array never moves under a copy
+  if (!h->win_copied) AM_CUDA(h, cudaEventCreateWithFlags(&h->win_copied, cudaEventDisableTiming));
+  if (h->win_copy_pending) AM_CUDA(h, cudaEventSynchronize(h->win_copied));  // the previous copy has left the pinned array
+  const size_t bytes = w.boxes.size() * sizeof(TickWords);
+  memcpy(h->win_pin.p, w.boxes.data(), bytes);
+  AM_CUDA(h, cudaMemcpyAsync(h->win_boxes.p, h->win_pin.p, bytes, cudaMemcpyHostToDevice, s));
+  AM_CUDA(h, cudaEventRecord(h->win_copied, s));
+  h->win_copy_pending = true;
+  return AM_OK;
+}
+
+int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStream_t s, const WindowPlan* win = nullptr) {
   if (h->n_records == 0) {
     // nothing to sweep: publish zeros without a launch
     if (o.stats) AM_CUDA(h, cudaMemsetAsync(o.stats, 0, sizeof(am_tick_stats_t), s));
@@ -498,7 +557,14 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   // boundary: every tick then reads the masks.)
   int64_t sec_of_min = T % 60;
   if (sec_of_min < 0) sec_of_min += 60;
-  const bool masks = sec_of_min == 0 || (mode & AM_SWEEP_FULL_SCAN) || (h->tz_n > 1 && !h->tz_aligned);
+  // A catch-up tick reads the canonical masks against the window's boxes instead of planes and zone words.
+  const bool window = win && win->any;
+  const bool masks = !window && (sec_of_min == 0 || (mode & AM_SWEEP_FULL_SCAN) || (h->tz_n > 1 && !h->tz_aligned));
+  if (window) {
+    const int rc = upload_window(h, *win, s);
+    if (rc != AM_OK) return rc;
+    p.tz_table = (const TickWords*)h->win_boxes.p;
+  }
   if (masks && h->tz_n > 1) {  // the tick's wall clock per zone, from the cached offsets
     AM_LAUNCH_PDL(tz_words_kernel, (h->tz_n + 63) / 64, 64, s, (const int32_t*)h->tz_off.p, (TickWords*)h->tz_table.p, T,
                   h->tz_n);
@@ -517,7 +583,12 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   }
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[0], s));
   const bool closed = (mode & AM_SWEEP_CLOSED_LOOP) != 0;
-  if (o.expand) {  // single-stream tick: the sweep's launch hides behind its predecessor (the previous tick's publish, the drain)
+  if (window) {  // (launched as the plain variants below are)
+    if (o.expand && closed) AM_LAUNCH_PDL(AM_SWEEP_WINDOW_KERNEL(true), p.n_tiles, kBlock, s, p);
+    else if (o.expand) AM_LAUNCH_PDL(AM_SWEEP_WINDOW_KERNEL(false), p.n_tiles, kBlock, s, p);
+    else if (closed) AM_LAUNCH(AM_SWEEP_WINDOW_KERNEL(true), p.n_tiles, kBlock, s, p);
+    else AM_LAUNCH(AM_SWEEP_WINDOW_KERNEL(false), p.n_tiles, kBlock, s, p);
+  } else if (o.expand) {  // single-stream tick: the sweep's launch hides behind its predecessor (the previous tick's publish, the drain)
     if (closed && masks) AM_LAUNCH_PDL(AM_SWEEP_KERNEL(true, true), p.n_tiles, kBlock, s, p);
     else if (closed) AM_LAUNCH_PDL(AM_SWEEP_KERNEL(true, false), p.n_tiles, kBlock, s, p);
     else if (masks) AM_LAUNCH_PDL(AM_SWEEP_KERNEL(false, true), p.n_tiles, kBlock, s, p);
@@ -580,8 +651,11 @@ int reserve_host_out(am_sweep* h, uint64_t entries) {
 
 // One host tick: drain, four kernels, one synchronisation; the list lands in h->host_out.
 int host_tick(am_sweep* h, int64_t unix_sec, uint32_t mode, am_tick_stats_t* stats) {
+  WindowPlan win;
+  int rc = plan_window(h, unix_sec, mode, &win);
+  if (rc != AM_OK) return rc;
   AM_CUDA(h, cudaSetDevice(h->device));
-  int rc = order_on(h, h->stream);
+  rc = order_on(h, h->stream);
   if (rc != AM_OK) return rc;
   rc = drain_staged(h, h->stream, &unix_sec, /*defer_clear=*/true);
   struct ClearOnExit {  // whatever happens below, the marks are cleared before the handle is used again
@@ -601,7 +675,7 @@ int host_tick(am_sweep* h, int64_t unix_sec, uint32_t mode, am_tick_stats_t* sta
   }
   o.stats = h->d_stats_mapped;
   AM_CUDA(h, cudaEventRecord(h->ev0, h->stream));
-  rc = launch_tick(h, unix_sec, mode, o, h->stream);
+  rc = launch_tick(h, unix_sec, mode, o, h->stream, &win);
   if (rc != AM_OK) return rc;
   AM_CUDA(h, cudaEventRecord(h->ev1, h->stream));
   rc = finish_deferred_clear(h, h->stream);  // behind the event the host waits for
@@ -613,6 +687,8 @@ int host_tick(am_sweep* h, int64_t unix_sec, uint32_t mode, am_tick_stats_t* sta
   am_tick_stats_t st = *h->h_stats;
   st.n_records = h->n_records;
   h->host_n = st.n_emitted;
+  h->has_prev = true;
+  h->prev_T = unix_sec;
   if (stats) *stats = st;
   return AM_OK;
 }
@@ -788,6 +864,8 @@ void am_sweep_destroy(am_sweep_t* h) {
   h->pin_in.release(); h->dev_in.release();
   h->tz_off.release(); h->tz_table.release(); h->tz_pin.release();
   if (h->tz_copied) cudaEventDestroy(h->tz_copied);
+  h->win_boxes.release(); h->win_pin.release();
+  if (h->win_copied) cudaEventDestroy(h->win_copied);
   if (h->ev_last) cudaEventDestroy(h->ev_last);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
@@ -1017,9 +1095,12 @@ int am_sweep_tick_device(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* d
   if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
+  WindowPlan win;
+  int rc = plan_window(h, unix_sec, mode, &win);
+  if (rc != AM_OK) return rc;
   AM_CUDA(h, cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)cuda_stream;  // NULL == CUDA default stream
-  int rc = order_on(h, s);
+  rc = order_on(h, s);
   if (rc != AM_OK) return rc;
   rc = drain_staged(h, s, &unix_sec);
   if (rc != AM_OK) return rc;
@@ -1029,7 +1110,9 @@ int am_sweep_tick_device(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* d
   o.cap = cap;
   o.count = (uint32_t*)d_count;
   o.stats = (am_tick_stats_t*)d_stats;
-  return launch_tick(h, unix_sec, mode, o, s);
+  rc = launch_tick(h, unix_sec, mode, o, s, &win);
+  if (rc == AM_OK) { h->has_prev = true; h->prev_T = unix_sec; }
+  return rc;
 }
 
 int am_sweep_tick_shard(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* cuda_stream) {
@@ -1037,9 +1120,12 @@ int am_sweep_tick_shard(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* cu
   if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
+  WindowPlan win;
+  int rc = plan_window(h, unix_sec, mode, &win);
+  if (rc != AM_OK) return rc;
   AM_CUDA(h, cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)cuda_stream;
-  int rc = order_on(h, s);
+  rc = order_on(h, s);
   if (rc != AM_OK) return rc;
   rc = drain_staged(h, s, &unix_sec);
   if (rc != AM_OK) return rc;
@@ -1047,14 +1133,18 @@ int am_sweep_tick_shard(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* cu
   ListOut o;
   o.expand = false;
   const int parity = (int)h->parity;
-  rc = launch_tick(h, unix_sec, mode, o, s);
-  if (rc == AM_OK) h->last_shard_parity = parity;
+  rc = launch_tick(h, unix_sec, mode, o, s, &win);
+  if (rc == AM_OK) {
+    h->last_shard_parity = parity;
+    h->has_prev = true;
+    h->prev_T = unix_sec;
+  }
   return rc;
 }
 
 int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint32_t mode,
                        uint64_t seed, am_tick_stats_t* stats_out) {
-  if (!h || !stats_out) return AM_E_INVAL;
+  if (!h || !stats_out || (mode & AM_SWEEP_CATCH_UP)) return AM_E_INVAL;
   if (n_ticks == 0) return AM_OK;
   if (n_ticks > (1ull << 24)) return AM_E_INVAL;
   if (unix_sec0 >= (1ll << 55) - (int64_t)n_ticks || unix_sec0 <= -(1ll << 55)) return AM_E_RANGE;
@@ -1127,6 +1217,7 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
     else h->last_ms = ms;
     if (blocked && rc == AM_OK)
       for (uint64_t k = 0; k < n_ticks; ++k) stats_out[k].n_records = h->n_records;
+    if (rc == AM_OK) { h->has_prev = true; h->prev_T = unix_sec0 + (int64_t)n_ticks - 1; }
   }
   cudaFree(d_stats);
   return rc;

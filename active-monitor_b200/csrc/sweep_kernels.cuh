@@ -302,8 +302,12 @@ __global__ void tz_words_kernel(const int32_t* __restrict__ tz_off, TickWords* _
 // spill stores) and loads both halves' remedy state at once in its dense result path; the other three run
 // at one more CTA per SM within 64 registers, one half at a time (the open-loop on-minute sweep measured
 // faster so): the open-loop ones in 59 and 60 without spills, the closed-loop off-minute one with 20 B.
-template <bool CLOSED, bool MASKS>
-__global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1)
+// WINDOW = a catch-up tick (AM_SWEEP_CATCH_UP, MASKS false): a 5-field schedule is due iff it fires somewhere in
+// the window's calendar boxes (p.tz_table, per zone).  A box covers many values of a field, so no plane
+// can answer it: the five canonical mask columns are read instead, 40 B per record, in warps that hold a
+// CRON_SPEC record.  Runs at AM_MIN_BLOCKS CTAs per SM like the closed-loop on-minute variant.
+template <bool CLOSED, bool MASKS, bool WINDOW = false>
+__global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1)
     sweep_tick_kernel(const SweepParams p) {
   // one row per warp, written unconditionally: no zero-initialisation, no shared
   // atomics, and therefore a single __syncthreads in the whole kernel
@@ -401,6 +405,39 @@ __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM
       }
     }
   }
+  if (WINDOW) {
+    // one vote per warp: warps without a 5-field schedule read no masks
+    uint32_t cron_lane = 0;  // bit (2h+j): the record is a CRON_SPEC one
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < 2; ++j) cron_lane |= (((j ? fl[h].y : fl[h].x) & AM_KIND_MASK) == AM_KIND_CRON_SPEC ? 1u : 0u) << (2 * h + j);
+    if (__any_sync(kFull, cron_lane != 0)) {
+      ulonglong2 mi[2], hr[2], dm[2], mo[2], dw[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mi[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.minute + r0[h]));
+        hr[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.hour + r0[h]));
+        dm[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.dom + r0[h]));
+        mo[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.month + r0[h]));
+        dw[h] = ld_stream(reinterpret_cast<const ulonglong2*>(p.c.dow + r0[h]));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          if ((cron_lane >> (2 * h + j)) & 1u) {
+            const TickWords* b = p.tz_table + ((j ? fl[h].y : fl[h].x) >> AM_F_TZ_SHIFT) * kWindowBoxes;
+            bool m = false;
+            for (int k = 0; k < kWindowBoxes && b[k].sec0; ++k)
+              m |= cron_matches(b[k], j ? mi[h].y : mi[h].x, j ? hr[h].y : hr[h].x, j ? dm[h].y : dm[h].x,
+                                j ? mo[h].y : mo[h].x, j ? dw[h].y : dw[h].x);
+            cron_bits |= (m ? 1u : 0u) << (2 * h + j);
+          }
+        }
+      }
+    }
+  }
 
   uint32_t act[2][2];
   uint32_t res_lane = 0;  // 4 x 8-bit counts of results applied by this lane
@@ -421,7 +458,7 @@ __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM
       // (an if, not `MASKS && ...`: with the latter ptxas hoisted this loop's arithmetic above the
       // __syncwarp fence in the MASKS=false variants and delayed the second half's loads behind it)
       bool due_cron = false;
-      if (MASKS) due_cron = ((cron_bits >> (2 * h + j)) & 1u) != 0;
+      if (MASKS || WINDOW) due_cron = ((cron_bits >> (2 * h + j)) & 1u) != 0;
       const uint32_t kind = f & AM_KIND_MASK;
       const bool due_iv = interval_due(f, j ? ras[h].y : ras[h].x, fav, T);
       const bool is_iv = is_interval_kind(kind);
@@ -489,7 +526,7 @@ __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM
         rfa[h] = ld_stream(reinterpret_cast<const longlong2*>(p.c.remedy_finished_at + r));
       }
     };
-    if (CLOSED && MASKS) {  // (the variants at 64 registers: one half at a time)
+    if (CLOSED && (MASKS || WINDOW)) {  // (the variants at 64 registers: one half at a time)
       load_half(0);
       load_half(1);
       __syncwarp();
@@ -497,7 +534,7 @@ __global__ void __launch_bounds__(kBlock, (CLOSED && MASKS) ? AM_MIN_BLOCKS : AM
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const uint32_t nb = (needy >> (2 * h)) & 3u;
-      if (!(CLOSED && MASKS)) load_half(h);
+      if (!(CLOSED && (MASKS || WINDOW))) load_half(h);
       if (nb) {
         const uint32_t r = r0[h];
         int32_t ns[2] = {sc[h].x, sc[h].y}, nf[2] = {fc[h].x, fc[h].y};

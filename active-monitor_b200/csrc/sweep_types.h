@@ -39,6 +39,7 @@
 #endif
 #endif
 #define AM_SWEEP_KERNEL(closed, masks) sweep_tick_kernel<closed, masks>  // one macro argument
+#define AM_SWEEP_WINDOW_KERNEL(closed) sweep_tick_kernel<closed, false, true>  // catch-up ticks
 
 namespace amsweep {
 
@@ -121,7 +122,9 @@ struct SweepParams {
   TickOut out;
   unsigned long long* acc;   // [kNumAcc] statistics accumulators (zero on entry)
   const TickWords* tz_table; // [zones + 1] T's LOCAL fields per registered time zone (entry 0 = UTC), written by
-                             // tz_words_kernel ahead of the sweep; NULL when no zone is registered
+                             // tz_words_kernel ahead of the sweep; NULL when no zone is registered.
+                             // WINDOW variant: [256 * kWindowBoxes] the catch-up window's calendar boxes per zone
+                             // (civil.h, window_boxes), the unused ones with sec0 = 0
 };
 
 struct ScanParams {

@@ -297,4 +297,31 @@ uint64_t offsets_at(int64_t utc, std::vector<int32_t>* offs, int64_t* valid_unti
   return g_version;
 }
 
+bool window_boxes(int64_t lo, int64_t hi, std::vector<amsweep::TickWords>* boxes, uint32_t* n_zones, bool* steady) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  const size_t nz = g_zones.size() + 1;
+  *n_zones = (uint32_t)nz;
+  *steady = true;
+  boxes->assign(nz * amsweep::kWindowBoxes, amsweep::TickWords{});
+  for (size_t k = 0; k < nz; ++k) {
+    amsweep::TickWords* out = boxes->data() + k * amsweep::kWindowBoxes;
+    int n = 0;
+    if (k == 0) {
+      if (!amsweep::window_boxes(lo, hi, out, &n, amsweep::kWindowBoxes)) return false;
+      continue;
+    }
+    const Zone& z = *g_zones[k - 1];
+    // seconds s .. e-1 of the window share one offset: the piece (s - 1, e - 1] in UTC
+    for (int64_t s = lo + 1; s <= hi;) {
+      const int32_t off = zone_offset(z, s);
+      const int64_t nc = next_change(z, s);
+      const int64_t e = nc <= hi ? nc : hi + 1;
+      if (s != lo + 1 || e != hi + 1 || off % 60 != 0) *steady = false;
+      if (!amsweep::window_boxes(s - 1 + off, e - 1 + off, out, &n, amsweep::kWindowBoxes)) return false;
+      s = e;
+    }
+  }
+  return true;
+}
+
 }  // namespace amsweep_tz

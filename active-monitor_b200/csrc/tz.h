@@ -40,5 +40,12 @@ uint64_t snapshot(std::vector<ZoneDesc>* descs, std::vector<int64_t>* trans, std
 // whether every offset is a whole number of minutes (the kernel may then skip the cron masks off the
 // minute: the local second-of-minute equals the UTC one).  Returns the registry version.
 uint64_t offsets_at(int64_t utc, std::vector<int32_t>* offs, int64_t* valid_until, bool* minute_aligned);
+// A catch-up tick's window (lo, hi] of UTC seconds as calendar boxes (civil.h, window_boxes), per zone:
+// the window is split where the zone changes its offset, each constant-offset piece mapped to the zone's
+// local seconds.  boxes[z * kWindowBoxes ..] for zone z = 0 (UTC) .. count(), unused entries with sec0 = 0.
+// *n_zones = count() + 1.  *steady: no zone may change its offset inside the window (next_change finds no instant
+// in it; a spurious one only costs the fast path) and every offset is a whole number of minutes — every zone's
+// local minute starts are then the UTC ones.  false: some zone needs more than kWindowBoxes boxes.
+bool window_boxes(int64_t lo, int64_t hi, std::vector<amsweep::TickWords>* boxes, uint32_t* n_zones, bool* steady);
 
 }  // namespace amsweep_tz

@@ -239,6 +239,22 @@ typedef struct am_tick_stats {
                                      hcc.go:751; its next cron minute) — per-tick statistics and the
                                      columns afterwards are identical to tick-by-tick evaluation, but
                                      no per-tick lists are produced                                */
+#define AM_SWEEP_CATCH_UP 0x8u    /* catch up on seconds the caller did not tick.  Let P be the second of the
+                                     handle's previous tick (every successful am_sweep_tick*, am_gather_tick_view
+                                     and am_sweep_run_ticks — its last second — sets it; a tick that returns
+                                     AM_E_NOSPACE counts).  A tick at T with this bit evaluates every record as a
+                                     plain tick at T does, except that a 5-field schedule is due iff it matches at
+                                     SOME second t of (P, T] (a zone-bound one: the zone's wall clock at t, with the
+                                     zone's offset at t).  A schedule that fired several times in the window is
+                                     emitted once, like a late timer of the reference (hcc.go:751).  Everything
+                                     else happens once, at T: interval and "@every" checks, posted results
+                                     (finishedAt = T), STOPPED, PARSE_ERROR, the closed-loop completion, the
+                                     statistics.  Records are evaluated as they stand after the tick's drain: an
+                                     upsert staged during a stall counts from the start of the window.
+                                     No previous tick, or T <= P: a plain tick.  T - P > 86400, or a window whose
+                                     calendar split exceeds the library's fixed per-zone budget: AM_E_RANGE and
+                                     nothing happens (nothing drained, P unchanged) — tick plainly instead.
+                                     am_sweep_run_ticks: AM_E_INVAL.                                         */
 
 /* One shard of the record array on one CUDA device.  `capacity` slots are
  * allocated up front; `shard_base` is added to local indices wherever a
