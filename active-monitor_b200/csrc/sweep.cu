@@ -1095,6 +1095,14 @@ int am_sweep_tick_device(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* d
   if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
+  // expand_kernel stores 16-B quads of indices and 4-B words of actions, scan_groups_kernel a u32 count and
+  // publish_kernel u64 statistics: a misaligned store would end the kernel with an error that takes the whole
+  // CUDA context down.  Refused before anything happens (nothing drained, P unchanged).
+  if (((uintptr_t)d_due_idx & 15u) || ((uintptr_t)d_due_action & 3u) || ((uintptr_t)d_count & 3u) ||
+      ((uintptr_t)d_stats & 7u)) {
+    h->last_error = "am_sweep_tick_device: d_due_idx must be 16-B aligned, d_due_action and d_count 4-B, d_stats 8-B";
+    return AM_E_INVAL;
+  }
   WindowPlan win;
   int rc = plan_window(h, unix_sec, mode, &win);
   if (rc != AM_OK) return rc;

@@ -334,6 +334,10 @@ int am_sweep_last_list(am_sweep_t*, uint64_t offset, uint64_t* due_idx, uint32_t
  * d_due_idx (u32 LOCAL indices), d_due_action (u8) hold `cap` entries;
  * d_count receives min(n_emitted, cap) (u32) — the number of valid list entries;
  * d_stats (may be NULL) receives an am_tick_stats_t whose n_emitted is the full count.
+ * Alignment: d_due_idx 16 B, d_due_action and d_count 4 B, d_stats 8 B (the kernels store
+ * whole quads and words); a misaligned pointer returns AM_E_INVAL before anything happens
+ * (nothing drained, the previous tick's second unchanged).  cudaMalloc returns 256-B
+ * aligned memory: carve several arrays out of one allocation at such offsets.
  * Used for device-resident pipelines.  Stream rule: every device operation of a handle
  * is ordered after the previous one, whatever streams they were issued on (the library
  * inserts the event waits); a stream passed here must stay alive until the next call on
