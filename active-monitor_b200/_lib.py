@@ -144,6 +144,8 @@ SYMBOLS = {
     "am_sweep_repeat_after_sec": (C.c_int, [C.c_void_p, i64, u64, u64, C.c_void_p]),
     "am_sweep_next_due": (C.c_int, [C.c_void_p, i64, P(i64)]),
     "am_sweep_read": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, P(AmRecordCols)]),
+    "am_sweep_set_hold_in_flight": (C.c_int, [C.c_void_p, C.c_int]),
+    "am_sweep_in_flight": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, C.c_void_p]),
     "am_sweep_size": (u64, [C.c_void_p]),
     "am_sweep_capacity": (u64, [C.c_void_p]),
     "am_sweep_device": (C.c_int, [C.c_void_p]),

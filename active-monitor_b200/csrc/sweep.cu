@@ -177,6 +177,10 @@ struct am_sweep {
   PinnedBuf win_pin;
   cudaEvent_t win_copied = nullptr;
   bool win_copy_pending = false;
+  // hold in flight (am_sweep_set_hold_in_flight): per slot the second of the tick that submitted its running health-check
+  // workflow, kNotInFlight when none ([cap_padded], allocated when the hold is first turned on)
+  bool hold = false;
+  int64_t* since = nullptr;
   std::string last_error;
   uint64_t launches = 0;
   double last_ms = -1.0;
@@ -391,6 +395,10 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
                   h->seg_dirty, d_ops, (uint32_t)n);
     h->launches += 2;
   }
+  if (h->hold) {  // a posted workflow phase or a remove ends the slot's run (an upsert keeps the hold)
+    AM_LAUNCH_PDL(clear_since_kernel, G, B, s, h->since, d_ops, (uint32_t)n);
+    h->launches++;
+  }
   // A tick's drain applies sparse results right away (apply_results_now_kernel: no second memory round trip
   // in the sweep, and the posted bits never pass through the flags as a separate step); a read's drain, or a
   // batch touching more than an eighth of the records, leaves them pending in the flags for the sweep's own
@@ -583,7 +591,15 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   }
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[0], s));
   const bool closed = (mode & AM_SWEEP_CLOSED_LOOP) != 0;
-  if (window) {  // (launched as the plain variants below are)
+  if (h->hold) {  // hold in flight: the open-loop variants that read and write since (closed loop is refused)
+    p.since = h->since;
+    if (window && o.expand) AM_LAUNCH_PDL(AM_SWEEP_HOLD_KERNEL(false, true), p.n_tiles, kBlock, s, p);
+    else if (window) AM_LAUNCH(AM_SWEEP_HOLD_KERNEL(false, true), p.n_tiles, kBlock, s, p);
+    else if (masks && o.expand) AM_LAUNCH_PDL(AM_SWEEP_HOLD_KERNEL(true, false), p.n_tiles, kBlock, s, p);
+    else if (masks) AM_LAUNCH(AM_SWEEP_HOLD_KERNEL(true, false), p.n_tiles, kBlock, s, p);
+    else if (o.expand) AM_LAUNCH_PDL(AM_SWEEP_HOLD_KERNEL(false, false), p.n_tiles, kBlock, s, p);
+    else AM_LAUNCH(AM_SWEEP_HOLD_KERNEL(false, false), p.n_tiles, kBlock, s, p);
+  } else if (window) {  // (launched as the plain variants below are)
     if (o.expand && closed) AM_LAUNCH_PDL(AM_SWEEP_WINDOW_KERNEL(true), p.n_tiles, kBlock, s, p);
     else if (o.expand) AM_LAUNCH_PDL(AM_SWEEP_WINDOW_KERNEL(false), p.n_tiles, kBlock, s, p);
     else if (closed) AM_LAUNCH(AM_SWEEP_WINDOW_KERNEL(true), p.n_tiles, kBlock, s, p);
@@ -649,10 +665,20 @@ int reserve_host_out(am_sweep* h, uint64_t entries) {
   return AM_OK;
 }
 
+// A closed-loop record completes in the tick that submits it: nothing is ever in flight to hold.  Refused before
+// anything happens (nothing drained, P unchanged).
+int refuse_closed_hold(am_sweep* h, uint32_t mode) {
+  if (!h->hold || !(mode & AM_SWEEP_CLOSED_LOOP)) return AM_OK;
+  h->last_error = "AM_SWEEP_CLOSED_LOOP while the hold in flight is on";
+  return AM_E_INVAL;
+}
+
 // One host tick: drain, four kernels, one synchronisation; the list lands in h->host_out.
 int host_tick(am_sweep* h, int64_t unix_sec, uint32_t mode, am_tick_stats_t* stats) {
+  int rc = refuse_closed_hold(h, mode);
+  if (rc != AM_OK) return rc;
   WindowPlan win;
-  int rc = plan_window(h, unix_sec, mode, &win);
+  rc = plan_window(h, unix_sec, mode, &win);
   if (rc != AM_OK) return rc;
   AM_CUDA(h, cudaSetDevice(h->device));
   rc = order_on(h, h->stream);
@@ -859,6 +885,7 @@ void am_sweep_destroy(am_sweep_t* h) {
     if (st.drained) cudaEventDestroy(st.drained);
   }
   if (h->marks) cudaFree(h->marks);
+  if (h->since) cudaFree(h->since);
   if (h->h_stats) cudaFreeHost(h->h_stats);
   h->host_out.release();
   h->pin_in.release(); h->dev_in.release();
@@ -930,8 +957,31 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
     h->launches++;
     AM_CUDA(h, cudaGetLastError());
   }
+  if (h->hold) {  // loaded records have nothing in flight
+    AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, h->stream, h->since + first, kNotInFlight, n);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
+  }
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   if (first + n > h->n_records) h->n_records = first + n;
+  return AM_OK;
+}
+
+int am_sweep_set_hold_in_flight(am_sweep_t* h, int on) {
+  if (!h) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if ((on != 0) == h->hold) return AM_OK;
+  if (on) {  // starts with nothing in flight
+    AM_CUDA(h, cudaSetDevice(h->device));
+    int rc = order_on(h, h->stream);
+    if (rc != AM_OK) return rc;
+    if (!h->since) AM_CUDA(h, cudaMalloc((void**)&h->since, h->cap_padded * sizeof(int64_t)));
+    AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, h->stream, h->since, kNotInFlight, h->cap_padded);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
+  }
+  h->hold = on != 0;
   return AM_OK;
 }
 
@@ -1103,8 +1153,10 @@ int am_sweep_tick_device(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* d
     h->last_error = "am_sweep_tick_device: d_due_idx must be 16-B aligned, d_due_action and d_count 4-B, d_stats 8-B";
     return AM_E_INVAL;
   }
+  int rc = refuse_closed_hold(h, mode);
+  if (rc != AM_OK) return rc;
   WindowPlan win;
-  int rc = plan_window(h, unix_sec, mode, &win);
+  rc = plan_window(h, unix_sec, mode, &win);
   if (rc != AM_OK) return rc;
   AM_CUDA(h, cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)cuda_stream;  // NULL == CUDA default stream
@@ -1128,8 +1180,10 @@ int am_sweep_tick_shard(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* cu
   if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
+  int rc = refuse_closed_hold(h, mode);
+  if (rc != AM_OK) return rc;
   WindowPlan win;
-  int rc = plan_window(h, unix_sec, mode, &win);
+  rc = plan_window(h, unix_sec, mode, &win);
   if (rc != AM_OK) return rc;
   AM_CUDA(h, cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)cuda_stream;
@@ -1158,6 +1212,10 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
   if (unix_sec0 >= (1ll << 55) - (int64_t)n_ticks || unix_sec0 <= -(1ll << 55)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
+  if (h->hold) {  // (neither the blocked kernel nor the run's plain ticks keep the hold: refused, nothing happens)
+    h->last_error = "am_sweep_run_ticks while the hold in flight is on";
+    return AM_E_INVAL;
+  }
   AM_CUDA(h, cudaSetDevice(h->device));
   int rc = order_on(h, h->stream);
   if (rc != AM_OK) return rc;
@@ -1295,8 +1353,8 @@ int am_sweep_next_due(am_sweep_t* h, int64_t unix_sec, int64_t* next_out) {
   AM_CUDA(h, h->dev_in.reserve(8));
   AM_CUDA(h, h->pin_in.reserve(8));
   AM_CUDA(h, cudaMemsetAsync(h->dev_in.p, 0xFF, 8, h->stream));
-  AM_LAUNCH(next_due_kernel, h->sms * 8, 256, h->stream, h->cols, h->n_records, unix_sec, zone_due,
-            (unsigned long long*)h->dev_in.p);
+  AM_LAUNCH(next_due_kernel, h->sms * 8, 256, h->stream, h->cols, (const int64_t*)(h->hold ? h->since : nullptr),
+            h->n_records, unix_sec, zone_due, (unsigned long long*)h->dev_in.p);
   h->launches++;
   AM_CUDA(h, cudaGetLastError());
   AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, 8, cudaMemcpyDeviceToHost, h->stream));
@@ -1322,6 +1380,45 @@ int am_sweep_read(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx
     if (rc != AM_OK) return rc;
   }
   return read_impl(h, first, n, idx, out);
+}
+
+int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
+  if (!h || (n && !since_out)) return AM_E_INVAL;
+  if (n == 0) return AM_OK;
+  if (n > 0xFFFFFFFFull || (!idx && (first + n > h->capacity || first + n < first))) return AM_E_INVAL;
+  if (idx)
+    for (uint64_t k = 0; k < n; ++k)
+      if (idx[k] >= h->capacity) return AM_E_RANGE;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  AM_CUDA(h, cudaSetDevice(h->device));
+  int rc = order_on(h, h->stream);
+  if (rc != AM_OK) return rc;
+  rc = drain_staged(h, h->stream);  // results posted by now release their holds (left pending for the next tick)
+  if (rc != AM_OK) return rc;
+  if (!h->hold) {
+    for (uint64_t k = 0; k < n; ++k) since_out[k] = kNotInFlight;
+    return AM_OK;
+  }
+  const size_t o_idx = n * 8, total = o_idx + (idx ? n * 4 : 0);
+  AM_CUDA(h, h->pin_in.reserve(total));
+  AM_CUDA(h, h->dev_in.reserve(total));
+  char* dp = (char*)h->dev_in.p;
+  const uint32_t* d_idx = nullptr;
+  if (idx) {
+    uint32_t* hidx = (uint32_t*)((char*)h->pin_in.p + o_idx);
+    for (uint64_t k = 0; k < n; ++k) hidx[k] = (uint32_t)idx[k];
+    AM_CUDA(h, cudaMemcpyAsync(dp + o_idx, hidx, n * 4, cudaMemcpyHostToDevice, h->stream));
+    d_idx = (const uint32_t*)(dp + o_idx);
+  }
+  AM_LAUNCH(in_flight_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols, (const int64_t*)h->since, (uint32_t)first,
+            d_idx, (uint32_t)n, (int64_t*)dp);
+  h->launches++;
+  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, dp, n * 8, cudaMemcpyDeviceToHost, h->stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  memcpy(since_out, h->pin_in.p, n * 8);
+  return AM_OK;
 }
 
 // (tick guard held, staged events drained, h->stream ordered)

@@ -306,7 +306,12 @@ __global__ void tz_words_kernel(const int32_t* __restrict__ tz_off, TickWords* _
 // the window's calendar boxes (p.tz_table, per zone).  A box covers many values of a field, so no plane
 // can answer it: the five canonical mask columns are read instead, 40 B per record, in warps that hold a
 // CRON_SPEC record.  Runs at AM_MIN_BLOCKS CTAs per SM like the closed-loop on-minute variant.
-template <bool CLOSED, bool MASKS, bool WINDOW = false>
+// HOLD = hold in flight (am_sweep_set_hold_in_flight; open loop only): after the due decision, a due record whose
+// health-check workflow is still running (p.since set, since >= finishedAt, no workflow phase pending) is not
+// submitted; every record that is submitted gets since = T.  The since word is loaded only for the halves that
+// hold a due record: one dependent round trip, in the warps that have one (DESIGN.md section 3 compares it with
+// streaming since for every record).
+template <bool CLOSED, bool MASKS, bool WINDOW = false, bool HOLD = false>
 __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1)
     sweep_tick_kernel(const SweepParams p) {
   // one row per warp, written unconditionally: no zero-initialisation, no shared
@@ -477,6 +482,30 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
       }
       if (live && (pending || (CLOSED && due))) needy |= 1u << (2 * h + j);
       if (due) due_bits |= 1u << (2 * h + j);
+    }
+  }
+
+  // ---- hold in flight: the reference's watch loop holds a check until its workflow ends (hcc.go:607-727) and only
+  //      then arms the next timer (hcc.go:745-752).  A posted phase clears since at the drain (clear_since_kernel).
+  if (HOLD && __any_sync(kFull, due_bits != 0)) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t db = (due_bits >> (2 * h)) & 3u;
+      if (db) {
+        const longlong2 sv = ld_stream(reinterpret_cast<const longlong2*>(p.since + r0[h]));
+        int64_t s[2] = {sv.x, sv.y};
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          if ((db >> j) & 1u) {
+            const uint32_t f = j ? fl[h].y : fl[h].x;
+            const int64_t fav = j ? fa[h].y : fa[h].x;
+            const bool held = s[j] != kNotInFlight && s[j] >= fav && !(f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL));
+            if (held) act[h][j] &= ~AM_ACT_SUBMIT_HC;
+            else s[j] = T;
+          }
+        }
+        if (s[0] != sv.x || s[1] != sv.y) st_stream(reinterpret_cast<longlong2*>(p.since + r0[h]), make_longlong2(s[0], s[1]));
+      }
     }
   }
 
@@ -991,8 +1020,11 @@ __global__ void next_fire_kernel(DevCols c, uint32_t first, uint32_t n, int64_t 
 // then.  Pending results, an unreported "Stopped" and parse errors (requeued after 1 s, hcc.go:204)
 // are due at once.  Grid-stride, one record per thread and step; lane -> warp (shuffles) -> global
 // atomicMin on a biased unsigned key.  `zone_due`: a lower bound, > T, of the first activation of any
-// schedule bound to a named time zone (the launcher derives it from the zones' offsets).
-__global__ void next_due_kernel(DevCols c, uint64_t n, int64_t T, int64_t zone_due, unsigned long long* out_biased) {
+// schedule bound to a named time zone (the launcher derives it from the zones' offsets).  `since`: the hold-in-flight
+// column (NULL when the hold is off): a held record is never due by its schedule — its next event is a posted phase
+// or a remove, each a reason for the caller to wake the ticker.
+__global__ void next_due_kernel(DevCols c, const int64_t* __restrict__ since, uint64_t n, int64_t T, int64_t zone_due,
+                                unsigned long long* out_biased) {
   unsigned long long best = ~0ull;
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t f = c.flags[i];
@@ -1002,6 +1034,8 @@ __global__ void next_due_kernel(DevCols c, uint64_t n, int64_t T, int64_t zone_d
     if ((f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING)) || kind == AM_KIND_PARSE_ERROR ||
         (kind == AM_KIND_STOPPED && !(f & AM_F_STOPPED_REPORTED))) {
       due = T + 1;
+    } else if (since && since[i] != kNotInFlight && since[i] >= c.finished_at[i]) {
+      // held (nothing pending: the branch above)
     } else if (kind == AM_KIND_INTERVAL || kind == AM_KIND_CRON_EVERY) {
       const int64_t at = (int64_t)((uint64_t)c.finished_at[i] + (uint64_t)(int64_t)c.ras[i]);
       due = ((f & AM_F_TIMER_ARMED) && at > T + 1) ? at : T + 1;
@@ -1219,6 +1253,39 @@ __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__
   const int lane = threadIdx.x & 31;
   const uint32_t v = warp_result_count(res, lane);
   if (lane < 4 && v) atomicAdd(&acc[10 + lane], (unsigned long long)v);
+}
+
+// Hold in flight: the drain's staged ops that end a run clear the slot's since.
+//   * a workflow phase (Succeeded / Failed): the run is over (hcc.go:635/:662), whatever else the drain does — also
+//     when a later upsert of the slot supersedes the result itself, and whatever second the next tick has;
+//   * a remove: no workflow in flight any more (hcc.go:175-186 stops its timer), also one followed by an upsert of the
+//     same slot (a new CR in an old slot).
+// A remedy phase alone does not (remedy workflows are not held).  Launched only while the hold is on.
+__global__ void clear_since_kernel(int64_t* since, const uint2* __restrict__ ops, uint32_t n) {
+  pdl_wait();  // (launched with programmatic stream serialisation: the previous tick's sweep writes since)
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint2 op = ops[k];
+  const uint32_t kind = op.y & kOpKindMask;
+  if (kind == kOpRemove || (kind == kOpResult && (op.y & kHcBits))) since[op.x] = kNotInFlight;
+}
+
+__global__ void fill_i64_kernel(int64_t* p, int64_t v, uint64_t n) {
+  uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) p[i] = v;
+}
+
+// am_sweep_in_flight: since of the slots the next tick would hold (the sweep's rule, on the drained state), else
+// kNotInFlight.  idx == NULL: the range [first, first + n).
+__global__ void in_flight_kernel(DevCols c, const int64_t* __restrict__ since, uint32_t first, const uint32_t* __restrict__ idx,
+                                 uint32_t n, int64_t* out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t i = idx ? idx[k] : first + k;
+  const int64_t s = since[i];
+  const bool held = s != kNotInFlight && s >= c.finished_at[i] && !(c.flags[i] & (AM_F_PENDING_OK | AM_F_PENDING_FAIL));
+  out[k] = held ? s : kNotInFlight;
 }
 
 __global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n) {

@@ -40,6 +40,7 @@
 #endif
 #define AM_SWEEP_KERNEL(closed, masks) sweep_tick_kernel<closed, masks>  // one macro argument
 #define AM_SWEEP_WINDOW_KERNEL(closed) sweep_tick_kernel<closed, false, true>  // catch-up ticks
+#define AM_SWEEP_HOLD_KERNEL(masks, window) sweep_tick_kernel<false, masks, window, true>  // hold in flight (open loop)
 
 namespace amsweep {
 
@@ -125,7 +126,10 @@ struct SweepParams {
                              // tz_words_kernel ahead of the sweep; NULL when no zone is registered.
                              // WINDOW variant: [256 * kWindowBoxes] the catch-up window's calendar boxes per zone
                              // (civil.h, window_boxes), the unused ones with sec0 = 0
+  int64_t* since;            // HOLD variants: [cap] the second of the tick that submitted the slot's running health-check
+                             // workflow, kNotInFlight when none (am_sweep_set_hold_in_flight); NULL otherwise
 };
+constexpr int64_t kNotInFlight = INT64_MIN;
 
 struct ScanParams {
   uint32_t* group_count;        // this tick's per-group sums; zeroed again once read

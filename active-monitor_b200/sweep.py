@@ -322,6 +322,24 @@ class Sweep:
                     "am_sweep_read")
         return cols
 
+    # -- hold in flight
+    def set_hold_in_flight(self, on: bool):
+        """one health-check workflow per check at a time (am_sweep_set_hold_in_flight)"""
+        self._check(self._lib.am_sweep_set_hold_in_flight(self._h, int(bool(on))), "am_sweep_set_hold_in_flight")
+
+    def in_flight(self, first: int = 0, n: int | None = None, idx=None) -> np.ndarray:
+        """i64 `since` of the slots [first, first+n) (or `idx`) the next tick would hold, INT64_MIN elsewhere.
+        n defaults to the swept slots from `first` on (am_sweep_size)."""
+        if idx is not None:
+            idx = np.ascontiguousarray(idx, dtype=np.uint64)
+            n = len(idx)
+        elif n is None:
+            n = max(self.size - first, 0)
+        out = np.zeros(n, dtype=np.int64)
+        self._check(self._lib.am_sweep_in_flight(self._h, first, n, None if idx is None else idx.ctypes.data,
+                                                 out.ctypes.data), "am_sweep_in_flight")
+        return out
+
     # -- introspection
     def set_seed(self, seed: int):
         self._check(self._lib.am_sweep_set_seed(self._h, seed), "am_sweep_set_seed")

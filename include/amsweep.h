@@ -381,6 +381,38 @@ int am_sweep_next_due(am_sweep_t*, int64_t unix_sec, int64_t* next_out);
 int am_sweep_read(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx,
                   am_record_cols_t* out);
 
+/* Hold in flight: one health-check workflow per check at a time, as the reference's watch loop
+ * keeps it (hcc.go:607-727 block until the workflow's terminal phase or its timeout; only then
+ * hcc.go:745-752 arm the next timer).  Off by default.  While on, the handle keeps per slot
+ * `since`, the second of the tick that submitted the check's running workflow, or none.  A record
+ * is HELD at a tick when since is set, since >= finishedAt, and no workflow phase (Succeeded /
+ * Failed) is pending for it.  A held record gets no AM_ACT_SUBMIT_HC; everything else about it is
+ * evaluated as usual (remedy results, RUN_REMEDY and the other one-shot actions, STOPPED,
+ * PARSE_ERROR).  Every record a tick emits with AM_ACT_SUBMIT_HC gets since = that tick's second,
+ * also in a tick that returns AM_E_NOSPACE (the rest of its list is in am_sweep_last_list).
+ * Release: a posted workflow phase clears since when the next tick or read drains it — also when
+ * an upsert of the slot staged after it supersedes the result itself, and whatever second the next
+ * tick has.  The caller's watch loop posts Failed itself when its workflow timeout expires
+ * (hcc.go:627-632).  am_sweep_remove and am_sweep_load_range clear since for their slots; a remedy
+ * phase alone does not.  An upsert keeps the hold (a status write during a run re-enters
+ * Reconcile; it must not submit the check again) unless its finishedAt is later than since.
+ * Only the health-check workflow is held: remedy workflows are not.
+ * Works with AM_SWEEP_CATCH_UP, AM_SWEEP_FULL_SCAN, named zones and every tick entry point
+ * (am_sweep_tick, _tick_view, _tick_device, _tick_shard and so am_gather_exchange /
+ * am_gather_tick_view).  While on, a tick with AM_SWEEP_CLOSED_LOOP and am_sweep_run_ticks return
+ * AM_E_INVAL before anything happens (nothing drained, P unchanged).  am_sweep_next_due skips held
+ * records: their next event is a post_result or a remove.
+ * Turning the hold on starts with nothing in flight (turn it on before the first tick); turning it
+ * off makes every slot read as not in flight.  The first call with on != 0 allocates 8 B per slot
+ * of capacity on the device.  Replaces the caller's own de-duplication of in-flight checks. */
+int am_sweep_set_hold_in_flight(am_sweep_t*, int on);
+
+/* For each slot of [first, first+n) (idx == NULL) or idx[0..n): the `since` of a slot the next
+ * tick would hold, INT64_MIN for every other slot (and for all of them while the hold is off).
+ * Drains staged calls like am_sweep_read.  `since` is the run's Status.StartedAt (`then`,
+ * hcc.go:609/638/665), which the caller can write back with the result. */
+int am_sweep_in_flight(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out);
+
 /* Introspection */
 uint64_t am_sweep_size(const am_sweep_t*);     /* high-water mark (slots swept) */
 uint64_t am_sweep_capacity(const am_sweep_t*);
