@@ -116,6 +116,9 @@ struct TickSet {
   unsigned long long* acc = nullptr;
   cudaEvent_t consumed = nullptr;
   bool consumed_pending = false;
+  // an am_sweep_tick_shard left its statistics in `acc` and no exchange has published (and so re-armed) them yet:
+  // the next tick on this set starts from zero
+  bool unpublished = false;
 };
 
 constexpr size_t kFlushOps = 32768;   // staged ops per early host-to-device chunk
@@ -409,6 +412,10 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
       AM_CUDA(h, cudaStreamWaitEvent(s, ts.consumed, 0));
       ts.consumed_pending = false;
     }
+    if (ts.unpublished) {
+      AM_CUDA(h, cudaMemsetAsync(ts.acc, 0, kNumAcc * 8, s));
+      ts.unpublished = false;
+    }
     AM_LAUNCH_PDL(apply_results_now_kernel, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc);
     h->launches++;
   } else if (st->n_result) {
@@ -544,6 +551,10 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   if (ts.consumed_pending) {  // an exchange on another stream may still be reading this buffer set
     AM_CUDA(h, cudaStreamWaitEvent(s, ts.consumed, 0));
     ts.consumed_pending = false;
+  }
+  if (ts.unpublished) {  // a tick_shard whose statistics no exchange published: not this tick's
+    AM_CUDA(h, cudaMemsetAsync(ts.acc, 0, kNumAcc * 8, s));
+    ts.unpublished = false;
   }
   SweepParams p{};
   p.c = h->cols;
@@ -759,6 +770,7 @@ int shard_mark_consumed(am_sweep* h, int parity, cudaStream_t s) {
   TickSet& ts = h->set[parity & 1];
   AM_CUDA(h, cudaEventRecord(ts.consumed, s));
   ts.consumed_pending = true;
+  ts.unpublished = false;  // (the exchange's publish_kernel re-armed the accumulators)
   return AM_OK;
 }
 }  // namespace amsweep
@@ -942,6 +954,11 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
   if (!g.ok) return AM_E_BUSY;
   AM_CUDA(h, cudaSetDevice(h->device));
   int rc = order_on(h, h->stream);
+  if (rc != AM_OK) return rc;
+  // a load is a call in the per-slot order: upserts, removes and results staged before it are applied first, so
+  // the load overwrites them (a result is left pending in the flags, which the load replaces; a posted workflow
+  // phase has released its slot's hold in this drain all the same)
+  rc = drain_staged(h, h->stream);
   if (rc != AM_OK) return rc;
   for (int k = 0; k < 16; ++k) {
     char* dst = (char*)h->col_ptr[k] + first * kColElem[k];
@@ -1198,6 +1215,7 @@ int am_sweep_tick_shard(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* cu
   rc = launch_tick(h, unix_sec, mode, o, s, &win);
   if (rc == AM_OK) {
     h->last_shard_parity = parity;
+    h->set[parity].unpublished = true;
     h->has_prev = true;
     h->prev_T = unix_sec;
   }

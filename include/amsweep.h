@@ -271,7 +271,10 @@ void am_sweep_destroy(am_sweep_t*);
  * registry (am_tz_lookup, handed out in order of first registration): records read
  * in another process, or before a restart that registered zones in another order,
  * must be re-classified.  A CRON_SPEC record naming an id that is not registered makes
- * this call and am_sweep_upsert return AM_E_INVAL without loading anything. */
+ * this call and am_sweep_upsert return AM_E_INVAL without loading anything.
+ * A load is a call in the per-slot order: upserts, removes and post_results staged before it
+ * take effect first, so the loaded records replace them (a result posted before the load is
+ * dropped, as it is by a later upsert; its workflow phase still releases the slot's hold). */
 int am_sweep_load_range(am_sweep_t*, uint64_t first, uint64_t n, const am_record_cols_t* cols);
 
 /* Reconcile of created/updated CRs (hcc.go:170-188): scatter n records to
@@ -281,7 +284,7 @@ int am_sweep_upsert(am_sweep_t*, uint64_t n, const uint64_t* idx, const am_recor
 /* CR deleted (hcc.go:175-186: Stop() its timer): tombstone the slots.  A removed
  * slot reads back as flags == AM_F_TOMBSTONE; its other columns are unspecified
  * until the next upsert.  Staged calls (upsert / remove / post_result) take effect
- * per slot in call order at the next tick or read. */
+ * per slot in call order at the next tick, read or load. */
 int am_sweep_remove(am_sweep_t*, uint64_t n, const uint64_t* idx);
 
 /* Terminal workflow phases observed by the watch loops (hcc.go:635, :662,
@@ -350,7 +353,9 @@ int am_sweep_tick_device(am_sweep_t*, int64_t unix_sec, uint32_t mode, void* d_d
  * inside the handle as a bitmap (1 bit per record) plus the non-default actions;
  * am_gather_exchange ships exactly that over NVLink and rebuilds the GLOBAL list on
  * every GPU.  Two buffer sets alternate, so the exchange of tick k (on another stream)
- * may overlap am_sweep_tick_shard of tick k+1; tick k+2 waits for exchange k by itself. */
+ * may overlap am_sweep_tick_shard of tick k+1; tick k+2 waits for exchange k by itself.
+ * A tick_shard that no exchange follows leaves no statistics behind: a later tick of any
+ * entry point counts only its own. */
 int am_sweep_tick_shard(am_sweep_t*, int64_t unix_sec, uint32_t mode, void* cuda_stream);
 
 /* Streaming: n_ticks consecutive one-second ticks starting at unix_sec0,
