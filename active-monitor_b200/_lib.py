@@ -61,7 +61,7 @@ class AmRecord(C.Structure):
                 ("finished_at", i64), ("remedy_finished_at", i64), ("ras", i32), ("flags", u32),
                 ("runs_limit", i32), ("reset_interval", i32), ("success", i32), ("failed", i32),
                 ("remedy_success", i32), ("remedy_failed", i32), ("remedy_total", i32),
-                ("reserved", i32)]
+                ("wf_timeout", i32)]
 
 
 RECORD_DTYPE = np.dtype([
@@ -69,7 +69,7 @@ RECORD_DTYPE = np.dtype([
     ("finished_at", "<i8"), ("remedy_finished_at", "<i8"), ("ras", "<i4"), ("flags", "<u4"),
     ("runs_limit", "<i4"), ("reset_interval", "<i4"), ("success", "<i4"), ("failed", "<i4"),
     ("remedy_success", "<i4"), ("remedy_failed", "<i4"), ("remedy_total", "<i4"),
-    ("reserved", "<i4")])
+    ("wf_timeout", "<i4")])
 assert RECORD_DTYPE.itemsize == C.sizeof(AmRecord) == 96
 
 # column order == am_record_cols_t member order == am_sweep_column_ptr ids
@@ -146,6 +146,7 @@ SYMBOLS = {
     "am_sweep_read": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, P(AmRecordCols)]),
     "am_sweep_set_hold_in_flight": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_in_flight": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, C.c_void_p]),
+    "am_sweep_last_timed_out": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
     "am_sweep_size": (u64, [C.c_void_p]),
     "am_sweep_capacity": (u64, [C.c_void_p]),
     "am_sweep_device": (C.c_int, [C.c_void_p]),

@@ -22,6 +22,7 @@
 //
 // There is deliberately no CPU path in this file: without a CUDA device
 // am_sweep_create fails with AM_E_DEVICE.
+#include <algorithm>
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
@@ -96,6 +97,7 @@ struct Staging {
   size_t n_ops = 0, n_recs = 0;
   size_t flushed_ops = 0, flushed_recs = 0;  // already enqueued for copy to the device twins
   uint32_t n_state = 0, n_result = 0;
+  bool any_wf = false;  // an upsert staged here carries a non-zero wf_timeout
   // am_sweep_post_result calls that have reserved a range of the op arrays and are filling it
   // OUTSIDE the lock (the controller's workers post concurrently, hcc.go:170-188): while there are
   // any, the arrays may not move, nothing past `flushed_ops` is known complete, and the drain waits
@@ -184,6 +186,18 @@ struct am_sweep {
   // workflow, kNotInFlight when none ([cap_padded], allocated when the hold is first turned on)
   bool hold = false;
   int64_t* since = nullptr;
+  // workflow timeouts (am_record_t.wf_timeout), allocated by the first drain that stages a non-zero one: per slot the
+  // latest upsert's timeout and the running workflow's deadline, per warp segment a lower bound of its deadlines, and
+  // the tick's timed-out list (room for every slot)
+  int32_t* wf_timeout = nullptr;
+  int64_t* deadline = nullptr;
+  unsigned long long* seg_deadline = nullptr;
+  uint32_t* to_idx = nullptr;
+  int64_t* to_since = nullptr;
+  uint32_t* to_count = nullptr;
+  bool to_ran = false;      // the last tick ran expire_runs_kernel: its list is on the device
+  bool to_fetched = false;  // ... and has been copied to to_host, sorted
+  std::vector<std::pair<uint32_t, int64_t>> to_host;
   std::string last_error;
   uint64_t launches = 0;
   double last_ms = -1.0;
@@ -350,13 +364,58 @@ int finish_deferred_clear(am_sweep* h, cudaStream_t s) {
   return AM_OK;
 }
 
+// Workflow timeouts: no deadline in [first, first + n) (the segment bounds stay lower bounds: a segment reached by its
+// bound finds nothing and gets its exact minimum); `all` also resets every bound.
+int drop_deadlines(am_sweep* h, cudaStream_t s, uint64_t first, uint64_t n, bool all) {
+  AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, s, h->deadline + first, kNoDeadline, n);
+  h->launches++;
+  if (all) AM_CUDA(h, cudaMemsetAsync(h->seg_deadline, 0xFF, h->cap_padded / kRecPerWarp * 8, s));
+  AM_CUDA(h, cudaGetLastError());
+  return AM_OK;
+}
+
+// The timeout state, allocated by the first drain that stages a non-zero wf_timeout: 24 B per slot (W 4, deadline 8,
+// the list's index 4 and since 8) and 8 B per 128-slot segment.
+int alloc_timeouts(am_sweep* h, cudaStream_t s) {
+  const size_t cap = h->cap_padded;
+  AM_CUDA(h, cudaMalloc((void**)&h->wf_timeout, cap * 4));
+  AM_CUDA(h, cudaMemsetAsync(h->wf_timeout, 0, cap * 4, s));
+  AM_CUDA(h, cudaMalloc((void**)&h->deadline, cap * 8));
+  AM_CUDA(h, cudaMalloc((void**)&h->seg_deadline, cap / kRecPerWarp * 8));
+  AM_CUDA(h, cudaMalloc((void**)&h->to_idx, cap * 4));
+  AM_CUDA(h, cudaMalloc((void**)&h->to_since, cap * 8));
+  AM_CUDA(h, cudaMalloc((void**)&h->to_count, 4));
+  AM_CUDA(h, cudaMemsetAsync(h->to_count, 0, 4, s));
+  return drop_deadlines(h, s, 0, cap, true);
+}
+
+// A tick's expiry pass (expire_runs_kernel), while the hold is on and the timeout state exists.  Every tick that gets
+// as far as its drain resets the timed-out list.
+int expire_runs(am_sweep* h, cudaStream_t s, int64_t T) {
+  h->to_ran = h->hold && h->wf_timeout;
+  h->to_fetched = false;
+  if (!h->to_ran) return AM_OK;
+  AM_CUDA(h, cudaMemsetAsync(h->to_count, 0, 4, s));
+  const uint64_t n_seg = (h->n_records + kRecPerWarp - 1) / kRecPerWarp;
+  if (n_seg) {  // one lane per segment bound, one warp per 32 of them
+    AM_LAUNCH_PDL(expire_runs_kernel, (unsigned)((n_seg + 255) / 256), 256, s, h->cols, h->since, h->deadline,
+                  h->seg_deadline, (uint32_t)n_seg, T, h->to_idx, h->to_since, h->to_count);
+    h->launches++;
+  }
+  AM_CUDA(h, cudaGetLastError());
+  return AM_OK;
+}
+
 int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, bool defer_clear = false) {
   Staging* st;
   {
     std::unique_lock<std::mutex> lk(h->mu);
     st = &h->stage[h->cur];
     h->cv.wait(lk, [&] { return st->writers == 0; });  // posting calls still filling their ranges
-    if (st->n_ops == 0) return AM_OK;
+    if (st->n_ops == 0) {
+      lk.unlock();
+      return tick_T ? expire_runs(h, s, *tick_T) : AM_OK;
+    }
     // callers are about to append to the other area: its previous copies must have left it
     Staging& nx = h->stage[h->cur ^ 1];
     if (nx.copy_pending) {
@@ -398,9 +457,23 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
                   h->seg_dirty, d_ops, (uint32_t)n);
     h->launches += 2;
   }
+  if (st->any_wf && !h->wf_timeout) {
+    const int rc = alloc_timeouts(h, s);
+    if (rc != AM_OK) return rc;
+  }
+  if (h->wf_timeout && st->n_state) {  // (upserts with W = 0 overwrite an older W as well)
+    AM_LAUNCH_PDL(store_wf_timeout_kernel, G, B, s, h->wf_timeout, h->marks, d_ops, d_recs, (uint32_t)n);
+    h->launches++;
+  }
   if (h->hold) {  // a posted workflow phase or a remove ends the slot's run (an upsert keeps the hold)
     AM_LAUNCH_PDL(clear_since_kernel, G, B, s, h->since, d_ops, (uint32_t)n);
     h->launches++;
+  }
+  // Workflow timeouts expire here, ahead of the result kernels: a remedy phase posted alone in this drain is then
+  // applied together with the synthetic Failed, as it is behind a Failed posted after it (the remedy gate sees both).
+  if (tick_T) {
+    const int rc = expire_runs(h, s, *tick_T);
+    if (rc != AM_OK) return rc;
   }
   // A tick's drain applies sparse results right away (apply_results_now_kernel: no second memory round trip
   // in the sweep, and the posted bits never pass through the flags as a separate step); a read's drain, or a
@@ -437,6 +510,7 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   st->done_ops = 0;
   st->done_ranges.clear();
   st->n_state = st->n_result = 0;
+  st->any_wf = false;
   st->hwm = 0;
   return AM_OK;
 }
@@ -602,7 +676,18 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   }
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[0], s));
   const bool closed = (mode & AM_SWEEP_CLOSED_LOOP) != 0;
-  if (h->hold) {  // hold in flight: the open-loop variants that read and write since (closed loop is refused)
+  if (h->hold && h->wf_timeout) {  // ... and workflow timeouts: the variants that also set deadlines
+    p.since = h->since;
+    p.wf_timeout = h->wf_timeout;
+    p.deadline = h->deadline;
+    p.seg_deadline = h->seg_deadline;
+    if (window && o.expand) AM_LAUNCH_PDL(AM_SWEEP_TIMEOUT_KERNEL(false, true), p.n_tiles, kBlock, s, p);
+    else if (window) AM_LAUNCH(AM_SWEEP_TIMEOUT_KERNEL(false, true), p.n_tiles, kBlock, s, p);
+    else if (masks && o.expand) AM_LAUNCH_PDL(AM_SWEEP_TIMEOUT_KERNEL(true, false), p.n_tiles, kBlock, s, p);
+    else if (masks) AM_LAUNCH(AM_SWEEP_TIMEOUT_KERNEL(true, false), p.n_tiles, kBlock, s, p);
+    else if (o.expand) AM_LAUNCH_PDL(AM_SWEEP_TIMEOUT_KERNEL(false, false), p.n_tiles, kBlock, s, p);
+    else AM_LAUNCH(AM_SWEEP_TIMEOUT_KERNEL(false, false), p.n_tiles, kBlock, s, p);
+  } else if (h->hold) {  // hold in flight: the open-loop variants that read and write since (closed loop is refused)
     p.since = h->since;
     if (window && o.expand) AM_LAUNCH_PDL(AM_SWEEP_HOLD_KERNEL(false, true), p.n_tiles, kBlock, s, p);
     else if (window) AM_LAUNCH(AM_SWEEP_HOLD_KERNEL(false, true), p.n_tiles, kBlock, s, p);
@@ -898,6 +983,9 @@ void am_sweep_destroy(am_sweep_t* h) {
   }
   if (h->marks) cudaFree(h->marks);
   if (h->since) cudaFree(h->since);
+  for (void* p : {(void*)h->wf_timeout, (void*)h->deadline, (void*)h->seg_deadline, (void*)h->to_idx, (void*)h->to_since,
+                  (void*)h->to_count})
+    if (p) cudaFree(p);
   if (h->h_stats) cudaFreeHost(h->h_stats);
   h->host_out.release();
   h->pin_in.release(); h->dev_in.release();
@@ -979,6 +1067,11 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
     h->launches++;
     AM_CUDA(h, cudaGetLastError());
   }
+  if (h->wf_timeout) {  // am_record_cols_t has no timeout column: loaded slots have none, and no deadline
+    AM_CUDA(h, cudaMemsetAsync(h->wf_timeout + first, 0, n * 4, h->stream));
+    rc = drop_deadlines(h, h->stream, first, n, false);
+    if (rc != AM_OK) return rc;
+  }
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   if (first + n > h->n_records) h->n_records = first + n;
   return AM_OK;
@@ -997,6 +1090,10 @@ int am_sweep_set_hold_in_flight(am_sweep_t* h, int on) {
     AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, h->stream, h->since, kNotInFlight, h->cap_padded);
     h->launches++;
     AM_CUDA(h, cudaGetLastError());
+    if (h->wf_timeout) {  // (the deadlines of runs from before the hold was turned off)
+      rc = drop_deadlines(h, h->stream, 0, h->cap_padded, true);
+      if (rc != AM_OK) return rc;
+    }
   }
   h->hold = on != 0;
   return AM_OK;
@@ -1007,6 +1104,11 @@ int am_sweep_upsert(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_rec
   if (n == 0) return AM_OK;
   if (amsweep_host::unknown_zones(n, &recs[0].flags, sizeof(am_record_t) / sizeof(uint32_t), (uint32_t)amsweep_tz::count()))
     return AM_E_INVAL;
+  bool any_wf = false;
+  for (uint64_t k = 0; k < n; ++k) {
+    if (recs[k].wf_timeout < 0) return AM_E_RANGE;  // (nothing staged)
+    any_wf |= recs[k].wf_timeout != 0;
+  }
   std::unique_lock<std::mutex> lk(h->mu);
   Staging* stp = nullptr;
   if (int rc = reserve_staging(h, lk, n, n, &stp)) return rc;
@@ -1020,10 +1122,10 @@ int am_sweep_upsert(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_rec
   for (uint64_t k = 0; k < n; ++k) {
     dst[k] = recs[k];
     dst[k].flags &= ~AM_F_TOMBSTONE;
-    dst[k].reserved = 0;
     if (idx[k] + 1 > hwm) hwm = idx[k] + 1;
   }
   st.hwm = hwm;
+  st.any_wf |= any_wf;
   complete_range(st, st.n_ops, st.n_ops + n);
   st.n_ops += n; st.n_recs += n;
   st.n_state += (uint32_t)n;
@@ -1237,6 +1339,7 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
   AM_CUDA(h, cudaSetDevice(h->device));
   int rc = order_on(h, h->stream);
   if (rc != AM_OK) return rc;
+  h->to_ran = false;  // (ticks: the timed-out list is reset; with the hold off nothing times out)
   // A blocked run publishes no tick's accumulators: its drain leaves posted results pending in the flags,
   // and the block kernel applies them at its first tick (and counts them in that tick's row).
   rc = drain_staged(h, h->stream, (mode & AM_SWEEP_BLOCKED) ? nullptr : &unix_sec0);
@@ -1372,7 +1475,8 @@ int am_sweep_next_due(am_sweep_t* h, int64_t unix_sec, int64_t* next_out) {
   AM_CUDA(h, h->pin_in.reserve(8));
   AM_CUDA(h, cudaMemsetAsync(h->dev_in.p, 0xFF, 8, h->stream));
   AM_LAUNCH(next_due_kernel, h->sms * 8, 256, h->stream, h->cols, (const int64_t*)(h->hold ? h->since : nullptr),
-            h->n_records, unix_sec, zone_due, (unsigned long long*)h->dev_in.p);
+            (const int64_t*)(h->hold ? h->deadline : nullptr), h->n_records, unix_sec, zone_due,
+            (unsigned long long*)h->dev_in.p);
   h->launches++;
   AM_CUDA(h, cudaGetLastError());
   AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, 8, cudaMemcpyDeviceToHost, h->stream));
@@ -1437,6 +1541,40 @@ int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   memcpy(since_out, h->pin_in.p, n * 8);
   return AM_OK;
+}
+
+int am_sweep_last_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t* since, uint64_t cap, uint64_t* n_out) {
+  if (!h || (cap && (!idx || !since))) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if (h->to_ran && !h->to_fetched) {  // the device list of the last tick, waited for (it may be on a caller stream)
+    AM_CUDA(h, cudaSetDevice(h->device));
+    int rc = order_on(h, h->stream);
+    if (rc != AM_OK) return rc;
+    AM_CUDA(h, h->pin_in.reserve(4));
+    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->to_count, 4, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    const uint32_t m = *(const uint32_t*)h->pin_in.p;
+    std::vector<uint32_t> li(m);
+    std::vector<int64_t> ls(m);
+    if (m) {
+      AM_CUDA(h, cudaMemcpy(li.data(), h->to_idx, m * 4ull, cudaMemcpyDeviceToHost));
+      AM_CUDA(h, cudaMemcpy(ls.data(), h->to_since, m * 8ull, cudaMemcpyDeviceToHost));
+    }
+    h->to_host.resize(m);
+    for (uint32_t k = 0; k < m; ++k) h->to_host[k] = {li[k], ls[k]};
+    std::sort(h->to_host.begin(), h->to_host.end());  // (appended one segment at a time, in no particular order)
+    h->to_fetched = true;
+  }
+  const uint64_t n = h->to_ran ? h->to_host.size() : 0;
+  if (offset > n) return AM_E_RANGE;
+  const uint64_t left = n - offset, ncopy = left < cap ? left : cap;
+  if (n_out) *n_out = left;
+  for (uint64_t k = 0; k < ncopy; ++k) {
+    idx[k] = h->shard_base + h->to_host[offset + k].first;
+    since[k] = h->to_host[offset + k].second;
+  }
+  return left > cap ? AM_E_NOSPACE : AM_OK;
 }
 
 // (tick guard held, staged events drained, h->stream ordered)

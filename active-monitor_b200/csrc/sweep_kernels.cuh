@@ -311,7 +311,10 @@ __global__ void tz_words_kernel(const int32_t* __restrict__ tz_off, TickWords* _
 // submitted; every record that is submitted gets since = T.  The since word is loaded only for the halves that
 // hold a due record: one dependent round trip, in the warps that have one (DESIGN.md section 3 compares it with
 // streaming since for every record).
-template <bool CLOSED, bool MASKS, bool WINDOW = false, bool HOLD = false>
+// TIMEOUT = workflow timeouts (HOLD only; the handle received a non-zero am_record_t.wf_timeout): the same round trip
+// also loads the slot's timeout W, and every submitted record gets deadline = T + W (none when W is 0); one atomicMin
+// per warp lowers the segment's bound (p.seg_deadline) that expire_runs_kernel reads.
+template <bool CLOSED, bool MASKS, bool WINDOW = false, bool HOLD = false, bool TIMEOUT = false>
 __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1)
     sweep_tick_kernel(const SweepParams p) {
   // one row per warp, written unconditionally: no zero-initialisation, no shared
@@ -488,11 +491,14 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
   // ---- hold in flight: the reference's watch loop holds a check until its workflow ends (hcc.go:607-727) and only
   //      then arms the next timer (hcc.go:745-752).  A posted phase clears since at the drain (clear_since_kernel).
   if (HOLD && __any_sync(kFull, due_bits != 0)) {
+    unsigned long long dmin = ~0ull;  // TIMEOUT: the least deadline this lane set (biased key)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const uint32_t db = (due_bits >> (2 * h)) & 3u;
       if (db) {
         const longlong2 sv = ld_stream(reinterpret_cast<const longlong2*>(p.since + r0[h]));
+        int2 wv = make_int2(0, 0);
+        if (TIMEOUT) wv = ld_stream(reinterpret_cast<const int2*>(p.wf_timeout + r0[h]));
         int64_t s[2] = {sv.x, sv.y};
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
@@ -500,12 +506,29 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
             const uint32_t f = j ? fl[h].y : fl[h].x;
             const int64_t fav = j ? fa[h].y : fa[h].x;
             const bool held = s[j] != kNotInFlight && s[j] >= fav && !(f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL));
-            if (held) act[h][j] &= ~AM_ACT_SUBMIT_HC;
-            else s[j] = T;
+            if (held) {
+              act[h][j] &= ~AM_ACT_SUBMIT_HC;
+            } else {
+              s[j] = T;
+              if (TIMEOUT) {  // the run's deadline is fixed at its submission (hcc.go:611-613); a new run replaces it
+                const int32_t W = j ? wv.y : wv.x;
+                const int64_t D = W > 0 ? T + W : kNoDeadline;
+                st_stream(p.deadline + r0[h] + j, D);
+                if (W > 0 && biased_key(D) < dmin) dmin = biased_key(D);
+              }
+            }
           }
         }
         if (s[0] != sv.x || s[1] != sv.y) st_stream(reinterpret_cast<longlong2*>(p.since + r0[h]), make_longlong2(s[0], s[1]));
       }
+    }
+    if (TIMEOUT && __any_sync(kFull, dmin != ~0ull)) {  // one atomic per warp into its segment's bound
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+        const unsigned long long v = __shfl_xor_sync(kFull, dmin, o);
+        dmin = v < dmin ? v : dmin;
+      }
+      if (lane == 0) atomicMin(p.seg_deadline + (tile_base + (uint32_t)(warp * kRecPerWarp)) / (uint32_t)kRecPerWarp, dmin);
     }
   }
 
@@ -1022,9 +1045,10 @@ __global__ void next_fire_kernel(DevCols c, uint32_t first, uint32_t n, int64_t 
 // atomicMin on a biased unsigned key.  `zone_due`: a lower bound, > T, of the first activation of any
 // schedule bound to a named time zone (the launcher derives it from the zones' offsets).  `since`: the hold-in-flight
 // column (NULL when the hold is off): a held record is never due by its schedule — its next event is a posted phase
-// or a remove, each a reason for the caller to wake the ticker.
-__global__ void next_due_kernel(DevCols c, const int64_t* __restrict__ since, uint64_t n, int64_t T, int64_t zone_due,
-                                unsigned long long* out_biased) {
+// or a remove, each a reason for the caller to wake the ticker — unless it has a workflow deadline D (`deadline`, NULL
+// without workflow timeouts): the tick at max(D, T + 1) times the run out (expire_runs_kernel).
+__global__ void next_due_kernel(DevCols c, const int64_t* __restrict__ since, const int64_t* __restrict__ deadline, uint64_t n,
+                                int64_t T, int64_t zone_due, unsigned long long* out_biased) {
   unsigned long long best = ~0ull;
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t f = c.flags[i];
@@ -1036,6 +1060,7 @@ __global__ void next_due_kernel(DevCols c, const int64_t* __restrict__ since, ui
       due = T + 1;
     } else if (since && since[i] != kNotInFlight && since[i] >= c.finished_at[i]) {
       // held (nothing pending: the branch above)
+      if (deadline && deadline[i] != kNoDeadline) due = deadline[i] > T + 1 ? deadline[i] : T + 1;
     } else if (kind == AM_KIND_INTERVAL || kind == AM_KIND_CRON_EVERY) {
       const int64_t at = (int64_t)((uint64_t)c.finished_at[i] + (uint64_t)(int64_t)c.ras[i]);
       due = ((f & AM_F_TIMER_ARMED) && at > T + 1) ? at : T + 1;
@@ -1288,6 +1313,90 @@ __global__ void in_flight_kernel(DevCols c, const int64_t* __restrict__ since, u
   out[k] = held ? s : kNotInFlight;
 }
 
+// Workflow timeouts: the drain's winning upserts (the marks decide, as in apply_state_ops_kernel) store their record's
+// wf_timeout.  The timeout of a run is read when the sweep submits it, so an upsert during a run changes the next run's.
+// Launched with every drain that has state ops once the handle has timeout state.
+__global__ void store_wf_timeout_kernel(int32_t* wf, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops,
+                                        const am_record_t* __restrict__ recs, uint32_t n) {
+  pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint2 op = ops[k];
+  const uint32_t i = op.x, arg = op.y;
+  if ((arg & kOpKindMask) != kOpUpsert || marks[3u * i] != k + 1u) return;
+  wf[i] = recs[arg & ~kOpKindMask].wf_timeout;
+}
+
+// Workflow timeouts at a tick (hcc.go:613 NewIEBWithTimeout with Spec.Workflow.Timeout; :627-632 the watch loop posts a
+// synthetic "Failed" when the run outlives it).  Runs in the tick's drain while the hold is on, after clear_since_kernel
+// and before the result kernels.  Lane L of a warp reads the bound of segment 32 w + L: 8 B per 128 slots when nothing
+// is due.  A segment whose bound is <= T is visited by the whole warp, 32 slots at a time: every deadline <= T is
+// dropped; a run that is still held (the sweep's rule) on a live record gets AM_F_PENDING_FAIL, exactly as a posted
+// Failed does, so the result kernel behind this one or the sweep's pending path applies it (counters, finishedAt = T,
+// timer, remedy gate); its since is cleared as clear_since_kernel clears it for a posted phase; and (slot, since) is
+// appended to the tick's list (one atomic per segment).  The bound becomes the exact minimum of what is left.
+__global__ void expire_runs_kernel(DevCols c, int64_t* since, int64_t* deadline, unsigned long long* seg_deadline,
+                                   uint32_t n_seg, int64_t T, uint32_t* out_idx, int64_t* out_since, uint32_t* out_count) {
+  pdl_wait();  // (launched with programmatic stream serialisation: the previous tick's sweep writes deadlines)
+  const int lane = threadIdx.x & 31;
+  const uint32_t seg0 = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 32u;
+  if (seg0 >= n_seg) return;  // warp-uniform
+  const unsigned long long tkey = biased_key(T);
+  uint32_t due = __ballot_sync(kFull, seg0 + (uint32_t)lane < n_seg && seg_deadline[seg0 + lane] <= tkey);
+  while (due) {  // warp-uniform
+    const uint32_t seg = seg0 + (uint32_t)(__ffs((int)due) - 1);
+    due &= due - 1;
+    unsigned long long left = ~0ull;
+    uint32_t hit = 0;  // bit q: slot 32 q + lane of the segment timed out
+    int64_t sv[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint32_t i = seg * (uint32_t)kRecPerWarp + 32u * q + (uint32_t)lane;
+      const int64_t D = deadline[i];
+      sv[q] = kNotInFlight;
+      if (D <= T) {
+        deadline[i] = kNoDeadline;
+        const uint32_t f = c.flags[i];
+        const int64_t s = since[i];
+        if (is_live(f) && s != kNotInFlight && s >= c.finished_at[i] && !(f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL))) {
+          c.flags[i] = f | AM_F_PENDING_FAIL;
+          since[i] = kNotInFlight;
+          sv[q] = s;
+          hit |= 1u << q;
+        }
+      } else if (biased_key(D) < left) {
+        left = biased_key(D);
+      }
+    }
+    const uint32_t cnt = (uint32_t)__popc(hit);
+    uint32_t incl = cnt;  // inclusive prefix over the lanes
+#pragma unroll
+    for (unsigned o = 1; o < 32; o <<= 1) {
+      const uint32_t v = __shfl_up_sync(kFull, incl, o);
+      if ((unsigned)lane >= o) incl += v;
+    }
+    const uint32_t total = __reduce_add_sync(kFull, cnt);
+    uint32_t base = 0;
+    if (total && lane == 0) base = atomicAdd(out_count, total);
+    base = __reduce_add_sync(kFull, base);  // (lane 0's, to every lane)
+    uint32_t pos = base + incl - cnt;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if ((hit >> q) & 1u) {
+        out_idx[pos] = seg * (uint32_t)kRecPerWarp + 32u * q + (uint32_t)lane;
+        out_since[pos] = sv[q];
+        ++pos;
+      }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+      const unsigned long long v = __shfl_xor_sync(kFull, left, o);
+      left = v < left ? v : left;
+    }
+    if (lane == 0) seg_deadline[seg] = left;
+  }
+}
+
 __global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1310,7 +1419,7 @@ __global__ void gather_records_kernel(DevCols c, const uint32_t* __restrict__ id
   r.runs_limit = c.runs_limit[i]; r.reset_interval = c.reset_interval[i];
   r.success = c.success[i]; r.failed = c.failed[i]; r.remedy_success = c.remedy_success[i];
   r.remedy_failed = c.remedy_failed[i]; r.remedy_total = c.remedy_total[i];
-  r.reserved = 0;
+  r.wf_timeout = 0;  // (not returned by am_sweep_read)
   out[k] = r;
 }
 

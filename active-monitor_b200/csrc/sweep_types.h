@@ -41,6 +41,7 @@
 #define AM_SWEEP_KERNEL(closed, masks) sweep_tick_kernel<closed, masks>  // one macro argument
 #define AM_SWEEP_WINDOW_KERNEL(closed) sweep_tick_kernel<closed, false, true>  // catch-up ticks
 #define AM_SWEEP_HOLD_KERNEL(masks, window) sweep_tick_kernel<false, masks, window, true>  // hold in flight (open loop)
+#define AM_SWEEP_TIMEOUT_KERNEL(masks, window) sweep_tick_kernel<false, masks, window, true, true>  // ... + workflow timeouts
 
 namespace amsweep {
 
@@ -128,8 +129,15 @@ struct SweepParams {
                              // (civil.h, window_boxes), the unused ones with sec0 = 0
   int64_t* since;            // HOLD variants: [cap] the second of the tick that submitted the slot's running health-check
                              // workflow, kNotInFlight when none (am_sweep_set_hold_in_flight); NULL otherwise
+  // TIMEOUT variants (workflow timeouts, am_record_t.wf_timeout): NULL otherwise
+  const int32_t* wf_timeout;           // [cap] the slot's workflow timeout in seconds, 0 = none (the latest upsert's)
+  int64_t* deadline;                   // [cap] the running workflow's deadline, kNoDeadline when none
+  unsigned long long* seg_deadline;    // [cap / kRecPerWarp] per warp segment a lower bound of its deadlines (biased key)
 };
 constexpr int64_t kNotInFlight = INT64_MIN;
+constexpr int64_t kNoDeadline = INT64_MAX;
+// a signed second as an unsigned key of the same order (the atomicMin idiom of next_due_kernel); kNoDeadline -> ~0
+__device__ __forceinline__ unsigned long long biased_key(int64_t t) { return (unsigned long long)t ^ (1ull << 63); }
 
 struct ScanParams {
   uint32_t* group_count;        // this tick's per-group sums; zeroed again once read

@@ -340,6 +340,24 @@ class Sweep:
                                                  out.ctypes.data), "am_sweep_in_flight")
         return out
 
+    def last_timed_out(self, offset: int = 0, cap: int | None = None):
+        """the runs the last tick timed out (workflow timeouts, am_sweep_last_timed_out): (global idx u64, since i64),
+        ascending by index, from entry `offset` on.  cap None: all of them."""
+        n = L.u64(0)
+        if cap is None:
+            rc = self._lib.am_sweep_last_timed_out(self._h, offset, None, None, 0, C.byref(n))
+            if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+                self._check(rc, "am_sweep_last_timed_out")
+            cap = int(n.value)
+        idx = np.empty(cap, dtype=np.uint64)
+        since = np.empty(cap, dtype=np.int64)
+        rc = self._lib.am_sweep_last_timed_out(self._h, offset, idx.ctypes.data if cap else None,
+                                               since.ctypes.data if cap else None, cap, C.byref(n))
+        if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+            self._check(rc, "am_sweep_last_timed_out")
+        k = min(int(n.value), cap)
+        return idx[:k], since[:k]
+
     # -- introspection
     def set_seed(self, seed: int):
         self._check(self._lib.am_sweep_set_seed(self._h, seed), "am_sweep_set_seed")

@@ -166,7 +166,12 @@ typedef struct am_record {
   uint32_t flags;
   int32_t runs_limit, reset_interval;
   int32_t success, failed, remedy_success, remedy_failed, remedy_total;
-  int32_t reserved;
+  int32_t wf_timeout;         /* workflow timeout in whole seconds, 0 = none: the effective
+                                 timeout of hcc.go:981-985 that the caller sets for
+                                 am_sweep_upsert (< 0: AM_E_RANGE).  Only read while the hold
+                                 in flight is on (see am_sweep_set_hold_in_flight).  The
+                                 classify and ingest calls write 0; am_sweep_read does not
+                                 return it; am_sweep_load_range sets it to 0.               */
 } am_record_t;
 
 /* Ladder classification at upsert, in the order hcc.go:227 -> 238 -> 251 ->
@@ -373,7 +378,9 @@ int am_sweep_run_ticks(am_sweep_t*, int64_t unix_sec0, uint64_t n_ticks, uint32_
  * checks, 0 otherwise.  On-demand query, not part of the per-tick path. */
 int am_sweep_repeat_after_sec(am_sweep_t*, int64_t unix_sec, uint64_t first, uint64_t n, int64_t* out);
 
-/* The earliest second after unix_sec at which a tick of this shard would emit anything, given
+/* The earliest second after unix_sec at which a tick of this shard would emit anything or time a
+ * run out (workflow timeouts, see am_sweep_set_hold_in_flight: a held run with deadline D counts as
+ * an event at max(D, unix_sec + 1), whether or not its expiry emits anything), given
  * the state as it stands (staged events included, no further ones assumed): the wake-up time of
  * the reference's earliest repeat timer (hcc.go:751) or cron activation (hcc.go:262), evaluated on
  * the device over every record (robfig SpecSchedule.Next for 5-field schedules).  The 1 Hz ticker
@@ -397,8 +404,8 @@ int am_sweep_read(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx,
  * also in a tick that returns AM_E_NOSPACE (the rest of its list is in am_sweep_last_list).
  * Release: a posted workflow phase clears since when the next tick or read drains it — also when
  * an upsert of the slot staged after it supersedes the result itself, and whatever second the next
- * tick has.  The caller's watch loop posts Failed itself when its workflow timeout expires
- * (hcc.go:627-632).  am_sweep_remove and am_sweep_load_range clear since for their slots; a remedy
+ * tick has.  Workflow timeouts (hcc.go:603-632: the watch loop gives up after Spec.Workflow.Timeout
+ * and posts a synthetic Failed) are kept on the device, below.  am_sweep_remove and am_sweep_load_range clear since for their slots; a remedy
  * phase alone does not.  An upsert keeps the hold (a status write during a run re-enters
  * Reconcile; it must not submit the check again) unless its finishedAt is later than since.
  * Only the health-check workflow is held: remedy workflows are not.
@@ -409,8 +416,31 @@ int am_sweep_read(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx,
  * records: their next event is a post_result or a remove.
  * Turning the hold on starts with nothing in flight (turn it on before the first tick); turning it
  * off makes every slot read as not in flight.  The first call with on != 0 allocates 8 B per slot
- * of capacity on the device.  Replaces the caller's own de-duplication of in-flight checks. */
+ * of capacity on the device.  Replaces the caller's own de-duplication of in-flight checks.
+ * Workflow timeouts, while the hold is on: every run a tick submits gets the deadline
+ * D = T + W when the slot's wf_timeout W (from its latest upsert) is > 0 at that tick, and none
+ * otherwise; a later submission of the slot replaces D, and a remove, a load_range and turning the
+ * hold off or on drop it.  So an upsert during a run changes the timeout of the next run only.  The
+ * first tick of any entry point with T >= D looks at the run after the tick's drain: if it is still
+ * held (a live record), the tick treats it exactly as if am_sweep_post_result(slot,
+ * AM_PHASE_FAILED, AM_PHASE_NONE) had been the last call before the tick (FailedCount + 1,
+ * finishedAt = T, the timer armed, the remedy gate and its actions, n_result_fail, the hold
+ * released, then the due decision at T: a 5-field check that matches T is submitted again in the
+ * same tick).  Either way D is dropped: a phase posted before that tick wins, a run released by
+ * then is not timed out, and a later upsert that holds it again does not bring D back.  A refused
+ * tick times nothing out.  The first upsert with a non-zero wf_timeout allocates 24 B per slot of
+ * capacity on the device; handles that never receive one launch nothing more.  Remedy workflows
+ * have no timeout here, and am_sweep_run_ticks is refused while the hold is on anyway. */
 int am_sweep_set_hold_in_flight(am_sweep_t*, int on);
+
+/* The runs the last tick (of any entry point) timed out, ascending by global index, from entry
+ * `offset` on: idx[k] the global index, since[k] the run's Status.StartedAt (hcc.go:609/665), for
+ * the status and the "Workflow timed out" event (hcc.go:631) the caller writes.  *n_out = entries
+ * from `offset` to the end; AM_E_NOSPACE if they exceed cap (the first cap entries are valid);
+ * AM_E_RANGE when offset is past the end.  Every tick resets the list (empty while the hold is off
+ * or no wf_timeout was ever set); it is valid until the next tick.  After am_sweep_tick_device /
+ * am_sweep_tick_shard the call waits for that tick to finish. */
+int am_sweep_last_timed_out(am_sweep_t*, uint64_t offset, uint64_t* idx, int64_t* since, uint64_t cap, uint64_t* n_out);
 
 /* For each slot of [first, first+n) (idx == NULL) or idx[0..n): the `since` of a slot the next
  * tick would hold, INT64_MIN for every other slot (and for all of them while the hold is off).
