@@ -18,7 +18,12 @@
 //     tick, no device-to-host copy call, and am_sweep_tick_view hands that memory to the
 //     caller without another pass;
 //   * every device operation of a handle is ordered after the previous one even when they
-//     are issued on different streams (am_sweep_tick_device takes the caller's stream).
+//     are issued on different streams (am_sweep_tick_device takes the caller's stream);
+//   * am_sweep_tick, _tick_view, _tick_device and _tick_shard run one path (run_tick): the
+//     refusals, the drain, the sweep and the commit of the previous tick's second; the sweep
+//     variant comes from one table (sweep_variant);
+//   * fixed-size device arrays, pinned host arrays and events are recorded on the handle as
+//     they are made (dev_array, host_array, new_event): am_sweep_destroy frees that list.
 //
 // There is deliberately no CPU path in this file: without a CUDA device
 // am_sweep_create fails with AM_E_DEVICE.
@@ -58,35 +63,37 @@ void set_create_error(const std::string& s) {
   g_create_error = s;
 }
 
-struct PinnedBuf {
+// A growable array in pinned host memory or in device memory; its contents do not survive growth.
+template <bool kPinned>
+struct Buf {
   void* p = nullptr;
   size_t cap = 0;
   cudaError_t reserve(size_t bytes, unsigned flags = cudaHostAllocDefault) {
     if (bytes <= cap) return cudaSuccess;
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    cap = 0;
+    release();
     size_t want = bytes + bytes / 2 + 4096;
-    cudaError_t e = cudaHostAlloc(&p, want, flags);
+    cudaError_t e = kPinned ? cudaHostAlloc(&p, want, flags) : cudaMalloc(&p, want);
     if (e == cudaSuccess) cap = want;
     return e;
   }
-  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
+  void release() { if (p) (void)(kPinned ? cudaFreeHost(p) : cudaFree(p)); p = nullptr; cap = 0; }
 };
-struct DevBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  cudaError_t reserve(size_t bytes) {
-    if (bytes <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    size_t want = bytes + bytes / 2 + 4096;
-    cudaError_t e = cudaMalloc(&p, want);
-    if (e == cudaSuccess) cap = want;
-    return e;
-  }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+using PinnedBuf = Buf<true>;
+using DevBuf = Buf<false>;
+
+// A small table uploaded from the host on the tick's stream.  The device array and the pinned copy are allocated
+// at their full size, the device one zeroed, at the first upload.
+struct Upload {
+  void* dev = nullptr;
+  void* pin = nullptr;
+  cudaEvent_t copied = nullptr;  // the last upload has left `pin`
+  bool pending = false;
+};
+
+// What am_sweep_destroy frees: every fixed-size allocation and every event of a handle, recorded as it is made.
+struct Owned {
+  enum Kind { kDevice, kPinned, kEvent } kind;
+  void* p;
 };
 
 // One of the two staging areas for controller events.  The pinned arrays are appended to
@@ -133,8 +140,6 @@ struct am_sweep {
   uint64_t capacity = 0, cap_padded = 0, shard_base = 0;
   uint64_t n_records = 0;  // high-water mark
   DevCols cols{};
-  void* col_ptr[16] = {};
-  size_t col_elem[16] = {};
   MaskPlanes planes{};             // the on-minute sweep's copy of the mask columns as bit planes
   uint32_t* seg_dirty = nullptr;   // [cap_padded / kRecPerWarp] segments a drain's state ops touched
   TickSet set[2];
@@ -170,18 +175,13 @@ struct am_sweep {
   uint32_t tz_n = 0;  // zones + 1; 0 or 1 = nothing registered
   int64_t tz_lo = 0, tz_hi = 0;
   bool tz_aligned = true;  // every offset a whole number of minutes
-  DevBuf tz_off, tz_table;
-  PinnedBuf tz_pin;
-  cudaEvent_t tz_copied = nullptr;
-  bool tz_copy_pending = false;
+  Upload tz_off;                 // [kMaxZones + 1] int32
+  TickWords* tz_table = nullptr;  // [kMaxZones + 1], written by tz_words_kernel
   // catch-up ticks (AM_SWEEP_CATCH_UP): the second of the previous tick, and the device table of a window's
   // calendar boxes ([kMaxZones + 1][kWindowBoxes], allocated at the first catch-up tick that needs it)
   bool has_prev = false;
   int64_t prev_T = 0;
-  DevBuf win_boxes;
-  PinnedBuf win_pin;
-  cudaEvent_t win_copied = nullptr;
-  bool win_copy_pending = false;
+  Upload win_boxes;
   // hold in flight (am_sweep_set_hold_in_flight): per slot the second of the tick that submitted its running health-check
   // workflow, kNotInFlight when none ([cap_padded], allocated when the hold is first turned on)
   bool hold = false;
@@ -205,6 +205,7 @@ struct am_sweep {
   bool early_results = true;  // AMSWEEP_EARLY_RESULTS=0: every posted result is applied inside the sweep
   Staging* pend_clear = nullptr;  // a host tick's drain leaves clear_marks_kernel for after the tick's kernels
   size_t pend_clear_n = 0;
+  std::vector<Owned> owned;
 };
 
 namespace {
@@ -262,6 +263,40 @@ int order_on(am_sweep* h, cudaStream_t s) {
   h->has_last = true;
   return AM_OK;
 }
+
+// The first half of every call's device work: the handle's device current and `s` ordered after its last operation.
+int set_stream(am_sweep* h, cudaStream_t s) {
+  AM_CUDA(h, cudaSetDevice(h->device));
+  return order_on(h, s);
+}
+
+// A fixed-size device array owned by the handle until am_sweep_destroy; zeroed on `s` when `zero`.
+template <class T>
+cudaError_t dev_array(am_sweep* h, T** p, size_t bytes, cudaStream_t s, bool zero = true) {
+  void* q = nullptr;
+  cudaError_t e = cudaMalloc(&q, bytes);
+  if (e != cudaSuccess) return e;
+  h->owned.push_back({Owned::kDevice, q});
+  *p = (T*)q;
+  return zero ? cudaMemsetAsync(q, 0, bytes, s) : cudaSuccess;
+}
+template <class T>
+cudaError_t host_array(am_sweep* h, T** p, size_t bytes, unsigned flags = cudaHostAllocDefault) {
+  void* q = nullptr;
+  cudaError_t e = cudaHostAlloc(&q, bytes, flags);
+  if (e != cudaSuccess) return e;
+  h->owned.push_back({Owned::kPinned, q});
+  *p = (T*)q;
+  return cudaSuccess;
+}
+cudaError_t new_event(am_sweep* h, cudaEvent_t* ev, bool timed = false) {
+  cudaError_t e = timed ? cudaEventCreate(ev) : cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) h->owned.push_back({Owned::kEvent, (void*)*ev});
+  return e;
+}
+
+// The seconds the calendar arithmetic takes: |unix_sec| < 2^55.
+bool time_ok(int64_t unix_sec) { return unix_sec < (1ll << 55) && unix_sec > -(1ll << 55); }
 
 // Grow a pinned staging array (called under h->mu); keeps the contents.  Copies out of the
 // old array may still be in flight on the copy stream: wait for them before it is freed.
@@ -378,14 +413,12 @@ int drop_deadlines(am_sweep* h, cudaStream_t s, uint64_t first, uint64_t n, bool
 // the list's index 4 and since 8) and 8 B per 128-slot segment.
 int alloc_timeouts(am_sweep* h, cudaStream_t s) {
   const size_t cap = h->cap_padded;
-  AM_CUDA(h, cudaMalloc((void**)&h->wf_timeout, cap * 4));
-  AM_CUDA(h, cudaMemsetAsync(h->wf_timeout, 0, cap * 4, s));
-  AM_CUDA(h, cudaMalloc((void**)&h->deadline, cap * 8));
-  AM_CUDA(h, cudaMalloc((void**)&h->seg_deadline, cap / kRecPerWarp * 8));
-  AM_CUDA(h, cudaMalloc((void**)&h->to_idx, cap * 4));
-  AM_CUDA(h, cudaMalloc((void**)&h->to_since, cap * 8));
-  AM_CUDA(h, cudaMalloc((void**)&h->to_count, 4));
-  AM_CUDA(h, cudaMemsetAsync(h->to_count, 0, 4, s));
+  AM_CUDA(h, dev_array(h, &h->wf_timeout, cap * 4, s));
+  AM_CUDA(h, dev_array(h, &h->deadline, cap * 8, s, false));
+  AM_CUDA(h, dev_array(h, &h->seg_deadline, cap / kRecPerWarp * 8, s, false));
+  AM_CUDA(h, dev_array(h, &h->to_idx, cap * 4, s, false));
+  AM_CUDA(h, dev_array(h, &h->to_since, cap * 8, s, false));
+  AM_CUDA(h, dev_array(h, &h->to_count, 4, s));
   return drop_deadlines(h, s, 0, cap, true);
 }
 
@@ -403,6 +436,20 @@ int expire_runs(am_sweep* h, cudaStream_t s, int64_t T) {
     h->launches++;
   }
   AM_CUDA(h, cudaGetLastError());
+  return AM_OK;
+}
+
+// Take buffer set `ts` for a tick on `s`: an exchange on another stream may still be reading it, and a tick_shard
+// whose statistics no exchange published left them in its accumulators (they are not this tick's).
+int claim_set(am_sweep* h, TickSet& ts, cudaStream_t s) {
+  if (ts.consumed_pending) {
+    AM_CUDA(h, cudaStreamWaitEvent(s, ts.consumed, 0));
+    ts.consumed_pending = false;
+  }
+  if (ts.unpublished) {
+    AM_CUDA(h, cudaMemsetAsync(ts.acc, 0, kNumAcc * 8, s));
+    ts.unpublished = false;
+  }
   return AM_OK;
 }
 
@@ -481,14 +528,7 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   // streaming path (apply_result_ops_kernel).
   if (tick_T && st->n_result && h->early_results && (uint64_t)st->n_result * 8 <= h->n_records) {
     TickSet& ts = h->set[h->parity];  // the buffer set of the tick being prepared
-    if (ts.consumed_pending) {        // (its statistics may still be read by an exchange on another stream)
-      AM_CUDA(h, cudaStreamWaitEvent(s, ts.consumed, 0));
-      ts.consumed_pending = false;
-    }
-    if (ts.unpublished) {
-      AM_CUDA(h, cudaMemsetAsync(ts.acc, 0, kNumAcc * 8, s));
-      ts.unpublished = false;
-    }
+    if (int rc = claim_set(h, ts, s)) return rc;
     AM_LAUNCH_PDL(apply_results_now_kernel, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc);
     h->launches++;
   } else if (st->n_result) {
@@ -515,6 +555,28 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   return AM_OK;
 }
 
+// The prologue of a call that is not a tick (tick guard held): on the handle's stream, after every upsert, remove
+// and result staged before it.
+int begin_call(am_sweep* h) {
+  const int rc = set_stream(h, h->stream);
+  return rc != AM_OK ? rc : drain_staged(h, h->stream);
+}
+
+// dev_in / pin_in for an on-demand kernel: `out_bytes` of results at the start, then (when `idx` is given) the n
+// slots as u32, copied to the device on the handle's stream.  *d_idx = that device copy, or NULL without `idx`.
+int stage_indices(am_sweep* h, size_t out_bytes, uint64_t n, const uint64_t* idx, const uint32_t** d_idx) {
+  AM_CUDA(h, h->pin_in.reserve(out_bytes + (idx ? n * 4 : 0)));
+  AM_CUDA(h, h->dev_in.reserve(out_bytes + (idx ? n * 4 : 0)));
+  *d_idx = nullptr;
+  if (!idx) return AM_OK;
+  uint32_t* hidx = (uint32_t*)((char*)h->pin_in.p + out_bytes);
+  for (uint64_t k = 0; k < n; ++k) hidx[k] = (uint32_t)idx[k];
+  uint32_t* didx = (uint32_t*)((char*)h->dev_in.p + out_bytes);
+  AM_CUDA(h, cudaMemcpyAsync(didx, hidx, n * 4, cudaMemcpyHostToDevice, h->stream));
+  *d_idx = didx;
+  return AM_OK;
+}
+
 // Where the rebuilt list goes: HBM (device-resident pipelines), mapped host memory (host
 // ticks) or nowhere (am_sweep_tick_shard: the exchange rebuilds the global list).
 struct ListOut {
@@ -525,6 +587,20 @@ struct ListOut {
   am_tick_stats_t* stats = nullptr;   // device or mapped host memory, may be NULL
   bool expand = true;
 };
+
+// Copy `bytes` of `src` into `u` on `s`.  Stream-ordered: a kernel still reading the previous contents runs before
+// the copy (every device operation of a handle is ordered).
+int upload(am_sweep* h, Upload& u, size_t full, const void* src, size_t bytes, cudaStream_t s) {
+  if (!u.dev) AM_CUDA(h, dev_array(h, &u.dev, full, s));
+  if (!u.pin) AM_CUDA(h, host_array(h, &u.pin, full));  // full size at once: the pinned array never moves under a copy
+  if (!u.copied) AM_CUDA(h, new_event(h, &u.copied));
+  if (u.pending) AM_CUDA(h, cudaEventSynchronize(u.copied));  // the previous copy has left the pinned array
+  memcpy(u.pin, src, bytes);
+  AM_CUDA(h, cudaMemcpyAsync(u.dev, u.pin, bytes, cudaMemcpyHostToDevice, s));
+  AM_CUDA(h, cudaEventRecord(u.copied, s));
+  u.pending = true;
+  return AM_OK;
+}
 
 // The zones' UTC offsets at T on the device.  Per tick: one uncontended lock for the registry version
 // and two compares; the offsets themselves are recomputed (tz_eval.h, host) and copied — a few hundred
@@ -545,22 +621,9 @@ int refresh_zones(am_sweep* h, int64_t T, cudaStream_t s) {
     h->tz_hi = INT64_MAX;
     return AM_OK;
   }
-  const size_t bytes = (amsweep_tz::kMaxZones + 1) * sizeof(int32_t);
-  if (!h->tz_off.p) {  // allocated once, for every id a record can carry; entries of zones not registered stay zero
-    AM_CUDA(h, h->tz_off.reserve(bytes));
-    AM_CUDA(h, cudaMemsetAsync(h->tz_off.p, 0, h->tz_off.cap, s));
-    AM_CUDA(h, h->tz_table.reserve((amsweep_tz::kMaxZones + 1) * sizeof(TickWords)));
-    AM_CUDA(h, cudaMemsetAsync(h->tz_table.p, 0, h->tz_table.cap, s));
-  }
-  AM_CUDA(h, h->tz_pin.reserve(bytes));
-  if (!h->tz_copied) AM_CUDA(h, cudaEventCreateWithFlags(&h->tz_copied, cudaEventDisableTiming));
-  if (h->tz_copy_pending) AM_CUDA(h, cudaEventSynchronize(h->tz_copied));  // the previous copy has left the pinned array
-  memcpy(h->tz_pin.p, offs.data(), offs.size() * sizeof(int32_t));
-  // (stream-ordered after every earlier tick of the handle: none of them still reads the old offsets)
-  AM_CUDA(h, cudaMemcpyAsync(h->tz_off.p, h->tz_pin.p, offs.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  AM_CUDA(h, cudaEventRecord(h->tz_copied, s));
-  h->tz_copy_pending = true;
-  return AM_OK;
+  // allocated once, for every id a record can carry; entries of zones not registered stay zero
+  if (!h->tz_table) AM_CUDA(h, dev_array(h, &h->tz_table, (amsweep_tz::kMaxZones + 1) * sizeof(TickWords), s));
+  return upload(h, h->tz_off, (amsweep_tz::kMaxZones + 1) * sizeof(int32_t), offs.data(), offs.size() * sizeof(int32_t), s);
 }
 
 // A catch-up tick's window (P, T] as calendar boxes per zone.  Computed before anything of the tick happens,
@@ -594,24 +657,25 @@ int plan_window(am_sweep* h, int64_t T, uint32_t mode, WindowPlan* w) {
   return AM_OK;
 }
 
-// The window's boxes on the device, stream-ordered like refresh_zones: a sweep still reading the previous
-// window's table runs before this copy on `s` (every device operation of a handle is ordered).  Zones
-// registered after the plan keep zero entries (sec0 = 0): no box, not due.
-int upload_window(am_sweep* h, const WindowPlan& w, cudaStream_t s) {
-  const size_t full = (size_t)(amsweep_tz::kMaxZones + 1) * kWindowBoxes * sizeof(TickWords);
-  if (!h->win_boxes.p) {
-    AM_CUDA(h, h->win_boxes.reserve(full));
-    AM_CUDA(h, cudaMemsetAsync(h->win_boxes.p, 0, h->win_boxes.cap, s));
-  }
-  AM_CUDA(h, h->win_pin.reserve(full));  // full size at once: the pinned array never moves under a copy
-  if (!h->win_copied) AM_CUDA(h, cudaEventCreateWithFlags(&h->win_copied, cudaEventDisableTiming));
-  if (h->win_copy_pending) AM_CUDA(h, cudaEventSynchronize(h->win_copied));  // the previous copy has left the pinned array
-  const size_t bytes = w.boxes.size() * sizeof(TickWords);
-  memcpy(h->win_pin.p, w.boxes.data(), bytes);
-  AM_CUDA(h, cudaMemcpyAsync(h->win_boxes.p, h->win_pin.p, bytes, cudaMemcpyHostToDevice, s));
-  AM_CUDA(h, cudaEventRecord(h->win_copied, s));
-  h->win_copy_pending = true;
-  return AM_OK;
+// The sweep variant of a tick: a row per loop mode, a column per way the masks are read (not at all, the planes of
+// T's minute, the canonical masks against a catch-up window's boxes).  These are the 12 instantiations of
+// sweep_tick_kernel there are.  Two combinations have none and never get here: closed loop with the hold on (refused
+// before the drain, and run_ticks refuses the hold) and a window with the planes (launch_tick sets `masks` only
+// without a window).
+using SweepFn = void (*)(const SweepParams);
+SweepFn sweep_variant(bool closed, bool masks, bool window, bool hold, bool timeout) {
+  static constexpr SweepFn kVariants[4][3] = {
+      // open loop
+      {sweep_tick_kernel<false, false>, sweep_tick_kernel<false, true>, sweep_tick_kernel<false, false, true>},
+      // closed loop
+      {sweep_tick_kernel<true, false>, sweep_tick_kernel<true, true>, sweep_tick_kernel<true, false, true>},
+      // hold in flight (open loop)
+      {sweep_tick_kernel<false, false, false, true>, sweep_tick_kernel<false, true, false, true>,
+       sweep_tick_kernel<false, false, true, true>},
+      // ... and workflow timeouts
+      {sweep_tick_kernel<false, false, false, true, true>, sweep_tick_kernel<false, true, false, true, true>,
+       sweep_tick_kernel<false, false, true, true, true>}};
+  return kVariants[hold ? 2 + timeout : closed][window ? 2 : masks];
 }
 
 int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStream_t s, const WindowPlan* win = nullptr) {
@@ -622,14 +686,7 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
     return AM_OK;
   }
   TickSet& ts = h->set[h->parity];
-  if (ts.consumed_pending) {  // an exchange on another stream may still be reading this buffer set
-    AM_CUDA(h, cudaStreamWaitEvent(s, ts.consumed, 0));
-    ts.consumed_pending = false;
-  }
-  if (ts.unpublished) {  // a tick_shard whose statistics no exchange published: not this tick's
-    AM_CUDA(h, cudaMemsetAsync(ts.acc, 0, kNumAcc * 8, s));
-    ts.unpublished = false;
-  }
+  if (int rc = claim_set(h, ts, s)) return rc;
   SweepParams p{};
   p.c = h->cols;
   p.n_records = h->n_records;
@@ -653,16 +710,16 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   // A catch-up tick reads the canonical masks against the window's boxes instead of planes and zone words.
   const bool window = win && win->any;
   const bool masks = !window && (sec_of_min == 0 || (mode & AM_SWEEP_FULL_SCAN) || (h->tz_n > 1 && !h->tz_aligned));
-  if (window) {
-    const int rc = upload_window(h, *win, s);
+  if (window) {  // zones registered after the plan keep zero entries (sec0 = 0): no box, not due
+    const int rc = upload(h, h->win_boxes, (size_t)(amsweep_tz::kMaxZones + 1) * kWindowBoxes * sizeof(TickWords),
+                          win->boxes.data(), win->boxes.size() * sizeof(TickWords), s);
     if (rc != AM_OK) return rc;
-    p.tz_table = (const TickWords*)h->win_boxes.p;
+    p.tz_table = (const TickWords*)h->win_boxes.dev;
   }
   if (masks && h->tz_n > 1) {  // the tick's wall clock per zone, from the cached offsets
-    AM_LAUNCH_PDL(tz_words_kernel, (h->tz_n + 63) / 64, 64, s, (const int32_t*)h->tz_off.p, (TickWords*)h->tz_table.p, T,
-                  h->tz_n);
+    AM_LAUNCH_PDL(tz_words_kernel, (h->tz_n + 63) / 64, 64, s, (const int32_t*)h->tz_off.dev, h->tz_table, T, h->tz_n);
     h->launches++;
-    p.tz_table = (const TickWords*)h->tz_table.p;
+    p.tz_table = h->tz_table;
   }
   if (masks) {  // the six planes of T's UTC fields
     const CivilTime ct = civil_from_unix(T);
@@ -675,45 +732,20 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
     p.pl.star = plane(kPlaneStar);
   }
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[0], s));
-  const bool closed = (mode & AM_SWEEP_CLOSED_LOOP) != 0;
-  if (h->hold && h->wf_timeout) {  // ... and workflow timeouts: the variants that also set deadlines
-    p.since = h->since;
+  const bool timeout = h->hold && h->wf_timeout;
+  if (h->hold) p.since = h->since;  // hold in flight: the variants that read and write since
+  if (timeout) {                    // ... and workflow timeouts: the variants that also set deadlines
     p.wf_timeout = h->wf_timeout;
     p.deadline = h->deadline;
     p.seg_deadline = h->seg_deadline;
-    if (window && o.expand) AM_LAUNCH_PDL(AM_SWEEP_TIMEOUT_KERNEL(false, true), p.n_tiles, kBlock, s, p);
-    else if (window) AM_LAUNCH(AM_SWEEP_TIMEOUT_KERNEL(false, true), p.n_tiles, kBlock, s, p);
-    else if (masks && o.expand) AM_LAUNCH_PDL(AM_SWEEP_TIMEOUT_KERNEL(true, false), p.n_tiles, kBlock, s, p);
-    else if (masks) AM_LAUNCH(AM_SWEEP_TIMEOUT_KERNEL(true, false), p.n_tiles, kBlock, s, p);
-    else if (o.expand) AM_LAUNCH_PDL(AM_SWEEP_TIMEOUT_KERNEL(false, false), p.n_tiles, kBlock, s, p);
-    else AM_LAUNCH(AM_SWEEP_TIMEOUT_KERNEL(false, false), p.n_tiles, kBlock, s, p);
-  } else if (h->hold) {  // hold in flight: the open-loop variants that read and write since (closed loop is refused)
-    p.since = h->since;
-    if (window && o.expand) AM_LAUNCH_PDL(AM_SWEEP_HOLD_KERNEL(false, true), p.n_tiles, kBlock, s, p);
-    else if (window) AM_LAUNCH(AM_SWEEP_HOLD_KERNEL(false, true), p.n_tiles, kBlock, s, p);
-    else if (masks && o.expand) AM_LAUNCH_PDL(AM_SWEEP_HOLD_KERNEL(true, false), p.n_tiles, kBlock, s, p);
-    else if (masks) AM_LAUNCH(AM_SWEEP_HOLD_KERNEL(true, false), p.n_tiles, kBlock, s, p);
-    else if (o.expand) AM_LAUNCH_PDL(AM_SWEEP_HOLD_KERNEL(false, false), p.n_tiles, kBlock, s, p);
-    else AM_LAUNCH(AM_SWEEP_HOLD_KERNEL(false, false), p.n_tiles, kBlock, s, p);
-  } else if (window) {  // (launched as the plain variants below are)
-    if (o.expand && closed) AM_LAUNCH_PDL(AM_SWEEP_WINDOW_KERNEL(true), p.n_tiles, kBlock, s, p);
-    else if (o.expand) AM_LAUNCH_PDL(AM_SWEEP_WINDOW_KERNEL(false), p.n_tiles, kBlock, s, p);
-    else if (closed) AM_LAUNCH(AM_SWEEP_WINDOW_KERNEL(true), p.n_tiles, kBlock, s, p);
-    else AM_LAUNCH(AM_SWEEP_WINDOW_KERNEL(false), p.n_tiles, kBlock, s, p);
-  } else if (o.expand) {  // single-stream tick: the sweep's launch hides behind its predecessor (the previous tick's publish, the drain)
-    if (closed && masks) AM_LAUNCH_PDL(AM_SWEEP_KERNEL(true, true), p.n_tiles, kBlock, s, p);
-    else if (closed) AM_LAUNCH_PDL(AM_SWEEP_KERNEL(true, false), p.n_tiles, kBlock, s, p);
-    else if (masks) AM_LAUNCH_PDL(AM_SWEEP_KERNEL(false, true), p.n_tiles, kBlock, s, p);
-    else AM_LAUNCH_PDL(AM_SWEEP_KERNEL(false, false), p.n_tiles, kBlock, s, p);
-  } else {
-    // am_sweep_tick_shard: a plain launch.  (An early-launched sweep could park its CTAs on every SM ahead of the
-    // previous tick's exchange on the other stream; measured at two GPUs it made no difference
-    // to the step — so the simpler form stays.)
-    if (closed && masks) AM_LAUNCH(AM_SWEEP_KERNEL(true, true), p.n_tiles, kBlock, s, p);
-    else if (closed) AM_LAUNCH(AM_SWEEP_KERNEL(true, false), p.n_tiles, kBlock, s, p);
-    else if (masks) AM_LAUNCH(AM_SWEEP_KERNEL(false, true), p.n_tiles, kBlock, s, p);
-    else AM_LAUNCH(AM_SWEEP_KERNEL(false, false), p.n_tiles, kBlock, s, p);
   }
+  const SweepFn sweep = sweep_variant((mode & AM_SWEEP_CLOSED_LOOP) != 0, masks, window, h->hold, timeout);
+  // A single-stream tick's sweep launches early and hides behind its predecessor (the previous tick's publish, the
+  // drain).  am_sweep_tick_shard's is a plain launch: an early-launched sweep could park its CTAs on every SM ahead
+  // of the previous tick's exchange on the other stream; measured at two GPUs it made no difference to the step, so
+  // the simpler form stays.
+  if (o.expand) AM_LAUNCH_PDL(sweep, p.n_tiles, kBlock, s, p);
+  else AM_LAUNCH(sweep, p.n_tiles, kBlock, s, p);
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[1], s));
   ScanParams sc{};
   sc.group_count = ts.out.group_count;
@@ -751,67 +783,83 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   return AM_OK;
 }
 
-// mapped pinned memory for the list of a host tick: u32 indices, then u8 actions
-int reserve_host_out(am_sweep* h, uint64_t entries) {
-  if (entries <= h->host_out_entries) return AM_OK;
-  const uint64_t want = (entries + entries / 4 + 4095) / 4096 * 4096;
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  AM_CUDA(h, h->host_out.reserve(want * 5, cudaHostAllocMapped));
-  h->host_out_entries = want;
-  return AM_OK;
-}
-
-// A closed-loop record completes in the tick that submits it: nothing is ever in flight to hold.  Refused before
-// anything happens (nothing drained, P unchanged).
-int refuse_closed_hold(am_sweep* h, uint32_t mode) {
-  if (!h->hold || !(mode & AM_SWEEP_CLOSED_LOOP)) return AM_OK;
-  h->last_error = "AM_SWEEP_CLOSED_LOOP while the hold in flight is on";
-  return AM_E_INVAL;
-}
-
-// One host tick: drain, four kernels, one synchronisation; the list lands in h->host_out.
-int host_tick(am_sweep* h, int64_t unix_sec, uint32_t mode, am_tick_stats_t* stats) {
-  int rc = refuse_closed_hold(h, mode);
-  if (rc != AM_OK) return rc;
-  WindowPlan win;
-  rc = plan_window(h, unix_sec, mode, &win);
-  if (rc != AM_OK) return rc;
-  AM_CUDA(h, cudaSetDevice(h->device));
-  rc = order_on(h, h->stream);
-  if (rc != AM_OK) return rc;
-  rc = drain_staged(h, h->stream, &unix_sec, /*defer_clear=*/true);
-  struct ClearOnExit {  // whatever happens below, the marks are cleared before the handle is used again
-    am_sweep* h;
-    ~ClearOnExit() { (void)finish_deferred_clear(h, h->stream); }
-  } clear_on_exit{h};
-  if (rc != AM_OK) return rc;
-  rc = reserve_host_out(h, h->n_records);
-  if (rc != AM_OK) return rc;
-  ListOut o;
+// A host tick's list goes to mapped pinned memory (u32 indices, then u8 actions), its statistics to the mapped struct.
+int host_list_out(am_sweep* h, ListOut* o) {
+  const uint64_t entries = h->n_records;
+  if (entries > h->host_out_entries) {
+    const uint64_t want = (entries + entries / 4 + 4095) / 4096 * 4096;
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    AM_CUDA(h, h->host_out.reserve(want * 5, cudaHostAllocMapped));
+    h->host_out_entries = want;
+  }
   if (h->host_out_entries) {
     void* d = nullptr;
     AM_CUDA(h, cudaHostGetDevicePointer(&d, h->host_out.p, 0));
-    o.idx = d;
-    o.act = (uint8_t*)d + h->host_out_entries * 4;
-    o.cap = h->host_out_entries;
+    o->idx = d;
+    o->act = (uint8_t*)d + h->host_out_entries * 4;
+    o->cap = h->host_out_entries;
   }
-  o.stats = h->d_stats_mapped;
-  AM_CUDA(h, cudaEventRecord(h->ev0, h->stream));
-  rc = launch_tick(h, unix_sec, mode, o, h->stream, &win);
+  o->stats = h->d_stats_mapped;
+  return AM_OK;
+}
+
+// Which entry point a tick came through: a host tick (am_sweep_tick, am_sweep_tick_view) writes the list into
+// h->host_out and waits for it, a device tick writes it where the caller said, a shard tick leaves it to the exchange.
+enum class TickKind { kHost, kDevice, kShard };
+
+// One tick of the handle, with the tick guard held and T in range.  Refusals come before anything happens (nothing
+// drained, P unchanged): closed loop with the hold on (a closed-loop record completes in the tick that submits it, so
+// nothing is ever in flight to hold), then the catch-up plan.  P, the second of the previous tick, moves only when
+// the tick succeeds.
+int run_tick(am_sweep* h, int64_t T, uint32_t mode, cudaStream_t s, TickKind kind, ListOut o = {},
+             am_tick_stats_t* stats = nullptr) {
+  if (h->hold && (mode & AM_SWEEP_CLOSED_LOOP)) {
+    h->last_error = "AM_SWEEP_CLOSED_LOOP while the hold in flight is on";
+    return AM_E_INVAL;
+  }
+  WindowPlan win;
+  int rc = plan_window(h, T, mode, &win);
   if (rc != AM_OK) return rc;
-  AM_CUDA(h, cudaEventRecord(h->ev1, h->stream));
-  rc = finish_deferred_clear(h, h->stream);  // behind the event the host waits for
+  rc = set_stream(h, s);
   if (rc != AM_OK) return rc;
-  AM_CUDA(h, cudaEventSynchronize(h->ev1));
-  float ms = 0;
-  AM_CUDA(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
-  h->last_ms = ms;
-  am_tick_stats_t st = *h->h_stats;
-  st.n_records = h->n_records;
-  h->host_n = st.n_emitted;
+  const bool host = kind == TickKind::kHost;
+  rc = drain_staged(h, s, &T, /*defer_clear=*/host);
+  struct ClearOnExit {  // whatever happens below, the marks are cleared before the handle is used again
+    am_sweep* h;
+    cudaStream_t s;
+    ~ClearOnExit() { (void)finish_deferred_clear(h, s); }
+  } clear_on_exit{h, s};
+  if (rc != AM_OK) return rc;
+  if (kind == TickKind::kShard) {
+    if (h->n_records == 0) return AM_E_INVAL;  // an empty shard has nothing to exchange
+    o.expand = false;
+  }
+  if (host) {
+    rc = host_list_out(h, &o);
+    if (rc != AM_OK) return rc;
+    AM_CUDA(h, cudaEventRecord(h->ev0, s));
+  }
+  const int parity = (int)h->parity;
+  rc = launch_tick(h, T, mode, o, s, &win);
+  if (rc != AM_OK) return rc;
+  if (host) {  // one synchronisation
+    AM_CUDA(h, cudaEventRecord(h->ev1, s));
+    rc = finish_deferred_clear(h, s);  // behind the event the host waits for
+    if (rc != AM_OK) return rc;
+    AM_CUDA(h, cudaEventSynchronize(h->ev1));
+    float ms = 0;
+    AM_CUDA(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+    h->last_ms = ms;
+    am_tick_stats_t st = *h->h_stats;
+    st.n_records = h->n_records;
+    h->host_n = st.n_emitted;
+    if (stats) *stats = st;
+  } else if (kind == TickKind::kShard) {
+    h->last_shard_parity = parity;
+    h->set[parity].unpublished = true;
+  }
   h->has_prev = true;
-  h->prev_T = unix_sec;
-  if (stats) *stats = st;
+  h->prev_T = T;
   return AM_OK;
 }
 
@@ -892,56 +940,35 @@ int am_sweep_create(am_sweep_t** out, int device_id, uint64_t capacity, uint64_t
     AM_CUDA(h, cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, device_id));
     AM_CUDA(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     AM_CUDA(h, cudaStreamCreateWithFlags(&h->cstream, cudaStreamNonBlocking));
-    AM_CUDA(h, cudaEventCreateWithFlags(&h->ev_last, cudaEventDisableTiming));
-    AM_CUDA(h, cudaEventCreate(&h->ev0));
-    AM_CUDA(h, cudaEventCreate(&h->ev1));
-    for (int k = 0; k < 3; ++k) AM_CUDA(h, cudaEventCreate(&h->evp[k]));
-    for (int b = 0; b < 2; ++b) {
-      AM_CUDA(h, cudaEventCreateWithFlags(&h->stage[b].copied, cudaEventDisableTiming));
-      AM_CUDA(h, cudaEventCreateWithFlags(&h->stage[b].drained, cudaEventDisableTiming));
-      AM_CUDA(h, cudaEventCreateWithFlags(&h->set[b].consumed, cudaEventDisableTiming));
-    }
-    for (int k = 0; k < 16; ++k) {
-      void* p = nullptr;
-      AM_CUDA(h, cudaMalloc(&p, h->cap_padded * kColElem[k]));
-      AM_CUDA(h, cudaMemsetAsync(p, 0, h->cap_padded * kColElem[k], h->stream));
-      *col_slot(h->cols, k) = p;
-      h->col_ptr[k] = p;
-      h->col_elem[k] = kColElem[k];
-    }
+    for (cudaEvent_t* e : {&h->ev_last, &h->stage[0].copied, &h->stage[0].drained, &h->stage[1].copied,
+                           &h->stage[1].drained, &h->set[0].consumed, &h->set[1].consumed})
+      AM_CUDA(h, new_event(h, e));
+    for (cudaEvent_t* e : {&h->ev0, &h->ev1, &h->evp[0], &h->evp[1], &h->evp[2]}) AM_CUDA(h, new_event(h, e, true));
+    for (int k = 0; k < 16; ++k) AM_CUDA(h, dev_array(h, col_slot(h->cols, k), h->cap_padded * kColElem[k], h->stream));
     AM_LAUNCH(fill_u32_kernel, h->sms * 8, 256, h->stream, h->cols.flags, AM_F_TOMBSTONE, h->cap_padded);
     h->launches++;
     // the mask planes: every slot is a tombstone, no record has a plane bit
     h->planes.words = h->cap_padded / 32;
-    AM_CUDA(h, cudaMalloc((void**)&h->planes.w, kPlanes * h->planes.words * 4));
-    AM_CUDA(h, cudaMemsetAsync(h->planes.w, 0, kPlanes * h->planes.words * 4, h->stream));
-    AM_CUDA(h, cudaMalloc((void**)&h->seg_dirty, h->cap_padded / kRecPerWarp * 4));
-    AM_CUDA(h, cudaMemsetAsync(h->seg_dirty, 0, h->cap_padded / kRecPerWarp * 4, h->stream));
+    AM_CUDA(h, dev_array(h, &h->planes.w, kPlanes * h->planes.words * 4, h->stream));
+    AM_CUDA(h, dev_array(h, &h->seg_dirty, h->cap_padded / kRecPerWarp * 4, h->stream));
     const size_t ntiles = h->cap_padded / kTile;
     const size_t ngroups = (ntiles + kGroupTiles - 1) / kGroupTiles;
-    for (int b = 0; b < 2; ++b) {
-      TickOut& t = h->set[b].out;
+    for (TickSet& ts : h->set) {
+      TickOut& t = ts.out;
       // bitmap words past the last tile of the last group are never written: they stay zero
-      AM_CUDA(h, cudaMalloc((void**)&t.bitmap, ngroups * kGroupWords * 4));
-      AM_CUDA(h, cudaMemsetAsync(t.bitmap, 0, ngroups * kGroupWords * 4, h->stream));
-      AM_CUDA(h, cudaMalloc((void**)&t.group_count, ngroups * 4));
-      AM_CUDA(h, cudaMemsetAsync(t.group_count, 0, ngroups * 4, h->stream));
-      AM_CUDA(h, cudaMalloc((void**)&t.group_prefix, (ngroups + 1) * 4));
-      AM_CUDA(h, cudaMemsetAsync(t.group_prefix, 0, (ngroups + 1) * 4, h->stream));
-      AM_CUDA(h, cudaMalloc((void**)&t.tile_exc, ntiles * 4));
-      AM_CUDA(h, cudaMemsetAsync(t.tile_exc, 0, ntiles * 4, h->stream));
-      AM_CUDA(h, cudaMalloc((void**)&t.exc_seg, h->cap_padded * 4));
-      AM_CUDA(h, cudaMemsetAsync(t.exc_seg, 0, h->cap_padded * 4, h->stream));  // expand_kernel prefetches past the counts
-      AM_CUDA(h, cudaMalloc((void**)&h->set[b].acc, kNumAcc * 8));
-      AM_CUDA(h, cudaMemsetAsync(h->set[b].acc, 0, kNumAcc * 8, h->stream));
+      AM_CUDA(h, dev_array(h, &t.bitmap, ngroups * kGroupWords * 4, h->stream));
+      AM_CUDA(h, dev_array(h, &t.group_count, ngroups * 4, h->stream));
+      AM_CUDA(h, dev_array(h, &t.group_prefix, (ngroups + 1) * 4, h->stream));
+      AM_CUDA(h, dev_array(h, &t.tile_exc, ntiles * 4, h->stream));
+      AM_CUDA(h, dev_array(h, &t.exc_seg, h->cap_padded * 4, h->stream));  // expand_kernel prefetches past the counts
+      AM_CUDA(h, dev_array(h, &ts.acc, kNumAcc * 8, h->stream));
     }
-    AM_CUDA(h, cudaMalloc((void**)&h->marks, h->cap_padded * 12));
-    AM_CUDA(h, cudaMemsetAsync(h->marks, 0, h->cap_padded * 12, h->stream));
+    AM_CUDA(h, dev_array(h, &h->marks, h->cap_padded * 12, h->stream));
     for (int b = 0; b < 2; ++b) {
-      AM_CUDA(h, cudaMalloc((void**)&h->due_idx[b], h->cap_padded * 4));
-      AM_CUDA(h, cudaMalloc((void**)&h->due_action[b], h->cap_padded));
+      AM_CUDA(h, dev_array(h, &h->due_idx[b], h->cap_padded * 4, h->stream, false));
+      AM_CUDA(h, dev_array(h, &h->due_action[b], h->cap_padded, h->stream, false));
     }
-    AM_CUDA(h, cudaHostAlloc((void**)&h->h_stats, sizeof(am_tick_stats_t), cudaHostAllocMapped));
+    AM_CUDA(h, host_array(h, &h->h_stats, sizeof(am_tick_stats_t), cudaHostAllocMapped));
     memset(h->h_stats, 0, sizeof(am_tick_stats_t));
     AM_CUDA(h, cudaHostGetDevicePointer((void**)&h->d_stats_mapped, h->h_stats, 0));
     AM_CUDA(h, cudaGetLastError());
@@ -961,42 +988,17 @@ void am_sweep_destroy(am_sweep_t* h) {
   if (!h) return;
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();  // ticks may have been issued on caller streams
-  for (int k = 0; k < 16; ++k) if (h->col_ptr[k]) cudaFree(h->col_ptr[k]);
-  if (h->planes.w) cudaFree(h->planes.w);
-  if (h->seg_dirty) cudaFree(h->seg_dirty);
-  for (int b = 0; b < 2; ++b) {
-    TickOut& t = h->set[b].out;
-    if (t.bitmap) cudaFree(t.bitmap);
-    if (t.group_count) cudaFree(t.group_count);
-    if (t.group_prefix) cudaFree(t.group_prefix);
-    if (t.tile_exc) cudaFree(t.tile_exc);
-    if (t.exc_seg) cudaFree(t.exc_seg);
-    if (h->set[b].acc) cudaFree(h->set[b].acc);
-    if (h->set[b].consumed) cudaEventDestroy(h->set[b].consumed);
-    if (h->due_idx[b]) cudaFree(h->due_idx[b]);
-    if (h->due_action[b]) cudaFree(h->due_action[b]);
-    Staging& st = h->stage[b];
+  for (const Owned& o : h->owned) {
+    if (o.kind == Owned::kDevice) cudaFree(o.p);
+    else if (o.kind == Owned::kPinned) cudaFreeHost(o.p);
+    else cudaEventDestroy((cudaEvent_t)o.p);
+  }
+  for (Staging& st : h->stage) {
     st.ops.release(); st.recs.release();
     st.d_ops.release(); st.d_recs.release();
-    if (st.copied) cudaEventDestroy(st.copied);
-    if (st.drained) cudaEventDestroy(st.drained);
   }
-  if (h->marks) cudaFree(h->marks);
-  if (h->since) cudaFree(h->since);
-  for (void* p : {(void*)h->wf_timeout, (void*)h->deadline, (void*)h->seg_deadline, (void*)h->to_idx, (void*)h->to_since,
-                  (void*)h->to_count})
-    if (p) cudaFree(p);
-  if (h->h_stats) cudaFreeHost(h->h_stats);
   h->host_out.release();
   h->pin_in.release(); h->dev_in.release();
-  h->tz_off.release(); h->tz_table.release(); h->tz_pin.release();
-  if (h->tz_copied) cudaEventDestroy(h->tz_copied);
-  h->win_boxes.release(); h->win_pin.release();
-  if (h->win_copied) cudaEventDestroy(h->win_copied);
-  if (h->ev_last) cudaEventDestroy(h->ev_last);
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
-  for (int k = 0; k < 3; ++k) if (h->evp[k]) cudaEventDestroy(h->evp[k]);
   if (h->stream) cudaStreamDestroy(h->stream);
   if (h->cstream) cudaStreamDestroy(h->cstream);
   delete h;
@@ -1008,7 +1010,7 @@ int am_sweep_device(const am_sweep_t* h) { return h ? h->device : -1; }
 double am_sweep_last_kernel_ms(const am_sweep_t* h) { return h ? h->last_ms : -1.0; }
 uint64_t am_sweep_launch_count(const am_sweep_t* h) { return h ? h->launches : 0; }
 void* am_sweep_column_ptr(am_sweep_t* h, int column) {
-  return (h && column >= 0 && column < 16) ? h->col_ptr[column] : nullptr;
+  return (h && column >= 0 && column < 16) ? *col_slot(h->cols, column) : nullptr;
 }
 int am_sweep_set_profiling(am_sweep_t* h, int on) {
   if (!h) return AM_E_INVAL;
@@ -1040,16 +1042,13 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
   if (cols->flags && amsweep_host::unknown_zones(n, cols->flags, 1, (uint32_t)amsweep_tz::count())) return AM_E_INVAL;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  AM_CUDA(h, cudaSetDevice(h->device));
-  int rc = order_on(h, h->stream);
-  if (rc != AM_OK) return rc;
   // a load is a call in the per-slot order: upserts, removes and results staged before it are applied first, so
   // the load overwrites them (a result is left pending in the flags, which the load replaces; a posted workflow
   // phase has released its slot's hold in this drain all the same)
-  rc = drain_staged(h, h->stream);
+  int rc = begin_call(h);
   if (rc != AM_OK) return rc;
   for (int k = 0; k < 16; ++k) {
-    char* dst = (char*)h->col_ptr[k] + first * kColElem[k];
+    char* dst = (char*)*col_slot(h->cols, k) + first * kColElem[k];
     const void* src = *cols_member(cols, k);
     if (src) AM_CUDA(h, cudaMemcpyAsync(dst, src, n * kColElem[k], cudaMemcpyHostToDevice, h->stream));
     else AM_CUDA(h, cudaMemsetAsync(dst, 0, n * kColElem[k], h->stream));
@@ -1083,10 +1082,9 @@ int am_sweep_set_hold_in_flight(am_sweep_t* h, int on) {
   if (!g.ok) return AM_E_BUSY;
   if ((on != 0) == h->hold) return AM_OK;
   if (on) {  // starts with nothing in flight
-    AM_CUDA(h, cudaSetDevice(h->device));
-    int rc = order_on(h, h->stream);
+    int rc = set_stream(h, h->stream);
     if (rc != AM_OK) return rc;
-    if (!h->since) AM_CUDA(h, cudaMalloc((void**)&h->since, h->cap_padded * sizeof(int64_t)));
+    if (!h->since) AM_CUDA(h, dev_array(h, &h->since, h->cap_padded * sizeof(int64_t), h->stream, false));
     AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, h->stream, h->since, kNotInFlight, h->cap_padded);
     h->launches++;
     AM_CUDA(h, cudaGetLastError());
@@ -1213,10 +1211,10 @@ int am_sweep_post_result(am_sweep_t* h, uint64_t n, const uint64_t* idx, const u
 int am_sweep_tick(am_sweep_t* h, int64_t unix_sec, uint32_t mode, uint64_t* due_idx,
                   uint32_t* due_action, uint64_t cap, uint64_t* n_out, am_tick_stats_t* stats) {
   if (!h || (cap && (!due_idx || !due_action))) return AM_E_INVAL;
-  if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
+  if (!time_ok(unix_sec)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  int rc = host_tick(h, unix_sec, mode, stats);
+  int rc = run_tick(h, unix_sec, mode, h->stream, TickKind::kHost, {}, stats);
   if (rc != AM_OK) return rc;
   const uint64_t n = h->host_n;
   if (n_out) *n_out = n;
@@ -1230,10 +1228,10 @@ int am_sweep_tick(am_sweep_t* h, int64_t unix_sec, uint32_t mode, uint64_t* due_
 int am_sweep_tick_view(am_sweep_t* h, int64_t unix_sec, uint32_t mode, am_tick_view_t* view,
                        am_tick_stats_t* stats) {
   if (!h || !view) return AM_E_INVAL;
-  if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
+  if (!time_ok(unix_sec)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  int rc = host_tick(h, unix_sec, mode, stats);
+  int rc = run_tick(h, unix_sec, mode, h->stream, TickKind::kHost, {}, stats);
   if (rc != AM_OK) return rc;
   view->idx_local = (const uint32_t*)h->host_out.p;
   view->action = h->host_out.p ? (const uint8_t*)h->host_out.p + h->host_out_entries * 4 : nullptr;
@@ -1261,7 +1259,7 @@ int am_sweep_tick_device(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* d
                          void* d_due_action, uint64_t cap, void* d_count, void* d_stats,
                          void* cuda_stream) {
   if (!h || (cap && (!d_due_idx || !d_due_action))) return AM_E_INVAL;
-  if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
+  if (!time_ok(unix_sec)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
   // expand_kernel stores 16-B quads of indices and 4-B words of actions, scan_groups_kernel a u32 count and
@@ -1272,56 +1270,16 @@ int am_sweep_tick_device(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* d
     h->last_error = "am_sweep_tick_device: d_due_idx must be 16-B aligned, d_due_action and d_count 4-B, d_stats 8-B";
     return AM_E_INVAL;
   }
-  int rc = refuse_closed_hold(h, mode);
-  if (rc != AM_OK) return rc;
-  WindowPlan win;
-  rc = plan_window(h, unix_sec, mode, &win);
-  if (rc != AM_OK) return rc;
-  AM_CUDA(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)cuda_stream;  // NULL == CUDA default stream
-  rc = order_on(h, s);
-  if (rc != AM_OK) return rc;
-  rc = drain_staged(h, s, &unix_sec);
-  if (rc != AM_OK) return rc;
-  ListOut o;
-  o.idx = d_due_idx;
-  o.act = (uint8_t*)d_due_action;
-  o.cap = cap;
-  o.count = (uint32_t*)d_count;
-  o.stats = (am_tick_stats_t*)d_stats;
-  rc = launch_tick(h, unix_sec, mode, o, s, &win);
-  if (rc == AM_OK) { h->has_prev = true; h->prev_T = unix_sec; }
-  return rc;
+  const ListOut o{d_due_idx, (uint8_t*)d_due_action, cap, (uint32_t*)d_count, (am_tick_stats_t*)d_stats};
+  return run_tick(h, unix_sec, mode, (cudaStream_t)cuda_stream, TickKind::kDevice, o);  // NULL == CUDA default stream
 }
 
 int am_sweep_tick_shard(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* cuda_stream) {
   if (!h) return AM_E_INVAL;
-  if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
+  if (!time_ok(unix_sec)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  int rc = refuse_closed_hold(h, mode);
-  if (rc != AM_OK) return rc;
-  WindowPlan win;
-  rc = plan_window(h, unix_sec, mode, &win);
-  if (rc != AM_OK) return rc;
-  AM_CUDA(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)cuda_stream;
-  rc = order_on(h, s);
-  if (rc != AM_OK) return rc;
-  rc = drain_staged(h, s, &unix_sec);
-  if (rc != AM_OK) return rc;
-  if (h->n_records == 0) return AM_E_INVAL;  // an empty shard has nothing to exchange
-  ListOut o;
-  o.expand = false;
-  const int parity = (int)h->parity;
-  rc = launch_tick(h, unix_sec, mode, o, s, &win);
-  if (rc == AM_OK) {
-    h->last_shard_parity = parity;
-    h->set[parity].unpublished = true;
-    h->has_prev = true;
-    h->prev_T = unix_sec;
-  }
-  return rc;
+  return run_tick(h, unix_sec, mode, (cudaStream_t)cuda_stream, TickKind::kShard);
 }
 
 int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint32_t mode,
@@ -1329,15 +1287,14 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
   if (!h || !stats_out || (mode & AM_SWEEP_CATCH_UP)) return AM_E_INVAL;
   if (n_ticks == 0) return AM_OK;
   if (n_ticks > (1ull << 24)) return AM_E_INVAL;
-  if (unix_sec0 >= (1ll << 55) - (int64_t)n_ticks || unix_sec0 <= -(1ll << 55)) return AM_E_RANGE;
+  if (!time_ok(unix_sec0) || !time_ok(unix_sec0 + (int64_t)n_ticks)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
   if (h->hold) {  // (neither the blocked kernel nor the run's plain ticks keep the hold: refused, nothing happens)
     h->last_error = "am_sweep_run_ticks while the hold in flight is on";
     return AM_E_INVAL;
   }
-  AM_CUDA(h, cudaSetDevice(h->device));
-  int rc = order_on(h, h->stream);
+  int rc = set_stream(h, h->stream);
   if (rc != AM_OK) return rc;
   h->to_ran = false;  // (ticks: the timed-out list is reset; with the hold off nothing times out)
   // A blocked run publishes no tick's accumulators: its drain leaves posted results pending in the flags,
@@ -1377,7 +1334,7 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
     b.seed = h->seed;
     b.T0 = T;
     b.K = (uint32_t)K;
-    b.tz_off = h->tz_n > 1 ? (const int32_t*)h->tz_off.p : nullptr;
+    b.tz_off = h->tz_n > 1 ? (const int32_t*)h->tz_off.dev : nullptr;
     b.stats = reinterpret_cast<unsigned long long*>(d_stats + k);
     const unsigned grid = (unsigned)((h->n_records + kBlockRecords - 1) / kBlockRecords);
     if (mode & AM_SWEEP_CLOSED_LOOP) AM_LAUNCH(sweep_block_kernel<true>, grid, kBlockThreads, h->stream, b);
@@ -1387,11 +1344,7 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
     k += K;
   }
   for (uint64_t k = 0; !blocked && k < n_ticks && rc == AM_OK; ++k) {
-    ListOut o;
-    o.idx = h->due_idx[k & 1];
-    o.act = h->due_action[k & 1];
-    o.cap = h->cap_padded;
-    o.stats = d_stats + k;
+    const ListOut o{h->due_idx[k & 1], h->due_action[k & 1], h->cap_padded, nullptr, d_stats + k};
     rc = launch_tick(h, unix_sec0 + (int64_t)k, mode, o, h->stream);
   }
   if (rc == AM_OK) {
@@ -1415,14 +1368,11 @@ static int read_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* 
 int am_sweep_repeat_after_sec(am_sweep_t* h, int64_t unix_sec, uint64_t first, uint64_t n, int64_t* out) {
   if (!h || (n && !out)) return AM_E_INVAL;
   if (first + n > h->capacity || first + n < first || n > 0xFFFFFFFFull) return AM_E_INVAL;
-  if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
+  if (!time_ok(unix_sec)) return AM_E_RANGE;
   if (n == 0) return AM_OK;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  AM_CUDA(h, cudaSetDevice(h->device));
-  int rc = order_on(h, h->stream);
-  if (rc != AM_OK) return rc;
-  rc = drain_staged(h, h->stream);
+  int rc = begin_call(h);
   if (rc != AM_OK) return rc;
   AM_CUDA(h, h->dev_in.reserve(n * 8));
   AM_CUDA(h, h->pin_in.reserve(n * 8));
@@ -1454,13 +1404,10 @@ int am_sweep_repeat_after_sec(am_sweep_t* h, int64_t unix_sec, uint64_t first, u
 
 int am_sweep_next_due(am_sweep_t* h, int64_t unix_sec, int64_t* next_out) {
   if (!h || !next_out) return AM_E_INVAL;
-  if (unix_sec >= (1ll << 55) || unix_sec <= -(1ll << 55)) return AM_E_RANGE;
+  if (!time_ok(unix_sec)) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  AM_CUDA(h, cudaSetDevice(h->device));
-  int rc = order_on(h, h->stream);
-  if (rc != AM_OK) return rc;
-  rc = drain_staged(h, h->stream);
+  int rc = begin_call(h);
   if (rc != AM_OK) return rc;
   *next_out = INT64_MAX;  // nothing will ever be due (empty shard, only tombstones / exhausted schedules)
   if (h->n_records == 0) return AM_OK;
@@ -1486,22 +1433,14 @@ int am_sweep_next_due(am_sweep_t* h, int64_t unix_sec, int64_t* next_out) {
   return AM_OK;
 }
 
-static int read_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, am_record_cols_t* out);
-
 int am_sweep_read(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx,
                   am_record_cols_t* out) {
   if (!h || !out) return AM_E_INVAL;
   if (n == 0) return AM_OK;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  AM_CUDA(h, cudaSetDevice(h->device));
-  {  // a read observes every upsert / remove / result staged before it
-    int rc = order_on(h, h->stream);
-    if (rc != AM_OK) return rc;
-    rc = drain_staged(h, h->stream);
-    if (rc != AM_OK) return rc;
-  }
-  return read_impl(h, first, n, idx, out);
+  const int rc = begin_call(h);  // a read observes every upsert / remove / result staged before it
+  return rc != AM_OK ? rc : read_impl(h, first, n, idx, out);
 }
 
 int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
@@ -1513,31 +1452,20 @@ int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t
       if (idx[k] >= h->capacity) return AM_E_RANGE;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  AM_CUDA(h, cudaSetDevice(h->device));
-  int rc = order_on(h, h->stream);
-  if (rc != AM_OK) return rc;
-  rc = drain_staged(h, h->stream);  // results posted by now release their holds (left pending for the next tick)
+  int rc = begin_call(h);  // results posted by now release their holds (left pending for the next tick)
   if (rc != AM_OK) return rc;
   if (!h->hold) {
     for (uint64_t k = 0; k < n; ++k) since_out[k] = kNotInFlight;
     return AM_OK;
   }
-  const size_t o_idx = n * 8, total = o_idx + (idx ? n * 4 : 0);
-  AM_CUDA(h, h->pin_in.reserve(total));
-  AM_CUDA(h, h->dev_in.reserve(total));
-  char* dp = (char*)h->dev_in.p;
-  const uint32_t* d_idx = nullptr;
-  if (idx) {
-    uint32_t* hidx = (uint32_t*)((char*)h->pin_in.p + o_idx);
-    for (uint64_t k = 0; k < n; ++k) hidx[k] = (uint32_t)idx[k];
-    AM_CUDA(h, cudaMemcpyAsync(dp + o_idx, hidx, n * 4, cudaMemcpyHostToDevice, h->stream));
-    d_idx = (const uint32_t*)(dp + o_idx);
-  }
+  const uint32_t* d_idx;
+  rc = stage_indices(h, n * 8, n, idx, &d_idx);
+  if (rc != AM_OK) return rc;
   AM_LAUNCH(in_flight_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols, (const int64_t*)h->since, (uint32_t)first,
-            d_idx, (uint32_t)n, (int64_t*)dp);
+            d_idx, (uint32_t)n, (int64_t*)h->dev_in.p);
   h->launches++;
   AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, dp, n * 8, cudaMemcpyDeviceToHost, h->stream));
+  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * 8, cudaMemcpyDeviceToHost, h->stream));
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   memcpy(since_out, h->pin_in.p, n * 8);
   return AM_OK;
@@ -1548,8 +1476,7 @@ int am_sweep_last_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
   if (h->to_ran && !h->to_fetched) {  // the device list of the last tick, waited for (it may be on a caller stream)
-    AM_CUDA(h, cudaSetDevice(h->device));
-    int rc = order_on(h, h->stream);
+    const int rc = set_stream(h, h->stream);
     if (rc != AM_OK) return rc;
     AM_CUDA(h, h->pin_in.reserve(4));
     AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->to_count, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1584,7 +1511,7 @@ static int read_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* 
     for (int k = 0; k < 16; ++k) {
       void* dst = *cols_member(out, k);
       if (!dst) continue;
-      AM_CUDA(h, cudaMemcpyAsync(dst, (char*)h->col_ptr[k] + first * kColElem[k], n * kColElem[k],
+      AM_CUDA(h, cudaMemcpyAsync(dst, (char*)*col_slot(h->cols, k) + first * kColElem[k], n * kColElem[k],
                                  cudaMemcpyDeviceToHost, h->stream));
     }
     AM_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -1593,18 +1520,14 @@ static int read_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* 
   if (n > 0xFFFFFFFFull) return AM_E_INVAL;
   for (uint64_t k = 0; k < n; ++k)
     if (idx[k] >= h->capacity) return AM_E_RANGE;
-  const size_t o_idx = n * sizeof(am_record_t), total = o_idx + n * 4;
-  AM_CUDA(h, h->pin_in.reserve(total));
-  AM_CUDA(h, h->dev_in.reserve(total));
-  uint32_t* hidx = (uint32_t*)((char*)h->pin_in.p + o_idx);
-  for (uint64_t k = 0; k < n; ++k) hidx[k] = (uint32_t)idx[k];
-  char* dp = (char*)h->dev_in.p;
-  AM_CUDA(h, cudaMemcpyAsync(dp + o_idx, hidx, n * 4, cudaMemcpyHostToDevice, h->stream));
-  AM_LAUNCH(gather_records_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols,
-            (const uint32_t*)(dp + o_idx), (am_record_t*)dp, (uint32_t)n);
+  const uint32_t* d_idx;
+  const int rc = stage_indices(h, n * sizeof(am_record_t), n, idx, &d_idx);
+  if (rc != AM_OK) return rc;
+  AM_LAUNCH(gather_records_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols, d_idx, (am_record_t*)h->dev_in.p,
+            (uint32_t)n);
   h->launches++;
   AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, dp, n * sizeof(am_record_t), cudaMemcpyDeviceToHost, h->stream));
+  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * sizeof(am_record_t), cudaMemcpyDeviceToHost, h->stream));
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   const am_record_t* r = (const am_record_t*)h->pin_in.p;
   for (uint64_t k = 0; k < n; ++k) {

@@ -38,10 +38,6 @@
 #define AM_LAUNCH_PDL(kernel, grid, block, stream, ...) ((void)(stream), emu::launch(kernel, dim3(grid), dim3(block), __VA_ARGS__))
 #endif
 #endif
-#define AM_SWEEP_KERNEL(closed, masks) sweep_tick_kernel<closed, masks>  // one macro argument
-#define AM_SWEEP_WINDOW_KERNEL(closed) sweep_tick_kernel<closed, false, true>  // catch-up ticks
-#define AM_SWEEP_HOLD_KERNEL(masks, window) sweep_tick_kernel<false, masks, window, true>  // hold in flight (open loop)
-#define AM_SWEEP_TIMEOUT_KERNEL(masks, window) sweep_tick_kernel<false, masks, window, true, true>  // ... + workflow timeouts
 
 namespace amsweep {
 
