@@ -186,6 +186,9 @@ struct am_sweep {
   // workflow, kNotInFlight when none ([cap_padded], allocated when the hold is first turned on)
   bool hold = false;
   int64_t* since = nullptr;
+  // remedy hold (am_sweep_set_hold_remedy, only with the hold): a running remedy workflow is kept in the same since and
+  // deadline words, its since as T + kRemedyRun
+  bool remedy = false;
   // workflow timeouts (am_record_t.wf_timeout), allocated by the first drain that stages a non-zero one: per slot the
   // latest upsert's timeout and the running workflow's deadline, per warp segment a lower bound of its deadlines, and
   // the tick's timed-out list (room for every slot)
@@ -196,8 +199,9 @@ struct am_sweep {
   int64_t* to_since = nullptr;
   uint32_t* to_count = nullptr;
   bool to_ran = false;      // the last tick ran expire_runs_kernel: its list is on the device
-  bool to_fetched = false;  // ... and has been copied to to_host, sorted
-  std::vector<std::pair<uint32_t, int64_t>> to_host;
+  bool to_fetched = false;  // ... and has been copied to to_host / rto_host, sorted
+  std::vector<std::pair<uint32_t, int64_t>> to_host;   // health-check runs: (slot, since)
+  std::vector<std::pair<uint32_t, int64_t>> rto_host;  // remedy runs: (slot, start)
   std::string last_error;
   uint64_t launches = 0;
   double last_ms = -1.0;
@@ -529,7 +533,12 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   if (tick_T && st->n_result && h->early_results && (uint64_t)st->n_result * 8 <= h->n_records) {
     TickSet& ts = h->set[h->parity];  // the buffer set of the tick being prepared
     if (int rc = claim_set(h, ts, s)) return rc;
-    AM_LAUNCH_PDL(apply_results_now_kernel, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc);
+    if (h->remedy)  // (remedy runs start here; the deadline words exist with the timeout state)
+      AM_LAUNCH_PDL(apply_results_now_kernel<true>, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc, h->since,
+                    h->deadline, (const int32_t*)h->wf_timeout, h->seg_deadline);
+    else
+      AM_LAUNCH_PDL(apply_results_now_kernel<false>, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc,
+                    (int64_t*)nullptr, (int64_t*)nullptr, (const int32_t*)nullptr, (unsigned long long*)nullptr);
     h->launches++;
   } else if (st->n_result) {
     AM_LAUNCH_PDL(apply_result_ops_kernel, G, B, s, h->cols.flags, h->marks, d_ops, (uint32_t)n);
@@ -658,13 +667,13 @@ int plan_window(am_sweep* h, int64_t T, uint32_t mode, WindowPlan* w) {
 }
 
 // The sweep variant of a tick: a row per loop mode, a column per way the masks are read (not at all, the planes of
-// T's minute, the canonical masks against a catch-up window's boxes).  These are the 12 instantiations of
+// T's minute, the canonical masks against a catch-up window's boxes).  These are the 18 instantiations of
 // sweep_tick_kernel there are.  Two combinations have none and never get here: closed loop with the hold on (refused
 // before the drain, and run_ticks refuses the hold) and a window with the planes (launch_tick sets `masks` only
 // without a window).
 using SweepFn = void (*)(const SweepParams);
-SweepFn sweep_variant(bool closed, bool masks, bool window, bool hold, bool timeout) {
-  static constexpr SweepFn kVariants[4][3] = {
+SweepFn sweep_variant(bool closed, bool masks, bool window, bool hold, bool timeout, bool remedy) {
+  static constexpr SweepFn kVariants[6][3] = {
       // open loop
       {sweep_tick_kernel<false, false>, sweep_tick_kernel<false, true>, sweep_tick_kernel<false, false, true>},
       // closed loop
@@ -674,8 +683,14 @@ SweepFn sweep_variant(bool closed, bool masks, bool window, bool hold, bool time
        sweep_tick_kernel<false, false, true, true>},
       // ... and workflow timeouts
       {sweep_tick_kernel<false, false, false, true, true>, sweep_tick_kernel<false, true, false, true, true>,
-       sweep_tick_kernel<false, false, true, true, true>}};
-  return kVariants[hold ? 2 + timeout : closed][window ? 2 : masks];
+       sweep_tick_kernel<false, false, true, true, true>},
+      // hold in flight with the remedy hold
+      {sweep_tick_kernel<false, false, false, true, false, true>, sweep_tick_kernel<false, true, false, true, false, true>,
+       sweep_tick_kernel<false, false, true, true, false, true>},
+      // ... and workflow timeouts
+      {sweep_tick_kernel<false, false, false, true, true, true>, sweep_tick_kernel<false, true, false, true, true, true>,
+       sweep_tick_kernel<false, false, true, true, true, true>}};
+  return kVariants[hold ? 2 + timeout + 2 * remedy : closed][window ? 2 : masks];
 }
 
 int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStream_t s, const WindowPlan* win = nullptr) {
@@ -739,7 +754,7 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
     p.deadline = h->deadline;
     p.seg_deadline = h->seg_deadline;
   }
-  const SweepFn sweep = sweep_variant((mode & AM_SWEEP_CLOSED_LOOP) != 0, masks, window, h->hold, timeout);
+  const SweepFn sweep = sweep_variant((mode & AM_SWEEP_CLOSED_LOOP) != 0, masks, window, h->hold, timeout, h->remedy);
   // A single-stream tick's sweep launches early and hides behind its predecessor (the previous tick's publish, the
   // drain).  am_sweep_tick_shard's is a plain launch: an early-launched sweep could park its CTAs on every SM ahead
   // of the previous tick's exchange on the other stream; measured at two GPUs it made no difference to the step, so
@@ -1094,6 +1109,27 @@ int am_sweep_set_hold_in_flight(am_sweep_t* h, int on) {
     }
   }
   h->hold = on != 0;
+  if (!on) h->remedy = false;  // (the since words are refilled when the hold is turned on again)
+  return AM_OK;
+}
+
+int am_sweep_set_hold_remedy(am_sweep_t* h, int on) {
+  if (!h) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if (!h->hold) {
+    h->last_error = "am_sweep_set_hold_remedy while the hold in flight is off";
+    return AM_E_INVAL;
+  }
+  if ((on != 0) == h->remedy) return AM_OK;
+  if (!on) {  // every remedy run ends (the segment bounds stay lower bounds)
+    int rc = set_stream(h, h->stream);
+    if (rc != AM_OK) return rc;
+    AM_LAUNCH(release_remedy_runs_kernel, h->sms * 8, 256, h->stream, h->since, h->deadline, h->cap_padded);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
+  }
+  h->remedy = on != 0;
   return AM_OK;
 }
 
@@ -1443,7 +1479,7 @@ int am_sweep_read(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx
   return rc != AM_OK ? rc : read_impl(h, first, n, idx, out);
 }
 
-int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
+static int in_flight_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out, bool remedy) {
   if (!h || (n && !since_out)) return AM_E_INVAL;
   if (n == 0) return AM_OK;
   if (n > 0xFFFFFFFFull || (!idx && (first + n > h->capacity || first + n < first))) return AM_E_INVAL;
@@ -1454,7 +1490,7 @@ int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t
   if (!g.ok) return AM_E_BUSY;
   int rc = begin_call(h);  // results posted by now release their holds (left pending for the next tick)
   if (rc != AM_OK) return rc;
-  if (!h->hold) {
+  if (!h->hold || (remedy && !h->remedy)) {
     for (uint64_t k = 0; k < n; ++k) since_out[k] = kNotInFlight;
     return AM_OK;
   }
@@ -1462,7 +1498,7 @@ int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t
   rc = stage_indices(h, n * 8, n, idx, &d_idx);
   if (rc != AM_OK) return rc;
   AM_LAUNCH(in_flight_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols, (const int64_t*)h->since, (uint32_t)first,
-            d_idx, (uint32_t)n, (int64_t*)h->dev_in.p);
+            d_idx, (uint32_t)n, (int64_t*)h->dev_in.p, remedy);
   h->launches++;
   AM_CUDA(h, cudaGetLastError());
   AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * 8, cudaMemcpyDeviceToHost, h->stream));
@@ -1471,7 +1507,18 @@ int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t
   return AM_OK;
 }
 
-int am_sweep_last_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t* since, uint64_t cap, uint64_t* n_out) {
+int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
+  return in_flight_impl(h, first, n, idx, since_out, false);
+}
+
+int am_sweep_remedy_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* started_out) {
+  return in_flight_impl(h, first, n, idx, started_out, true);
+}
+
+// One of the last tick's two timed-out lists, entries [offset, ...) as global indices: the health-check runs, or the
+// remedy runs with their start.
+static int timed_out_impl(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t* since, uint64_t cap, uint64_t* n_out,
+                          bool remedy) {
   if (!h || (cap && (!idx || !since))) return AM_E_INVAL;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
@@ -1488,20 +1535,35 @@ int am_sweep_last_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64
       AM_CUDA(h, cudaMemcpy(li.data(), h->to_idx, m * 4ull, cudaMemcpyDeviceToHost));
       AM_CUDA(h, cudaMemcpy(ls.data(), h->to_since, m * 8ull, cudaMemcpyDeviceToHost));
     }
-    h->to_host.resize(m);
-    for (uint32_t k = 0; k < m; ++k) h->to_host[k] = {li[k], ls[k]};
+    h->to_host.clear();
+    h->rto_host.clear();
+    for (uint32_t k = 0; k < m; ++k) {  // a remedy run's since word is its start + kRemedyRun
+      if (ls[k] >= kRemedyRun / 2) h->rto_host.push_back({li[k], ls[k] - kRemedyRun});
+      else h->to_host.push_back({li[k], ls[k]});
+    }
     std::sort(h->to_host.begin(), h->to_host.end());  // (appended one segment at a time, in no particular order)
+    std::sort(h->rto_host.begin(), h->rto_host.end());
     h->to_fetched = true;
   }
-  const uint64_t n = h->to_ran ? h->to_host.size() : 0;
+  const std::vector<std::pair<uint32_t, int64_t>>& list = remedy ? h->rto_host : h->to_host;
+  const uint64_t n = h->to_ran ? list.size() : 0;
   if (offset > n) return AM_E_RANGE;
   const uint64_t left = n - offset, ncopy = left < cap ? left : cap;
   if (n_out) *n_out = left;
   for (uint64_t k = 0; k < ncopy; ++k) {
-    idx[k] = h->shard_base + h->to_host[offset + k].first;
-    since[k] = h->to_host[offset + k].second;
+    idx[k] = h->shard_base + list[offset + k].first;
+    since[k] = list[offset + k].second;
   }
   return left > cap ? AM_E_NOSPACE : AM_OK;
+}
+
+int am_sweep_last_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t* since, uint64_t cap, uint64_t* n_out) {
+  return timed_out_impl(h, offset, idx, since, cap, n_out, false);
+}
+
+int am_sweep_last_remedy_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t* started, uint64_t cap,
+                                   uint64_t* n_out) {
+  return timed_out_impl(h, offset, idx, started, cap, n_out, true);
 }
 
 // (tick guard held, staged events drained, h->stream ordered)

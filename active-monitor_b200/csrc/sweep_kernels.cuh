@@ -258,6 +258,28 @@ __device__ __forceinline__ uint32_t carry_of_actions(uint32_t a) { return ((a & 
 static_assert(AM_F_CARRY_SHIFT == 11 && AM_ACT_RUN_REMEDY == 0x02u && AM_ACT_REMEDY_SKIP == 0x10u && AM_ACT_ANOMALY == 0x80u,
               "carry bit layout");
 
+// Remedy hold: a result step whose actions `a` run the remedy starts a remedy run unless a remedy outcome (`f`, the flags
+// it was applied to) completed the remedy at once.  In the reference the Failed branch blocks in watchRemedyWorkflow
+// (hcc.go:683-714, :788-852) until the remedy ends; only then is the next run scheduled.
+__device__ __forceinline__ bool starts_remedy_run(uint32_t a, uint32_t f) {
+  return (a & AM_ACT_RUN_REMEDY) && !(f & AM_F_REMEDY_PENDING);
+}
+// The run of slot i started at T: since = T + kRemedyRun, and with timeout state (TIMEOUT) the deadline T + W of the
+// slot's workflow timeout W (hcc.go:791-799 watch the remedy with Spec.Workflow.Timeout), none when W is 0 — stored
+// either way, since the word may still hold the health-check run's deadline — and the segment's bound lowered to it.
+// Starts are rare (a failure of a check with a remedy workflow): one atomic per start and no register kept live for it
+// (a per-warp minimum cost the open-loop on-minute sweep 16 B of spills at 64 registers).
+template <bool TIMEOUT>
+__device__ __forceinline__ void start_remedy_run(int64_t* since, int64_t* deadline, const int32_t* wf_timeout,
+                                                 unsigned long long* seg_deadline, uint32_t i, int64_t T) {
+  since[i] = T + kRemedyRun;
+  if (TIMEOUT) {
+    const int32_t W = wf_timeout[i];
+    deadline[i] = W > 0 ? T + W : kNoDeadline;
+    if (W > 0) atomicMin(seg_deadline + i / (uint32_t)kRecPerWarp, biased_key(T + W));
+  }
+}
+
 // robfig SpecSchedule matching against the tick's one-hot wall-clock words (Appendix A: five ANDs and
 // the dom/dow star rule).  Branch-free: every term is evaluated (no short-circuit control flow).
 __device__ __forceinline__ bool cron_matches(const TickWords& t, uint64_t mi, uint64_t hr, uint64_t dm, uint64_t mo, uint64_t dw) {
@@ -314,7 +336,9 @@ __global__ void tz_words_kernel(const int32_t* __restrict__ tz_off, TickWords* _
 // TIMEOUT = workflow timeouts (HOLD only; the handle received a non-zero am_record_t.wf_timeout): the same round trip
 // also loads the slot's timeout W, and every submitted record gets deadline = T + W (none when W is 0); one atomicMin
 // per warp lowers the segment's bound (p.seg_deadline) that expire_runs_kernel reads.
-template <bool CLOSED, bool MASKS, bool WINDOW = false, bool HOLD = false, bool TIMEOUT = false>
+// REMEDY = remedy hold (HOLD only, am_sweep_set_hold_remedy): a record whose posted result this sweep applies and which
+// gains AM_ACT_RUN_REMEDY without a remedy outcome merged starts a remedy run (start_remedy_run): it is not submitted.
+template <bool CLOSED, bool MASKS, bool WINDOW = false, bool HOLD = false, bool TIMEOUT = false, bool REMEDY = false>
 __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1)
     sweep_tick_kernel(const SweepParams p) {
   // one row per warp, written unconditionally: no zero-initialisation, no shared
@@ -598,7 +622,12 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
           if ((nb >> j) & 1u) {
             RecState s{nfl[h][j], nfa[h][j], ns[j], nf[j], nrs[j], nrf[j], nrt[j], nrfa[j], limv[j], rstv[j]};
             uint32_t res = 0;
-            act[h][j] |= result_step<CLOSED>(s, T, (due_bits >> (2 * h + j)) & 1u, p.seed, p.shard_base + r + (uint32_t)j, res);
+            const uint32_t a = result_step<CLOSED>(s, T, (due_bits >> (2 * h + j)) & 1u, p.seed, p.shard_base + r + (uint32_t)j, res);
+            act[h][j] |= a;
+            if (REMEDY && starts_remedy_run(a, nfl[h][j])) {
+              start_remedy_run<TIMEOUT>(p.since, p.deadline, p.wf_timeout, p.seg_deadline, r + (uint32_t)j, T);
+              act[h][j] &= ~AM_ACT_SUBMIT_HC;
+            }
             res_lane += res;
             nfl[h][j] = s.flags; nfa[h][j] = s.fa;
             ns[j] = s.s; nf[j] = s.f; nrs[j] = s.rs; nrf[j] = s.rf; nrt[j] = s.rt; nrfa[j] = s.rfa;
@@ -633,6 +662,8 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
       const uint32_t a = result_step<CLOSED>(s, T, (due_bits >> b) & 1u, p.seed, p.shard_base + i, res);
       res_lane += res;  // per lane at most 4 records x 2 results per byte
       store_changed_state(p.c, i, s, s0);
+      const bool run = REMEDY && starts_remedy_run(a, s0.flags);
+      if (run) start_remedy_run<TIMEOUT>(p.since, p.deadline, p.wf_timeout, p.seg_deadline, i, T);
       // (a record "Stopped" in this very tick already carries STOPPED_REPORTED and
       // finishedAt = T in nfl/nfa, and apply_result preserves both: the pause rule of
       // hcc.go:238-250 and a posted result commute)
@@ -640,6 +671,7 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
       for (int q = 0; q < 4; ++q) {
         if (q == b) {
           act[q >> 1][q & 1] |= a;
+          if (run) act[q >> 1][q & 1] &= ~AM_ACT_SUBMIT_HC;
           nfl[q >> 1][q & 1] = s.flags;
           nfa[q >> 1][q & 1] = s.fa;
         }
@@ -1220,8 +1252,12 @@ __global__ void apply_result_ops_kernel(uint32_t* flags, const uint32_t* __restr
 // timer-armed state it leaves is exactly what the sweep's own step 1 would have decided on.  Only the
 // tick's drain does this (T is the tick's second) and only when results are sparse; a read drains
 // without it, and a dense batch is cheaper as the sweep's streaming path.
+// REMEDY (remedy hold): a result that runs the remedy without a remedy outcome merged starts a remedy run here
+// (start_remedy_run; `deadline` NULL without timeout state), and the sweep of the same tick holds the record.
+template <bool REMEDY>
 __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops, uint32_t n,
-                                         int64_t T, unsigned long long* acc) {
+                                         int64_t T, unsigned long long* acc, int64_t* since, int64_t* deadline,
+                                         const int32_t* __restrict__ wf_timeout, unsigned long long* seg_deadline) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   constexpr uint32_t kPend = AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING;
@@ -1271,6 +1307,10 @@ __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__
         if (s.rt != b.rt) c.remedy_total[i] = s.rt;
         if (s.rfa != b.rfa) c.remedy_finished_at[i] = s.rfa;
         c.flags[i] = s.flags | carry_of_actions(a);  // pending bits cleared, timer armed, action bits for this tick's sweep
+        if (REMEDY && starts_remedy_run(a, f)) {
+          if (deadline) start_remedy_run<true>(since, deadline, wf_timeout, seg_deadline, i, T);
+          else start_remedy_run<false>(since, deadline, wf_timeout, seg_deadline, i, T);
+        }
       }
     }
   }
@@ -1285,7 +1325,8 @@ __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__
 //     when a later upsert of the slot supersedes the result itself, and whatever second the next tick has;
 //   * a remove: no workflow in flight any more (hcc.go:175-186 stops its timer), also one followed by an upsert of the
 //     same slot (a new CR in an old slot).
-// A remedy phase alone does not (remedy workflows are not held).  Launched only while the hold is on.
+// A remedy phase alone ends a remedy run (remedy hold: hcc.go:821-851 end watchRemedyWorkflow), not a health-check run.
+// Launched only while the hold is on.
 __global__ void clear_since_kernel(int64_t* since, const uint2* __restrict__ ops, uint32_t n) {
   pdl_wait();  // (launched with programmatic stream serialisation: the previous tick's sweep writes since)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1293,6 +1334,17 @@ __global__ void clear_since_kernel(int64_t* since, const uint2* __restrict__ ops
   const uint2 op = ops[k];
   const uint32_t kind = op.y & kOpKindMask;
   if (kind == kOpRemove || (kind == kOpResult && (op.y & kHcBits))) since[op.x] = kNotInFlight;
+  else if (kind == kOpResult && (op.y & AM_F_REMEDY_PENDING) && is_remedy_run(since[op.x])) since[op.x] = kNotInFlight;
+}
+
+// Turning the remedy hold off: every remedy run ends, with its deadline (`deadline` NULL without timeout state).
+__global__ void release_remedy_runs_kernel(int64_t* since, int64_t* deadline, uint64_t n) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    if (is_remedy_run(since[i])) {
+      since[i] = kNotInFlight;
+      if (deadline) deadline[i] = kNoDeadline;
+    }
+  }
 }
 
 __global__ void fill_i64_kernel(int64_t* p, int64_t v, uint64_t n) {
@@ -1301,16 +1353,17 @@ __global__ void fill_i64_kernel(int64_t* p, int64_t v, uint64_t n) {
   for (; i < n; i += stride) p[i] = v;
 }
 
-// am_sweep_in_flight: since of the slots the next tick would hold (the sweep's rule, on the drained state), else
-// kNotInFlight.  idx == NULL: the range [first, first + n).
+// am_sweep_in_flight: since of the slots the next tick would hold (the sweep's rule, on the drained state) for a
+// health-check run, else kNotInFlight.  `remedy` (am_sweep_remedy_in_flight): the start of a held remedy run instead.
+// idx == NULL: the range [first, first + n).
 __global__ void in_flight_kernel(DevCols c, const int64_t* __restrict__ since, uint32_t first, const uint32_t* __restrict__ idx,
-                                 uint32_t n, int64_t* out) {
+                                 uint32_t n, int64_t* out, bool remedy) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const uint32_t i = idx ? idx[k] : first + k;
   const int64_t s = since[i];
   const bool held = s != kNotInFlight && s >= c.finished_at[i] && !(c.flags[i] & (AM_F_PENDING_OK | AM_F_PENDING_FAIL));
-  out[k] = held ? s : kNotInFlight;
+  out[k] = held && is_remedy_run(s) == remedy ? (remedy ? s - kRemedyRun : s) : kNotInFlight;
 }
 
 // Workflow timeouts: the drain's winning upserts (the marks decide, as in apply_state_ops_kernel) store their record's
@@ -1334,7 +1387,9 @@ __global__ void store_wf_timeout_kernel(int32_t* wf, const uint32_t* __restrict_
 // dropped; a run that is still held (the sweep's rule) on a live record gets AM_F_PENDING_FAIL, exactly as a posted
 // Failed does, so the result kernel behind this one or the sweep's pending path applies it (counters, finishedAt = T,
 // timer, remedy gate); its since is cleared as clear_since_kernel clears it for a posted phase; and (slot, since) is
-// appended to the tick's list (one atomic per segment).  The bound becomes the exact minimum of what is left.
+// appended to the tick's list (one atomic per segment).  The bound becomes the exact minimum of what is left.  A remedy
+// run (remedy hold) gets AM_F_REMEDY_PENDING without the OK bit instead, and its since word goes into the list as it
+// is: the host tells the two kinds apart.
 __global__ void expire_runs_kernel(DevCols c, int64_t* since, int64_t* deadline, unsigned long long* seg_deadline,
                                    uint32_t n_seg, int64_t T, uint32_t* out_idx, int64_t* out_since, uint32_t* out_count) {
   pdl_wait();  // (launched with programmatic stream serialisation: the previous tick's sweep writes deadlines)
@@ -1359,7 +1414,8 @@ __global__ void expire_runs_kernel(DevCols c, int64_t* since, int64_t* deadline,
         const uint32_t f = c.flags[i];
         const int64_t s = since[i];
         if (is_live(f) && s != kNotInFlight && s >= c.finished_at[i] && !(f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL))) {
-          c.flags[i] = f | AM_F_PENDING_FAIL;
+          // a remedy run (remedy hold, hcc.go:813-818) times out as a posted remedy "Failed"
+          c.flags[i] = is_remedy_run(s) ? ((f & ~AM_F_REMEDY_OUTCOME_OK) | AM_F_REMEDY_PENDING) : (f | AM_F_PENDING_FAIL);
           since[i] = kNotInFlight;
           sv[q] = s;
           hit |= 1u << q;

@@ -132,6 +132,12 @@ struct SweepParams {
 };
 constexpr int64_t kNotInFlight = INT64_MIN;
 constexpr int64_t kNoDeadline = INT64_MAX;
+// Remedy hold (am_sweep_set_hold_remedy): a running remedy workflow started at T is kept in the slot's since word as
+// T + kRemedyRun.  Every tick second is |T| < 2^55, so a since word >= kRemedyRun / 2 is a remedy run and anything
+// below is a health-check run; a check has at most one run of either kind in flight, so they share the word (and the
+// deadline word).
+constexpr int64_t kRemedyRun = 1ll << 60;
+__device__ __forceinline__ bool is_remedy_run(int64_t since) { return since >= kRemedyRun / 2; }
 // a signed second as an unsigned key of the same order (the atomicMin idiom of next_due_kernel); kNoDeadline -> ~0
 __device__ __forceinline__ unsigned long long biased_key(int64_t t) { return (unsigned long long)t ^ (1ull << 63); }
 

@@ -327,36 +327,55 @@ class Sweep:
         """one health-check workflow per check at a time (am_sweep_set_hold_in_flight)"""
         self._check(self._lib.am_sweep_set_hold_in_flight(self._h, int(bool(on))), "am_sweep_set_hold_in_flight")
 
-    def in_flight(self, first: int = 0, n: int | None = None, idx=None) -> np.ndarray:
-        """i64 `since` of the slots [first, first+n) (or `idx`) the next tick would hold, INT64_MIN elsewhere.
-        n defaults to the swept slots from `first` on (am_sweep_size)."""
+    def set_hold_remedy(self, on: bool):
+        """no HealthCheck submitted while the check's remedy workflow runs (am_sweep_set_hold_remedy; needs the hold)"""
+        self._check(self._lib.am_sweep_set_hold_remedy(self._h, int(bool(on))), "am_sweep_set_hold_remedy")
+
+    def _per_slot(self, fn: str, first: int, n: int | None, idx) -> np.ndarray:
         if idx is not None:
             idx = np.ascontiguousarray(idx, dtype=np.uint64)
             n = len(idx)
         elif n is None:
             n = max(self.size - first, 0)
         out = np.zeros(n, dtype=np.int64)
-        self._check(self._lib.am_sweep_in_flight(self._h, first, n, None if idx is None else idx.ctypes.data,
-                                                 out.ctypes.data), "am_sweep_in_flight")
+        self._check(getattr(self._lib, fn)(self._h, first, n, None if idx is None else idx.ctypes.data, out.ctypes.data), fn)
         return out
+
+    def in_flight(self, first: int = 0, n: int | None = None, idx=None) -> np.ndarray:
+        """i64 `since` of the slots [first, first+n) (or `idx`) the next tick would hold for their health-check run,
+        INT64_MIN elsewhere.  n defaults to the swept slots from `first` on (am_sweep_size)."""
+        return self._per_slot("am_sweep_in_flight", first, n, idx)
+
+    def remedy_in_flight(self, first: int = 0, n: int | None = None, idx=None) -> np.ndarray:
+        """i64 start of the running remedy workflow of the slots the next tick would hold for it (remedy hold,
+        am_sweep_remedy_in_flight), INT64_MIN elsewhere; arguments as in_flight"""
+        return self._per_slot("am_sweep_remedy_in_flight", first, n, idx)
+
+    def _timed_out(self, fn: str, offset: int, cap: int | None):
+        n = L.u64(0)
+        call = getattr(self._lib, fn)
+        if cap is None:
+            rc = call(self._h, offset, None, None, 0, C.byref(n))
+            if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+                self._check(rc, fn)
+            cap = int(n.value)
+        idx = np.empty(cap, dtype=np.uint64)
+        since = np.empty(cap, dtype=np.int64)
+        rc = call(self._h, offset, idx.ctypes.data if cap else None, since.ctypes.data if cap else None, cap, C.byref(n))
+        if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+            self._check(rc, fn)
+        k = min(int(n.value), cap)
+        return idx[:k], since[:k]
 
     def last_timed_out(self, offset: int = 0, cap: int | None = None):
         """the runs the last tick timed out (workflow timeouts, am_sweep_last_timed_out): (global idx u64, since i64),
         ascending by index, from entry `offset` on.  cap None: all of them."""
-        n = L.u64(0)
-        if cap is None:
-            rc = self._lib.am_sweep_last_timed_out(self._h, offset, None, None, 0, C.byref(n))
-            if rc not in (L.AM_OK, L.AM_E_NOSPACE):
-                self._check(rc, "am_sweep_last_timed_out")
-            cap = int(n.value)
-        idx = np.empty(cap, dtype=np.uint64)
-        since = np.empty(cap, dtype=np.int64)
-        rc = self._lib.am_sweep_last_timed_out(self._h, offset, idx.ctypes.data if cap else None,
-                                               since.ctypes.data if cap else None, cap, C.byref(n))
-        if rc not in (L.AM_OK, L.AM_E_NOSPACE):
-            self._check(rc, "am_sweep_last_timed_out")
-        k = min(int(n.value), cap)
-        return idx[:k], since[:k]
+        return self._timed_out("am_sweep_last_timed_out", offset, cap)
+
+    def last_remedy_timed_out(self, offset: int = 0, cap: int | None = None):
+        """the remedy runs the last tick timed out (remedy hold, am_sweep_last_remedy_timed_out): (global idx u64,
+        start i64), as last_timed_out"""
+        return self._timed_out("am_sweep_last_remedy_timed_out", offset, cap)
 
     # -- introspection
     def set_seed(self, seed: int):

@@ -408,7 +408,7 @@ int am_sweep_read(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx,
  * and posts a synthetic Failed) are kept on the device, below.  am_sweep_remove and am_sweep_load_range clear since for their slots; a remedy
  * phase alone does not.  An upsert keeps the hold (a status write during a run re-enters
  * Reconcile; it must not submit the check again) unless its finishedAt is later than since.
- * Only the health-check workflow is held: remedy workflows are not.
+ * Only the health-check workflow is held unless the remedy hold is on (am_sweep_set_hold_remedy).
  * Works with AM_SWEEP_CATCH_UP, AM_SWEEP_FULL_SCAN, named zones and every tick entry point
  * (am_sweep_tick, _tick_view, _tick_device, _tick_shard and so am_gather_exchange /
  * am_gather_tick_view).  While on, a tick with AM_SWEEP_CLOSED_LOOP and am_sweep_run_ticks return
@@ -430,8 +430,53 @@ int am_sweep_read(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx,
  * then is not timed out, and a later upsert that holds it again does not bring D back.  A refused
  * tick times nothing out.  The first upsert with a non-zero wf_timeout allocates 24 B per slot of
  * capacity on the device; handles that never receive one launch nothing more.  Remedy workflows
- * have no timeout here, and am_sweep_run_ticks is refused while the hold is on anyway. */
+ * time out only under the remedy hold, and am_sweep_run_ticks is refused while the hold is on
+ * anyway.  Turning the hold off also turns the remedy hold off. */
 int am_sweep_set_hold_in_flight(am_sweep_t*, int on);
+
+/* Remedy hold: a check is not submitted while its remedy workflow runs, as in the reference, where
+ * the Failed branch of the watch loop runs the remedy and blocks in watchRemedyWorkflow until it
+ * ends or times out (hcc.go:683-714, :788-852); only then is the status written and the next timer
+ * armed.  Without it the check keeps its schedule while the remedy runs, and every failure in that
+ * time reads RemedyTotalRuns before the running remedy's phase is posted: a slow remedy can be
+ * started many times over its runs limit.  Off by default; AM_E_INVAL (nothing changes) while the
+ * hold in flight is off.  While on:
+ *  - A remedy run STARTS at a tick T whose action for a check carries AM_ACT_RUN_REMEDY when no
+ *    remedy outcome was applied with it (a remedy phase posted in the same call as the Failed, or
+ *    in an earlier call before the tick: then the remedy completed at once and nothing is held) —
+ *    whether the Failed was posted or is a workflow timeout's, and also in a tick that returns
+ *    AM_E_NOSPACE.  Its start is T (RemedyStartedAt, the `then` of hcc.go:790).  With the timeout
+ *    state (a non-zero wf_timeout was ever upserted) it gets the deadline D = T + W when the slot's
+ *    wf_timeout W is > 0 at T, none otherwise: the remedy watch uses Spec.Workflow.Timeout.
+ *  - While it runs the check is HELD: no AM_ACT_SUBMIT_HC, also at the tick T that starts it (a
+ *    5-field check matching T at the tick its Failed is applied is not submitted).  Everything
+ *    else about it is evaluated as usual.  am_sweep_in_flight reads INT64_MIN for it and
+ *    am_sweep_remedy_in_flight its start; am_sweep_next_due skips it and counts D as an event at
+ *    max(D, unix_sec + 1).
+ *  - It ENDS at the drain of a posted remedy phase (also when a later upsert supersedes the result
+ *    itself) or a posted workflow phase (applied as always), at a remove, at am_sweep_load_range
+ *    and when either hold is turned off.  An upsert keeps it.  The check is then due by its usual
+ *    rule (finishedAt + RepeatAfterSec, or its schedule): one that became due while the remedy ran
+ *    is submitted at the tick that ends it.  (The reference re-arms its timer RepeatAfterSec after
+ *    the remedy ends, hcc.go:751: a divergence, see INTEGRATION.md section 5.)
+ *  - TIMEOUT: the first tick of any entry point with T >= D looks at the run after its drain; if it
+ *    is still held on a live record, the tick treats it exactly as if am_sweep_post_result(slot,
+ *    AM_PHASE_NONE, AM_PHASE_FAILED) had been the last call before it (RemedyFailedCount + 1,
+ *    RemedyTotalRuns = success + failed, RemedyFinishedAt = T, n_remedy_fail, the run ended, then
+ *    the due decision at T) and lists it in am_sweep_last_remedy_timed_out.  D is dropped either way.
+ * Turning it off ends every remedy run (one pass over the slots); it costs no memory of its own. */
+int am_sweep_set_hold_remedy(am_sweep_t*, int on);
+
+/* The remedy runs the last tick timed out (remedy hold): the contract of am_sweep_last_timed_out,
+ * with started[k] the run's start (RemedyStartedAt), for the status and the "remedy workflow is
+ * timedout" event (hcc.go:813-818) the caller writes. */
+int am_sweep_last_remedy_timed_out(am_sweep_t*, uint64_t offset, uint64_t* idx, int64_t* started, uint64_t cap,
+                                   uint64_t* n_out);
+
+/* For each slot of [first, first+n) (idx == NULL) or idx[0..n): the start of the slot's running
+ * remedy workflow the next tick would hold (remedy hold), INT64_MIN for every other slot (and for all
+ * of them while the remedy hold is off).  Drains staged calls like am_sweep_read. */
+int am_sweep_remedy_in_flight(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* started_out);
 
 /* The runs the last tick (of any entry point) timed out, ascending by global index, from entry
  * `offset` on: idx[k] the global index, since[k] the run's Status.StartedAt (hcc.go:609/665), for
@@ -443,7 +488,8 @@ int am_sweep_set_hold_in_flight(am_sweep_t*, int on);
 int am_sweep_last_timed_out(am_sweep_t*, uint64_t offset, uint64_t* idx, int64_t* since, uint64_t cap, uint64_t* n_out);
 
 /* For each slot of [first, first+n) (idx == NULL) or idx[0..n): the `since` of a slot the next
- * tick would hold, INT64_MIN for every other slot (and for all of them while the hold is off).
+ * tick would hold for its health-check run, INT64_MIN for every other slot (and for all of them
+ * while the hold is off; a slot whose remedy runs is in am_sweep_remedy_in_flight).
  * Drains staged calls like am_sweep_read.  `since` is the run's Status.StartedAt (`then`,
  * hcc.go:609/638/665), which the caller can write back with the result. */
 int am_sweep_in_flight(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out);

@@ -1,0 +1,177 @@
+"""Child process of tests/test_remedy_hold_emulator.py: the remedy hold through the sharded whole step, as
+run_gather_timeout.py runs workflow timeouts.  `world` ranks as Python threads drive the REAL C-ABI of the emulated
+library: every rank owns an index-range shard of ONE amgen population (half of it with a remedy workflow), turns the hold
+and the remedy hold on, upserts its records with a wf_timeout and calls am_gather_tick_view (am_sweep_tick_shard with
+the remedy variants, then the exchange).  Between ticks a few workflow phases are posted for checks in flight and a few
+remedy phases for running remedies, each to the rank that owns it; the rest time out.  Every rank's global list must
+equal the remedy-hold oracle (tests/remedy_hold_oracle.py) of the UNSHARDED population, its view, its
+am_sweep_last_timed_out and its am_sweep_last_remedy_timed_out the part it owns; at the end its columns,
+am_sweep_in_flight and am_sweep_remedy_in_flight the oracle's.
+
+usage: run_gather_remedy_hold.py <world> <idx_bytes> <records in total> <config>
+Prints "ok ..." and exits 0 on success."""
+import ctypes as C
+import importlib
+import os
+import sys
+import threading
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tools", "amgen"), os.path.join(ROOT, "tests")):
+    sys.path.insert(0, p)
+abi = importlib.import_module("active-monitor_b200._lib")
+assert "emu" in os.path.basename(abi.LIB_PATH), "run with AMSWEEP_LIB pointing at libamsweep_emu.so"
+am = importlib.import_module("active-monitor_b200")
+gather = importlib.import_module("active-monitor_b200.gather")
+lib = abi.load()
+
+import amgen  # noqa: E402
+import hold_oracle  # noqa: E402
+import remedy_hold_oracle  # noqa: E402
+import timeout_oracle  # noqa: E402
+from adversarial import ZoneMap, product_lookup  # noqa: E402
+
+world, idx_bytes, n_total, config = (int(a) for a in sys.argv[1:5])
+T0 = 1790898290  # 2026-10-01 23:44:50 UTC
+TICKS = [(T0, False), (T0 + 1, False), (T0 + 2, False), (T0 + 9, True), (T0 + 70, True), (T0 + 71, False),
+         (T0 + 72, False), (T0 + 700, True), (T0 + 701, False), (T0 + 3700, True), (T0 + 3701, False)]
+
+zmap = ZoneMap(product_lookup(lib))  # zone ids in the generator's order, before anything is classified
+whole = amgen.fill(config, 4, 0, n_total, T0, lib.am_healthcheck_classify, threads=2)
+whole["flags"] |= np.where(np.random.default_rng(config).random(n_total) < 0.5, abi.F_HAS_REMEDY, 0).astype(np.uint32)
+shards = [gather.shard_range(n_total, r, world) for r in range(world)]
+bases = np.array([s[0] for s in shards], dtype=np.uint64)
+sizes = np.array([s[1] for s in shards], dtype=np.uint64)
+
+# the oracle run first: it decides which in-flight checks post a phase before each tick
+rng = np.random.default_rng(world * 1000 + config)
+ocols = {k: v.copy() for k, v in whole.items()}
+ocols["flags"] &= np.uint32(~abi.F_TOMBSTONE & 0xFFFFFFFF)  # (upserted, not loaded: an upsert is never a tombstone)
+since = hold_oracle.none_in_flight(n_total)
+deadline = timeout_oracle.no_deadlines(n_total)
+rsince = hold_oracle.none_in_flight(n_total)
+rdeadline = timeout_oracle.no_deadlines(n_total)
+wf = np.random.default_rng(world * 77 + config).integers(0, 120, n_total).astype(np.int32)
+want, posts, P = [], [], None
+hc = np.uint32(abi.F_PENDING_OK | abi.F_PENDING_FAIL)
+for k, (T, catch_up) in enumerate(TICKS):
+    fl = np.flatnonzero(since != hold_oracle.NOT_IN_FLIGHT)
+    sl = np.sort(rng.choice(fl, min(len(fl), 60), replace=False)) if k and len(fl) else np.zeros(0, np.int64)
+    ph = rng.integers(1, 3, len(sl)).astype(np.uint8)
+    ph = np.where(rng.random(len(sl)) < 0.8, 2, 1).astype(np.uint8)
+    ocols["flags"][sl] = (ocols["flags"][sl] & ~hc) | np.where(ph == 1, abi.F_PENDING_OK, abi.F_PENDING_FAIL).astype(np.uint32)
+    hold_oracle.post(since, sl, ph)
+    rl = np.flatnonzero(rsince != hold_oracle.NOT_IN_FLIGHT)
+    rl = np.sort(rng.choice(rl, min(len(rl), 20), replace=False)) if len(rl) else np.zeros(0, np.int64)
+    ocols["flags"][rl] |= np.uint32(abi.F_REMEDY_PENDING | abi.F_REMEDY_OUTCOME_OK)
+    rsince[rl] = hold_oracle.NOT_IN_FLIGHT
+    rdeadline[rl] = timeout_oracle.NO_DEADLINE
+    posts.append((sl, ph, rl))
+    want.append(remedy_hold_oracle.sweep(zmap, ocols, since, deadline, wf, rsince, rdeadline, T, P=P if catch_up else None))
+    P = T
+assert sum(int(((w[1] & abi.ACT_SUBMIT_HC) != 0).sum()) for w in want[1:]) > 0
+assert sum(len(w[3][0]) for w in want) > 100 and sum(len(w[4][0]) for w in want) > 20
+
+handles = [None] * world
+n_timed = [0] * world
+n_rtimed = [0] * world
+errors = []
+bar = threading.Barrier(world)
+
+
+def view(ptr, n, ctype, dtype):
+    if n == 0:
+        return np.zeros(0, dtype)
+    return np.frombuffer((ctype * n).from_address(ptr), dtype=dtype).copy()
+
+
+def rank_main(rank):
+    try:
+        first, cnt = shards[rank]
+        s = am.Sweep(capacity=cnt, device=rank, shard_base=first)
+        s.set_hold_in_flight(True)
+        s.set_hold_remedy(True)
+        recs = am.columns_to_records({k: np.ascontiguousarray(v[first:first + cnt]) for k, v in whole.items()})
+        recs["wf_timeout"] = wf[first:first + cnt]
+        s.upsert(np.arange(cnt), recs)
+        h = C.c_void_p()
+        assert lib.am_gather_create(C.byref(h), rank, rank, world, n_total, idx_bytes) == 0
+        mine = C.create_string_buffer(abi.IPC_HANDLE_BYTES)
+        assert lib.am_gather_export(h, mine) == 0
+        handles[rank] = bytes(mine.raw)
+        bar.wait()
+        assert lib.am_gather_connect(h, b"".join(handles)) == 0
+        assert lib.am_gather_set_layout(h, bases.ctypes.data, sizes.ctypes.data) == 0
+        assert lib.am_gather_bind(h, s._h, None, None) == 0
+        st = np.zeros(1, dtype=abi.STATS_DTYPE)
+        it, dt = (C.c_uint32, np.uint32) if idx_bytes == 4 else (C.c_uint64, np.uint64)
+        for k, (T, catch_up) in enumerate(TICKS):
+            sl, ph, rl = posts[k]
+            own = (sl >= first) & (sl < first + cnt)
+            if own.any():
+                s.post_result(sl[own] - first, ph[own])
+            own = (rl >= first) & (rl < first + cnt)
+            if own.any():
+                s.post_result(rl[own] - first, np.zeros(int(own.sum()), np.uint8), np.ones(int(own.sum()), np.uint8))
+            v = abi.AmTickView()
+            rc = lib.am_gather_tick_view(h, T, abi.SWEEP_CATCH_UP if catch_up else 0, C.byref(v),
+                                         C.cast(st.ctypes.data, C.POINTER(abi.AmTickStats)))
+            assert rc == 0, (rc, lib.am_gather_last_error(h))
+            counts = view(lib.am_gather_out_counts(h), world + 1, C.c_uint32, np.uint32)
+            total = int(counts[world])
+            gi = view(lib.am_gather_out_idx(h), total, it, dt).astype(np.uint64)
+            ga = view(lib.am_gather_out_act(h), total, C.c_uint8, np.uint8)
+            wi, wa, _, timed, rtimed = want[k]
+            np.testing.assert_array_equal(gi, wi, err_msg=f"rank {rank} tick {k} idx")
+            np.testing.assert_array_equal(ga.astype(np.uint32), wa, err_msg=f"rank {rank} tick {k} act")
+            part = (wi >= first) & (wi < first + cnt)
+            vi = view(C.cast(v.idx_local, C.c_void_p).value, int(v.n), C.c_uint32, np.uint32)
+            va = view(C.cast(v.action, C.c_void_p).value, int(v.n), C.c_uint8, np.uint8)
+            np.testing.assert_array_equal(vi.astype(np.uint64) + np.uint64(first), wi[part], err_msg=f"rank {rank} tick {k} view")
+            np.testing.assert_array_equal(va.astype(np.uint32), wa[part], err_msg=f"rank {rank} tick {k} view act")
+            ti, ts = s.last_timed_out()
+            mine = (timed[0] >= first) & (timed[0] < first + cnt)
+            np.testing.assert_array_equal(ti, timed[0][mine], err_msg=f"rank {rank} tick {k} timed out")
+            np.testing.assert_array_equal(ts, timed[1][mine], err_msg=f"rank {rank} tick {k} timed-out since")
+            n_timed[rank] += len(ti)
+            ri, rs = s.last_remedy_timed_out()
+            mine = (rtimed[0] >= first) & (rtimed[0] < first + cnt)
+            np.testing.assert_array_equal(ri, rtimed[0][mine], err_msg=f"rank {rank} tick {k} remedy timed out")
+            np.testing.assert_array_equal(rs, rtimed[1][mine], err_msg=f"rank {rank} tick {k} remedy start")
+            n_rtimed[rank] += len(ri)
+        bar.wait()
+        dev = s.read_range(0, cnt)
+        for name in abi.COLUMN_NAMES:
+            np.testing.assert_array_equal(dev[name], ocols[name][first:first + cnt], err_msg=f"rank {rank} column {name}")
+        np.testing.assert_array_equal(s.in_flight(0, cnt), hold_oracle.in_flight(ocols, since)[first:first + cnt],
+                                      err_msg=f"rank {rank} in_flight")
+        np.testing.assert_array_equal(s.remedy_in_flight(0, cnt), remedy_hold_oracle.in_flight(ocols, rsince)[first:first + cnt],
+                                      err_msg=f"rank {rank} remedy_in_flight")
+        # a closed-loop step is refused on every rank before anything happens (no exchange needed)
+        rc = lib.am_sweep_tick_shard(s._h, TICKS[-1][0] + 1, abi.SWEEP_CLOSED_LOOP, None)
+        assert rc == abi.AM_E_INVAL, (rank, rc)
+        bar.wait()
+        lib.am_gather_destroy(h)
+        s.close()
+    except BaseException as e:  # noqa: BLE001
+        import traceback
+        errors.append((rank, repr(e), traceback.format_exc()[-1500:]))
+        try:
+            bar.abort()
+        except Exception:
+            pass
+
+
+th = [threading.Thread(target=rank_main, args=(r,)) for r in range(world)]
+for t in th:
+    t.start()
+for t in th:
+    t.join()
+if errors:
+    print("FAILED", errors)
+    sys.exit(1)
+assert all(v > 0 for v in n_rtimed), n_rtimed  # every shard timed out remedy runs of its own
+print(f"ok remedy hold remedy_timed_out_per_rank={n_rtimed} timed_out_per_rank={n_timed} world={world} idx_bytes={idx_bytes} n={n_total} config={config} "
+      f"emitted={[len(w[0]) for w in want]} remedy_held={int(remedy_hold_oracle.held(ocols, rsince).sum())}")
