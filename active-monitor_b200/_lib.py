@@ -150,6 +150,8 @@ SYMBOLS = {
     "am_sweep_set_hold_remedy": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_remedy_in_flight": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, C.c_void_p]),
     "am_sweep_last_remedy_timed_out": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
+    "am_sweep_set_track_changes": (C.c_int, [C.c_void_p, C.c_int]),
+    "am_sweep_last_changes": (C.c_int, [C.c_void_p, u64, C.c_void_p, P(AmRecordCols), u64, P(u64)]),
     "am_sweep_size": (u64, [C.c_void_p]),
     "am_sweep_capacity": (u64, [C.c_void_p]),
     "am_sweep_device": (C.c_int, [C.c_void_p]),

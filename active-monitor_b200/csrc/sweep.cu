@@ -202,6 +202,18 @@ struct am_sweep {
   bool to_fetched = false;  // ... and has been copied to to_host / rto_host, sorted
   std::vector<std::pair<uint32_t, int64_t>> to_host;   // health-check runs: (slot, since)
   std::vector<std::pair<uint32_t, int64_t>> rto_host;  // remedy runs: (slot, start)
+  // status changes (am_sweep_set_track_changes), allocated at the first enable: one bit per slot that the coming tick
+  // changes ([n_groups * kGroupWords], drains and the tick add to it, the list kernel clears it), the last tick's
+  // ascending slot list ([cap_padded]), and the per-group counts, offsets and total of the compaction
+  bool track = false;
+  uint32_t* chg_bits = nullptr;
+  uint32_t* chg_list = nullptr;
+  uint32_t* chg_group = nullptr;
+  uint32_t* chg_prefix = nullptr;
+  unsigned long long* chg_acc = nullptr;  // scan_groups_kernel's accumulators: [1] = entries in chg_list
+  bool chg_listed = false;   // the last tick built its list on the device
+  bool chg_fetched = false;  // ... and its length has been read into chg_n
+  uint64_t chg_n = 0;
   std::string last_error;
   uint64_t launches = 0;
   double last_ms = -1.0;
@@ -438,8 +450,44 @@ int expire_runs(am_sweep* h, cudaStream_t s, int64_t T) {
     AM_LAUNCH_PDL(expire_runs_kernel, (unsigned)((n_seg + 255) / 256), 256, s, h->cols, h->since, h->deadline,
                   h->seg_deadline, (uint32_t)n_seg, T, h->to_idx, h->to_since, h->to_count);
     h->launches++;
+    if (h->track) {  // status changes: every timed-out run gets its Failed applied by this tick
+      AM_LAUNCH_PDL(note_slots_kernel, h->sms, 256, s, h->chg_bits, (const uint32_t*)h->to_idx, (const uint32_t*)h->to_count);
+      h->launches++;
+    }
   }
   AM_CUDA(h, cudaGetLastError());
+  return AM_OK;
+}
+
+// Status changes: the bits of slots [first, first + n) from the flags as they stand (a live record with a pending result
+// is changed by the next tick), for turning tracking on and for am_sweep_load_range.
+int seed_changes(am_sweep* h, cudaStream_t s, uint64_t first, uint64_t n) {
+  AM_LAUNCH(seed_changes_kernel, h->sms * 8, 256, s, h->chg_bits, (const uint32_t*)h->cols.flags, first, n);
+  h->launches++;
+  AM_CUDA(h, cudaGetLastError());
+  return AM_OK;
+}
+
+// Status changes after a tick's sweep (buffer set `parity`): STOPPED in, ANOMALY out (and in closed loop every completed
+// submission in), then the bits compacted into the ascending list, which clears them.  A host tick launches this behind
+// the event it waits for: am_sweep_last_changes waits for it.
+int list_changes(am_sweep* h, cudaStream_t s, int parity, bool closed) {
+  if (h->n_records == 0) return AM_OK;  // (nothing swept: the list stays empty)
+  const TickSet& ts = h->set[parity];
+  const uint32_t n_tiles = tiles_of(h->n_records), n_groups = groups_of(h->n_records);
+  AM_LAUNCH_PDL(note_exceptions_kernel, (n_tiles + kWarps - 1) / kWarps, kBlock, s, h->chg_bits, ts.out, n_tiles, closed);
+  AM_LAUNCH_PDL(count_changes_kernel, n_groups, kGroupWords, s, h->chg_bits, (const uint32_t*)h->cols.flags, h->chg_group);
+  ScanParams sc{};
+  sc.group_count = h->chg_group;
+  sc.group_prefix = h->chg_prefix;
+  sc.acc = h->chg_acc;
+  sc.n_groups = n_groups;
+  sc.cap = 0xFFFFFFFFu;
+  AM_LAUNCH_PDL(scan_groups_kernel, 1, 1024, s, sc);
+  AM_LAUNCH_PDL(list_changes_kernel, n_groups, kGroupWords, s, h->chg_bits, (const uint32_t*)h->chg_prefix, h->chg_list);
+  h->launches += 4;
+  AM_CUDA(h, cudaGetLastError());
+  h->chg_listed = true;
   return AM_OK;
 }
 
@@ -507,6 +555,10 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
     AM_LAUNCH_PDL(build_planes_dirty_kernel, (unsigned)((n + kWarps - 1) / kWarps), kBlock, s, h->cols, h->planes,
                   h->seg_dirty, d_ops, (uint32_t)n);
     h->launches += 2;
+  }
+  if (h->track) {  // status changes: the phases of this drain that survive, and what its upserts and removes overwrote
+    AM_LAUNCH_PDL(note_ops_kernel, G, B, s, h->chg_bits, (const uint32_t*)h->cols.flags, h->marks, d_ops, (uint32_t)n);
+    h->launches++;
   }
   if (st->any_wf && !h->wf_timeout) {
     const int rc = alloc_timeouts(h, s);
@@ -838,6 +890,7 @@ int run_tick(am_sweep* h, int64_t T, uint32_t mode, cudaStream_t s, TickKind kin
   rc = set_stream(h, s);
   if (rc != AM_OK) return rc;
   const bool host = kind == TickKind::kHost;
+  h->chg_listed = h->chg_fetched = false;  // (every tick that drains resets the list of status changes)
   rc = drain_staged(h, s, &T, /*defer_clear=*/host);
   struct ClearOnExit {  // whatever happens below, the marks are cleared before the handle is used again
     am_sweep* h;
@@ -857,10 +910,16 @@ int run_tick(am_sweep* h, int64_t T, uint32_t mode, cudaStream_t s, TickKind kin
   const int parity = (int)h->parity;
   rc = launch_tick(h, T, mode, o, s, &win);
   if (rc != AM_OK) return rc;
-  if (host) {  // one synchronisation
+  if (host) {
     AM_CUDA(h, cudaEventRecord(h->ev1, s));
     rc = finish_deferred_clear(h, s);  // behind the event the host waits for
     if (rc != AM_OK) return rc;
+  }
+  if (h->track) {  // (a host tick: behind that event as well)
+    rc = list_changes(h, s, parity, (mode & AM_SWEEP_CLOSED_LOOP) != 0);
+    if (rc != AM_OK) return rc;
+  }
+  if (host) {  // one synchronisation
     AM_CUDA(h, cudaEventSynchronize(h->ev1));
     float ms = 0;
     AM_CUDA(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
@@ -1086,6 +1145,10 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
     rc = drop_deadlines(h, h->stream, first, n, false);
     if (rc != AM_OK) return rc;
   }
+  if (h->track) {  // the load replaced whatever the drains had noted for the range
+    rc = seed_changes(h, h->stream, first, n);
+    if (rc != AM_OK) return rc;
+  }
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   if (first + n > h->n_records) h->n_records = first + n;
   return AM_OK;
@@ -1130,6 +1193,30 @@ int am_sweep_set_hold_remedy(am_sweep_t* h, int on) {
     AM_CUDA(h, cudaGetLastError());
   }
   h->remedy = on != 0;
+  return AM_OK;
+}
+
+int am_sweep_set_track_changes(am_sweep_t* h, int on) {
+  if (!h) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if ((on != 0) == h->track) return AM_OK;
+  h->chg_listed = h->chg_fetched = false;
+  if (on) {  // 4.125 B per slot of capacity at the first enable; every enable starts from the flags as they stand
+    int rc = set_stream(h, h->stream);
+    if (rc != AM_OK) return rc;
+    if (!h->chg_acc) {  // (the last of them: an enable that failed half-way allocates again)
+      const size_t ngroups = groups_of(h->cap_padded);
+      AM_CUDA(h, dev_array(h, &h->chg_bits, ngroups * kGroupWords * 4, h->stream));
+      AM_CUDA(h, dev_array(h, &h->chg_list, h->cap_padded * 4, h->stream, false));
+      AM_CUDA(h, dev_array(h, &h->chg_group, ngroups * 4, h->stream));
+      AM_CUDA(h, dev_array(h, &h->chg_prefix, (ngroups + 1) * 4, h->stream));
+      AM_CUDA(h, dev_array(h, &h->chg_acc, kNumAcc * 8, h->stream));
+    }
+    rc = seed_changes(h, h->stream, 0, h->cap_padded);
+    if (rc != AM_OK) return rc;
+  }
+  h->track = on != 0;
   return AM_OK;
 }
 
@@ -1333,6 +1420,7 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
   int rc = set_stream(h, h->stream);
   if (rc != AM_OK) return rc;
   h->to_ran = false;  // (ticks: the timed-out list is reset; with the hold off nothing times out)
+  h->chg_listed = h->chg_fetched = false;  // (and the list of status changes: a run's ticks are not tracked)
   // A blocked run publishes no tick's accumulators: its drain leaves posted results pending in the flags,
   // and the block kernel applies them at its first tick (and counts them in that tick's row).
   rc = drain_staged(h, h->stream, (mode & AM_SWEEP_BLOCKED) ? nullptr : &unix_sec0);
@@ -1396,6 +1484,10 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
     if (rc == AM_OK) { h->has_prev = true; h->prev_T = unix_sec0 + (int64_t)n_ticks - 1; }
   }
   cudaFree(d_stats);
+  if (h->track) {  // the run applied what its drain noted: start again from the flags
+    const int rs = seed_changes(h, h->stream, 0, h->cap_padded);
+    if (rc == AM_OK) rc = rs;
+  }
   return rc;
 }
 
@@ -1564,6 +1656,65 @@ int am_sweep_last_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64
 int am_sweep_last_remedy_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t* started, uint64_t cap,
                                    uint64_t* n_out) {
   return timed_out_impl(h, offset, idx, started, cap, n_out, true);
+}
+
+int am_sweep_last_changes(am_sweep_t* h, uint64_t offset, uint64_t* idx, am_record_cols_t* cols, uint64_t cap,
+                          uint64_t* n_out) {
+  if (!h || (cap && !idx)) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if (!h->track) {
+    h->last_error = "am_sweep_last_changes while tracking is off";
+    return AM_E_INVAL;
+  }
+  int rc = set_stream(h, h->stream);  // (after the last tick, on whatever stream it ran; staged calls are not drained)
+  if (rc != AM_OK) return rc;
+  if (h->chg_listed && !h->chg_fetched) {
+    AM_CUDA(h, h->pin_in.reserve(8));
+    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->chg_acc + 1, 8, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    h->chg_n = *(const unsigned long long*)h->pin_in.p;
+    h->chg_fetched = true;
+  }
+  const uint64_t n = h->chg_listed ? h->chg_n : 0;
+  if (offset > n) return AM_E_RANGE;
+  const uint64_t left = n - offset, ncopy = left < cap ? left : cap;
+  if (n_out) *n_out = left;
+  if (ncopy) {
+    // pin_in / dev_in: the list's entries, then each requested column (8-B aligned), gathered on the device
+    GatherCols gc{};
+    size_t at[16], bytes = (ncopy * 4 + 7) / 8 * 8;
+    unsigned nc = 0;
+    for (int k = 0; k < 16; ++k) {
+      if (!cols || !*cols_member(cols, k)) continue;
+      at[nc] = bytes;
+      gc.src[nc] = *col_slot(h->cols, k);
+      gc.elem[nc] = (uint32_t)kColElem[k];
+      bytes += (ncopy * kColElem[k] + 7) / 8 * 8;
+      ++nc;
+    }
+    AM_CUDA(h, h->pin_in.reserve(bytes));
+    AM_CUDA(h, h->dev_in.reserve(bytes));
+    const uint32_t* d_idx = h->chg_list + offset;
+    for (unsigned c = 0; c < nc; ++c) gc.dst[c] = (char*)h->dev_in.p + at[c];
+    if (nc) {
+      AM_LAUNCH(gather_columns_kernel, dim3((unsigned)((ncopy + 255) / 256), nc), 256, h->stream, gc, d_idx, (uint32_t)ncopy);
+      h->launches++;
+      AM_CUDA(h, cudaGetLastError());
+      AM_CUDA(h, cudaMemcpyAsync((char*)h->pin_in.p + at[0], (char*)h->dev_in.p + at[0], bytes - at[0],
+                                 cudaMemcpyDeviceToHost, h->stream));
+    }
+    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, d_idx, ncopy * 4, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    const uint32_t* li = (const uint32_t*)h->pin_in.p;
+    for (uint64_t k = 0; k < ncopy; ++k) idx[k] = h->shard_base + li[k];
+    for (int k = 0, c = 0; k < 16; ++k) {
+      void* dst = cols ? *cols_member(cols, k) : nullptr;
+      if (!dst) continue;
+      memcpy(dst, (const char*)h->pin_in.p + at[c++], ncopy * kColElem[k]);
+    }
+  }
+  return left > cap ? AM_E_NOSPACE : AM_OK;
 }
 
 // (tick guard held, staged events drained, h->stream ordered)

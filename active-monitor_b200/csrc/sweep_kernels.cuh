@@ -1463,6 +1463,166 @@ __global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ op
   marks[3u * i + 2u] = 0;
 }
 
+// ---- status changes (am_sweep_set_track_changes) --------------------------------------------------------------
+// The handle keeps one bit per slot, bit i & 31 of word i / 32: "the coming tick changes this slot's columns".  Drains
+// add to it (a read's drain too: the results it leaves pending belong to the next tick), the tick adds and removes what
+// only the sweep decides, and after the sweep the bits are compacted into the tick's ascending slot list and cleared.
+// A set bit whose slot is not live when the list is built is dropped: the result kernels and the sweep apply nothing to
+// such a slot, and nothing between the drain and the list changes a kind or a tombstone.
+constexpr uint32_t kPendBits = AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING;
+
+// A drain's staged ops, after apply_state_ops_kernel and before anything applies a result.  One thread per slot decides
+// (the marks' rules, as in apply_results_now_kernel): the slot's latest upsert / remove, else its workflow-phase winner,
+// else its remedy-phase winner.  With an upsert or remove the bit is set exactly when a phase posted after it survives
+// or the upserted record itself carries pending results; an older bit (a read's drain left a result pending) goes, as
+// the state op overwrote that result.  Without one, a surviving phase sets the bit.
+__global__ void note_ops_kernel(uint32_t* bits, const uint32_t* __restrict__ flags, const uint32_t* __restrict__ marks,
+                                const uint2* __restrict__ ops, uint32_t n) {
+  pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t i = ops[k].x;
+  const uint32_t s_state = marks[3u * i], hcw = marks[3u * i + 1u], rmw = marks[3u * i + 2u];
+  const bool hc_valid = hcw != 0u && hcw >= s_state, rm_valid = rmw != 0u && rmw >= s_state;
+  uint32_t* w = bits + i / 32u;
+  const uint32_t b = 1u << (i & 31u);
+  if (s_state) {
+    if (s_state != k + 1u) return;
+    if (hc_valid || rm_valid || (flags[i] & kPendBits)) atomicOr(w, b);
+    else atomicAnd(w, ~b);
+  } else if (hcw == k + 1u || (rmw == k + 1u && !hc_valid)) {
+    atomicOr(w, b);
+  }
+}
+
+// The slots of a device list of *count entries (the expiry pass's timed-out runs, each given a pending Failed): set.
+// Grid-stride: the count is known on the device only.
+__global__ void note_slots_kernel(uint32_t* bits, const uint32_t* __restrict__ idx, const uint32_t* __restrict__ count) {
+  pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
+  const uint32_t n = *count;
+  for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
+    atomicOr(bits + idx[k] / 32u, 1u << (idx[k] & 31u));
+}
+
+// The bits of slots [first, first + n) from their flags alone: set where a live record carries a pending result.  Turning
+// tracking on (every slot) and am_sweep_load_range (its range) start from here.  One thread per word; the partial words
+// at either end keep their other bits.
+__global__ void seed_changes_kernel(uint32_t* bits, const uint32_t* __restrict__ flags, uint64_t first, uint64_t n) {
+  const uint64_t w0 = first / 32u, w1 = (first + n + 31u) / 32u;
+  for (uint64_t w = w0 + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < w1; w += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t in = 0, v = 0;
+    for (uint32_t b = 0; b < 32u; ++b) {
+      const uint64_t i = w * 32u + b;
+      if (i < first || i >= first + n) continue;
+      in |= 1u << b;
+      const uint32_t f = flags[i];
+      if (is_live(f) && (f & kPendBits)) v |= 1u << b;
+    }
+    if (in == kFull) {
+      bits[w] = v;
+    } else {
+      atomicAnd(bits + w, ~in);
+      atomicOr(bits + w, v);
+    }
+  }
+}
+
+// After the sweep, one warp per tile, over the tile's exceptions (the non-default actions it emitted): a record reported
+// STOPPED is in (finishedAt = T and STOPPED_REPORTED); otherwise one whose result came out AM_ACT_ANOMALY is out (the
+// reference panics at hcc.go:690 before it writes a status, DESIGN.md section 6 item 5).  `closed` (closed loop): every
+// record emitted with SUBMIT_HC completed in this tick, so the tile's emitted bits are OR-ed in first (lane L: word L),
+// and an exception without SUBMIT_HC keeps the bit it had before (a result, if any, set it at the drain).
+__global__ void note_exceptions_kernel(uint32_t* bits, const TickOut out, uint32_t n_tiles, bool closed) {
+  __shared__ uint32_t s_before[kWarps][kTileWords];
+  pdl_wait();  // (launched with programmatic stream serialisation: the sweep writes the exceptions)
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t tile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (tile >= n_tiles) return;  // warp-uniform
+  uint32_t* w = bits + (size_t)tile * kTileWords;
+  if (closed) {
+    const uint32_t before = w[lane];
+    s_before[warp][lane] = before;
+    w[lane] = before | out.bitmap[(size_t)tile * kTileWords + lane];
+  }
+  __syncwarp();
+  const uint32_t ne = out.tile_exc[tile];
+  for (uint32_t e = (uint32_t)lane; e < ne; e += 32u) {
+    const uint32_t x = out.exc_seg[(size_t)tile * kTile + e];
+    const uint32_t off = x >> 8, a = x & 0xFFu, b = 1u << (off & 31u);
+    if (a & AM_ACT_STOPPED) atomicOr(w + off / 32u, b);
+    else if ((a & AM_ACT_ANOMALY) || (closed && !(a & AM_ACT_SUBMIT_HC) && !(s_before[warp][off / 32u] & b)))
+      atomicAnd(w + off / 32u, ~b);
+  }
+}
+
+// The list, in two passes of one CTA per 8192-slot group (thread t: word t of the group) around scan_groups_kernel.
+// Counting drops the bits of slots that are not live; listing writes the group's slots at its offset, ascending, and
+// clears the words.  Groups with nothing listed are not read twice.
+__global__ void __launch_bounds__(kGroupWords) count_changes_kernel(uint32_t* bits, const uint32_t* __restrict__ flags,
+                                                                    uint32_t* group_count) {
+  __shared__ uint32_t s_warp[kGroupWords / 32];
+  pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t wi = (size_t)blockIdx.x * kGroupWords + threadIdx.x;
+  uint32_t v = bits[wi];
+  if (v) {
+    uint32_t keep = v;
+    for (uint32_t m = v; m; m &= m - 1u) {
+      const uint32_t b = (uint32_t)__ffs((int)m) - 1u;
+      if (!is_live(flags[wi * 32u + b])) keep &= ~(1u << b);
+    }
+    if (keep != v) bits[wi] = keep;
+    v = keep;
+  }
+  const uint32_t c = __reduce_add_sync(kFull, (uint32_t)__popc(v));
+  if (lane == 0) s_warp[warp] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t t = 0;
+    for (uint32_t k = 0; k < kGroupWords / 32u; ++k) t += s_warp[k];
+    group_count[blockIdx.x] = t;
+  }
+}
+
+__global__ void __launch_bounds__(kGroupWords) list_changes_kernel(uint32_t* bits, const uint32_t* __restrict__ group_prefix,
+                                                                   uint32_t* list) {
+  __shared__ uint32_t s_warp[kGroupWords / 32];
+  pdl_wait();  // (launched with programmatic stream serialisation: scan_groups_kernel writes the offsets)
+  const uint32_t g = blockIdx.x;
+  const uint32_t base = group_prefix[g];
+  if (group_prefix[g + 1u] == base) return;  // block-uniform
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t wi = (size_t)g * kGroupWords + threadIdx.x;
+  const uint32_t v = bits[wi];
+  const uint32_t c = (uint32_t)__popc(v);
+  uint32_t incl = c;
+#pragma unroll
+  for (unsigned d = 1; d < 32; d <<= 1) {
+    const uint32_t up = __shfl_up_sync(kFull, incl, d);
+    if ((unsigned)lane >= d) incl += up;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  uint32_t pos = base + incl - c;
+  for (int k = 0; k < warp; ++k) pos += s_warp[k];
+  for (uint32_t m = v; m; m &= m - 1u) list[pos++] = (uint32_t)(wi * 32u) + (uint32_t)__ffs((int)m) - 1u;
+  if (v) bits[wi] = 0;
+}
+
+// am_sweep_last_changes: the requested columns of the listed slots idx[0..n), column-major into dst[c] (blockIdx.y = c).
+struct GatherCols {
+  const void* src[16];
+  void* dst[16];
+  uint32_t elem[16];  // 4 or 8 bytes
+};
+__global__ void gather_columns_kernel(const GatherCols g, const uint32_t* __restrict__ idx, uint32_t n) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t c = blockIdx.y, i = idx[k];
+  if (g.elem[c] == 8u) ((uint64_t*)g.dst[c])[k] = ((const uint64_t*)g.src[c])[i];
+  else ((uint32_t*)g.dst[c])[k] = ((const uint32_t*)g.src[c])[i];
+}
+
 __global__ void gather_records_kernel(DevCols c, const uint32_t* __restrict__ idx, am_record_t* out,
                                       uint32_t n) {
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;

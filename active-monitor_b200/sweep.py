@@ -377,6 +377,31 @@ class Sweep:
         start i64), as last_timed_out"""
         return self._timed_out("am_sweep_last_remedy_timed_out", offset, cap)
 
+    # -- status changes
+    def set_track_changes(self, on: bool):
+        """record every tick's changed set, the checks whose status to write back (am_sweep_set_track_changes)"""
+        self._check(self._lib.am_sweep_set_track_changes(self._h, int(bool(on))), "am_sweep_set_track_changes")
+
+    def last_changes(self, offset: int = 0, cap: int | None = None, names=None):
+        """the slots the last tick changed (am_sweep_last_changes) from entry `offset` on: (global idx u64, cols dict)
+        with the columns `names` (None: all sixteen) of those slots as they stand.  cap None: all of them."""
+        n = L.u64(0)
+        fn = "am_sweep_last_changes"
+        if cap is None:
+            rc = self._lib.am_sweep_last_changes(self._h, offset, None, None, 0, C.byref(n))
+            if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+                self._check(rc, fn)
+            cap = int(n.value)
+        idx = np.empty(cap, dtype=np.uint64)
+        cols = {name: np.empty(cap, dtype=dt) for name, dt in L.COLUMNS if names is None or name in names}
+        cs = cols_struct(cols)
+        rc = self._lib.am_sweep_last_changes(self._h, offset, idx.ctypes.data if cap else None, C.byref(cs), cap,
+                                             C.byref(n))
+        if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+            self._check(rc, fn)
+        k = min(int(n.value), cap)
+        return idx[:k], {name: a[:k] for name, a in cols.items()}
+
     # -- introspection
     def set_seed(self, seed: int):
         self._check(self._lib.am_sweep_set_seed(self._h, seed), "am_sweep_set_seed")

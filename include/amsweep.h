@@ -494,6 +494,42 @@ int am_sweep_last_timed_out(am_sweep_t*, uint64_t offset, uint64_t* idx, int64_t
  * hcc.go:609/638/665), which the caller can write back with the result. */
 int am_sweep_in_flight(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out);
 
+/* Status changes: which checks need their status written back after a tick (the reference writes
+ * the status subresource after every phase it applies, updateHealthCheckStatus, hcc.go:734 and
+ * :1445-1462).  Off by default.  While on, every tick of every entry point (am_sweep_tick,
+ * _tick_view, _tick_device, _tick_shard and so am_gather_exchange / am_gather_tick_view) records
+ * its CHANGED SET: the slots whose columns, as am_sweep_read returns them, the tick changed, not
+ * counting the library-internal bits AM_F_CARRY_MASK and the posted-result bits AM_F_PENDING_* /
+ * AM_F_REMEDY_* the tick consumes.  That is every live record to which the tick applied a
+ * workflow result (a posted Succeeded / Failed, a workflow timeout's Failed, a closed-loop
+ * completion) or a remedy result (a posted remedy phase, a remedy timeout, an attached outcome),
+ * except those whose result the tick reported AM_ACT_ANOMALY (the reference writes no status for
+ * them, DESIGN.md section 6 item 5), and every record the tick reported AM_ACT_STOPPED.  Results
+ * resolve in the per-slot call order: one superseded by a later upsert or remove is not listed, and
+ * one a read's drain left pending belongs to the next tick that applies it.  Upserts, removes,
+ * loads, submissions and the holds' bookkeeping are never listed by themselves.  The list is reset
+ * by every tick that reaches its drain (a refused tick leaves it; an AM_E_NOSPACE tick records it
+ * as usual).  am_sweep_run_ticks does not track its ticks: it empties the list, and the next tick
+ * lists only what it changes itself.
+ * Turning it on allocates 4.125 B per slot of capacity on the device at the first such call (none
+ * for a handle that never turns it on); the first tick after it starts a fresh set.  Turning it off
+ * frees nothing; a handle with it off launches nothing for it. */
+int am_sweep_set_track_changes(am_sweep_t*, int on);
+
+/* The last tick's changed set (am_sweep_set_track_changes), ascending by global index, from entry
+ * `offset` on: idx[k] the global index and, for every non-NULL column of `cols` (cols itself may be
+ * NULL), element k the slot's value, gathered on the device (NULL columns are not read, as in
+ * am_sweep_read: fetch only what a status write needs).  *n_out = entries from `offset` to the end;
+ * AM_E_NOSPACE if they exceed cap (the first cap entries are valid); AM_E_RANGE when offset is past
+ * the end; AM_E_INVAL while tracking is off.  After am_sweep_tick_device / am_sweep_tick_shard the
+ * call waits for that tick to finish.  It does NOT drain staged calls: the values are the columns
+ * as they stand, which are the tick's results unless a call that drains (am_sweep_read,
+ * am_sweep_in_flight, am_sweep_next_due, am_sweep_load_range, ...) has applied upserts staged since
+ * the tick.  A run's StartedAt is not here: the caller has it from am_work_item_t.unix_sec and the
+ * timed-out lists. */
+int am_sweep_last_changes(am_sweep_t*, uint64_t offset, uint64_t* idx, am_record_cols_t* cols, uint64_t cap,
+                          uint64_t* n_out);
+
 /* Introspection */
 uint64_t am_sweep_size(const am_sweep_t*);     /* high-water mark (slots swept) */
 uint64_t am_sweep_capacity(const am_sweep_t*);
