@@ -1511,9 +1511,9 @@ int am_sweep_repeat_after_sec(am_sweep_t* h, int64_t unix_sec, uint64_t first, u
   AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * 8, cudaMemcpyDeviceToHost, h->stream));
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   memcpy(out, h->pin_in.p, n * 8);
-  {  // schedules bound to a named time zone (marked -1, never a real value): Next() on the host
+  {  // schedules bound to a named time zone (marked kZoneBoundMark): Next() on the host
     std::vector<uint64_t> zi;
-    for (uint64_t k = 0; k < n; ++k) if (out[k] == -1) zi.push_back(first + k);
+    for (uint64_t k = 0; k < n; ++k) if (out[k] == kZoneBoundMark) zi.push_back(first + k);
     if (!zi.empty()) {
       std::vector<uint64_t> mi(zi.size()), hr(zi.size()), dm(zi.size()), mo(zi.size()), dw(zi.size());
       std::vector<uint32_t> fl(zi.size());

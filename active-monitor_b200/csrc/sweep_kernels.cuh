@@ -1051,6 +1051,11 @@ __global__ void fill_u32_kernel(uint32_t* p, uint32_t v, uint64_t n) {
 // "@every d" and interval checks the stored interval, 0 for everything else.  One
 // thread per record; the day scan diverges, which is fine for an on-demand query
 // (status display, timer-wheel bucketing) that is not part of the per-tick path.
+// A schedule bound to a named time zone is written as kZoneBoundMark: the host evaluates its Next()
+// (am_cron_next).  No answer takes that value: a 5-field schedule's is > 0 or -9223372035 (|T| < 2^55),
+// an interval's is an i32, whatever its sign.
+constexpr int64_t kZoneBoundMark = INT64_MIN;
+
 __global__ void next_fire_kernel(DevCols c, uint32_t first, uint32_t n, int64_t T, int64_t* out) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
@@ -1060,7 +1065,7 @@ __global__ void next_fire_kernel(DevCols c, uint32_t first, uint32_t n, int64_t 
   int64_t v = 0;
   if (!(f & AM_F_TOMBSTONE)) {
     if (kind == AM_KIND_CRON_SPEC && (f >> AM_F_TZ_SHIFT) != 0)
-      v = -1;  // bound to a named time zone: the host evaluates Next() (am_cron_next), marked here
+      v = kZoneBoundMark;
     else if (kind == AM_KIND_CRON_SPEC)
       v = repeat_after_from_next(cron_next_utc(c.minute[i], c.hour[i], c.dom[i], c.month[i], c.dow[i], T), T);
     else if (kind == AM_KIND_INTERVAL || kind == AM_KIND_CRON_EVERY)

@@ -374,8 +374,8 @@ int am_sweep_run_ticks(am_sweep_t*, int64_t unix_sec0, uint64_t n_ticks, uint32_
 /* RepeatAfterSec of records [first, first+n) as the reference derives it at
  * reconcile time (hcc.go:259-262): Next(unix_sec) - unix_sec for a 5-field
  * schedule (robfig SpecSchedule.Next evaluated on the device; -9223372035 when
- * nothing fires within five years), the stored interval for "@every"/interval
- * checks, 0 otherwise.  On-demand query, not part of the per-tick path. */
+ * nothing fires within five years), the stored interval (whatever its sign) for
+ * "@every"/interval checks, 0 otherwise.  On-demand query, not part of the per-tick path. */
 int am_sweep_repeat_after_sec(am_sweep_t*, int64_t unix_sec, uint64_t first, uint64_t n, int64_t* out);
 
 /* The earliest second after unix_sec at which a tick of this shard would emit anything or time a
