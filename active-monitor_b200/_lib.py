@@ -34,6 +34,10 @@ F_TZ_SHIFT = 24
 
 ACT_SUBMIT_HC, ACT_RUN_REMEDY, ACT_STOPPED, ACT_PARSE_ERROR = 0x01, 0x02, 0x04, 0x08
 ACT_REMEDY_SKIP, ACT_RESET_ON_PASS, ACT_RESET_ON_INTERVAL, ACT_ANOMALY = 0x10, 0x20, 0x40, 0x80
+CHG_SUCCEEDED, CHG_FAILED, CHG_TIMED_OUT, CHG_REMEDY_SUCCEEDED = 0x01, 0x02, 0x04, 0x08
+CHG_REMEDY_FAILED, CHG_REMEDY_TIMED_OUT, CHG_STOPPED, CHG_CLOSED_LOOP = 0x10, 0x20, 0x40, 0x80
+# am_change_detail_t
+CHANGE_DETAIL = np.dtype([("started", "<i8"), ("remedy_started", "<i8"), ("applied", "<u4"), ("action", "<u4")])
 
 SWEEP_CLOSED_LOOP, SWEEP_FULL_SCAN, SWEEP_BLOCKED, SWEEP_CATCH_UP = 0x1, 0x2, 0x4, 0x8
 PHASE_NONE, PHASE_SUCCEEDED, PHASE_FAILED = 0, 1, 2
@@ -152,6 +156,8 @@ SYMBOLS = {
     "am_sweep_last_remedy_timed_out": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
     "am_sweep_set_track_changes": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_last_changes": (C.c_int, [C.c_void_p, u64, C.c_void_p, P(AmRecordCols), u64, P(u64)]),
+    "am_sweep_set_change_details": (C.c_int, [C.c_void_p, C.c_int]),
+    "am_sweep_last_change_details": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
     "am_sweep_size": (u64, [C.c_void_p]),
     "am_sweep_capacity": (u64, [C.c_void_p]),
     "am_sweep_device": (C.c_int, [C.c_void_p]),

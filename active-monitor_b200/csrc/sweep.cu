@@ -214,6 +214,19 @@ struct am_sweep {
   bool chg_listed = false;   // the last tick built its list on the device
   bool chg_fetched = false;  // ... and its length has been read into chg_n
   uint64_t chg_n = 0;
+  // change details (am_sweep_set_change_details, only with tracking), allocated at the first enable: per slot the
+  // AM_CHG_* bits and the run start a pass captured ([cap_padded] each, meaningful while the slot's bit is set), the
+  // same of the last tick's list by entry, and the tick the list belongs to (its buffer set, second and closed-loop
+  // mode) for the action bytes
+  bool details = false;
+  uint8_t* det_applied = nullptr;
+  int64_t* det_start = nullptr;
+  uint8_t* det_e_applied = nullptr;  // ... and the pairs of the last tick's list, by entry ([cap_padded] each)
+  int64_t* det_e_start = nullptr;
+  int chg_parity = 0;
+  int64_t chg_T = 0;
+  bool chg_closed = false;
+  bool det_listed = false;  // the last list was built with details on (a list from before they were on has none)
   std::string last_error;
   uint64_t launches = 0;
   double last_ms = -1.0;
@@ -450,6 +463,11 @@ int expire_runs(am_sweep* h, cudaStream_t s, int64_t T) {
     AM_LAUNCH_PDL(expire_runs_kernel, (unsigned)((n_seg + 255) / 256), 256, s, h->cols, h->since, h->deadline,
                   h->seg_deadline, (uint32_t)n_seg, T, h->to_idx, h->to_since, h->to_count);
     h->launches++;
+    if (h->details) {  // (before note_slots_kernel: a clear bit means the slot's pair is stale)
+      AM_LAUNCH_PDL(capture_timeouts_kernel, h->sms, 256, s, h->det_applied, h->det_start, (const uint32_t*)h->chg_bits,
+                    (const uint32_t*)h->to_idx, (const int64_t*)h->to_since, (const uint32_t*)h->to_count);
+      h->launches++;
+    }
     if (h->track) {  // status changes: every timed-out run gets its Failed applied by this tick
       AM_LAUNCH_PDL(note_slots_kernel, h->sms, 256, s, h->chg_bits, (const uint32_t*)h->to_idx, (const uint32_t*)h->to_count);
       h->launches++;
@@ -464,6 +482,10 @@ int expire_runs(am_sweep* h, cudaStream_t s, int64_t T) {
 int seed_changes(am_sweep* h, cudaStream_t s, uint64_t first, uint64_t n) {
   AM_LAUNCH(seed_changes_kernel, h->sms * 8, 256, s, h->chg_bits, (const uint32_t*)h->cols.flags, first, n);
   h->launches++;
+  if (h->details) {
+    AM_LAUNCH(seed_details_kernel, h->sms * 8, 256, s, h->det_applied, h->det_start, (const uint32_t*)h->cols.flags, first, n);
+    h->launches++;
+  }
   AM_CUDA(h, cudaGetLastError());
   return AM_OK;
 }
@@ -471,10 +493,19 @@ int seed_changes(am_sweep* h, cudaStream_t s, uint64_t first, uint64_t n) {
 // Status changes after a tick's sweep (buffer set `parity`): STOPPED in, ANOMALY out (and in closed loop every completed
 // submission in), then the bits compacted into the ascending list, which clears them.  A host tick launches this behind
 // the event it waits for: am_sweep_last_changes waits for it.
-int list_changes(am_sweep* h, cudaStream_t s, int parity, bool closed) {
+int list_changes(am_sweep* h, cudaStream_t s, int parity, bool closed, int64_t T) {
+  h->chg_parity = parity;
+  h->chg_T = T;
+  h->chg_closed = closed;
+  h->det_listed = h->details;
   if (h->n_records == 0) return AM_OK;  // (nothing swept: the list stays empty)
   const TickSet& ts = h->set[parity];
   const uint32_t n_tiles = tiles_of(h->n_records), n_groups = groups_of(h->n_records);
+  if (h->details) {
+    AM_LAUNCH_PDL(capture_sweep_kernel, (n_tiles + kWarps - 1) / kWarps, kBlock, s, h->det_applied, h->det_start,
+                  (const uint32_t*)h->chg_bits, ts.out, n_tiles, closed);
+    h->launches++;
+  }
   AM_LAUNCH_PDL(note_exceptions_kernel, (n_tiles + kWarps - 1) / kWarps, kBlock, s, h->chg_bits, ts.out, n_tiles, closed);
   AM_LAUNCH_PDL(count_changes_kernel, n_groups, kGroupWords, s, h->chg_bits, (const uint32_t*)h->cols.flags, h->chg_group);
   ScanParams sc{};
@@ -486,6 +517,12 @@ int list_changes(am_sweep* h, cudaStream_t s, int parity, bool closed) {
   AM_LAUNCH_PDL(scan_groups_kernel, 1, 1024, s, sc);
   AM_LAUNCH_PDL(list_changes_kernel, n_groups, kGroupWords, s, h->chg_bits, (const uint32_t*)h->chg_prefix, h->chg_list);
   h->launches += 4;
+  if (h->details) {
+    AM_LAUNCH_PDL(snapshot_details_kernel, h->sms * 4, 256, s, (const uint32_t*)h->chg_list,
+                  (const unsigned long long*)(h->chg_acc + 1), (const uint8_t*)h->det_applied, (const int64_t*)h->det_start,
+                  h->det_e_applied, h->det_e_start);
+    h->launches++;
+  }
   AM_CUDA(h, cudaGetLastError());
   h->chg_listed = true;
   return AM_OK;
@@ -559,6 +596,12 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   if (h->track) {  // status changes: the phases of this drain that survive, and what its upserts and removes overwrote
     AM_LAUNCH_PDL(note_ops_kernel, G, B, s, h->chg_bits, (const uint32_t*)h->cols.flags, h->marks, d_ops, (uint32_t)n);
     h->launches++;
+  }
+  if (h->details) {  // change details: what the surviving phases apply and the runs they end (since not yet cleared)
+    AM_LAUNCH_PDL(capture_ops_kernel, G, B, s, h->det_applied, h->det_start, h->cols,
+                  (const int64_t*)(h->hold ? h->since : nullptr), (const uint32_t*)h->marks, d_ops, (uint32_t)n);
+    AM_LAUNCH_PDL(capture_superseded_kernel, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n);
+    h->launches += 2;
   }
   if (st->any_wf && !h->wf_timeout) {
     const int rc = alloc_timeouts(h, s);
@@ -916,7 +959,7 @@ int run_tick(am_sweep* h, int64_t T, uint32_t mode, cudaStream_t s, TickKind kin
     if (rc != AM_OK) return rc;
   }
   if (h->track) {  // (a host tick: behind that event as well)
-    rc = list_changes(h, s, parity, (mode & AM_SWEEP_CLOSED_LOOP) != 0);
+    rc = list_changes(h, s, parity, (mode & AM_SWEEP_CLOSED_LOOP) != 0, T);
     if (rc != AM_OK) return rc;
   }
   if (host) {  // one synchronisation
@@ -1217,6 +1260,34 @@ int am_sweep_set_track_changes(am_sweep_t* h, int on) {
     if (rc != AM_OK) return rc;
   }
   h->track = on != 0;
+  if (!on) h->details = false;
+  return AM_OK;
+}
+
+int am_sweep_set_change_details(am_sweep_t* h, int on) {
+  if (!h) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if (!h->track) {
+    h->last_error = "am_sweep_set_change_details while tracking is off";
+    return AM_E_INVAL;
+  }
+  if ((on != 0) == h->details) return AM_OK;
+  if (on) {  // 18 B per slot of capacity at the first enable; the staged calls first, so that what they post is pending
+    int rc = begin_call(h);
+    if (rc != AM_OK) return rc;
+    if (!h->det_e_start) {  // (the last of them: an enable that failed half-way allocates again)
+      AM_CUDA(h, dev_array(h, &h->det_applied, h->cap_padded, h->stream, false));
+      AM_CUDA(h, dev_array(h, &h->det_start, h->cap_padded * 8, h->stream, false));
+      AM_CUDA(h, dev_array(h, &h->det_e_applied, h->cap_padded, h->stream, false));
+      AM_CUDA(h, dev_array(h, &h->det_e_start, h->cap_padded * 8, h->stream, false));
+    }
+    AM_LAUNCH(seed_details_kernel, h->sms * 8, 256, h->stream, h->det_applied, h->det_start, (const uint32_t*)h->cols.flags,
+              (uint64_t)0, h->cap_padded);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
+  }
+  h->details = on != 0;
   return AM_OK;
 }
 
@@ -1290,12 +1361,15 @@ int am_sweep_post_result(am_sweep_t* h, uint64_t n, const uint64_t* idx, const u
   // validate and stage in vectorised passes of one copy chunk each; a single large post hands every
   // finished chunk to the copy stream before staging the next (when no other call is staging).
   // phase -> flag bits: {none, Succeeded, Failed} -> {0, PENDING_OK, PENDING_FAIL}
+  // Every entry carries the call's tag (its first op index, mod 2^22; capture_superseded_kernel): the entries of one
+  // call see the in-flight state from before the call.
+  const uint32_t kind = kOpResult | (((uint32_t)a << kCallTagShift) & kCallTagMask);
   unsigned bad = 0;
   cudaError_t ce = cudaSuccess;
   for (uint64_t off = 0; off < n && !bad; off += kFlushOps) {
     const uint64_t m = n - off < kFlushOps ? n - off : kFlushOps;
     bad = amsweep_host::stage_results(m, idx + off, phase + off, remedy_phase ? remedy_phase + off : nullptr, h->capacity,
-                                      kOpResult, oo + off);
+                                      kind, oo + off);
     if (!bad && off + m < n) {
       lk.lock();
       if (st.writers == 1 && ce == cudaSuccess && cudaSetDevice(h->device) == cudaSuccess)
@@ -1713,6 +1787,51 @@ int am_sweep_last_changes(am_sweep_t* h, uint64_t offset, uint64_t* idx, am_reco
       if (!dst) continue;
       memcpy(dst, (const char*)h->pin_in.p + at[c++], ncopy * kColElem[k]);
     }
+  }
+  return left > cap ? AM_E_NOSPACE : AM_OK;
+}
+
+int am_sweep_last_change_details(am_sweep_t* h, uint64_t offset, uint64_t* idx, am_change_detail_t* out, uint64_t cap,
+                                 uint64_t* n_out) {
+  if (!h || (cap && (!idx || !out))) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if (!h->details) {
+    h->last_error = "am_sweep_last_change_details while change details are off";
+    return AM_E_INVAL;
+  }
+  int rc = set_stream(h, h->stream);  // (after the last tick, on whatever stream it ran; staged calls are not drained)
+  if (rc != AM_OK) return rc;
+  const bool listed = h->chg_listed && h->det_listed;
+  if (listed && !h->chg_fetched) {
+    AM_CUDA(h, h->pin_in.reserve(8));
+    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->chg_acc + 1, 8, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    h->chg_n = *(const unsigned long long*)h->pin_in.p;
+    h->chg_fetched = true;
+  }
+  const uint64_t n = listed ? h->chg_n : 0;
+  if (offset > n) return AM_E_RANGE;
+  const uint64_t left = n - offset, ncopy = left < cap ? left : cap;
+  if (n_out) *n_out = left;
+  if (ncopy) {
+    // pin_in / dev_in: the details, then the list's entries
+    const size_t at = ncopy * sizeof(am_change_detail_t), bytes = at + ncopy * 4;
+    AM_CUDA(h, h->pin_in.reserve(bytes));
+    AM_CUDA(h, h->dev_in.reserve(bytes));
+    const uint32_t* d_idx = h->chg_list + offset;
+    AM_LAUNCH(gather_details_kernel, (unsigned)((ncopy + 255) / 256), 256, h->stream, d_idx, (uint32_t)ncopy,
+              (const uint8_t*)h->det_e_applied + offset, (const int64_t*)h->det_e_start + offset, h->set[h->chg_parity].out,
+              h->chg_closed,
+              h->chg_T, (am_change_detail_t*)h->dev_in.p);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, at, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaMemcpyAsync((char*)h->pin_in.p + at, d_idx, ncopy * 4, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    memcpy(out, h->pin_in.p, at);
+    const uint32_t* li = (const uint32_t*)((const char*)h->pin_in.p + at);
+    for (uint64_t k = 0; k < ncopy; ++k) idx[k] = h->shard_base + li[k];
   }
   return left > cap ? AM_E_NOSPACE : AM_OK;
 }

@@ -1246,6 +1246,17 @@ __global__ void apply_result_ops_kernel(uint32_t* flags, const uint32_t* __restr
   }
 }
 
+// The posted bits a drain leaves in a slot's flags `f` (the rule above): the winner of the workflow phase and the
+// winner of the remedy phase, each when posted after the slot's latest upsert / remove, replace their own bit groups.
+// A winner's arg is fetched only when it is valid.  apply_results_now_kernel spells the same two lines out with its
+// own winner's arg in hand (calling this there reorders its machine code); capture_ops_kernel calls it.
+template <typename HcArg, typename RmArg>
+__device__ __forceinline__ uint32_t merge_phases(uint32_t f, bool hc_valid, HcArg hc_arg, bool rm_valid, RmArg rm_arg) {
+  if (hc_valid) f = (f & ~kHcBits) | (hc_arg() & kHcBits);
+  if (rm_valid) f = (f & ~kRemedyBits) | (rm_arg() & kRemedyBits);
+  return f;
+}
+
 // Results posted between two ticks, applied while the tick drains them instead of inside its sweep.
 // In the sweep a record with a posted result costs its warp a second, dependent memory round trip
 // (the remedy / counter columns) behind the streaming loads; with a result on ~2 % of the records
@@ -1612,6 +1623,180 @@ __global__ void __launch_bounds__(kGroupWords) list_changes_kernel(uint32_t* bit
   for (int k = 0; k < warp; ++k) pos += s_warp[k];
   for (uint32_t m = v; m; m &= m - 1u) list[pos++] = (uint32_t)(wi * 32u) + (uint32_t)__ffs((int)m) - 1u;
   if (v) bits[wi] = 0;
+}
+
+// ---- change details (am_sweep_set_change_details) -------------------------------------------------------------
+// Per slot, beside the status-change bit: `applied`, the AM_CHG_* bits of the results the coming tick applies, and
+// `start`, the start of the run whose phase it applies as a since word (T, or T + kRemedyRun for a remedy run;
+// kNotInFlight when none).  A slot has at most one run in flight, so one word serves both kinds.  The pair is
+// meaningful exactly while the slot's status-change bit is set: every pass that sets the bit writes the pair first,
+// and a pass that finds the bit clear starts from (0, kNotInFlight).  Nothing clears them after a tick: the tick
+// copies the pairs of its list, by entry, into a second pair of arrays (snapshot_details_kernel).
+// A result op carries its post call's tag in arg bits 8..29 (am_sweep_post_result: the call's first op index, mod
+// 2^22), which no other kernel reads: two entries of one call see the same in-flight state, as they do in call order.
+constexpr uint32_t kCallTagShift = 8, kCallTagMask = 0x3FFFFFu << kCallTagShift;
+static_assert((kCallTagMask & (kOpKindMask | AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING |
+                               AM_F_REMEDY_OUTCOME_OK)) == 0, "call tag bits");
+
+// The AM_CHG_* bits of a flags word's posted-result bits.
+__device__ __forceinline__ uint32_t applied_of(uint32_t f) {
+  return ((f & AM_F_PENDING_OK) ? AM_CHG_SUCCEEDED : 0u) | ((f & AM_F_PENDING_FAIL) ? AM_CHG_FAILED : 0u) |
+         ((f & AM_F_REMEDY_PENDING) ? ((f & AM_F_REMEDY_OUTCOME_OK) ? AM_CHG_REMEDY_SUCCEEDED : AM_CHG_REMEDY_FAILED) : 0u);
+}
+
+// A drain's ops, after apply_state_ops_kernel and before clear_since_kernel and the result kernels (the flags hold the
+// already-pending bits, since the in-flight state before the drain).  The slot's owner (note_ops_kernel's: its latest
+// upsert / remove, else its workflow-phase winner, else its remedy-phase winner) writes the pair: applied from the
+// posted bits the drain leaves (merge_phases, the result kernels' rule); start from the held run (in_flight_kernel's
+// rule) when a winner of its kind ends it, else an earlier drain's capture whose phase is still pending and not
+// replaced.  A state op drops the earlier capture (the record's own pending bits report no start).  `since` NULL:
+// the hold is off.  capture_superseded_kernel then drops a capture that an earlier call of the drain ended first.
+__global__ void capture_ops_kernel(uint8_t* applied, int64_t* start, const DevCols c, const int64_t* __restrict__ since,
+                                   const uint32_t* __restrict__ marks, const uint2* __restrict__ ops, uint32_t n) {
+  pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t i = ops[k].x;
+  const uint32_t s_state = marks[3u * i], hcw = marks[3u * i + 1u], rmw = marks[3u * i + 2u];
+  const bool hc_valid = hcw != 0u && hcw >= s_state, rm_valid = rmw != 0u && rmw >= s_state;
+  if (s_state ? s_state != k + 1u : !(hcw == k + 1u || (rmw == k + 1u && !hc_valid))) return;
+  const uint32_t f = c.flags[i];
+  const uint32_t fm = merge_phases(f, hc_valid, [&] { return ops[hcw - 1u].y; }, rm_valid, [&] { return ops[rmw - 1u].y; });
+  int64_t w = kNotInFlight;
+  if (!s_state) {
+    const int64_t old = start[i];
+    const bool rem = is_remedy_run(old);
+    if (old != kNotInFlight && !(rem ? rm_valid : hc_valid) && (f & (rem ? AM_F_REMEDY_PENDING : kHcBits))) w = old;
+  }
+  if (since) {
+    const int64_t s = since[i];
+    if (s != kNotInFlight && s >= c.finished_at[i] && !(f & kHcBits) && (is_remedy_run(s) ? rm_valid : hc_valid)) w = s;
+  }
+  start[i] = w;
+  applied[i] = (uint8_t)applied_of(fm);
+}
+
+// After capture_ops_kernel, one thread per op: an op that ended the captured run before the winner's call did (a
+// remove; a workflow phase; for a remedy run any phase) leaves the winner's call nothing in flight.
+__global__ void capture_superseded_kernel(int64_t* start, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops,
+                                          uint32_t n) {
+  pdl_wait();  // (launched with programmatic stream serialisation: capture_ops_kernel writes start)
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint2 op = ops[k];
+  const uint32_t i = op.x, arg = op.y, kind = arg & kOpKindMask;
+  if (kind == kOpUpsert) return;
+  const int64_t w = start[i];
+  if (w == kNotInFlight) return;
+  const bool rem = is_remedy_run(w);
+  const uint32_t win = marks[3u * i + (rem ? 2u : 1u)];
+  if (k + 1u >= win) return;  // (win == 0: an earlier drain's capture, which this drain does not replace)
+  if (kind == kOpResult) {
+    if (!((arg & kHcBits) || (rem && (arg & AM_F_REMEDY_PENDING)))) return;
+    if (((arg ^ ops[win - 1u].y) & kCallTagMask) == 0u) return;  // an entry of the winner's own call
+  }
+  start[i] = kNotInFlight;
+}
+
+// The expiry pass's timed-out runs (before note_slots_kernel sets their bits): the timeout's Failed and its run's start.
+__global__ void capture_timeouts_kernel(uint8_t* applied, int64_t* start, const uint32_t* __restrict__ bits,
+                                        const uint32_t* __restrict__ idx, const int64_t* __restrict__ since,
+                                        const uint32_t* __restrict__ count) {
+  pdl_wait();  // (launched with programmatic stream serialisation: expire_runs_kernel writes the list)
+  const uint32_t n = *count;
+  for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
+    const uint32_t i = idx[k];
+    const int64_t s = since[k];
+    const uint32_t before = ((bits[i / 32u] >> (i & 31u)) & 1u) ? applied[i] : 0u;
+    applied[i] = (uint8_t)(before | (is_remedy_run(s) ? AM_CHG_REMEDY_FAILED | AM_CHG_REMEDY_TIMED_OUT
+                                                      : AM_CHG_FAILED | AM_CHG_TIMED_OUT));
+    start[i] = s;
+  }
+}
+
+// After the sweep, before note_exceptions_kernel, one warp per tile: a slot the sweep alone adds to the list (STOPPED,
+// or in closed loop a completed submission) whose bit is clear starts from (0, kNotInFlight).
+__global__ void capture_sweep_kernel(uint8_t* applied, int64_t* start, const uint32_t* __restrict__ bits, const TickOut out,
+                                     uint32_t n_tiles, bool closed) {
+  pdl_wait();  // (launched with programmatic stream serialisation: the sweep writes the exceptions)
+  const int lane = threadIdx.x & 31;
+  const uint32_t tile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (tile >= n_tiles) return;  // warp-uniform
+  const size_t w0 = (size_t)tile * kTileWords;
+  if (closed) {
+    for (uint32_t m = out.bitmap[w0 + lane] & ~bits[w0 + lane]; m; m &= m - 1u) {
+      const size_t i = (w0 + lane) * 32u + (uint32_t)__ffs((int)m) - 1u;
+      applied[i] = 0;
+      start[i] = kNotInFlight;
+    }
+  }
+  const uint32_t ne = out.tile_exc[tile];
+  for (uint32_t e = (uint32_t)lane; e < ne; e += 32u) {
+    const uint32_t x = out.exc_seg[(size_t)tile * kTile + e];
+    const size_t i = (size_t)tile * kTile + (x >> 8);
+    if ((x & AM_ACT_STOPPED) && !((bits[i / 32u] >> (i & 31u)) & 1u)) {
+      applied[i] = 0;
+      start[i] = kNotInFlight;
+    }
+  }
+}
+
+// Turning details on (every slot), am_sweep_load_range (its range) and the end of am_sweep_run_ticks: the pair from the
+// flags as they stand, with no start (results pending from before report none).
+__global__ void seed_details_kernel(uint8_t* applied, int64_t* start, const uint32_t* __restrict__ flags, uint64_t first,
+                                    uint64_t n) {
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < n; k += (uint64_t)gridDim.x * blockDim.x) {
+    applied[first + k] = (uint8_t)applied_of(flags[first + k]);
+    start[first + k] = kNotInFlight;
+  }
+}
+
+// After list_changes_kernel: the pair of every listed slot, by list entry, so that the drains of later calls (which
+// capture for the next tick) leave the list's details as the tick left them.  Grid-stride: the count is known on the
+// device only.
+__global__ void snapshot_details_kernel(const uint32_t* __restrict__ list, const unsigned long long* __restrict__ count,
+                                        const uint8_t* __restrict__ applied, const int64_t* __restrict__ start,
+                                        uint8_t* e_applied, int64_t* e_start) {
+  pdl_wait();  // (launched with programmatic stream serialisation: list_changes_kernel writes the list)
+  const uint32_t n = (uint32_t)*count;
+  for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
+    const uint32_t i = list[k];
+    e_applied[k] = applied[i];
+    e_start[k] = start[i];
+  }
+}
+
+// am_sweep_last_change_details: the details of list entries [0, n) (slots idx, pairs e_applied / e_start) of the tick
+// whose output is `out`.  The action is the slot's exception (a binary search of its tile's ascending exceptions), else
+// SUBMIT_HC from the bitmap.
+__global__ void gather_details_kernel(const uint32_t* __restrict__ idx, uint32_t n, const uint8_t* __restrict__ e_applied,
+                                      const int64_t* __restrict__ e_start, const TickOut out, bool closed, int64_t T,
+                                      am_change_detail_t* dst) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t i = idx[k], tile = i / (uint32_t)kTile, off = i % (uint32_t)kTile;
+  uint32_t act = ((out.bitmap[i / 32u] >> (i & 31u)) & 1u) ? AM_ACT_SUBMIT_HC : 0u;
+  const uint32_t* e = out.exc_seg + (size_t)tile * kTile;
+  uint32_t lo = 0, hi = out.tile_exc[tile];
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) / 2u;
+    if ((e[mid] >> 8) < off) lo = mid + 1u;
+    else hi = mid;
+  }
+  if (lo < out.tile_exc[tile] && (e[lo] >> 8) == off) act = e[lo] & 0xFFu;
+  uint32_t a = e_applied[k];
+  const int64_t w = e_start[k];
+  am_change_detail_t d;
+  d.started = (a & (AM_CHG_SUCCEEDED | AM_CHG_FAILED)) && w != kNotInFlight && !is_remedy_run(w) ? w : kNotInFlight;
+  d.remedy_started = (a & (AM_CHG_REMEDY_SUCCEEDED | AM_CHG_REMEDY_FAILED)) && is_remedy_run(w) ? w - kRemedyRun : kNotInFlight;
+  if (act & AM_ACT_STOPPED) a |= AM_CHG_STOPPED;
+  if (closed && (act & AM_ACT_SUBMIT_HC)) {
+    a |= AM_CHG_CLOSED_LOOP;
+    d.started = T;
+  }
+  d.applied = a;
+  d.action = act;
+  dst[k] = d;
 }
 
 // am_sweep_last_changes: the requested columns of the listed slots idx[0..n), column-major into dst[c] (blockIdx.y = c).

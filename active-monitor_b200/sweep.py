@@ -402,6 +402,30 @@ class Sweep:
         k = min(int(n.value), cap)
         return idx[:k], {name: a[:k] for name, a in cols.items()}
 
+    def set_change_details(self, on: bool):
+        """keep what every tick applied to the checks it changed, with the runs' starts (am_sweep_set_change_details;
+        needs tracking on)"""
+        self._check(self._lib.am_sweep_set_change_details(self._h, int(bool(on))), "am_sweep_set_change_details")
+
+    def last_change_details(self, offset: int = 0, cap: int | None = None):
+        """the details of the last tick's changed set (am_sweep_last_change_details) from entry `offset` on: (global idx
+        u64, structured array of L.CHANGE_DETAIL: started, remedy_started, applied, action).  cap None: all of them."""
+        n = L.u64(0)
+        fn = "am_sweep_last_change_details"
+        if cap is None:
+            rc = self._lib.am_sweep_last_change_details(self._h, offset, None, None, 0, C.byref(n))
+            if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+                self._check(rc, fn)
+            cap = int(n.value)
+        idx = np.empty(cap, dtype=np.uint64)
+        det = np.zeros(cap, dtype=L.CHANGE_DETAIL)
+        rc = self._lib.am_sweep_last_change_details(self._h, offset, idx.ctypes.data if cap else None,
+                                                    det.ctypes.data if cap else None, cap, C.byref(n))
+        if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+            self._check(rc, fn)
+        k = min(int(n.value), cap)
+        return idx[:k], det[:k]
+
     # -- introspection
     def set_seed(self, seed: int):
         self._check(self._lib.am_sweep_set_seed(self._h, seed), "am_sweep_set_seed")

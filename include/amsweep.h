@@ -530,6 +530,48 @@ int am_sweep_set_track_changes(am_sweep_t*, int on);
 int am_sweep_last_changes(am_sweep_t*, uint64_t offset, uint64_t* idx, am_record_cols_t* cols, uint64_t cap,
                           uint64_t* n_out);
 
+/* Change details: what the last tick applied to each check of its changed set, and the start of
+ * the run whose phase it applied, so that a status write and the per-check metrics need no shadow
+ * state (hcc.go:627-661, :673-721, :813-851; internal/metrics/collector.go).  One entry per entry
+ * of am_sweep_last_changes, same order. */
+typedef struct am_change_detail {
+  int64_t started;        /* StartedAt of the health-check run whose workflow phase this tick applied, else INT64_MIN */
+  int64_t remedy_started; /* RemedyStartedAt of the remedy run whose remedy phase this tick applied, else INT64_MIN */
+  uint32_t applied;       /* AM_CHG_* bits */
+  uint32_t action;        /* the AM_ACT_* bits the tick emitted for the slot, 0 if it emitted none */
+} am_change_detail_t;
+
+#define AM_CHG_SUCCEEDED 0x01u        /* a workflow Succeeded was applied (hcc.go:635-661)             */
+#define AM_CHG_FAILED 0x02u           /* a workflow Failed was applied (hcc.go:662-722)                */
+#define AM_CHG_TIMED_OUT 0x04u        /* ... that Failed is a workflow timeout's (hcc.go:627-632)      */
+#define AM_CHG_REMEDY_SUCCEEDED 0x08u /* a remedy Succeeded was applied (hcc.go:821-835)               */
+#define AM_CHG_REMEDY_FAILED 0x10u    /* a remedy Failed was applied (hcc.go:836-851)                  */
+#define AM_CHG_REMEDY_TIMED_OUT 0x20u /* ... that remedy Failed is a remedy timeout's (hcc.go:813-818) */
+#define AM_CHG_STOPPED 0x40u          /* the tick reported AM_ACT_STOPPED (hcc.go:238-250)            */
+#define AM_CHG_CLOSED_LOOP 0x80u      /* the result is the closed-loop harness completion             */
+
+/* Off by default; AM_E_INVAL, changing nothing, while status changes are not tracked (turning
+ * tracking off turns details off).  Turning details on applies the calls staged before it, as a
+ * read does, and allocates 18 B per slot of capacity on the device at the first such call (none
+ * for a handle that never turns them on; a handle with them off launches nothing for them).
+ * applied: the posted results the tick applied, as the per-slot call order resolved them (a
+ * phase superseded by a later upsert, remove or load is not there; of several phases of one group
+ * the latest; a remedy phase merged with the Failed it was posted with or behind; an attached
+ * remedy outcome is FAILED | REMEDY_*), plus TIMED_OUT / REMEDY_TIMED_OUT with the Failed of a
+ * timeout, STOPPED, and CLOSED_LOOP.  STARTED RULE: with the hold on, started (remedy_started) is
+ * what am_sweep_in_flight (am_sweep_remedy_in_flight) would have returned for the slot right
+ * before the am_sweep_post_result call that staged the applied workflow (remedy) phase; for a
+ * timeout it is the timed-out run's start, for a closed-loop completion T, and otherwise,
+ * including whenever the hold is off and for results pending from before details were turned on,
+ * INT64_MIN.  action: the slot's entry in the tick's own list. */
+int am_sweep_set_change_details(am_sweep_t*, int on);
+
+/* The last tick's change details: out[k] for entry offset + k of am_sweep_last_changes, idx[k]
+ * its global index.  Same contract as am_sweep_last_changes (offset, cap, *n_out, AM_E_NOSPACE,
+ * AM_E_RANGE; it waits for a device tick and drains nothing); AM_E_INVAL while details are off. */
+int am_sweep_last_change_details(am_sweep_t*, uint64_t offset, uint64_t* idx, am_change_detail_t* out, uint64_t cap,
+                                 uint64_t* n_out);
+
 /* Introspection */
 uint64_t am_sweep_size(const am_sweep_t*);     /* high-water mark (slots swept) */
 uint64_t am_sweep_capacity(const am_sweep_t*);

@@ -53,7 +53,17 @@ struct HealthCheckStatus {
   std::optional<int64_t> FinishedAt, RemedyFinishedAt;  // *metav1.Time as unix seconds
   int64_t SuccessCount = 0, FailedCount = 0, TotalHealthCheckRuns = 0;
   int64_t RemedySuccessCount = 0, RemedyFailedCount = 0, RemedyTotalRuns = 0;
-  std::string Status;  // "Stopped" | "" (workflow phases are written by the Go side)
+  std::string Status;  // GetStatus: "Stopped" | ""; StatusWrites: also "Succeeded" | "Failed"
+  // written by StatusWrites only (nullopt / "": not assigned by the tick, or set to nil by a remedy reset)
+  std::optional<int64_t> StartedAt, LastFailedAt, RemedyStartedAt, RemedyLastFailedAt;
+  std::string RemedyStatus;
+};
+
+// One status write of a tick (StatusWrites): the check and the fields hcc.go assigns for what the tick applied.
+struct StatusWrite {
+  std::string Key;
+  HealthCheckStatus Status;
+  am_change_detail_t Detail;
 };
 
 struct HealthCheck {
@@ -179,6 +189,70 @@ class HealthCheckReconciler {
     s.RemedyTotalRuns = r.remedy_total;
     if ((r.flags & AM_KIND_MASK) == AM_KIND_STOPPED && (r.flags & AM_F_STOPPED_REPORTED)) s.Status = "Stopped";
     return s;
+  }
+
+  // Status changes with their details (am_sweep_set_track_changes + am_sweep_set_change_details), for StatusWrites.
+  int EnableStatusWrites() {
+    const int rc = am_sweep_set_track_changes(h_, 1);
+    return rc != AM_OK ? rc : am_sweep_set_change_details(h_, 1);
+  }
+
+  // After a tick at `now` (EnableStatusWrites first): the status writes updateHealthCheckStatus (hcc.go:1445) would
+  // persist, one per check the tick changed, built from am_sweep_last_changes and am_sweep_last_change_details alone.
+  // The counters and TotalHealthCheckRuns are the check's columns.  As the watch loops assign them:
+  //   Succeeded (hcc.go:636-661): Status, StartedAt = then, FinishedAt = now; on the reset (AM_ACT_RESET_ON_PASS) the
+  //     remedy timestamps are nil and RemedyStatus = "HealthCheck Passed so Remedy is reset";
+  //   Failed (:663-721, a timeout's too, :627-632): Status, StartedAt = then, FinishedAt = LastFailedAt = now; on the
+  //     interval reset (AM_ACT_RESET_ON_INTERVAL) RemedyStatus = "RemedyResetInterval elapsed so Remedy is reset";
+  //   a remedy phase (:821-851), when the tick applied it (alone, or behind a Failed that runs the remedy):
+  //     RemedyStatus, RemedyStartedAt = then, RemedyFinishedAt = now, and RemedyLastFailedAt = now for a Failed;
+  //   AM_CHG_STOPPED: Status = "Stopped".
+  // `then` is the detail's start; a field it leaves at INT64_MIN (the hold off, or no run seen) is not written.
+  std::vector<StatusWrite> StatusWrites(int64_t now) {
+    std::vector<StatusWrite> out;
+    uint64_t n = 0;
+    int rc = am_sweep_last_changes(h_, 0, nullptr, nullptr, 0, &n);
+    if ((rc != AM_OK && rc != AM_E_NOSPACE) || n == 0) return out;
+    std::vector<uint64_t> idx(n), idx2(n);
+    std::vector<am_change_detail_t> det(n);
+    std::vector<uint32_t> flags(n);
+    std::vector<int64_t> fa(n), rfa(n);
+    std::vector<int32_t> sc(n), fc(n), rs(n), rf(n), rt(n);
+    am_record_cols_t c{};
+    c.flags = flags.data(); c.finished_at = fa.data(); c.remedy_finished_at = rfa.data();
+    c.success = sc.data(); c.failed = fc.data(); c.remedy_success = rs.data(); c.remedy_failed = rf.data();
+    c.remedy_total = rt.data();
+    if (am_sweep_last_changes(h_, 0, idx.data(), &c, n, &n) != AM_OK) return out;
+    if (am_sweep_last_change_details(h_, 0, idx2.data(), det.data(), n, &n) != AM_OK) return out;
+    const int64_t kNone = INT64_MIN;
+    for (uint64_t k = 0; k < n; ++k) {
+      const am_change_detail_t& d = det[k];
+      StatusWrite w{names_[idx[k]], {}, d};
+      HealthCheckStatus& s = w.Status;
+      s.SuccessCount = sc[k]; s.FailedCount = fc[k]; s.TotalHealthCheckRuns = (int64_t)sc[k] + fc[k];
+      s.RemedySuccessCount = rs[k]; s.RemedyFailedCount = rf[k]; s.RemedyTotalRuns = rt[k];
+      const bool ok = (d.applied & AM_CHG_SUCCEEDED) != 0, fail = !ok && (d.applied & AM_CHG_FAILED) != 0;
+      if (ok || fail) {
+        s.Status = ok ? "Succeeded" : "Failed";
+        if (d.started != kNone) s.StartedAt = d.started;
+        s.FinishedAt = now;
+        if (fail) s.LastFailedAt = now;
+      }
+      if (ok && (d.action & AM_ACT_RESET_ON_PASS)) s.RemedyStatus = "HealthCheck Passed so Remedy is reset";
+      if (fail && (d.action & AM_ACT_RESET_ON_INTERVAL)) s.RemedyStatus = "RemedyResetInterval elapsed so Remedy is reset";
+      const bool rem = (d.applied & (AM_CHG_REMEDY_SUCCEEDED | AM_CHG_REMEDY_FAILED)) != 0 &&
+                       (!(ok || fail) || (fail && (d.action & AM_ACT_RUN_REMEDY)));
+      if (rem) {
+        const bool rok = (d.applied & AM_CHG_REMEDY_SUCCEEDED) != 0;
+        s.RemedyStatus = rok ? "Succeeded" : "Failed";
+        if (d.remedy_started != kNone) s.RemedyStartedAt = d.remedy_started;
+        s.RemedyFinishedAt = now;
+        if (!rok) s.RemedyLastFailedAt = now;
+      }
+      if (d.applied & AM_CHG_STOPPED) s.Status = "Stopped";
+      out.push_back(std::move(w));
+    }
+    return out;
   }
 
   int LastTickError() const { return last_rc_; }
