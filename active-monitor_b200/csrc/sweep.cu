@@ -1405,6 +1405,28 @@ int am_sweep_post_result(am_sweep_t* h, uint64_t n, const uint64_t* idx, const u
   return AM_OK;
 }
 
+// The last tick's lists are read in pages: of n entries, those from `offset` on are left (*n_out), min(left, cap) are
+// copied (*ncopy); AM_E_RANGE past the end (nothing copied), AM_E_NOSPACE when more are left than fit.
+static int list_page(uint64_t n, uint64_t offset, uint64_t cap, uint64_t* n_out, uint64_t* ncopy) {
+  if (offset > n) return AM_E_RANGE;
+  const uint64_t left = n - offset;
+  *ncopy = left < cap ? left : cap;
+  if (n_out) *n_out = left;
+  return left > cap ? AM_E_NOSPACE : AM_OK;
+}
+
+// Entries [offset, ...) of the last tick's host list, widened into the caller's (Go) memory.
+static int copy_host_list(am_sweep_t* h, uint64_t offset, uint64_t* due_idx, uint32_t* due_action, uint64_t cap,
+                          uint64_t* n_out) {
+  uint64_t ncopy;
+  const int page = list_page(h->host_n, offset, cap, n_out, &ncopy);
+  if (page == AM_E_RANGE) return page;
+  if (ncopy)
+    amsweep_host::widen_list(ncopy, h->shard_base, (const uint32_t*)h->host_out.p + offset,
+                             (const uint8_t*)h->host_out.p + h->host_out_entries * 4 + offset, due_idx, due_action);
+  return page;
+}
+
 int am_sweep_tick(am_sweep_t* h, int64_t unix_sec, uint32_t mode, uint64_t* due_idx,
                   uint32_t* due_action, uint64_t cap, uint64_t* n_out, am_tick_stats_t* stats) {
   if (!h || (cap && (!due_idx || !due_action))) return AM_E_INVAL;
@@ -1413,13 +1435,7 @@ int am_sweep_tick(am_sweep_t* h, int64_t unix_sec, uint32_t mode, uint64_t* due_
   if (!g.ok) return AM_E_BUSY;
   int rc = run_tick(h, unix_sec, mode, h->stream, TickKind::kHost, {}, stats);
   if (rc != AM_OK) return rc;
-  const uint64_t n = h->host_n;
-  if (n_out) *n_out = n;
-  const uint64_t ncopy = n < cap ? n : cap;
-  if (ncopy)  // widen into the caller's (Go) memory
-    amsweep_host::widen_list(ncopy, h->shard_base, (const uint32_t*)h->host_out.p,
-                             (const uint8_t*)h->host_out.p + h->host_out_entries * 4, due_idx, due_action);
-  return n > cap ? AM_E_NOSPACE : AM_OK;
+  return copy_host_list(h, 0, due_idx, due_action, cap, n_out);
 }
 
 int am_sweep_tick_view(am_sweep_t* h, int64_t unix_sec, uint32_t mode, am_tick_view_t* view,
@@ -1442,14 +1458,7 @@ int am_sweep_last_list(am_sweep_t* h, uint64_t offset, uint64_t* due_idx, uint32
   if (!h || (cap && (!due_idx || !due_action))) return AM_E_INVAL;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  const uint64_t n = h->host_n;
-  if (offset > n) return AM_E_RANGE;
-  const uint64_t left = n - offset, ncopy = left < cap ? left : cap;
-  if (n_out) *n_out = left;
-  if (ncopy)
-    amsweep_host::widen_list(ncopy, h->shard_base, (const uint32_t*)h->host_out.p + offset,
-                             (const uint8_t*)h->host_out.p + h->host_out_entries * 4 + offset, due_idx, due_action);
-  return left > cap ? AM_E_NOSPACE : AM_OK;
+  return copy_host_list(h, offset, due_idx, due_action, cap, n_out);
 }
 
 int am_sweep_tick_device(am_sweep_t* h, int64_t unix_sec, uint32_t mode, void* d_due_idx,
@@ -1703,24 +1712,33 @@ static int timed_out_impl(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t
     }
     h->to_host.clear();
     h->rto_host.clear();
-    for (uint32_t k = 0; k < m; ++k) {  // a remedy run's since word is its start + kRemedyRun
-      if (ls[k] >= kRemedyRun / 2) h->rto_host.push_back({li[k], ls[k] - kRemedyRun});
-      else h->to_host.push_back({li[k], ls[k]});
-    }
+    for (uint32_t k = 0; k < m; ++k)
+      (is_remedy_run(ls[k]) ? h->rto_host : h->to_host).push_back({li[k], run_start(ls[k])});
     std::sort(h->to_host.begin(), h->to_host.end());  // (appended one segment at a time, in no particular order)
     std::sort(h->rto_host.begin(), h->rto_host.end());
     h->to_fetched = true;
   }
   const std::vector<std::pair<uint32_t, int64_t>>& list = remedy ? h->rto_host : h->to_host;
-  const uint64_t n = h->to_ran ? list.size() : 0;
-  if (offset > n) return AM_E_RANGE;
-  const uint64_t left = n - offset, ncopy = left < cap ? left : cap;
-  if (n_out) *n_out = left;
+  uint64_t ncopy;
+  const int page = list_page(h->to_ran ? list.size() : 0, offset, cap, n_out, &ncopy);
+  if (page == AM_E_RANGE) return page;
   for (uint64_t k = 0; k < ncopy; ++k) {
     idx[k] = h->shard_base + list[offset + k].first;
     since[k] = list[offset + k].second;
   }
-  return left > cap ? AM_E_NOSPACE : AM_OK;
+  return page;
+}
+
+// list_page over the last tick's change list (empty unless `listed`); its length is fetched once per tick.
+static int change_page(am_sweep_t* h, bool listed, uint64_t offset, uint64_t cap, uint64_t* n_out, uint64_t* ncopy) {
+  if (listed && !h->chg_fetched) {
+    AM_CUDA(h, h->pin_in.reserve(8));
+    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->chg_acc + 1, 8, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    h->chg_n = *(const unsigned long long*)h->pin_in.p;
+    h->chg_fetched = true;
+  }
+  return list_page(listed ? h->chg_n : 0, offset, cap, n_out, ncopy);
 }
 
 int am_sweep_last_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t* since, uint64_t cap, uint64_t* n_out) {
@@ -1743,17 +1761,9 @@ int am_sweep_last_changes(am_sweep_t* h, uint64_t offset, uint64_t* idx, am_reco
   }
   int rc = set_stream(h, h->stream);  // (after the last tick, on whatever stream it ran; staged calls are not drained)
   if (rc != AM_OK) return rc;
-  if (h->chg_listed && !h->chg_fetched) {
-    AM_CUDA(h, h->pin_in.reserve(8));
-    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->chg_acc + 1, 8, cudaMemcpyDeviceToHost, h->stream));
-    AM_CUDA(h, cudaStreamSynchronize(h->stream));
-    h->chg_n = *(const unsigned long long*)h->pin_in.p;
-    h->chg_fetched = true;
-  }
-  const uint64_t n = h->chg_listed ? h->chg_n : 0;
-  if (offset > n) return AM_E_RANGE;
-  const uint64_t left = n - offset, ncopy = left < cap ? left : cap;
-  if (n_out) *n_out = left;
+  uint64_t ncopy;
+  const int page = change_page(h, h->chg_listed, offset, cap, n_out, &ncopy);
+  if (page != AM_OK && page != AM_E_NOSPACE) return page;
   if (ncopy) {
     // pin_in / dev_in: the list's entries, then each requested column (8-B aligned), gathered on the device
     GatherCols gc{};
@@ -1788,7 +1798,7 @@ int am_sweep_last_changes(am_sweep_t* h, uint64_t offset, uint64_t* idx, am_reco
       memcpy(dst, (const char*)h->pin_in.p + at[c++], ncopy * kColElem[k]);
     }
   }
-  return left > cap ? AM_E_NOSPACE : AM_OK;
+  return page;
 }
 
 int am_sweep_last_change_details(am_sweep_t* h, uint64_t offset, uint64_t* idx, am_change_detail_t* out, uint64_t cap,
@@ -1802,18 +1812,9 @@ int am_sweep_last_change_details(am_sweep_t* h, uint64_t offset, uint64_t* idx, 
   }
   int rc = set_stream(h, h->stream);  // (after the last tick, on whatever stream it ran; staged calls are not drained)
   if (rc != AM_OK) return rc;
-  const bool listed = h->chg_listed && h->det_listed;
-  if (listed && !h->chg_fetched) {
-    AM_CUDA(h, h->pin_in.reserve(8));
-    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->chg_acc + 1, 8, cudaMemcpyDeviceToHost, h->stream));
-    AM_CUDA(h, cudaStreamSynchronize(h->stream));
-    h->chg_n = *(const unsigned long long*)h->pin_in.p;
-    h->chg_fetched = true;
-  }
-  const uint64_t n = listed ? h->chg_n : 0;
-  if (offset > n) return AM_E_RANGE;
-  const uint64_t left = n - offset, ncopy = left < cap ? left : cap;
-  if (n_out) *n_out = left;
+  uint64_t ncopy;
+  const int page = change_page(h, h->chg_listed && h->det_listed, offset, cap, n_out, &ncopy);
+  if (page != AM_OK && page != AM_E_NOSPACE) return page;
   if (ncopy) {
     // pin_in / dev_in: the details, then the list's entries
     const size_t at = ncopy * sizeof(am_change_detail_t), bytes = at + ncopy * 4;
@@ -1833,7 +1834,7 @@ int am_sweep_last_change_details(am_sweep_t* h, uint64_t offset, uint64_t* idx, 
     const uint32_t* li = (const uint32_t*)((const char*)h->pin_in.p + at);
     for (uint64_t k = 0; k < ncopy; ++k) idx[k] = h->shard_base + li[k];
   }
-  return left > cap ? AM_E_NOSPACE : AM_OK;
+  return page;
 }
 
 // (tick guard held, staged events drained, h->stream ordered)

@@ -87,7 +87,6 @@ __device__ __forceinline__ void block_constant(BlockStats& S, int which, int64_t
 // One record through the block, event by event (see the header of this file).
 template <bool CLOSED>
 __device__ __forceinline__ void block_record(const BlockParams& p, BlockStats& S, uint64_t cta_base, uint32_t loc) {
-  constexpr uint32_t kPend = AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING;
   const int64_t K = (int64_t)p.K;
   const uint64_t i = cta_base + loc;
   const uint64_t g = p.shard_base + i;
@@ -107,7 +106,7 @@ __device__ __forceinline__ void block_record(const BlockParams& p, BlockStats& S
   }
   // remedy / counter state: every due record needs it in closed loop, a posted result in open loop
   RecState s{};
-  const bool with_state = CLOSED || (f & kPend) != 0;
+  const bool with_state = CLOSED || (f & kPendBits) != 0;
   if (with_state) load_state(p.c, i, s);
   const RecState s0 = s;
   const uint32_t f0 = f;
@@ -124,11 +123,11 @@ __device__ __forceinline__ void block_record(const BlockParams& p, BlockStats& S
     return next_local_minute(p.T0, t, zoff);  // 5-field schedule
   };
 
-  int64_t t = (f & (kPend | AM_F_CARRY_MASK)) ? 0 : next_event(-1);
+  int64_t t = (f & (kPendBits | AM_F_CARRY_MASK)) ? 0 : next_event(-1);
   while (t < K) {
     const int64_t T = p.T0 + t;
     // ---- exactly sweep_tick_kernel's decision for (record, T) ----
-    const bool pending = (f & kPend) != 0;
+    const bool pending = (f & kPendBits) != 0;
     const bool due_iv = interval_due(f, rasv, fa, T);
     bool due_cron = false;
     if (is_cron) {
@@ -199,7 +198,6 @@ __global__ void __launch_bounds__(kBlockThreads, AM_BLOCK_MIN_CTAS) sweep_block_
 
   const uint64_t cta_base = (uint64_t)blockIdx.x * kBlockRecords;
   const int64_t K = (int64_t)p.K;
-  constexpr uint32_t kPend = AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING;
 
   // ---- pass 1: classify.  16 B per record (flags, repeatAfterSec, finishedAt), four records per thread.
   //      Records that cannot act inside the block — the majority: an armed timer that fires later — cost
@@ -222,7 +220,7 @@ __global__ void __launch_bounds__(kBlockThreads, AM_BLOCK_MIN_CTAS) sweep_block_
       const uint32_t loc = loc0 + (uint32_t)q;
       const uint32_t kind = f & AM_KIND_MASK;
       if (!is_live(f)) continue;  // tombstones, NO_RESOURCE (hcc.go:227), host-fallback: never evaluated
-      const bool first_tick = (f & (kPend | AM_F_CARRY_MASK)) != 0;  // a posted result / carried action: an event at tick 0
+      const bool first_tick = (f & (kPendBits | AM_F_CARRY_MASK)) != 0;  // posted result / carried action: tick 0
       const uint64_t g = p.shard_base + cta_base + loc;
       int64_t n_ev = 0;  // expected events in the block (an upper bound is fine: it only picks the list)
       if (kind == AM_KIND_PARSE_ERROR) {

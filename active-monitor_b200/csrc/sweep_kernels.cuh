@@ -92,6 +92,36 @@ inline void st_keep_u32(uint32_t* p, uint32_t v, uint64_t) { *p = v; }
 inline void st_keep_u8(uint8_t* p, uint32_t v, uint64_t) { *p = (uint8_t)v; }
 #endif
 
+// ---- the posted-result bits of the flags word ---------------------------------
+constexpr uint32_t kHcBits = AM_F_PENDING_OK | AM_F_PENDING_FAIL;               // a workflow phase
+constexpr uint32_t kRemedyBits = AM_F_REMEDY_PENDING | AM_F_REMEDY_OUTCOME_OK;  // a remedy phase and its outcome
+constexpr uint32_t kPendBits = kHcBits | AM_F_REMEDY_PENDING;                   // any posted result
+
+// ---- warp collectives (every lane calls them): the inclusive prefix sum of v over lanes 0 .. lane
+__device__ __forceinline__ uint32_t warp_inclusive_scan(uint32_t v, int lane) {
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t up = __shfl_up_sync(kFull, v, d);
+    if (lane >= d) v += up;
+  }
+  return v;
+}
+// the least v of the warp, in every lane
+__device__ __forceinline__ unsigned long long warp_min(unsigned long long v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const unsigned long long u = __shfl_xor_sync(kFull, v, o);
+    v = u < v ? u : v;
+  }
+  return v;
+}
+// four 8-bit counters per lane (byte q: counter q) summed over the warp: .x = 0 | 1 << 16, .y = 2 | 3 << 16
+__device__ __forceinline__ uint2 warp_byte_sums(uint32_t c) {
+  const uint32_t lo = __reduce_add_sync(kFull, (c & 0xFFu) | ((c & 0xFF00u) << 8));
+  const uint32_t hi = __reduce_add_sync(kFull, ((c >> 16) & 0xFFu) | ((c >> 8) & 0xFF0000u));
+  return make_uint2(lo, hi);
+}
+
 __device__ __forceinline__ uint64_t sm64(uint64_t z) {
   z += 0x9E3779B97F4A7C15ull;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -140,7 +170,7 @@ __device__ __forceinline__ uint32_t apply_result(RecState& r, int64_t T, uint32_
   uint32_t act = 0;
   const uint32_t f = r.flags;
   // watchWorkflowReschedule re-arms the repeat timer after either outcome (hcc.go:745-752)
-  const uint32_t armed = (f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL)) ? AM_F_TIMER_ARMED : 0u;
+  const uint32_t armed = (f & kHcBits) ? AM_F_TIMER_ARMED : 0u;
   if (f & AM_F_PENDING_OK) {  // hcc.go:635-661
     r.s = (int32_t)((uint32_t)r.s + 1u);
     r.fa = T;
@@ -186,7 +216,7 @@ __device__ __forceinline__ uint32_t apply_result(RecState& r, int64_t T, uint32_
   } else if (f & AM_F_REMEDY_PENDING) {  // remedy finished on its own
     remedy_result(r, T, (f & AM_F_REMEDY_OUTCOME_OK) != 0, res);
   }
-  r.flags = (f & ~(AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING | AM_F_REMEDY_OUTCOME_OK)) | armed;
+  r.flags = (f & ~(kHcBits | kRemedyBits)) | armed;
   return act;
 }
 
@@ -228,11 +258,8 @@ __device__ __forceinline__ void store_changed_state(const DevCols& c, I i, const
 // The lanes' result counts (four 8-bit counts each, as apply_result adds them) summed over the warp: lane
 // q < 4 gets counter q {ok, fail, remedy ok, remedy fail}.  Two redux over 16-bit halves; every lane calls it.
 __device__ __forceinline__ uint32_t warp_result_count(uint32_t res, int lane) {
-  uint32_t lo = 0, hi = 0;
-  if (__any_sync(kFull, res != 0)) {
-    lo = __reduce_add_sync(kFull, (res & 0xFFu) | ((res & 0xFF00u) << 8));           // ok | fail<<16
-    hi = __reduce_add_sync(kFull, ((res >> 16) & 0xFFu) | ((res >> 8) & 0xFF0000u));  // remedy ok | fail<<16
-  }
+  uint32_t lo = 0, hi = 0;  // ok | fail << 16, remedy ok | remedy fail << 16
+  if (__any_sync(kFull, res != 0)) { const uint2 s = warp_byte_sums(res); lo = s.x; hi = s.y; }
   return ((lane < 2 ? lo : hi) >> ((lane & 1) * 16)) & 0xFFFFu;
 }
 
@@ -245,10 +272,17 @@ __device__ __forceinline__ bool is_interval_kind(uint32_t kind) { return ((0x14u
 // is applied first (step 1): finishedAt = T and the timer re-armed.  Without a timer (controller restart,
 // hcc.go:161) the reference submits whatever finishedAt says.
 __device__ __forceinline__ bool interval_due(uint32_t f, int32_t ras, int64_t fa, int64_t T) {
-  const bool has_result = (f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL)) != 0;
+  const bool has_result = (f & kHcBits) != 0;
   const int64_t elapsed = (int64_t)((uint64_t)T - (uint64_t)(has_result ? T : fa));
   const bool armed = has_result || (f & AM_F_TIMER_ARMED) != 0;
   return !((elapsed < (int64_t)ras) & armed);
+}
+
+// The hold rule: the run in a since word is still in flight — it started no earlier than the record's finishedAt and
+// no workflow phase is pending.  finishedAt and the flags are callables, read only when the terms before them hold.
+template <typename FinishedAt, typename Flags>
+__device__ __forceinline__ bool held_run(int64_t since, FinishedAt finished_at, Flags flags) {
+  return since != kNotInFlight && since >= finished_at() && !(flags() & kHcBits);
 }
 
 // Action bits of apply_result <-> the carry bits of the flags word (AM_F_CARRY_MASK): RUN_REMEDY (0x02)
@@ -329,7 +363,7 @@ __global__ void tz_words_kernel(const int32_t* __restrict__ tz_off, TickWords* _
 // can answer it: the five canonical mask columns are read instead, 40 B per record, in warps that hold a
 // CRON_SPEC record.  Runs at AM_MIN_BLOCKS CTAs per SM like the closed-loop on-minute variant.
 // HOLD = hold in flight (am_sweep_set_hold_in_flight; open loop only): after the due decision, a due record whose
-// health-check workflow is still running (p.since set, since >= finishedAt, no workflow phase pending) is not
+// health-check workflow is still running (held_run on p.since) is not
 // submitted; every record that is submitted gets since = T.  The since word is loaded only for the halves that
 // hold a due record: one dependent round trip, in the warps that have one (DESIGN.md section 3 compares it with
 // streaming since for every record).
@@ -486,7 +520,7 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
       const uint32_t f = j ? fl[h].y : fl[h].x;
       const int64_t fav = j ? fa[h].y : fa[h].x;
       const bool live = is_live(f);
-      const bool pending = (f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING)) != 0;
+      const bool pending = (f & kPendBits) != 0;
       // (an if, not `MASKS && ...`: with the latter ptxas hoisted this loop's arithmetic above the
       // __syncwarp fence in the MASKS=false variants and delayed the second half's loads behind it)
       bool due_cron = false;
@@ -529,8 +563,8 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
           if ((db >> j) & 1u) {
             const uint32_t f = j ? fl[h].y : fl[h].x;
             const int64_t fav = j ? fa[h].y : fa[h].x;
-            const bool held = s[j] != kNotInFlight && s[j] >= fav && !(f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL));
-            if (held) {
+            // held_run, written out: through the call the hold variants compile to different machine code
+            if (s[j] != kNotInFlight && s[j] >= fav && !(f & kHcBits)) {
               act[h][j] &= ~AM_ACT_SUBMIT_HC;
             } else {
               s[j] = T;
@@ -547,11 +581,7 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
       }
     }
     if (TIMEOUT && __any_sync(kFull, dmin != ~0ull)) {  // one atomic per warp into its segment's bound
-#pragma unroll
-      for (int o = 16; o; o >>= 1) {
-        const unsigned long long v = __shfl_xor_sync(kFull, dmin, o);
-        dmin = v < dmin ? v : dmin;
-      }
+      dmin = warp_min(dmin);
       if (lane == 0) atomicMin(p.seg_deadline + (tile_base + (uint32_t)(warp * kRecPerWarp)) / (uint32_t)kRecPerWarp, dmin);
     }
   }
@@ -757,7 +787,7 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
       for (int j = 0; j < 2; ++j)
         if (act[h][j] > 1u) {
           const uint32_t off = (uint32_t)(warp * kRecPerWarp + h * 64 + lane * 2 + j);  // record within the tile
-          st_keep_u32(p.out.exc_seg + pos, (off << 8) | act[h][j], keep);
+          st_keep_u32(p.out.exc_seg + pos, exc_entry(off, act[h][j]), keep);
           ++pos;
         }
     }
@@ -782,23 +812,12 @@ __global__ void __launch_bounds__(1024) scan_groups_kernel(const ScanParams p) {
   for (uint32_t g0 = 0; g0 < p.n_groups; g0 += blockDim.x) {
     const uint32_t g = g0 + (uint32_t)tid;
     const uint32_t c = g < p.n_groups ? p.group_count[g] : 0u;
-    uint32_t incl = c;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t up = __shfl_up_sync(kFull, incl, d);
-      if (lane >= d) incl += up;
-    }
+    const uint32_t incl = warp_inclusive_scan(c, lane);
     if (lane == 31) s_warp[warp] = incl;
     __syncthreads();
     if (warp == 0) {  // exclusive scan of the 32 warp totals
       const uint32_t t = s_warp[lane];
-      uint32_t wi = t;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t up = __shfl_up_sync(kFull, wi, d);
-        if (lane >= d) wi += up;
-      }
-      s_warp[lane] = wi - t;
+      s_warp[lane] = warp_inclusive_scan(t, lane) - t;
     }
     __syncthreads();
     const uint32_t carry = s_carry;
@@ -870,12 +889,7 @@ __global__ void __launch_bounds__(kExpandThreads, 8) expand_kernel(const ExpandP
 
   // ---- ranks: exclusive popcount prefix over the group's 256 words (two per thread)
   const uint32_t c_lo = (uint32_t)__popc(w2.x), c = c_lo + (uint32_t)__popc(w2.y);
-  uint32_t incl = c;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t up = __shfl_up_sync(kFull, incl, d);
-    if (lane >= d) incl += up;
-  }
+  const uint32_t incl = warp_inclusive_scan(c, lane);
   if (lane == 31) s_warp[warp] = incl;
   if (l16 == 0) s_nx[tsub] = nx;
   *reinterpret_cast<uint2*>(&s_w[2 * tid]) = w2;
@@ -907,23 +921,21 @@ __global__ void __launch_bounds__(kExpandThreads, 8) expand_kernel(const ExpandP
   uint32_t c0 = 0, c1 = 0;
   for (uint32_t i = l16; i < nx; i += 16u) {
     const uint32_t e = i < 16u ? e_first : __ldcs(src.exc_seg + (size_t)tile * kTile + i);
-    const uint32_t off = tsub * (uint32_t)kTile + (e >> 8);
+    const uint32_t off = tsub * (uint32_t)kTile + exc_offset(e), a = exc_action(e);
     const uint32_t wd = off >> 5;
     const uint32_t rk = (uint32_t)s_wpre[wd] + (uint32_t)__popc(s_w[wd] & ((1u << (off & 31u)) - 1u));
-    s_act[sh + rk] = (uint8_t)e;
-    c0 += spread4(e);
-    c1 += spread4(e >> 4);
+    s_act[sh + rk] = (uint8_t)a;
+    c0 += spread4(a);
+    c1 += spread4(e >> 4);  // the action's high nibble (spread4 reads 4 bits: masking a first costs instructions)
   }
   if (stats) {
     // statistics of this warp's slice of the group: action bits from the exceptions (a lane holds
     // at most 64 of them: byte counters), index checksums from the bitmap words themselves — the
     // sum over the set bits b of word t of (32 t + b) = popc(w) 32 t + sum_j 2^j popc(w & M_j)
-    uint32_t a0 = 0, a1 = 0, a2 = 0, a3 = 0;
+    uint32_t a0 = 0, a1 = 0, a2 = 0, a3 = 0;  // action bits 0 | 1 << 16, ..., 6 | 7 << 16
     if (__any_sync(kFull, nx != 0)) {
-      a0 = __reduce_add_sync(kFull, (c0 & 0xFFu) | ((c0 & 0xFF00u) << 8));
-      a1 = __reduce_add_sync(kFull, ((c0 >> 16) & 0xFFu) | ((c0 >> 8) & 0xFF0000u));
-      a2 = __reduce_add_sync(kFull, (c1 & 0xFFu) | ((c1 & 0xFF00u) << 8));
-      a3 = __reduce_add_sync(kFull, ((c1 >> 16) & 0xFFu) | ((c1 >> 8) & 0xFF0000u));
+      const uint2 s0 = warp_byte_sums(c0), s1 = warp_byte_sums(c1);
+      a0 = s0.x; a1 = s0.y; a2 = s1.x; a3 = s1.y;
     }
     if (lane < 8) {
       const uint32_t qv = lane < 2 ? a0 : (lane < 4 ? a1 : (lane < 6 ? a2 : a3));
@@ -1092,11 +1104,9 @@ __global__ void next_due_kernel(DevCols c, const int64_t* __restrict__ since, co
     const uint32_t kind = f & AM_KIND_MASK;
     if (!is_live(f)) continue;
     int64_t due = INT64_MAX;
-    if ((f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING)) || kind == AM_KIND_PARSE_ERROR ||
-        (kind == AM_KIND_STOPPED && !(f & AM_F_STOPPED_REPORTED))) {
+    if ((f & kPendBits) || kind == AM_KIND_PARSE_ERROR || (kind == AM_KIND_STOPPED && !(f & AM_F_STOPPED_REPORTED))) {
       due = T + 1;
-    } else if (since && since[i] != kNotInFlight && since[i] >= c.finished_at[i]) {
-      // held (nothing pending: the branch above)
+    } else if (since && held_run(since[i], [&] { return c.finished_at[i]; }, [&] { return f; })) {
       if (deadline && deadline[i] != kNoDeadline) due = deadline[i] > T + 1 ? deadline[i] : T + 1;
     } else if (kind == AM_KIND_INTERVAL || kind == AM_KIND_CRON_EVERY) {
       const int64_t at = (int64_t)((uint64_t)c.finished_at[i] + (uint64_t)(int64_t)c.ras[i]);
@@ -1110,11 +1120,7 @@ __global__ void next_due_kernel(DevCols c, const int64_t* __restrict__ since, co
     const unsigned long long key = (unsigned long long)due ^ (1ull << 63);  // order-preserving bias
     best = key < best ? key : best;
   }
-#pragma unroll
-  for (int d = 16; d; d >>= 1) {
-    const unsigned long long o = __shfl_xor_sync(kFull, best, d);
-    best = o < best ? o : best;
-  }
+  best = warp_min(best);
   if ((threadIdx.x & 31) == 0 && best != ~0ull) atomicMin(out_biased, best);
 }
 
@@ -1132,8 +1138,32 @@ __global__ void next_due_kernel(DevCols c, const int64_t* __restrict__ since, co
 // A staged op is a uint2 (slot, arg): arg = kind in the top 2 bits; low 30 bits: record index
 // (upsert) or flag bits (result).
 constexpr uint32_t kOpUpsert = 0u << 30, kOpRemove = 1u << 30, kOpResult = 2u << 30, kOpKindMask = 3u << 30;
-constexpr uint32_t kHcBits = AM_F_PENDING_OK | AM_F_PENDING_FAIL;
-constexpr uint32_t kRemedyBits = AM_F_REMEDY_PENDING | AM_F_REMEDY_OUTCOME_OK;
+
+// The mark triple of slot i: word x (kMarkState, kMarkHc, kMarkRm) is the 1-based sequence (op k: k + 1) of the slot's
+// latest state op (upsert / remove), workflow phase and remedy phase in this drain, 0 for none.  The winner rule below
+// works on the words as scalars (held in a struct, they cost the readers registers).
+enum : uint32_t { kMarkState = 0u, kMarkHc = 1u, kMarkRm = 2u };
+template <typename W>
+__device__ __forceinline__ W& mark(W* marks, uint32_t i, uint32_t x) { return marks[3u * i + x]; }
+__device__ __forceinline__ bool mark_is(uint32_t word, uint32_t k) { return word == k + 1u; }
+__device__ __forceinline__ bool state_op_won(const uint32_t* marks, uint32_t i, uint32_t k) {  // one word read
+  return mark(marks, i, kMarkState) == k + 1u;
+}
+// a phase winner counts when posted after the slot's latest state op (an older result belongs to the replaced CR)
+__device__ __forceinline__ bool phase_valid(uint32_t phase, uint32_t state) { return phase != 0u && phase >= state; }
+// op k won a phase group: it is the group's winner (`phase`) and that one counts (`valid`)
+__device__ __forceinline__ bool phase_won(uint32_t phase, bool valid, uint32_t k) { return valid && mark_is(phase, k); }
+// the slot's phases are owned by the workflow-phase winner if it counts, else by the remedy-phase winner
+__device__ __forceinline__ bool phase_owner(bool won_hc, bool won_rm, bool hc_valid) {
+  return won_hc || (won_rm && !hc_valid);
+}
+// the posted bits a drain leaves in flags f: each valid winner's arg (fetched only then) replaces its own bit group
+template <typename HcArg, typename RmArg>
+__device__ __forceinline__ uint32_t merge_phases(uint32_t f, bool hc_valid, HcArg hc_arg, bool rm_valid, RmArg rm_arg) {
+  if (hc_valid) f = (f & ~kHcBits) | (hc_arg() & kHcBits);
+  if (rm_valid) f = (f & ~kRemedyBits) | (rm_arg() & kRemedyBits);
+  return f;
+}
 
 __global__ void mark_ops_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
@@ -1141,9 +1171,9 @@ __global__ void mark_ops_kernel(uint32_t* marks, const uint2* __restrict__ ops, 
   if (k >= n) return;
   const uint2 op = ops[k];
   const uint32_t i = op.x, arg = op.y;
-  if ((arg & kOpKindMask) != kOpResult) { atomicMax(&marks[3u * i], k + 1u); return; }
-  if (arg & kHcBits) atomicMax(&marks[3u * i + 1u], k + 1u);
-  if (arg & AM_F_REMEDY_PENDING) atomicMax(&marks[3u * i + 2u], k + 1u);
+  if ((arg & kOpKindMask) != kOpResult) { atomicMax(&mark(marks, i, kMarkState), k + 1u); return; }
+  if (arg & kHcBits) atomicMax(&mark(marks, i, kMarkHc), k + 1u);
+  if (arg & AM_F_REMEDY_PENDING) atomicMax(&mark(marks, i, kMarkRm), k + 1u);
 }
 
 // upserts (hcc.go:170-188 Reconcile) and removes (hcc.go:175-186).  Both may change the slot's kind or
@@ -1156,7 +1186,7 @@ __global__ void apply_state_ops_kernel(DevCols c, const uint32_t* __restrict__ m
   const uint2 op = ops[k];
   const uint32_t i = op.x, arg = op.y;
   const uint32_t kind = arg & kOpKindMask;
-  if (kind == kOpResult || marks[3u * i] != k + 1u) return;
+  if (kind == kOpResult || !state_op_won(marks, i, k)) return;
   seg_dirty[i / kRecPerWarp] = 1u;
   if (kind == kOpRemove) { c.flags[i] = AM_F_TOMBSTONE; return; }
   const am_record_t r = recs[arg & ~kOpKindMask];
@@ -1235,26 +1265,15 @@ __global__ void apply_result_ops_kernel(uint32_t* flags, const uint32_t* __restr
   const uint2 op = ops[k];
   const uint32_t i = op.x, arg = op.y;
   if ((arg & kOpKindMask) != kOpResult) return;
-  const uint32_t s = marks[3u * i];
-  if (k + 1u < s) return;  // posted before the slot's latest upsert / remove
+  // the winner rule with one word read per test, spelled as compares (through mark_is the kernel compiles differently)
+  if (k + 1u < mark(marks, i, kMarkState)) return;
   uint32_t clr = 0, set = 0;
-  if ((arg & kHcBits) && marks[3u * i + 1u] == k + 1u) { clr |= kHcBits; set |= arg & kHcBits; }
-  if ((arg & AM_F_REMEDY_PENDING) && marks[3u * i + 2u] == k + 1u) { clr |= kRemedyBits; set |= arg & kRemedyBits; }
+  if ((arg & kHcBits) && mark(marks, i, kMarkHc) == k + 1u) { clr |= kHcBits; set |= arg & kHcBits; }
+  if ((arg & AM_F_REMEDY_PENDING) && mark(marks, i, kMarkRm) == k + 1u) { clr |= kRemedyBits; set |= arg & kRemedyBits; }
   if (clr) {
     atomicAnd(&flags[i], ~clr);
     atomicOr(&flags[i], set);
   }
-}
-
-// The posted bits a drain leaves in a slot's flags `f` (the rule above): the winner of the workflow phase and the
-// winner of the remedy phase, each when posted after the slot's latest upsert / remove, replace their own bit groups.
-// A winner's arg is fetched only when it is valid.  apply_results_now_kernel spells the same two lines out with its
-// own winner's arg in hand (calling this there reorders its machine code); capture_ops_kernel calls it.
-template <typename HcArg, typename RmArg>
-__device__ __forceinline__ uint32_t merge_phases(uint32_t f, bool hc_valid, HcArg hc_arg, bool rm_valid, RmArg rm_arg) {
-  if (hc_valid) f = (f & ~kHcBits) | (hc_arg() & kHcBits);
-  if (rm_valid) f = (f & ~kRemedyBits) | (rm_arg() & kRemedyBits);
-  return f;
 }
 
 // Results posted between two ticks, applied while the tick drains them instead of inside its sweep.
@@ -1276,24 +1295,21 @@ __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__
                                          const int32_t* __restrict__ wf_timeout, unsigned long long* seg_deadline) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-  constexpr uint32_t kPend = AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING;
   uint32_t res = 0;
   uint2 op = make_uint2(0u, 0u);
   if (k < n) op = ops[k];
   if (k < n && (op.y & kOpKindMask) == kOpResult) {
     const uint32_t i = op.x, arg = op.y;
-    const uint32_t s_state = marks[3u * i], hcw = marks[3u * i + 1u], rmw = marks[3u * i + 2u];
-    // The winners of the slot's two phase groups (apply_result_ops_kernel's rule: the latest op of a group, if
-    // it was posted after the slot's latest upsert / remove) may be two different ops; ONE thread owns the
-    // slot here — the workflow-phase winner, else the remedy-phase winner — and takes the other group's
-    // bits from that op, so the flags are read and written once, without atomics.
-    const bool hc_valid = hcw != 0u && hcw >= s_state, rm_valid = rmw != 0u && rmw >= s_state;
-    const bool mine_hc = hc_valid && hcw == k + 1u, mine_rm = rm_valid && rmw == k + 1u;
-    if (mine_hc || (mine_rm && !hc_valid)) {
-      uint32_t f = c.flags[i];
-      if (mine_hc) f = (f & ~kHcBits) | (arg & kHcBits);
-      if (rm_valid) f = (f & ~kRemedyBits) | ((mine_rm ? arg : ops[rmw - 1u].y) & kRemedyBits);
-      if (!is_live(f) || !(f & kPend)) {
+    const uint32_t s_state = mark(marks, i, kMarkState), hcw = mark(marks, i, kMarkHc), rmw = mark(marks, i, kMarkRm);
+    const bool hc_valid = phase_valid(hcw, s_state), rm_valid = phase_valid(rmw, s_state);
+    // The winners of the slot's two phase groups may be two different ops; ONE thread owns the slot here
+    // (phase_owner) and takes the other group's bits from that op, so the flags are read and written once, without
+    // atomics.  The owner is the workflow-phase winner whenever that one is valid.
+    const bool won_hc = phase_won(hcw, hc_valid, k), won_rm = phase_won(rmw, rm_valid, k);
+    if (phase_owner(won_hc, won_rm, hc_valid)) {  // (so a valid workflow winner is this op: won_hc == hc_valid)
+      const uint32_t f = merge_phases(c.flags[i], won_hc, [&] { return arg; }, rm_valid,
+                                      [&] { return won_rm ? arg : ops[rmw - 1u].y; });
+      if (!is_live(f) || !(f & kPendBits)) {
         c.flags[i] = f;  // (a record the sweep does not evaluate keeps its posted result)
       } else {
         // Gather only what this result can touch (every column is its own 32-B sector of a random record):
@@ -1378,8 +1394,8 @@ __global__ void in_flight_kernel(DevCols c, const int64_t* __restrict__ since, u
   if (k >= n) return;
   const uint32_t i = idx ? idx[k] : first + k;
   const int64_t s = since[i];
-  const bool held = s != kNotInFlight && s >= c.finished_at[i] && !(c.flags[i] & (AM_F_PENDING_OK | AM_F_PENDING_FAIL));
-  out[k] = held && is_remedy_run(s) == remedy ? (remedy ? s - kRemedyRun : s) : kNotInFlight;
+  const bool held = held_run(s, [&] { return c.finished_at[i]; }, [&] { return c.flags[i]; });
+  out[k] = held && is_remedy_run(s) == remedy ? run_start(s) : kNotInFlight;
 }
 
 // Workflow timeouts: the drain's winning upserts (the marks decide, as in apply_state_ops_kernel) store their record's
@@ -1392,7 +1408,7 @@ __global__ void store_wf_timeout_kernel(int32_t* wf, const uint32_t* __restrict_
   if (k >= n) return;
   const uint2 op = ops[k];
   const uint32_t i = op.x, arg = op.y;
-  if ((arg & kOpKindMask) != kOpUpsert || marks[3u * i] != k + 1u) return;
+  if ((arg & kOpKindMask) != kOpUpsert || !state_op_won(marks, i, k)) return;
   wf[i] = recs[arg & ~kOpKindMask].wf_timeout;
 }
 
@@ -1429,7 +1445,8 @@ __global__ void expire_runs_kernel(DevCols c, int64_t* since, int64_t* deadline,
         deadline[i] = kNoDeadline;
         const uint32_t f = c.flags[i];
         const int64_t s = since[i];
-        if (is_live(f) && s != kNotInFlight && s >= c.finished_at[i] && !(f & (AM_F_PENDING_OK | AM_F_PENDING_FAIL))) {
+        // held_run, written out: through the call this kernel compiles to different machine code
+        if (is_live(f) && s != kNotInFlight && s >= c.finished_at[i] && !(f & kHcBits)) {
           // a remedy run (remedy hold, hcc.go:813-818) times out as a posted remedy "Failed"
           c.flags[i] = is_remedy_run(s) ? ((f & ~AM_F_REMEDY_OUTCOME_OK) | AM_F_REMEDY_PENDING) : (f | AM_F_PENDING_FAIL);
           since[i] = kNotInFlight;
@@ -1441,12 +1458,7 @@ __global__ void expire_runs_kernel(DevCols c, int64_t* since, int64_t* deadline,
       }
     }
     const uint32_t cnt = (uint32_t)__popc(hit);
-    uint32_t incl = cnt;  // inclusive prefix over the lanes
-#pragma unroll
-    for (unsigned o = 1; o < 32; o <<= 1) {
-      const uint32_t v = __shfl_up_sync(kFull, incl, o);
-      if ((unsigned)lane >= o) incl += v;
-    }
+    const uint32_t incl = warp_inclusive_scan(cnt, lane);
     const uint32_t total = __reduce_add_sync(kFull, cnt);
     uint32_t base = 0;
     if (total && lane == 0) base = atomicAdd(out_count, total);
@@ -1460,11 +1472,7 @@ __global__ void expire_runs_kernel(DevCols c, int64_t* since, int64_t* deadline,
         ++pos;
       }
     }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-      const unsigned long long v = __shfl_xor_sync(kFull, left, o);
-      left = v < left ? v : left;
-    }
+    left = warp_min(left);
     if (lane == 0) seg_deadline[seg] = left;
   }
 }
@@ -1474,9 +1482,8 @@ __global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ op
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const uint32_t i = ops[k].x;
-  marks[3u * i] = 0;
-  marks[3u * i + 1u] = 0;
-  marks[3u * i + 2u] = 0;
+#pragma unroll
+  for (uint32_t x = kMarkState; x <= kMarkRm; ++x) mark(marks, i, x) = 0;
 }
 
 // ---- status changes (am_sweep_set_track_changes) --------------------------------------------------------------
@@ -1485,7 +1492,6 @@ __global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ op
 // only the sweep decides, and after the sweep the bits are compacted into the tick's ascending slot list and cleared.
 // A set bit whose slot is not live when the list is built is dropped: the result kernels and the sweep apply nothing to
 // such a slot, and nothing between the drain and the list changes a kind or a tombstone.
-constexpr uint32_t kPendBits = AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING;
 
 // A drain's staged ops, after apply_state_ops_kernel and before anything applies a result.  One thread per slot decides
 // (the marks' rules, as in apply_results_now_kernel): the slot's latest upsert / remove, else its workflow-phase winner,
@@ -1498,15 +1504,15 @@ __global__ void note_ops_kernel(uint32_t* bits, const uint32_t* __restrict__ fla
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const uint32_t i = ops[k].x;
-  const uint32_t s_state = marks[3u * i], hcw = marks[3u * i + 1u], rmw = marks[3u * i + 2u];
-  const bool hc_valid = hcw != 0u && hcw >= s_state, rm_valid = rmw != 0u && rmw >= s_state;
+  const uint32_t s_state = mark(marks, i, kMarkState), hcw = mark(marks, i, kMarkHc), rmw = mark(marks, i, kMarkRm);
+  const bool hc_valid = phase_valid(hcw, s_state), rm_valid = phase_valid(rmw, s_state);
   uint32_t* w = bits + i / 32u;
   const uint32_t b = 1u << (i & 31u);
   if (s_state) {
-    if (s_state != k + 1u) return;
+    if (!mark_is(s_state, k)) return;
     if (hc_valid || rm_valid || (flags[i] & kPendBits)) atomicOr(w, b);
     else atomicAnd(w, ~b);
-  } else if (hcw == k + 1u || (rmw == k + 1u && !hc_valid)) {
+  } else if (phase_owner(phase_won(hcw, hc_valid, k), phase_won(rmw, rm_valid, k), hc_valid)) {
     atomicOr(w, b);
   }
 }
@@ -1564,7 +1570,7 @@ __global__ void note_exceptions_kernel(uint32_t* bits, const TickOut out, uint32
   const uint32_t ne = out.tile_exc[tile];
   for (uint32_t e = (uint32_t)lane; e < ne; e += 32u) {
     const uint32_t x = out.exc_seg[(size_t)tile * kTile + e];
-    const uint32_t off = x >> 8, a = x & 0xFFu, b = 1u << (off & 31u);
+    const uint32_t off = exc_offset(x), a = exc_action(x), b = 1u << (off & 31u);
     if (a & AM_ACT_STOPPED) atomicOr(w + off / 32u, b);
     else if ((a & AM_ACT_ANOMALY) || (closed && !(a & AM_ACT_SUBMIT_HC) && !(s_before[warp][off / 32u] & b)))
       atomicAnd(w + off / 32u, ~b);
@@ -1611,12 +1617,7 @@ __global__ void __launch_bounds__(kGroupWords) list_changes_kernel(uint32_t* bit
   const size_t wi = (size_t)g * kGroupWords + threadIdx.x;
   const uint32_t v = bits[wi];
   const uint32_t c = (uint32_t)__popc(v);
-  uint32_t incl = c;
-#pragma unroll
-  for (unsigned d = 1; d < 32; d <<= 1) {
-    const uint32_t up = __shfl_up_sync(kFull, incl, d);
-    if ((unsigned)lane >= d) incl += up;
-  }
+  const uint32_t incl = warp_inclusive_scan(c, lane);
   if (lane == 31) s_warp[warp] = incl;
   __syncthreads();
   uint32_t pos = base + incl - c;
@@ -1635,8 +1636,7 @@ __global__ void __launch_bounds__(kGroupWords) list_changes_kernel(uint32_t* bit
 // A result op carries its post call's tag in arg bits 8..29 (am_sweep_post_result: the call's first op index, mod
 // 2^22), which no other kernel reads: two entries of one call see the same in-flight state, as they do in call order.
 constexpr uint32_t kCallTagShift = 8, kCallTagMask = 0x3FFFFFu << kCallTagShift;
-static_assert((kCallTagMask & (kOpKindMask | AM_F_PENDING_OK | AM_F_PENDING_FAIL | AM_F_REMEDY_PENDING |
-                               AM_F_REMEDY_OUTCOME_OK)) == 0, "call tag bits");
+static_assert((kCallTagMask & (kOpKindMask | kHcBits | kRemedyBits)) == 0, "call tag bits");
 
 // The AM_CHG_* bits of a flags word's posted-result bits.
 __device__ __forceinline__ uint32_t applied_of(uint32_t f) {
@@ -1647,19 +1647,20 @@ __device__ __forceinline__ uint32_t applied_of(uint32_t f) {
 // A drain's ops, after apply_state_ops_kernel and before clear_since_kernel and the result kernels (the flags hold the
 // already-pending bits, since the in-flight state before the drain).  The slot's owner (note_ops_kernel's: its latest
 // upsert / remove, else its workflow-phase winner, else its remedy-phase winner) writes the pair: applied from the
-// posted bits the drain leaves (merge_phases, the result kernels' rule); start from the held run (in_flight_kernel's
-// rule) when a winner of its kind ends it, else an earlier drain's capture whose phase is still pending and not
-// replaced.  A state op drops the earlier capture (the record's own pending bits report no start).  `since` NULL:
-// the hold is off.  capture_superseded_kernel then drops a capture that an earlier call of the drain ended first.
+// posted bits the drain leaves (merge_phases, the result kernels' rule); start from the held run (held_run) when
+// a winner of its kind ends it, else an earlier drain's capture whose phase is still pending and not replaced.  A
+// state op drops the earlier capture (the record's own pending bits report no start).  `since` NULL: the hold is off.
+// capture_superseded_kernel then drops a capture that an earlier call of the drain ended first.
 __global__ void capture_ops_kernel(uint8_t* applied, int64_t* start, const DevCols c, const int64_t* __restrict__ since,
                                    const uint32_t* __restrict__ marks, const uint2* __restrict__ ops, uint32_t n) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const uint32_t i = ops[k].x;
-  const uint32_t s_state = marks[3u * i], hcw = marks[3u * i + 1u], rmw = marks[3u * i + 2u];
-  const bool hc_valid = hcw != 0u && hcw >= s_state, rm_valid = rmw != 0u && rmw >= s_state;
-  if (s_state ? s_state != k + 1u : !(hcw == k + 1u || (rmw == k + 1u && !hc_valid))) return;
+  const uint32_t s_state = mark(marks, i, kMarkState), hcw = mark(marks, i, kMarkHc), rmw = mark(marks, i, kMarkRm);
+  const bool hc_valid = phase_valid(hcw, s_state), rm_valid = phase_valid(rmw, s_state);
+  if (s_state ? !mark_is(s_state, k) : !phase_owner(phase_won(hcw, hc_valid, k), phase_won(rmw, rm_valid, k), hc_valid))
+    return;
   const uint32_t f = c.flags[i];
   const uint32_t fm = merge_phases(f, hc_valid, [&] { return ops[hcw - 1u].y; }, rm_valid, [&] { return ops[rmw - 1u].y; });
   int64_t w = kNotInFlight;
@@ -1670,7 +1671,8 @@ __global__ void capture_ops_kernel(uint8_t* applied, int64_t* start, const DevCo
   }
   if (since) {
     const int64_t s = since[i];
-    if (s != kNotInFlight && s >= c.finished_at[i] && !(f & kHcBits) && (is_remedy_run(s) ? rm_valid : hc_valid)) w = s;
+    if (held_run(s, [&] { return c.finished_at[i]; }, [&] { return f; }) && (is_remedy_run(s) ? rm_valid : hc_valid))
+      w = s;
   }
   start[i] = w;
   applied[i] = (uint8_t)applied_of(fm);
@@ -1689,7 +1691,7 @@ __global__ void capture_superseded_kernel(int64_t* start, const uint32_t* __rest
   const int64_t w = start[i];
   if (w == kNotInFlight) return;
   const bool rem = is_remedy_run(w);
-  const uint32_t win = marks[3u * i + (rem ? 2u : 1u)];
+  const uint32_t win = mark(marks, i, rem ? kMarkRm : kMarkHc);
   if (k + 1u >= win) return;  // (win == 0: an earlier drain's capture, which this drain does not replace)
   if (kind == kOpResult) {
     if (!((arg & kHcBits) || (rem && (arg & AM_F_REMEDY_PENDING)))) return;
@@ -1733,8 +1735,8 @@ __global__ void capture_sweep_kernel(uint8_t* applied, int64_t* start, const uin
   const uint32_t ne = out.tile_exc[tile];
   for (uint32_t e = (uint32_t)lane; e < ne; e += 32u) {
     const uint32_t x = out.exc_seg[(size_t)tile * kTile + e];
-    const size_t i = (size_t)tile * kTile + (x >> 8);
-    if ((x & AM_ACT_STOPPED) && !((bits[i / 32u] >> (i & 31u)) & 1u)) {
+    const size_t i = (size_t)tile * kTile + exc_offset(x);
+    if ((exc_action(x) & AM_ACT_STOPPED) && !((bits[i / 32u] >> (i & 31u)) & 1u)) {
       applied[i] = 0;
       start[i] = kNotInFlight;
     }
@@ -1780,15 +1782,16 @@ __global__ void gather_details_kernel(const uint32_t* __restrict__ idx, uint32_t
   uint32_t lo = 0, hi = out.tile_exc[tile];
   while (lo < hi) {
     const uint32_t mid = (lo + hi) / 2u;
-    if ((e[mid] >> 8) < off) lo = mid + 1u;
+    if (exc_offset(e[mid]) < off) lo = mid + 1u;
     else hi = mid;
   }
-  if (lo < out.tile_exc[tile] && (e[lo] >> 8) == off) act = e[lo] & 0xFFu;
+  if (lo < out.tile_exc[tile] && exc_offset(e[lo]) == off) act = exc_action(e[lo]);
   uint32_t a = e_applied[k];
   const int64_t w = e_start[k];
   am_change_detail_t d;
   d.started = (a & (AM_CHG_SUCCEEDED | AM_CHG_FAILED)) && w != kNotInFlight && !is_remedy_run(w) ? w : kNotInFlight;
-  d.remedy_started = (a & (AM_CHG_REMEDY_SUCCEEDED | AM_CHG_REMEDY_FAILED)) && is_remedy_run(w) ? w - kRemedyRun : kNotInFlight;
+  d.remedy_started =
+      (a & (AM_CHG_REMEDY_SUCCEEDED | AM_CHG_REMEDY_FAILED)) && is_remedy_run(w) ? run_start(w) : kNotInFlight;
   if (act & AM_ACT_STOPPED) a |= AM_CHG_STOPPED;
   if (closed && (act & AM_ACT_SUBMIT_HC)) {
     a |= AM_CHG_CLOSED_LOOP;

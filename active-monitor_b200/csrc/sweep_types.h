@@ -104,8 +104,12 @@ struct TickOut {
   uint32_t* group_count;   // [n_groups] emitted records per group (REDs of the tiles; zero on entry)
   uint32_t* group_prefix;  // [n_groups + 1] exclusive prefix of group_count (scan_groups_kernel)
   uint32_t* tile_exc;      // [n_tiles] exceptions per tile
-  uint32_t* exc_seg;       // [n_tiles * 1024] per tile: (offset in tile << 8) | action, ascending
+  uint32_t* exc_seg;       // [n_tiles * 1024] per tile: exception entries (exc_entry), ascending
 };
+// An exception entry: the record's offset in its tile above its 8 action bits (a tile's entries ascend by record).
+AM_HD uint32_t exc_entry(uint32_t off, uint32_t act) { return (off << 8) | act; }
+AM_HD uint32_t exc_offset(uint32_t e) { return e >> 8; }
+AM_HD uint32_t exc_action(uint32_t e) { return e & 0xFFu; }
 
 struct SweepParams {
   DevCols c;
@@ -137,7 +141,9 @@ constexpr int64_t kNoDeadline = INT64_MAX;
 // below is a health-check run; a check has at most one run of either kind in flight, so they share the word (and the
 // deadline word).
 constexpr int64_t kRemedyRun = 1ll << 60;
-__device__ __forceinline__ bool is_remedy_run(int64_t since) { return since >= kRemedyRun / 2; }
+AM_HD bool is_remedy_run(int64_t since) { return since >= kRemedyRun / 2; }
+// the start of the run a since word holds, of either kind (kNotInFlight stays kNotInFlight)
+AM_HD int64_t run_start(int64_t since) { return is_remedy_run(since) ? since - kRemedyRun : since; }
 // a signed second as an unsigned key of the same order (the atomicMin idiom of next_due_kernel); kNoDeadline -> ~0
 __device__ __forceinline__ unsigned long long biased_key(int64_t t) { return (unsigned long long)t ^ (1ull << 63); }
 
