@@ -1,5 +1,5 @@
 """Hand-derived cases of the change details (am_sweep_set_change_details), written against a driver: the oracle alone
-(change_details_oracle.Model, tests/test_change_details_oracle.py) or a handle compared with it after every tick
+(tests/handle_model.py, tests/test_change_details_oracle.py) or a handle compared with it after every tick
 (tests/test_change_details_gpu.py, through every tick entry point).  A driver has upsert, remove, post, read(slots),
 load(first, cols), set_details(on), tick(T, mode=0) -> (global idx, action, stats, ...), changes() and details() -> the
 last tick's details (change_details_oracle.DETAIL, one per listed slot).  `hold` and `n` as in changes_cases.

@@ -1,5 +1,5 @@
 """The change details of a tick (am_sweep_set_change_details / am_sweep_last_change_details), defined from the existing
-models alone, around changes_oracle.Model (which gives the listed slots):
+models alone, around changes_oracle.changed (which gives the listed slots); tests/handle_model.py takes the starts:
 
   applied         the posted-result bits of the state just before the tick (every call before it applied, as the
                   models apply them) that the tick consumed, as AM_CHG_* bits; plus FAILED | TIMED_OUT for a slot in
@@ -17,8 +17,6 @@ An upsert, remove or load of a slot drops what was taken for it (its pending pha
 are off, and turning them on drops everything: results pending from before report INT64_MIN.  Nothing is taken from
 the device's mechanism (drain marks, since words, call tags)."""
 import numpy as np
-
-import changes_oracle
 
 NONE = np.int64(np.iinfo(np.int64).min)
 F_PENDING_OK, F_PENDING_FAIL, F_REMEDY_PENDING, F_REMEDY_OUTCOME_OK = 1 << 4, 1 << 5, 1 << 6, 1 << 7
@@ -83,72 +81,3 @@ def details(listed, before_flags, out, T, mode, hc, rm, shard_base=0):
     d = np.zeros(len(listed), dtype=DETAIL)
     d["started"], d["remedy_started"], d["applied"], d["action"] = st, rst, a, act
     return d
-
-
-class Model(changes_oracle.Model):
-    """changes_oracle.Model and the details of its last tick; details on from the start unless `details` is False"""
-
-    def __init__(self, zmap, n, hold=None, shard_base=0, seed=0, details=True):
-        super().__init__(zmap, n, hold, shard_base, seed)
-        self.on = details
-        self.hc, self.rm = {}, {}
-        self.det = np.zeros(0, dtype=DETAIL)
-
-    def in_flight(self):
-        """(in_flight(), remedy_in_flight()) of every slot, as the models have them"""
-        if self.hold == "remedy":
-            return self.m.in_flight(), self.m.remedy_in_flight()
-        return self.m.in_flight(0, self.n), np.full(self.n, NONE, dtype=np.int64)
-
-    def set_details(self, on):
-        if on and not self.on:
-            self.det = np.zeros(0, dtype=DETAIL)  # (the last tick's list has no details)
-        self.on = bool(on)
-        self.hc, self.rm = {}, {}
-
-    def _drop(self, slots):
-        for i in np.asarray(slots, dtype=np.int64).tolist():
-            self.hc.pop(i, None)
-            self.rm.pop(i, None)
-
-    def upsert(self, slots, recs):
-        super().upsert(slots, recs)
-        self._drop(slots)
-
-    def remove(self, slots):
-        super().remove(slots)
-        self._drop(slots)
-
-    def load(self, first, cols):
-        super().load(first, cols)
-        self._drop(np.arange(first, first + len(cols["flags"])))
-
-    def post(self, slots, phase, rphase=None):
-        if self.on:
-            v, rv = self.in_flight()
-            sl = np.asarray(slots, dtype=np.int64)
-            ph = np.asarray(phase)
-            rp = np.asarray(rphase) if rphase is not None else np.zeros(len(sl), np.uint8)
-            for k, i in enumerate(sl.tolist()):
-                if ph[k]:
-                    self.hc[i] = v[i]
-                if rp[k]:
-                    self.rm[i] = rv[i]
-        super().post(slots, phase, rphase)
-
-    def tick(self, T, mode=0):
-        before = self.cols["flags"].copy()
-        out = super().tick(T, mode)
-        if self.on:
-            self.det = details(self.last, before, out, T, mode, self.hc, self.rm, self.shard_base)
-        self.hc, self.rm = {}, {}
-        return out
-
-    def run_ticks(self, T0, n, mode=0, seed=0):
-        rows = super().run_ticks(T0, n, mode, seed)
-        self.det = np.zeros(0, dtype=DETAIL)
-        self.hc, self.rm = {}, {}
-        return rows
-
-    def details(self):
-        return self.det

@@ -1,5 +1,5 @@
 """Hand-derived cases of the status changes (am_sweep_set_track_changes), written against a driver: the oracle alone
-(changes_oracle.Model, tests/test_changes_oracle.py) or a handle compared with it after every tick
+(tests/handle_model.py, tests/test_changes_oracle.py) or a handle compared with it after every tick
 (tests/test_status_changes_gpu.py, through every tick entry point).  A driver has upsert, remove, post, read(slots),
 tick(T, mode=0) -> (global idx, action, stats, ...) and changes() -> the last tick's changed set (global idx).  Each case
 names the hold it needs in its `hold` attribute (None, "hold" or "remedy": the hold with timeouts and the remedy

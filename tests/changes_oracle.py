@@ -5,14 +5,11 @@ carry bits (AM_F_CARRY_MASK) and the posted-result bits AM_F_PENDING_* / AM_F_RE
 records whose action carries AM_ACT_ANOMALY without AM_ACT_STOPPED are taken out: the reference panics at hcc.go:690
 before it writes a status (DESIGN.md section 6 item 5), although the oracles count the Failed.
 
-The states come from sequence_model.SequenceModel (plain ticks, catch-up ticks, closed loop, the hold in flight) or
-remedy_hold_oracle.State (the hold with workflow timeouts and the remedy hold).  Nothing is taken from the device's
-mechanism (drain marks, exceptions, bitmaps)."""
+The states come from tests/handle_model.py.  Nothing is taken from the device's mechanism (drain marks, exceptions,
+bitmaps)."""
 import numpy as np
 
 import oracle_c
-import remedy_hold_oracle
-from sequence_model import SequenceModel
 
 COLUMN_NAMES = [n for n, _ in oracle_c.COLUMNS]
 F_RESULT_BITS = (1 << 4) | (1 << 5) | (1 << 6) | (1 << 7)
@@ -47,53 +44,3 @@ def empty_columns(n):
     cols = {name: np.zeros(n, dtype=dt) for name, dt in oracle_c.COLUMNS}
     cols["flags"][:] = F_TOMBSTONE
     return cols
-
-
-class Model:
-    """one oracle state and the changed set of its last tick.  hold: None (off), "hold" (the hold in flight) or
-    "remedy" (the hold, workflow timeouts and the remedy hold).  Calls as the models have them; a read drains on the
-    handle and changes nothing here."""
-
-    def __init__(self, zmap, n, hold=None, shard_base=0, seed=0):
-        self.hold, self.n, self.shard_base = hold, n, shard_base
-        if hold == "remedy":
-            self.m = remedy_hold_oracle.State(zmap, empty_columns(n), shard_base)
-        else:
-            self.m = SequenceModel(zmap, n, shard_base, seed=seed)
-            self.m.set_hold(hold == "hold")
-        self.last = EMPTY
-
-    @property
-    def cols(self):
-        return self.m.ocols if self.hold == "remedy" else self.m.cols
-
-    def upsert(self, slots, recs):
-        self.m.upsert(slots, recs)
-
-    def remove(self, slots):
-        self.m.remove(slots)
-
-    def post(self, slots, phase, rphase=None):
-        self.m.post(slots, phase, rphase)
-
-    def load(self, first, cols):
-        self.m.load(first, cols)
-
-    def read(self, slots):
-        pass
-
-    def tick(self, T, mode=0):
-        """the oracle's tick: (global idx, action, stats[, timed-out, remedy timed-out])"""
-        before = snapshot(self.cols)
-        out = self.m.tick(T, mode)
-        self.last = changed(before, self.cols, out[0], out[1], self.shard_base)
-        return out
-
-    def run_ticks(self, T0, n, mode=0, seed=0):
-        """am_sweep_run_ticks: it tracks nothing and empties the list"""
-        rows = self.m.run_ticks(T0, n, mode, seed)
-        self.last = EMPTY
-        return rows
-
-    def changes(self):
-        return self.last

@@ -28,6 +28,7 @@ lib = abi.load()
 
 import amgen  # noqa: E402
 import change_details_oracle  # noqa: E402
+from handle_model import HandleModel  # noqa: E402
 from adversarial import ZoneMap, product_lookup  # noqa: E402
 
 world, idx_bytes, n_total, config = (int(a) for a in sys.argv[1:5])
@@ -43,7 +44,7 @@ bases = np.array([s[0] for s in shards], dtype=np.uint64)
 sizes = np.array([s[1] for s in shards], dtype=np.uint64)
 
 rng = np.random.default_rng(world * 1000 + config)
-model = change_details_oracle.Model(zmap, n_total)
+model = HandleModel(zmap, n_total, track=True, details=True)
 model.upsert(np.arange(n_total), am.columns_to_records(whole))
 want, posts = [], []
 for k, (T, catch_up) in enumerate(TICKS):

@@ -4,7 +4,7 @@ population (half of it with a remedy workflow), turns tracking on, upserts its r
 (am_sweep_tick_shard, then the exchange).  Between ticks results are posted, each to the rank that owns its slot (one
 tick's batch dense enough for the sweep to apply it), and some ranks read in between.  Every rank's global list must
 equal the oracle of the UNSHARDED population, and its am_sweep_last_changes the part of the changed-set oracle
-(tests/changes_oracle.py) it owns, with the oracle's columns.
+(tests/changes_oracle.py, through tests/handle_model.py) it owns, with the oracle's columns.
 
 usage: run_gather_changes.py <world> <idx_bytes> <records in total> <config>
 Prints "ok ..." and exits 0 on success."""
@@ -26,8 +26,8 @@ gather = importlib.import_module("active-monitor_b200.gather")
 lib = abi.load()
 
 import amgen  # noqa: E402
-import changes_oracle  # noqa: E402
 from adversarial import ZoneMap, product_lookup  # noqa: E402
+from handle_model import HandleModel  # noqa: E402
 
 world, idx_bytes, n_total, config = (int(a) for a in sys.argv[1:5])
 T0 = 1790898290  # 2026-10-01 23:44:50 UTC
@@ -42,7 +42,7 @@ bases = np.array([s[0] for s in shards], dtype=np.uint64)
 sizes = np.array([s[1] for s in shards], dtype=np.uint64)
 
 rng = np.random.default_rng(world * 1000 + config)
-model = changes_oracle.Model(zmap, n_total)
+model = HandleModel(zmap, n_total, track=True)
 model.upsert(np.arange(n_total), am.columns_to_records(whole))
 want, posts = [], []
 for k, (T, catch_up) in enumerate(TICKS):
@@ -53,7 +53,7 @@ for k, (T, catch_up) in enumerate(TICKS):
     model.post(sl, ph, rp)
     posts.append((sl, ph, rp))
     out = model.tick(T, abi.SWEEP_CATCH_UP if catch_up else 0)
-    want.append((out[0], out[1], model.changes(), {n: model.cols[n][model.changes()].copy() for n in abi.COLUMN_NAMES}))
+    want.append((out[0], out[1], model.changes(), {n: model.cols()[n][model.changes()].copy() for n in abi.COLUMN_NAMES}))
 assert sum(len(w[2]) for w in want) > n_total // 8
 
 handles = [None] * world

@@ -28,10 +28,8 @@ gather = importlib.import_module("active-monitor_b200.gather")
 lib = abi.load()
 
 import amgen  # noqa: E402
-import hold_oracle  # noqa: E402
-import remedy_hold_oracle  # noqa: E402
-import timeout_oracle  # noqa: E402
 from adversarial import ZoneMap, product_lookup  # noqa: E402
+from handle_model import NONE, HandleModel  # noqa: E402
 
 world, idx_bytes, n_total, config = (int(a) for a in sys.argv[1:5])
 T0 = 1790898290  # 2026-10-01 23:44:50 UTC
@@ -45,32 +43,25 @@ shards = [gather.shard_range(n_total, r, world) for r in range(world)]
 bases = np.array([s[0] for s in shards], dtype=np.uint64)
 sizes = np.array([s[1] for s in shards], dtype=np.uint64)
 
-# the oracle run first: it decides which in-flight checks post a phase before each tick
+# the model run first: it decides which in-flight checks post a phase before each tick
 rng = np.random.default_rng(world * 1000 + config)
-ocols = {k: v.copy() for k, v in whole.items()}
-ocols["flags"] &= np.uint32(~abi.F_TOMBSTONE & 0xFFFFFFFF)  # (upserted, not loaded: an upsert is never a tombstone)
-since = hold_oracle.none_in_flight(n_total)
-deadline = timeout_oracle.no_deadlines(n_total)
-rsince = hold_oracle.none_in_flight(n_total)
-rdeadline = timeout_oracle.no_deadlines(n_total)
 wf = np.random.default_rng(world * 77 + config).integers(0, 120, n_total).astype(np.int32)
-want, posts, P = [], [], None
-hc = np.uint32(abi.F_PENDING_OK | abi.F_PENDING_FAIL)
+model = HandleModel(zmap, n_total, hold=True, remedy=True)
+recs = am.columns_to_records(whole)
+recs["wf_timeout"] = wf
+model.upsert(np.arange(n_total), recs)
+want, posts = [], []
 for k, (T, catch_up) in enumerate(TICKS):
-    fl = np.flatnonzero(since != hold_oracle.NOT_IN_FLIGHT)
+    fl = np.flatnonzero(model.since != NONE)
     sl = np.sort(rng.choice(fl, min(len(fl), 60), replace=False)) if k and len(fl) else np.zeros(0, np.int64)
     ph = rng.integers(1, 3, len(sl)).astype(np.uint8)
     ph = np.where(rng.random(len(sl)) < 0.8, 2, 1).astype(np.uint8)
-    ocols["flags"][sl] = (ocols["flags"][sl] & ~hc) | np.where(ph == 1, abi.F_PENDING_OK, abi.F_PENDING_FAIL).astype(np.uint32)
-    hold_oracle.post(since, sl, ph)
-    rl = np.flatnonzero(rsince != hold_oracle.NOT_IN_FLIGHT)
+    model.post(sl, ph)
+    rl = np.flatnonzero(model.rsince != NONE)
     rl = np.sort(rng.choice(rl, min(len(rl), 20), replace=False)) if len(rl) else np.zeros(0, np.int64)
-    ocols["flags"][rl] |= np.uint32(abi.F_REMEDY_PENDING | abi.F_REMEDY_OUTCOME_OK)
-    rsince[rl] = hold_oracle.NOT_IN_FLIGHT
-    rdeadline[rl] = timeout_oracle.NO_DEADLINE
+    model.post(rl, np.zeros(len(rl), np.uint8), np.ones(len(rl), np.uint8))
     posts.append((sl, ph, rl))
-    want.append(remedy_hold_oracle.sweep(zmap, ocols, since, deadline, wf, rsince, rdeadline, T, P=P if catch_up else None))
-    P = T
+    want.append(model.tick(T, abi.SWEEP_CATCH_UP if catch_up else 0))
 assert sum(int(((w[1] & abi.ACT_SUBMIT_HC) != 0).sum()) for w in want[1:]) > 0
 assert sum(len(w[3][0]) for w in want) > 100 and sum(len(w[4][0]) for w in want) > 20
 
@@ -144,10 +135,10 @@ def rank_main(rank):
         bar.wait()
         dev = s.read_range(0, cnt)
         for name in abi.COLUMN_NAMES:
-            np.testing.assert_array_equal(dev[name], ocols[name][first:first + cnt], err_msg=f"rank {rank} column {name}")
-        np.testing.assert_array_equal(s.in_flight(0, cnt), hold_oracle.in_flight(ocols, since)[first:first + cnt],
+            np.testing.assert_array_equal(dev[name], model.cols()[name][first:first + cnt], err_msg=f"rank {rank} column {name}")
+        np.testing.assert_array_equal(s.in_flight(0, cnt), model.in_flight()[first:first + cnt],
                                       err_msg=f"rank {rank} in_flight")
-        np.testing.assert_array_equal(s.remedy_in_flight(0, cnt), remedy_hold_oracle.in_flight(ocols, rsince)[first:first + cnt],
+        np.testing.assert_array_equal(s.remedy_in_flight(0, cnt), model.remedy_in_flight()[first:first + cnt],
                                       err_msg=f"rank {rank} remedy_in_flight")
         # a closed-loop step is refused on every rank before anything happens (no exchange needed)
         rc = lib.am_sweep_tick_shard(s._h, TICKS[-1][0] + 1, abi.SWEEP_CLOSED_LOOP, None)
@@ -174,4 +165,4 @@ if errors:
     sys.exit(1)
 assert all(v > 0 for v in n_rtimed), n_rtimed  # every shard timed out remedy runs of its own
 print(f"ok remedy hold remedy_timed_out_per_rank={n_rtimed} timed_out_per_rank={n_timed} world={world} idx_bytes={idx_bytes} n={n_total} config={config} "
-      f"emitted={[len(w[0]) for w in want]} remedy_held={int(remedy_hold_oracle.held(ocols, rsince).sum())}")
+      f"emitted={[len(w[0]) for w in want]} remedy_held={int((model.remedy_in_flight() != NONE).sum())}")

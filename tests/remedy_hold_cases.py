@@ -1,14 +1,24 @@
 """Hand-derived cases of the remedy hold (am_sweep_set_hold_remedy, with the hold in flight on), written against a
-`driver`: the remedy-hold oracle alone (tests/test_remedy_hold_oracle.py) or a handle compared with it after every tick
+`driver`: the model alone (tests/handle_model.py) or a handle compared with it after every tick
 (tests/test_remedy_hold_gpu.py, through every tick entry point).  A driver starts with the hold and the remedy hold on
 and has upsert(slots, recs), remove(slots), load(first, cols), post(slots, phase, rphase=None), tick(T, mode=0) ->
 (global idx, action, stats, (timed-out idx, since), (remedy timed-out idx, start)), in_flight(), remedy_in_flight(),
-cols(), set_hold(on) and set_remedy(on) -> return code."""
+cols(), set_hold(on) and set_remedy(on), which raise handle_model.Refused when refused."""
 import numpy as np
 
+from handle_model import Refused
 from timeout_cases import M0, NONE, REMEDY_SKIP, RUN_REMEDY, SUBMIT, _acts, _timed, rec
 
 OK, FAIL = 1, 2
+
+
+def _rc(call, on):
+    """the return code of a switch: 0, or the code it was refused with"""
+    try:
+        call(on)
+    except Refused as r:
+        return r.code
+    return 0
 
 
 def _rtimed(out):
@@ -53,7 +63,7 @@ def slow_remedy_limit(am, d):
 def slow_remedy_without_the_hold(am, d):
     """the same sequence without the remedy hold: every failure while a remedy runs reads RemedyTotalRuns == 0 and
     starts another (the defect the remedy hold removes)"""
-    assert d.set_remedy(False) == 0
+    assert _rc(d.set_remedy, False) == 0
     started, skips, most = _slow_remedies(am, d)
     assert started > 2 and most > 2, (started, skips, most)
 
@@ -152,13 +162,13 @@ def releases(am, d):
     out = d.tick(M0 + 61)
     assert out[2]["n_result_ok"] == 1 and len(out[0]) == 0
     assert d.remedy_in_flight()[:5].tolist() == [NONE, NONE, NONE, M0 + 60, M0 + 60]
-    assert d.set_remedy(False) == 0 and d.set_remedy(True) == 0
+    assert _rc(d.set_remedy, False) == 0 and _rc(d.set_remedy, True) == 0
     assert (d.remedy_in_flight() == NONE).all()
     d.post([3], [FAIL])
     out = d.tick(M0 + 120)
     assert _acts(out) == {0: SUBMIT, 2: SUBMIT, 3: RUN_REMEDY, 4: SUBMIT}
     assert d.remedy_in_flight()[3] == M0 + 120
-    assert d.set_hold(False) == 0 and d.set_hold(True) == 0
+    assert _rc(d.set_hold, False) == 0 and _rc(d.set_hold, True) == 0
     assert (d.remedy_in_flight() == NONE).all() and (d.in_flight() == NONE).all()
     d.post([4], [FAIL])
     assert _acts(d.tick(M0 + 180)) == {k: SUBMIT for k in (0, 2, 3)} | {4: SUBMIT | RUN_REMEDY}
@@ -166,14 +176,14 @@ def releases(am, d):
 
 def refused_without_the_hold(am, d):
     """am_sweep_set_hold_remedy while the hold in flight is off returns AM_E_INVAL and changes nothing"""
-    assert d.set_hold(False) == 0
-    assert d.set_remedy(True) == am.AM_E_INVAL and d.set_remedy(False) == am.AM_E_INVAL
-    assert d.set_hold(True) == 0
+    assert _rc(d.set_hold, False) == 0
+    assert _rc(d.set_remedy, True) == am.AM_E_INVAL and _rc(d.set_remedy, False) == am.AM_E_INVAL
+    assert _rc(d.set_hold, True) == 0
     d.upsert([0], rec(am, 0, cron="* * * * *", has_remedy=True))
     assert _acts(d.tick(M0)) == {0: SUBMIT}
     d.post([0], [FAIL])
     assert _acts(d.tick(M0 + 60)) == {0: SUBMIT | RUN_REMEDY}  # the remedy hold stayed off
-    assert d.set_remedy(True) == 0
+    assert _rc(d.set_remedy, True) == 0
 
 
 CASES = [slow_remedy_limit, slow_remedy_without_the_hold, merged_remedy_holds_nothing,

@@ -13,8 +13,8 @@ place of since).  A tick at T:
      SUBMIT_HC is dropped and n_submit_hc decremented (an open-loop submit writes no column), rsince = T,
      rdeadline = T + W when the slot's W > 0, and the health-check since and deadline are cleared; every entry still
      submitted ends the slot's remedy run (a check has one run in flight).
-A posted workflow or remedy phase, a remove, a load and toggling either hold end a remedy run; an upsert does not.
-With the remedy hold off the state is timeout_oracle.State's alone."""
+A posted workflow or remedy phase, a remove, a load and toggling either hold end a remedy run; an upsert does not
+(tests/handle_model.py keeps the runs for one handle, in call order)."""
 import numpy as np
 
 import hold_oracle
@@ -76,80 +76,3 @@ def sweep(zmap, ocols, since, deadline, wf, rsince, rdeadline, T, P=None, shard_
     rdeadline[sl] = np.where(w > 0, T + w, NO_DEADLINE)
     since[:] = np.where(shown == ALWAYS_HELD, np.int64(NONE), shown)
     return idx, act, st, timed, rtimed
-
-
-def first_event(zmap, ocols, since, deadline, wf, rsince, rdeadline, T, horizon):
-    """the first second of (T, T + horizon] at which a plain tick emits anything, applies a result or times a run of
-    either kind out, by brute force over copies; None when there is none"""
-    c = {k: v.copy() for k, v in ocols.items()}
-    s, d, rs, rd = since.copy(), deadline.copy(), rsince.copy(), rdeadline.copy()
-    for t in range(T + 1, T + horizon + 1):
-        idx, _, st, timed, rtimed = sweep(zmap, c, s, d, wf, rs, rd, t)
-        if (len(idx) or len(timed[0]) or len(rtimed[0]) or st["n_result_ok"] or st["n_result_fail"] or st["n_remedy_ok"]
-                or st["n_remedy_fail"]):
-            return t
-    return None
-
-
-class State(timeout_oracle.State):
-    """the oracle side of one handle with the hold on: timeout_oracle.State plus the remedy runs and the switch"""
-
-    def __init__(self, zmap, cols, shard_base=0, remedy=True):
-        super().__init__(zmap, cols, shard_base)
-        self.rsince = hold_oracle.none_in_flight(self.n)
-        self.rdeadline = timeout_oracle.no_deadlines(self.n)
-        self.remedy = remedy
-
-    def _end(self, slots):
-        self.rsince[slots] = NONE
-        self.rdeadline[slots] = NO_DEADLINE
-
-    def remove(self, slots):
-        super().remove(slots)
-        self._end(np.asarray(slots, dtype=np.int64))
-
-    def post(self, slots, phase, rphase=None):
-        super().post(slots, phase, rphase)
-        slots = np.asarray(slots, dtype=np.int64)
-        ends = np.asarray(phase) != 0
-        if rphase is not None:
-            ends |= np.asarray(rphase) != 0
-        self._end(slots[ends])
-
-    def load(self, first, cols):
-        super().load(first, cols)
-        self._end(np.arange(first, first + len(cols["flags"])))
-
-    def hold_on_again(self):
-        """am_sweep_set_hold_in_flight off, then on: the remedy hold is off as well"""
-        super().hold_on_again()
-        self._end(slice(None))
-        self.remedy = False
-
-    def set_remedy(self, on):
-        """am_sweep_set_hold_remedy while the hold is on"""
-        if not on:
-            self._end(slice(None))
-        self.remedy = bool(on)
-
-    def tick(self, T, mode=0):
-        """(global idx, action, stats, timed_out, remedy_timed_out)"""
-        P = self.P if (mode & timeout_oracle.CATCH_UP) and self.P is not None and T > self.P else None
-        if self.remedy:
-            out = sweep(self.zmap, self.ocols, self.since, self.deadline, self.wf, self.rsince, self.rdeadline, T, P=P,
-                        shard_base=self.shard_base)
-        else:
-            out = timeout_oracle.sweep(self.zmap, self.ocols, self.since, self.deadline, self.wf, T, P=P,
-                                       shard_base=self.shard_base)
-            out = out + ((np.zeros(0, dtype=np.uint64), np.zeros(0, dtype=np.int64)),)
-        self.P = T
-        return out
-
-    def remedy_in_flight(self):
-        return in_flight(self.ocols, self.rsince)
-
-    def next_event(self, T, horizon):
-        if not self.remedy:
-            return super().next_event(T, horizon)
-        return first_event(self.zmap, self.ocols, self.since, self.deadline, self.wf, self.rsince, self.rdeadline, T,
-                           horizon)

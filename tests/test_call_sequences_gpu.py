@@ -1,5 +1,5 @@
 """Random call sequences through every entry point of a sweep handle, compared after every call with one sequential
-model (tests/sequence_model.py): upserts with duplicate slots that flip kinds and zones, removes, sparse and dense
+model (tests/handle_model.py): upserts with duplicate slots that flip kinds and zones, removes, sparse and dense
 posts (some from four threads), calls past the 32 K-op copy chunk, loads at ragged offsets over slots with staged
 calls, the hold turned on and off, every query, and ticks through am_sweep_tick (short buffers and last_list
 included), _tick_view, _tick_device (the handle's stream, a torch stream, the default stream), _tick_shard and
@@ -15,10 +15,10 @@ import zlib
 import numpy as np
 import pytest
 
-import hold_oracle
 import oracle_c
 from adversarial import MONROVIA, ZoneMap, first_difference, oracle_lookup, population, zones_usable
-from sequence_model import NONE, Refused, SequenceModel
+from handle_model import NONE, HandleModel, Refused
+from handle_pair import DevOut, check_changes, check_details, emulated
 
 pytestmark = pytest.mark.gpu
 
@@ -31,10 +31,6 @@ CHUNK = 32 * 1024  # ops per copy chunk of the staging arrays (kFlushOps)
 @pytest.fixture(scope="module")
 def zmap(am, orc):
     return ZoneMap()
-
-
-def _emulated(am):
-    return "emu" in os.path.basename(am.abi.LIB_PATH)
 
 
 def _interval(am, n, ras, fa):
@@ -57,7 +53,7 @@ def test_load_range_after_staged_calls(am, zmap, case):
     if case in ("probe", "probe_hold"):
         A = am.records_to_columns(_interval(am, 8, 60, T - 60))        # due at T
         B = _interval(am, 1, 60, T)                                    # not due at T
-        m = SequenceModel(zmap, 8)
+        m = HandleModel(zmap, 8)
         with am.Sweep(capacity=8) as s:
             if case == "probe_hold":
                 s.set_hold_in_flight(True)
@@ -95,7 +91,7 @@ def test_load_range_after_staged_calls(am, zmap, case):
         assert idx.tolist() == ([0, 1, 2] if case == "probe_hold" else list(range(8))), idx.tolist()
         assert (act == am.ACT_SUBMIT_HC).all()
         assert st["n_result_fail"] == 0 and st["n_result_ok"] == (case == "probe_hold"), st
-        assert first_difference(am, got, want, dev, m.cols) is None
+        assert first_difference(am, got, want[:3], dev, m.cols()) is None
         for name in am.COLUMN_NAMES:  # three fresh copies of A
             np.testing.assert_array_equal(dev[name][:3], three[name], err_msg=name)
     else:
@@ -105,7 +101,7 @@ def test_load_range_after_staged_calls(am, zmap, case):
         every = am.records_to_columns(_cron(am, n, "* * * * *"))
         paris = _cron(am, 11, "CRON_TZ=Europe/Paris 30 3 * * *")  # another kind and zone, not due at T
         quiet = _interval(am, 4, 3600, T)
-        m = SequenceModel(zmap, n)
+        m = HandleModel(zmap, n)
         with am.Sweep(capacity=n) as s:
             s.load_range(0, every)
             m.load(0, every)
@@ -118,14 +114,14 @@ def test_load_range_after_staged_calls(am, zmap, case):
             m.load(133, part)
             for t in (T, T + 60):
                 gi, ga, gs = s.tick(t)
-                wi, wa, ws = m.tick(t, 0)
+                wi, wa, ws = m.tick(t, 0)[:3]
                 assert gs == ws, (t, gs, ws)
                 np.testing.assert_array_equal(gi, wi)
                 np.testing.assert_array_equal(ga, wa)
             assert {130, 131, 132, 129, 200}.isdisjoint(gi.tolist()) and {133, 140, 150, 151, 152} <= set(gi.tolist())
             got = s.read_range(0, n)
             for name in am.COLUMN_NAMES:
-                np.testing.assert_array_equal(got[name], m.cols[name], err_msg=name)
+                np.testing.assert_array_equal(got[name], m.cols()[name], err_msg=name)
 
 
 def test_a_tick_shard_without_an_exchange_leaves_no_statistics(am, zmap):
@@ -133,7 +129,7 @@ def test_a_tick_shard_without_an_exchange_leaves_no_statistics(am, zmap):
     without one counts only its own"""
     T = 1790812800 + 7
     recs = _interval(am, 64, 3600, T - 10)
-    m = SequenceModel(zmap, 64)
+    m = HandleModel(zmap, 64)
     with am.Sweep(capacity=64) as s:
         for c in (s, m):
             c.upsert(np.arange(64), recs)
@@ -170,38 +166,11 @@ def _capacity(k, cap):
     return int(env.split(",")[k]) if env else cap
 
 
-class DevOut:
-    """output arrays of am_sweep_tick_device: torch device memory, or host memory on the CPU emulator"""
-
-    def __init__(self, am, n):
-        self.emu = _emulated(am)
-        self.n = n
-        if self.emu:
-            self.t = [np.zeros(n + 4, np.uint32), np.zeros(n + 4, np.uint8), np.zeros(4, np.uint32), np.zeros(16, np.uint64)]
-            self.ptr = [a.ctypes.data for a in self.t]
-        else:
-            import torch
-            self.t = [torch.zeros(n + 4, dtype=torch.int32, device="cuda"), torch.zeros(n + 4, dtype=torch.uint8, device="cuda"),
-                      torch.zeros(4, dtype=torch.int32, device="cuda"), torch.zeros(16, dtype=torch.int64, device="cuda")]
-            self.ptr = [a.data_ptr() for a in self.t]
-
-    def tick(self, am, s, T, mode, cap, stream):
-        s.tick_device(T, mode, self.ptr[0], self.ptr[1], cap, self.ptr[2], self.ptr[3], stream=stream)
-        if self.emu:
-            idx, act, cnt, st = self.t
-        else:
-            import torch
-            torch.cuda.synchronize()
-            idx, act, cnt, st = [a.cpu().numpy() for a in self.t]
-        k = int(cnt.view(np.uint32)[0])
-        stats = dict(zip(am.abi.STAT_FIELDS, [int(v) for v in st.view(np.uint64)]))
-        return idx.view(np.uint32)[:k].astype(np.uint64) + np.uint64(s.shard_base), act[:k].astype(np.uint32), stats
-
-
 class Walk:
-    """one handle and its model, driven by one seeded generator; every check names (walk, seed, step, call)"""
+    """one handle and its model, driven by one seeded generator; every check names (walk, seed, step, call).  With
+    `track` (and `details`) on, every tick and run_ticks also compares the changed set (and the details)."""
 
-    def __init__(self, am, zmap, name, seed, capacity, base, T0):
+    def __init__(self, am, zmap, name, seed, capacity, base, T0, track=False, details=False):
         self.am, self.zmap, self.name, self.seed = am, zmap, name, seed
         self.rng = np.random.default_rng(seed)
         self.n = capacity
@@ -209,12 +178,15 @@ class Walk:
         self.zones = zones_usable(T0 - DAY, T0 + 2 * DAY)
         self.tz_ids = zmap.ids_of(self.zones)
         self.s = am.Sweep(capacity=capacity, shard_base=base)
-        self.m = SequenceModel(zmap, capacity, base, seed=seed)
+        self.m = HandleModel(zmap, capacity, base, seed=seed)
         self.s.set_seed(seed)
+        self.details = details
+        if track:
+            self.set_track()
         self.dev = DevOut(am, capacity)
         self.step = 0
         self.call = "create"
-        self.streams = ["handle"] if _emulated(am) else ["handle", "torch", "default"]
+        self.streams = ["handle"] if emulated(am) else ["handle", "torch", "default"]
         self.torch_stream = None
         self.calls = {}
         self.reached = dict(held=0, catch_up_minutes=0, nospace=0, dense_posts=0, zone_transitions=0, big_calls=0)
@@ -311,6 +283,15 @@ class Walk:
         self.s.set_hold_in_flight(on)
         self.m.set_hold(on)
 
+    def set_track(self):
+        """tracking on (again: off first), with details if the walk has them: an empty changed set"""
+        for on in ([False, True] if self.m.track else [True]):
+            self.s.set_track_changes(on)
+            self.m.set_track(on)
+        if self.details:
+            self.s.set_change_details(True)
+            self.m.set_details(True)
+
     # ---- queries (each drains the staged calls) ----
     def read(self):
         if self.rng.integers(0, 2):
@@ -326,7 +307,7 @@ class Walk:
         live = self.m.live(sl)
         for c in self.am.COLUMN_NAMES:
             keep = live | (c == "flags")
-            np.testing.assert_array_equal(got[c][keep], self.m.cols[c][sl][keep], err_msg=f"{self.where} {c}")
+            np.testing.assert_array_equal(got[c][keep], self.m.cols()[c][sl][keep], err_msg=f"{self.where} {c}")
 
     def in_flight(self):
         if self.rng.integers(0, 2):
@@ -374,7 +355,7 @@ class Walk:
 
     def compare(self, got, want, every_column):
         gi, ga, gs = got
-        wi, wa, ws = want
+        wi, wa, ws = want[:3]
         assert gs == ws, (self.where, {k: (gs[k], ws[k]) for k in gs if gs[k] != ws[k]})
         np.testing.assert_array_equal(gi, wi, err_msg=str(self.where))
         np.testing.assert_array_equal(ga, wa, err_msg=str(self.where))
@@ -388,15 +369,15 @@ class Walk:
         got = self.s.read_range(0, hwm, names)
         live = self.m.live(np.arange(hwm))
         for c in names:
-            bad = np.flatnonzero((got[c] != self.m.cols[c][:hwm]) & (live | (c == "flags")))
-            assert len(bad) == 0, (self.where, c, int(bad[0]), int(got[c][bad[0]]), int(self.m.cols[c][bad[0]]))
+            want = self.m.cols()[c]
+            bad = np.flatnonzero((got[c] != want[:hwm]) & (live | (c == "flags")))
+            assert len(bad) == 0, (self.where, c, int(bad[0]), int(got[c][bad[0]]), int(want[bad[0]]))
         if every_column:
             np.testing.assert_array_equal(self.s.in_flight(0, self.n), self.m.in_flight(0, self.n), err_msg=str(self.where))
 
     def tick(self, T, mode, every_column, entry=None):
         am, s, m = self.am, self.s, self.m
-        if m.hold:
-            self.reached["held"] += int(hold_oracle.held(m.view(), m.since[:m.hwm]).sum())
+        self.reached["held"] += int(m.held().sum())
         P = m.window_of(T, mode)
         if P is not None and T - P <= DAY and any(t % 60 == 0 for t in range(P + 1, T + 1)):
             self.reached["catch_up_minutes"] += 1
@@ -412,18 +393,30 @@ class Walk:
                 self._call(entry, T, mode, None)
             assert e.value.code == r.code, (self.where, e.value.code, r.code)
             assert s.launch_count == before, self.where
+            self.check_lists(False)
             return False
         self.device_cap = None
         got = self._call(entry, T, mode, want)
-        if m.hold:  # submitted by this tick and held from now on
-            self.reached["held"] += int(hold_oracle.held(m.view(), m.since[:m.hwm]).sum())
+        self.reached["held"] += int(m.held().sum())  # submitted by this tick and held from now on
         if got is None:  # tick_shard: the list stays on the device
             self.check_columns(True)
         else:
             if self.device_cap is not None:  # a short device buffer holds the list's first cap entries
                 want = (want[0][:self.device_cap], want[1][:self.device_cap], want[2])
             self.compare(got, want, every_column)
+        self.check_lists(True)
         return True
+
+    def check_lists(self, ticked):
+        """the changed set with tracking on (its columns after a tick), the details with details on"""
+        m, s = self.m, self.s
+        if m.track and ticked:
+            check_changes(s, m.changes(), m.cols(), self.where)
+        elif m.track:
+            np.testing.assert_array_equal(s.last_changes(names=[])[0], m.changes(), err_msg=str(self.where))
+        if m.details_on:
+            det = m.details()
+            check_details(s, m.changes() if len(det) else np.zeros(0, np.uint64), det, self.where)
 
     def _call(self, entry, T, mode, want):
         am, s = self.am, self.s
@@ -484,6 +477,7 @@ class Walk:
                 with pytest.raises(am.AmError) as e:
                     s.run_ticks(T, k, mode=mode, seed=seed)
                 assert e.value.code == r.code and s.launch_count == before, self.where
+                self.check_lists(False)
                 return 0
             got = s.run_ticks(T, k, mode=mode, seed=seed)
         finally:
@@ -495,6 +489,7 @@ class Walk:
             row = {f: int(got[j][f]) for f in am.abi.STAT_FIELDS}
             assert row == want[j], (self.where, j, {f: (row[f], want[j][f]) for f in row if row[f] != want[j][f]})
         self.check_columns(every_column)
+        self.check_lists(False)
         return k
 
     # ---- the walk ----

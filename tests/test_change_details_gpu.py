@@ -1,9 +1,10 @@
 """Change details (am_sweep_set_change_details / am_sweep_last_change_details): after every tick the handle's details
-must equal the change-details oracle's (tests/change_details_oracle.py, built on the existing models alone), entry by
+must equal the change-details oracle's (tests/change_details_oracle.py, in tests/handle_model.py), entry by
 entry with the changed set.  Through every tick entry point: the hand-derived cases, the sparse and the dense result
 routes with reads between posts and ticks, the hold, the hold with timeouts and the remedy hold, catch-up ticks on named
 zones with AM_SWEEP_FULL_SCAN, closed loop, short buffers and refused ticks, the call contract, run_ticks, toggling
-details and tracking, random call sequences through tests/sequence_model.py, launch counts and 10 M records."""
+details and tracking, random call sequences through tests/test_call_sequences_gpu.py's walk, launch counts and 10 M
+records."""
 import zlib
 
 import numpy as np
@@ -14,8 +15,9 @@ import change_details_cases
 import change_details_oracle as cdo
 import changes_oracle
 from adversarial import ZoneMap, population, zones_usable
+from handle_pair import check_details, emulated
 from test_call_sequences_gpu import WALKS
-from test_status_changes_gpu import CATCH, CLOSED, ENTRIES, FULL, ChangesWalk, Pair, _emulated
+from test_status_changes_gpu import CATCH, CLOSED, ENTRIES, FULL, ChangesWalk, pair
 from timeout_cases import M0, rec
 
 pytestmark = pytest.mark.gpu
@@ -28,42 +30,11 @@ def zmap(am, orc):
     return ZoneMap()
 
 
-def check_details(s, want_idx, want, where):
-    idx, det = s.last_change_details()
-    np.testing.assert_array_equal(idx, want_idx, err_msg=f"{where}: listed slots")
-    for name in cdo.DETAIL.names:
-        np.testing.assert_array_equal(det[name], want[name], err_msg=f"{where}: {name}")
-    return len(idx)
-
-
-class DetailsPair(Pair):
-    """test_status_changes_gpu.Pair with details on: every tick also compares the details with the oracle's"""
-
-    def __init__(self, am, zmap, n, hold=None, entry="tick", shard_base=0):
-        super().__init__(am, zmap, n, hold, entry, shard_base)
-        self.o = cdo.Model(zmap, n, hold, shard_base)
-        self.s.set_change_details(True)
-        self.detailed = 0
-
-    def set_details(self, on):
-        self.s.set_change_details(on)
-        self.o.set_details(on)
-
-    def details(self):
-        return self.o.details()
-
-    def tick(self, T, mode=0, entry=None, names=None):
-        want = super().tick(T, mode, entry, names)
-        if self.o.on:
-            self.detailed += check_details(self.s, self.o.changes(), self.o.details(), (entry or self.entry, mode, T))
-        return want
-
-
 # ---- 1. the hand-derived cases, through every tick entry point -------------------------------------------------------
 @pytest.mark.parametrize("entry", ENTRIES)
 @pytest.mark.parametrize("case", change_details_cases.CASES, ids=lambda c: c.__name__)
 def test_hand_derived_cases(am, zmap, case, entry):
-    p = DetailsPair(am, zmap, case.n, case.hold, entry)
+    p = pair(am, zmap, case.n, case.hold, entry=entry, details=True)
     try:
         case(am, p)
     finally:
@@ -86,7 +57,7 @@ def _walk(am, zmap, hold, early, mode, seed_text, monkeypatch, n=3000):
         return r
 
     monkeypatch.setenv("AMSWEEP_EARLY_RESULTS", str(early))
-    p = DetailsPair(am, zmap, n, hold)
+    p = pair(am, zmap, n, hold, details=True)
     try:
         p.upsert(np.arange(n), records(n))
         entries = ENTRIES + ["tick_short"]
@@ -136,7 +107,7 @@ def test_closed_loop(am, zmap):
     n = 4000
     rng = np.random.default_rng(7)
     T = M0 + 3
-    p = DetailsPair(am, zmap, n)
+    p = pair(am, zmap, n, details=True)
     try:
         p.upsert(np.arange(n), am.columns_to_records(population(rng, n, T, True, zmap.ids_of(zones_usable(T - DAY, T + DAY)))))
         for k, step in enumerate([0, 1, 57, 60, 1, 3600]):
@@ -157,7 +128,7 @@ def test_catch_up_on_named_zones(am, zmap):
     cols = amgen.fill(22, 2, 0, n, T, am.load().am_healthcheck_classify)
     rng = np.random.default_rng(23)
     cols["flags"] |= np.where(rng.random(n) < 0.5, am.F_HAS_REMEDY, 0).astype(np.uint32)
-    p = DetailsPair(am, zmap, n, "remedy")
+    p = pair(am, zmap, n, "remedy", details=True)
     try:
         recs = am.columns_to_records(cols)
         recs["wf_timeout"] = rng.integers(0, 400, n)
@@ -170,7 +141,7 @@ def test_catch_up_on_named_zones(am, zmap):
                        np.where(rng.random(1500) < 0.3, 1, 0).astype(np.uint8))
             p.tick(T, CATCH | (FULL if k % 3 == 0 else 0), entry=ENTRIES[k % 4])
         assert p.detailed > 5000, p.detailed
-        det = p.o.details()
+        det = p.m.details()
         assert (det["started"] != cdo.NONE).any()
     finally:
         p.close()
@@ -227,73 +198,10 @@ def test_contract(am):
 
 
 # ---- 5. random call sequences through the sequence model ------------------------------------------------------------------
-class DetailsWalk(ChangesWalk):
-    """test_status_changes_gpu.ChangesWalk with details on: the model's posts are wrapped to take in_flight() before
-    they delegate; after every tick the details against change_details_oracle.details"""
-
-    def __init__(self, *a):
-        super().__init__(*a)
-        self.hc, self.rm = {}, {}
-        self.want_det = np.zeros(0, cdo.DETAIL)
-        m, s = self.m, self.s
-        post, upsert, remove, load, stc = m.post, m.upsert, m.remove, m.load, s.set_track_changes
-
-        def posted(idx, phase, rphase=None):
-            v = m.in_flight(idx=idx)
-            for k, i in enumerate(np.asarray(idx, dtype=np.int64).tolist()):
-                if phase[k]:
-                    self.hc[i] = v[k]
-            post(idx, phase, rphase)
-
-        def dropped(f):
-            def g(idx, *rest):
-                f(idx, *rest)
-                for i in np.asarray(idx, dtype=np.int64).tolist():
-                    self.hc.pop(i, None)
-            return g
-
-        def loaded(first, cols):
-            load(first, cols)
-            for i in range(first, first + len(cols["flags"])):
-                self.hc.pop(i, None)
-
-        def tracked(on):  # (turning tracking off turns details off: on again at once)
-            stc(on)
-            if on:
-                s.set_change_details(True)
-                self.hc.clear()
-                self.want_det = np.zeros(0, cdo.DETAIL)
-
-        m.post, m.upsert, m.remove, m.load, s.set_track_changes = posted, dropped(upsert), dropped(remove), loaded, tracked
-        s.set_change_details(True)
-
-    def tick(self, T, mode, every_column, entry=None):
-        before = self.m.cols["flags"].copy()
-        ok = super().tick(T, mode, every_column, entry)  # (it may turn tracking off and on: details start afresh)
-        if ok:
-            self.want_det = cdo.details(self.want, before, self.out, T, mode, self.hc, {}, self.s.shard_base)
-            self.hc.clear()
-        idx, det = self.s.last_change_details()
-        if len(self.want_det):
-            np.testing.assert_array_equal(idx, self.want, err_msg=str(self.where))
-        assert len(det) == len(self.want_det), self.where
-        for name in cdo.DETAIL.names:
-            np.testing.assert_array_equal(det[name], self.want_det[name], err_msg=f"{self.where}: {name}")
-        return ok
-
-    def run_ticks(self, T, every_column):
-        k = super().run_ticks(T, every_column)
-        if k:
-            self.hc.clear()
-            self.want_det = np.zeros(0, cdo.DETAIL)
-        assert len(self.s.last_change_details()[0]) == len(self.want_det), self.where
-        return k
-
-
 @pytest.mark.parametrize("k", [0, 2, 3, 5], ids=[WALKS[k][3] for k in (0, 2, 3, 5)])
 def test_random_call_sequences(am, zmap, k):
     cap, base, T0, name = WALKS[k]
-    walk = DetailsWalk(am, zmap, name, zlib.crc32(f"details {name}".encode()), cap, base, T0)
+    walk = ChangesWalk(am, zmap, name, zlib.crc32(f"details {name}".encode()), cap, base, T0, details=True)
     walk.run()
     assert walk.checked > 20
 
@@ -331,7 +239,7 @@ def test_launch_counts(am):
 def test_one_check_through_its_phases(am, zmap):
     """one check through Succeeded, Failed with a remedy, a remedy timeout and a reset: what a status write needs for
     each phase hcc.go:636-851 applies (StartedAt / RemedyStartedAt = then, the reset) is in the details alone"""
-    p = DetailsPair(am, zmap, 4, "remedy")
+    p = pair(am, zmap, 4, "remedy", details=True)
     try:
         p.upsert([0], rec(am, 40, repeat_after_sec=60, finished_at=M0 - 100, has_remedy=True, remedy_runs_limit=5,
                           remedy_reset_interval=100000))
@@ -339,20 +247,20 @@ def test_one_check_through_its_phases(am, zmap):
         p.tick(T)  # submitted at M0
         p.post([0], [1])
         p.tick(T + 5)
-        (d,) = p.o.details()
+        (d,) = p.m.details()
         assert (d["started"], d["applied"]) == (M0, cdo.CHG_SUCCEEDED)  # Succeeded: StartedAt = then, FinishedAt = now
         p.tick(T + 65)  # submitted again
         p.post([0], [2])
         p.tick(T + 70)  # Failed: LastFailedAt = now, the remedy run starts
-        (d,) = p.o.details()
+        (d,) = p.m.details()
         assert (d["started"], d["applied"]) == (T + 65, cdo.CHG_FAILED) and d["action"] & 0x02
         p.tick(T + 110)  # the remedy run outlives W = 40: RemedyFailed, RemedyStartedAt = then
-        (d,) = p.o.details()
+        (d,) = p.m.details()
         assert (d["remedy_started"], d["applied"]) == (T + 70, cdo.CHG_REMEDY_FAILED | cdo.CHG_REMEDY_TIMED_OUT)
         p.tick(T + 200)  # submitted again
         p.post([0], [1])
         p.tick(T + 205)  # Succeeded with RemedyTotalRuns >= 1: "HealthCheck Passed so Remedy is reset"
-        (d,) = p.o.details()
+        (d,) = p.m.details()
         assert d["action"] & 0x20 and d["applied"] == cdo.CHG_SUCCEEDED and d["started"] == T + 200
     finally:
         p.close()
@@ -361,7 +269,7 @@ def test_one_check_through_its_phases(am, zmap):
 # ---- 8. full size, on the GPU only -----------------------------------------------------------------------------------------
 def test_full_size_config3(am, zmap):
     """one 10 M-record config 3 tick (the dense route), the details compared in full"""
-    if _emulated(am):
+    if emulated(am):
         pytest.skip("10 M records: GPU only")
     n = 10_000_000
     T0 = amgen.T0_MON_0915

@@ -5,6 +5,7 @@ import pytest
 import change_details_cases
 import change_details_oracle
 from adversarial import ZoneMap
+from handle_model import HandleModel
 
 
 @pytest.fixture(scope="module")
@@ -14,7 +15,7 @@ def zmap(am, orc):
 
 @pytest.mark.parametrize("case", change_details_cases.CASES, ids=lambda c: c.__name__)
 def test_hand_derived_cases(am, zmap, case):
-    case(am, change_details_oracle.Model(zmap, case.n, case.hold))
+    case(am, HandleModel(zmap, case.n, hold=case.hold is not None, remedy=case.hold == "remedy", track=True, details=True))
 
 
 def test_applied_of_maps_every_posted_bit():

@@ -5,6 +5,7 @@ import pytest
 import changes_cases
 import changes_oracle
 from adversarial import ZoneMap
+from handle_model import HandleModel
 
 
 @pytest.fixture(scope="module")
@@ -14,7 +15,7 @@ def zmap(am, orc):
 
 @pytest.mark.parametrize("case", changes_cases.CASES, ids=lambda c: c.__name__)
 def test_hand_derived_cases(am, zmap, case):
-    case(am, changes_oracle.Model(zmap, case.n, case.hold))
+    case(am, HandleModel(zmap, case.n, hold=case.hold is not None, remedy=case.hold == "remedy", track=True))
 
 
 def test_masked_bits_and_anomaly():

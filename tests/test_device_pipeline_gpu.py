@@ -3,9 +3,9 @@ a delay kernel, with staged calls, host ticks and reads between them; posting th
 output buffers shorter than the list; shard bases past 2^32; the exchange of a one-GPU world; and output
 pointers that are not aligned for the kernels' stores.
 
-Every tick is compared with the sequential model: the C oracle's columns with every staged call applied in call
-order, each tick the oracle's sweep at its second (a catch-up tick: the window oracle over (P, T]).  The device
-work is checked after one synchronisation at the end, so a tick that read a staging area, a zone offset or a
+Every tick is compared with the sequential model (tests/handle_model.py): the C oracle's columns with every staged
+call applied in call order, each tick the oracle's sweep at its second (a catch-up tick: the window oracle over
+(P, T]).  The device work is checked after one synchronisation at the end, so a tick that read a staging area, a zone offset or a
 window box before (or after) the host wrote it shows up as a difference.
 
 The stream tests need a GPU.  The misalignment test also runs on the emulated library (AMSWEEP_LIB), with numpy
@@ -17,8 +17,8 @@ import threading
 import numpy as np
 import pytest
 
-import window_oracle
 from adversarial import ZoneMap, population, zones_usable
+from handle_model import HandleModel
 
 pytestmark = pytest.mark.gpu
 
@@ -94,7 +94,7 @@ def _stats(am, words):
 
 def check_device_tick(am, out, want, base, what, count=True, stats=True):
     """the list prefix, the count, the full statistics; canaries everywhere nothing was to be written"""
-    wi, wa, ws = want
+    wi, wa, ws = want[:3]
     idx, act, cnt, st = out.fetch()
     m = min(len(wi), out.cap)
     if count:
@@ -115,7 +115,7 @@ def check_device_tick(am, out, want, base, what, count=True, stats=True):
 
 def check_host_tick(got, want, what):
     gi, ga, gs = got
-    wi, wa, ws = want
+    wi, wa, ws = want[:3]
     assert gs == ws, (what, {f: (gs[f], ws[f]) for f in ws if gs[f] != ws[f]})
     np.testing.assert_array_equal(np.asarray(gi, np.uint64), wi, err_msg=f"{what}: idx")
     np.testing.assert_array_equal(np.asarray(ga, np.uint32), wa, err_msg=f"{what}: act")
@@ -129,49 +129,11 @@ def check_columns(am, dev, model, what):
         np.testing.assert_array_equal(dev[name][live], model[name][live], err_msg=f"{what}: {name}")
 
 
-class Model:
-    """The oracle's columns with every staged call applied in call order; a tick is the oracle's sweep at T, a
-    catch-up tick the window oracle over (P, T]."""
-
-    def __init__(self, am, zmap, cols, base=0):
-        self.am, self.zmap, self.base = am, zmap, base
-        self.c = {k: v.copy() for k, v in cols.items()}
-        self.P = None
-        self.hc = np.uint32(am.F_PENDING_OK | am.F_PENDING_FAIL)
-        self.rm = np.uint32(am.F_REMEDY_PENDING | am.F_REMEDY_OUTCOME_OK)
-        self.pb = np.array([0, am.F_PENDING_OK, am.F_PENDING_FAIL], np.uint32)
-        self.rb = np.array([0, am.F_REMEDY_PENDING | am.F_REMEDY_OUTCOME_OK, am.F_REMEDY_PENDING], np.uint32)
-
-    def post(self, slots, phase, rphase=None):
-        """one post_result call (slots distinct): each phase that is not "none" replaces its bit group"""
-        f = self.c["flags"][slots]
-        f = np.where(phase != 0, (f & ~self.hc) | self.pb[phase], f)
-        if rphase is not None:
-            f = np.where(rphase != 0, (f & ~self.rm) | self.rb[rphase], f)
-        self.c["flags"][slots] = f
-
-    def upsert(self, idx, recs):
-        for name in self.am.COLUMN_NAMES:
-            self.c[name][idx] = recs[name]
-        self.c["flags"][idx] &= ~np.uint32(self.am.F_TOMBSTONE)
-
-    def remove(self, idx):
-        self.c["flags"][idx] = self.am.F_TOMBSTONE
-
-    def tick(self, T, mode):
-        if mode & self.am.SWEEP_CATCH_UP and self.P is not None and T > self.P:
-            want = window_oracle.sweep_window(self.zmap, self.c, self.P, T, mode=mode, seed=SEED, shard_base=self.base)
-        else:
-            want = self.zmap.sweep(self.c, T, mode=mode & 1, seed=SEED, shard_base=self.base)
-        self.P = T
-        return want
-
-    def next_due(self, T, horizon=120):
-        for t in range(T + 1, T + horizon + 1):
-            probe = {k: v.copy() for k, v in self.c.items()}
-            if self.zmap.sweep(probe, t, seed=SEED, shard_base=self.base)[2]["n_emitted"]:
-                return t
-        return None
+def _model(zmap, cols, base=0):
+    """the model of a handle without the hold, `cols` loaded into slots 0.."""
+    m = HandleModel(zmap, len(cols["flags"]), base, seed=SEED)
+    m.load(0, cols)
+    return m
 
 
 def _results(rng, n, every, offset=None):
@@ -221,7 +183,7 @@ def test_queued_ticks_on_four_streams_equal_the_oracle_sequence(am, zmap):
     rng = np.random.default_rng(101)
     tz_ids = zmap.ids_of(zones_usable(T_NOV - HOUR, T_NOV + 3 * HOUR))
     cols = population(rng, n, T_NOV, True, tz_ids)
-    model = Model(am, zmap, cols)
+    model = _model(zmap, cols)
 
     def fresh(k):
         idx = rng.choice(n, k, replace=False).astype(np.uint64)
@@ -297,12 +259,12 @@ def test_queued_ticks_on_four_streams_equal_the_oracle_sequence(am, zmap):
             elif op[0] == "host":
                 check_host_tick(seen[k], model.tick(op[1], op[2]), what)
             elif op[0] == "next_due":
-                assert seen[k] == model.next_due(op[1]), what
+                assert seen[k] == model.first_active_tick(op[1], 120), what
             elif op[0] == "read":
-                check_columns(am, seen[k], model.c, what)
+                check_columns(am, seen[k], model.cols(), what)
             else:
                 _apply(None, model, op)
-        check_columns(am, s.read_range(0, n), model.c, "final")
+        check_columns(am, s.read_range(0, n), model.cols(), "final")
 
 
 # ---- 2. posting threads between device ticks that are still in flight -------------------------------------------
@@ -314,7 +276,7 @@ def test_posting_threads_between_queued_device_ticks(am, zmap):
     rng = np.random.default_rng(202)
     tz_ids = zmap.ids_of(zones_usable(T0, T0 + HOUR))
     cols = population(rng, n, T0, True, tz_ids)
-    model = Model(am, zmap, cols)
+    model = _model(zmap, cols)
     up_slots = np.arange(3, n, 97, dtype=np.uint64)              # the upserting thread's slots
     free = np.setdiff1d(np.arange(n, dtype=np.uint64), up_slots)
     lanes = [free[w::4] for w in range(4)]                        # four posting threads, disjoint slots
@@ -376,7 +338,7 @@ def test_posting_threads_between_queued_device_ticks(am, zmap):
             for u, r in ups:
                 model.upsert(u.astype(np.int64), r)
             check_device_tick(am, outs[k], model.tick(T, mode), 0, (k, T, mode))
-        check_columns(am, s.read_range(0, n), model.c, "final")
+        check_columns(am, s.read_range(0, n), model.cols(), "final")
 
 
 # ---- 3. device buffers shorter than the list ------------------------------------------------------------------------
@@ -403,7 +365,7 @@ def test_short_device_buffers(am, zmap, n, how):
     rng = np.random.default_rng(n + len(how))
     cols = population(rng, n, T, True, zmap.ids_of(zones_usable(P, T + 1)))
     staged = _results(rng, n, 23)
-    model = Model(am, zmap, cols)
+    model = _model(zmap, cols)
     want_P = model.tick(P, 0) if how == "catch-up" else None
     for op in staged:
         _apply(None, model, op)
@@ -427,7 +389,7 @@ def test_short_device_buffers(am, zmap, n, how):
             check_device_tick(am, out, want, 0, (how, n, cap, count, stats), count, stats)
             # the short tick consumed its one-shot actions like any other: the next one equals the oracle's
             check_host_tick(s.tick(T + 1, mode & am.SWEEP_CLOSED_LOOP), want_next, (how, n, cap, "next"))
-            check_columns(am, s.read_range(0, n), model.c, (how, n, cap))
+            check_columns(am, s.read_range(0, n), model.cols(), (how, n, cap))
 
 
 # ---- 4. shard bases past 2^32 -----------------------------------------------------------------------------------------
@@ -441,7 +403,7 @@ def test_shard_bases_across_2_32(am, zmap, base):
     T0 = T_OCT + 14 * HOUR
     rng = np.random.default_rng(base & 0xFFFF)
     cols = population(rng, n, T0, True, zmap.ids_of(zones_usable(T0, T0 + HOUR)))
-    model = Model(am, zmap, cols, base)
+    model = _model(zmap, cols, base)
     CU, CL = am.SWEEP_CATCH_UP, am.SWEEP_CLOSED_LOOP
     with am.Sweep(capacity=n, shard_base=base) as s:
         s.load_range(0, cols)
@@ -470,7 +432,7 @@ def test_shard_bases_across_2_32(am, zmap, base):
                 got = {f: int(rows[k][f]) for f in am.abi.STAT_FIELDS}
                 ws = model.tick(t0 + k, CL)[2]
                 assert got == ws, (blocked, k, {f: (got[f], ws[f]) for f in ws if got[f] != ws[f]})
-        check_columns(am, s.read_range(0, n), model.c, "final")
+        check_columns(am, s.read_range(0, n), model.cols(), "final")
 
 
 # ---- 5. the exchange of a one-GPU world ------------------------------------------------------------------------------
@@ -483,7 +445,7 @@ def test_exchange_of_a_one_gpu_world(am, zmap, idx_bytes, base):
     T0 = T_OCT + 16 * HOUR
     rng = np.random.default_rng(idx_bytes)
     cols = population(rng, n, T0, True, zmap.ids_of(zones_usable(T0, T0 + HOUR)))
-    model = Model(am, zmap, cols, base)
+    model = _model(zmap, cols, base)
     CU, CL, FS = am.SWEEP_CATCH_UP, am.SWEEP_CLOSED_LOOP, am.SWEEP_FULL_SCAN
     # two steps before the gate: the exchange's kernels are loaded and both staging areas have their size
     WARM = 2
@@ -524,7 +486,7 @@ def test_exchange_of_a_one_gpu_world(am, zmap, idx_bytes, base):
             for k, (T, mode) in enumerate(ticks):
                 for op in posts[k]:
                     _apply(None, model, op)
-                wi, wa, ws = model.tick(T, mode)
+                wi, wa, ws = model.tick(T, mode)[:3]
                 cnt = got_cnt[k].cpu().numpy()
                 assert cnt[0] == len(wi) and cnt[1] == len(wi), (k, cnt, len(wi))
                 gi = got_idx[k].cpu().numpy()[: len(wi)].astype(np.int64).astype(np.uint64) & np.uint64(mask)
@@ -550,7 +512,7 @@ def test_exchange_of_a_one_gpu_world(am, zmap, idx_bytes, base):
             assert pc == [len(want[0])]
             np.testing.assert_array_equal(pi.cpu().numpy().astype(np.int64).astype(np.uint64) & np.uint64(mask), want[0])
             np.testing.assert_array_equal(pa.cpu().numpy().astype(np.uint32), want[1])
-            check_columns(am, s.read_range(0, n), model.c, "final")
+            check_columns(am, s.read_range(0, n), model.cols(), "final")
         finally:
             g.close()
 
@@ -577,7 +539,7 @@ def test_misaligned_outputs_are_refused_before_anything_happens(am, zmap):
     rng = np.random.default_rng(606)
     tz_ids = zmap.ids_of(zones_usable(P, T))
     cols = population(rng, n, P, True, tz_ids)
-    model = Model(am, zmap, cols)
+    model = _model(zmap, cols)
     staged = _results(rng, n, 2) + [("upsert", np.arange(5, 25, dtype=np.uint64),
                                      am.columns_to_records(population(rng, 20, P, True, tz_ids))),
                                     ("remove", np.array([7, 900], np.uint64))] + _results(rng, n, 7)
@@ -604,4 +566,4 @@ def test_misaligned_outputs_are_refused_before_anything_happens(am, zmap):
         want = model.tick(T, CU)
         assert want[2]["n_result_ok"] + want[2]["n_result_fail"] > 0
         check_device_tick(am, out, want, 0, "aligned")
-        check_columns(am, s.read_range(0, n), model.c, "final")
+        check_columns(am, s.read_range(0, n), model.cols(), "final")

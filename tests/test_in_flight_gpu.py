@@ -1,9 +1,9 @@
 """Hold in flight (am_sweep_set_hold_in_flight): a check whose health-check workflow is running is not submitted again
 until a workflow phase is posted for it, it is removed or its slot is loaded.  Compared after every tick with the hold
-oracle (tests/hold_oracle.py) — list, statistics, all sixteen columns and am_sweep_in_flight — and checked against an
+oracle (tests/hold_oracle.py, through tests/handle_pair.py) — list, statistics, all sixteen columns and
+am_sweep_in_flight — and checked against an
 invariant that needs no oracle, the release / clear / keep cases, the refusals, short buffers, turning the hold off
 and next_due."""
-import os
 import zlib
 
 import numpy as np
@@ -11,7 +11,8 @@ import pytest
 
 import amgen
 import hold_oracle
-from adversarial import ZoneMap, first_difference, population, zones_usable
+from adversarial import ZoneMap, population, zones_usable
+from handle_pair import Pair, emulated
 
 pytestmark = pytest.mark.gpu
 
@@ -24,121 +25,6 @@ FULL, CATCH = 0x2, 0x8
 @pytest.fixture(scope="module")
 def zmap(am, orc):
     return ZoneMap()
-
-
-def _emulated(am):
-    return "emu" in os.path.basename(am.abi.LIB_PATH)
-
-
-class DevOut:
-    """the four output arrays of am_sweep_tick_device: torch device memory, or host memory on the CPU emulator"""
-
-    def __init__(self, am, n):
-        self.emu = _emulated(am)
-        if self.emu:
-            self.t = [np.zeros(n, np.uint32), np.zeros(n + 4, np.uint8), np.zeros(4, np.uint32), np.zeros(16, np.uint64)]
-            self.ptr = [a.ctypes.data for a in self.t]
-        else:
-            import torch
-            self.t = [torch.zeros(n, dtype=torch.int32, device="cuda"), torch.zeros(n + 4, dtype=torch.uint8, device="cuda"),
-                      torch.zeros(4, dtype=torch.int32, device="cuda"), torch.zeros(16, dtype=torch.int64, device="cuda")]
-            self.ptr = [a.data_ptr() for a in self.t]
-        self.n = n
-
-    def tick(self, am, s, T, mode):
-        s.tick_device(T, mode, self.ptr[0], self.ptr[1], self.n, self.ptr[2], self.ptr[3], stream=s.stream)
-        if self.emu:
-            idx, act, cnt, st = self.t
-        else:
-            import torch
-            torch.cuda.synchronize()
-            idx, act, cnt, st = [a.cpu().numpy() for a in self.t]
-        k = int(cnt.view(np.uint32)[0])
-        stats = dict(zip(am.abi.STAT_FIELDS, [int(v) for v in st.view(np.uint64)]))
-        return (idx.view(np.uint32)[:k].astype(np.uint64) + np.uint64(s.shard_base), act[:k].astype(np.uint32), stats)
-
-
-class Pair:
-    """a handle with the hold on and its oracle state (columns + since), kept in step by every call"""
-
-    def __init__(self, am, zmap, cols, seed=0):
-        self.am, self.zmap = am, zmap
-        self.n = len(cols["flags"])
-        self.s = am.Sweep(capacity=self.n)
-        self.s.set_hold_in_flight(True)
-        self.s.set_seed(seed)
-        self.s.load_range(0, cols)
-        self.ocols = {k: v.copy() for k, v in cols.items()}
-        self.since = hold_oracle.none_in_flight(self.n)
-        self.P = None
-        self.dev = None
-
-    def close(self):
-        self.s.close()
-
-    def post(self, slots, phase, rphase=None):
-        am = self.am
-        slots = np.asarray(slots, dtype=np.int64)
-        phase = np.asarray(phase, dtype=np.uint8)
-        self.s.post_result(slots, phase, rphase)
-        hc = np.uint32(am.F_PENDING_OK | am.F_PENDING_FAIL)
-        rm = np.uint32(am.F_REMEDY_PENDING | am.F_REMEDY_OUTCOME_OK)
-        for k, i in enumerate(slots):  # in call order: a later post of the same slot wins
-            f = self.ocols["flags"][i]
-            if phase[k]:
-                f = (f & ~hc) | np.uint32(am.F_PENDING_OK if phase[k] == am.PHASE_SUCCEEDED else am.F_PENDING_FAIL)
-            if rphase is not None and rphase[k]:
-                f = (f & ~rm) | (rm if rphase[k] == am.PHASE_SUCCEEDED else np.uint32(am.F_REMEDY_PENDING))
-            self.ocols["flags"][i] = f
-        hold_oracle.post(self.since, slots, phase)
-
-    def upsert(self, slots, recs):
-        self.s.upsert(slots, recs)
-        for k, i in enumerate(slots):
-            for name in self.am.COLUMN_NAMES:
-                self.ocols[name][i] = recs[name][k]
-            self.ocols["flags"][i] &= ~np.uint32(self.am.F_TOMBSTONE)
-
-    def remove(self, slots):
-        self.s.remove(slots)
-        self.ocols["flags"][np.asarray(slots, dtype=np.int64)] = self.am.F_TOMBSTONE
-        hold_oracle.clear(self.since, slots)
-
-    def load(self, first, cols):
-        self.s.load_range(first, cols)
-        m = len(cols["flags"])
-        for name in self.am.COLUMN_NAMES:
-            self.ocols[name][first:first + m] = cols[name]
-        hold_oracle.clear(self.since, np.arange(first, first + m))
-
-    def tick(self, T, mode=0, entry="tick"):
-        am, s = self.am, self.s
-        P = self.P if (mode & CATCH) and self.P is not None and T > self.P else None
-        want = hold_oracle.sweep(self.zmap, self.ocols, self.since, T, P=P, mode=0, seed=0)
-        if entry == "tick":
-            got = s.tick(T, mode=mode)
-        elif entry == "tick_view":
-            i, a, st = s.tick_view(T, mode=mode)
-            got = (i.astype(np.uint64), a.astype(np.uint32), st)
-        elif entry == "tick_device":
-            self.dev = self.dev or DevOut(am, self.n)
-            got = self.dev.tick(am, s, T, mode)
-        else:
-            s.tick_shard(T, mode=mode)
-            got = None
-        self.P = T
-        return got, want
-
-    def check(self, got, want, what):
-        dev = self.s.read_range(0, self.n)
-        if got is None:  # tick_shard: the list stays on the device (the exchange rebuilds it)
-            for name in self.am.COLUMN_NAMES:
-                np.testing.assert_array_equal(dev[name], self.ocols[name], err_msg=f"{what} {name}")
-        else:
-            bad = first_difference(self.am, got, want, dev, self.ocols)
-            assert bad is None, (what, bad)
-        np.testing.assert_array_equal(self.s.in_flight(0, self.n), hold_oracle.in_flight(self.ocols, self.since),
-                                      err_msg=str(what))
 
 
 def _past(cols, T):
@@ -162,7 +48,7 @@ def test_ticks_equal_the_hold_oracle(am, zmap, entry, mode):
     n = 3000
     rng = np.random.default_rng(zlib.crc32(f"{entry} {mode}".encode()))
     T = T_OCT + 12 * DAY + 14 * HOUR - 3
-    p = Pair(am, zmap, population(rng, n, T, True, zmap.ids_of(zones_usable(T - DAY, T + 2 * DAY))))
+    p = Pair(am, zmap, population(rng, n, T, True, zmap.ids_of(zones_usable(T - DAY, T + 2 * DAY))), hold=True, entry=entry)
     held_seen = released = superseded = 0
     try:
         for k, step in enumerate(STEPS):
@@ -177,7 +63,7 @@ def test_ticks_equal_the_hold_oracle(am, zmap, entry, mode):
                 elif r < 0.55:
                     first = int(rng.integers(0, n - 200))
                     p.load(first, population(rng, 200, T, True, zmap.ids_of(zones_usable(T - DAY, T + 2 * DAY))))
-                fl = np.flatnonzero(p.since != NONE)
+                fl = np.flatnonzero(p.m.since != NONE)
                 if len(fl):
                     dense = k % 5 == 3
                     sl = rng.choice(fl, min(len(fl), 2000 if dense else 40), replace=False)
@@ -190,11 +76,10 @@ def test_ticks_equal_the_hold_oracle(am, zmap, entry, mode):
                         p.upsert(up, _records(am, rng, len(up), T, zmap))
                         superseded += len(up)
                 if k % 4 == 2:  # a read's drain: the results stay pending for the sweep
-                    np.testing.assert_array_equal(p.s.in_flight(0, n), hold_oracle.in_flight(p.ocols, p.since))
+                    np.testing.assert_array_equal(p.s.in_flight(0, n), p.m.in_flight())
             T += step
-            held_seen += int(hold_oracle.held(p.ocols, p.since).sum())
-            got, want = p.tick(T, mode, entry)
-            p.check(got, want, (entry, mode, k, T))
+            held_seen += int(p.m.held().sum())
+            p.tick(T, mode)
         assert held_seen > 1000 and released > 100 and superseded > 30
     finally:
         p.close()
@@ -204,7 +89,7 @@ def test_ticks_equal_the_hold_oracle(am, zmap, entry, mode):
 @pytest.mark.parametrize("with_results", [False, True])
 def test_no_second_submission_while_in_flight(am, zmap, with_results):
     n = 2000
-    ticks = 600 if _emulated(am) else 3600
+    ticks = 600 if emulated(am) else 3600
     rng = np.random.default_rng(17 + with_results)
     T0 = T_OCT + 5 * DAY + 9 * HOUR + 13
     cols = _past(population(rng, n, T0, True, zmap.ids_of(zones_usable(T0 - DAY, T0 + DAY))), T0)
@@ -432,23 +317,16 @@ def test_next_due_is_the_first_tick_that_emits(am, zmap):
     recs = np.concatenate([am.classify(**kw)[1] for kw in specs])
     n = len(recs)
     cols = am.records_to_columns(recs)
-    p = Pair(am, zmap, cols)
+    p = Pair(am, zmap, cols, hold=True)
     try:
         for k, (step, post) in enumerate([(0, None), (1, None), (13, [0]), (1, None), (200, [1, 2]), (1, None)]):
             T += step
             if post:
                 p.post(post, [am.PHASE_SUCCEEDED] * len(post))
-            got, want = p.tick(T)
-            p.check(got, want, k)
+            p.tick(T)
             nd = p.s.next_due(T)
-            # brute force: oracle ticks on copies, one second at a time
-            oc = {kk: v.copy() for kk, v in p.ocols.items()}
-            since = p.since.copy()
-            t = T + 1
-            while len(hold_oracle.sweep(zmap, oc, since, t)[0]) == 0:
-                t += 1
-                assert t < T + 4000
-            assert nd == t, (k, nd, t)
+            t = p.m.first_active_tick(T, 4000)  # (no result is pending: the first tick that emits)
+            assert t is not None and nd == t, (k, nd, t)
     finally:
         p.close()
 
@@ -465,13 +343,13 @@ def test_next_due_on_the_adversarial_population(am, zmap, parse_errors):
     if not parse_errors:  # (a PARSE_ERROR record is due every second: next_due would always be T + 1)
         pe = (cols["flags"] & np.uint32(am.KIND_MASK)) == am.KIND_PARSE_ERROR
         cols["flags"][pe] = am.F_TOMBSTONE
-    p = Pair(am, zmap, cols)
+    p = Pair(am, zmap, cols, hold=True)
     checked = 0
     try:
         for k, step in enumerate([0, 1, 1, 29, 1, 1, 61]):
             T += step
             if k == 2:  # paused / broken during their runs: held STOPPED and PARSE_ERROR records
-                sub = np.flatnonzero(p.since != NONE)[:6]
+                sub = np.flatnonzero(p.m.since != NONE)[:6]
                 assert len(sub) == 6
                 rc, stopped = am.classify(repeat_after_sec=0, finished_at=T - 3)
                 rc2, broken = am.classify(cron="bad cron", finished_at=T - 3)
@@ -479,18 +357,17 @@ def test_next_due_on_the_adversarial_population(am, zmap, parse_errors):
                 assert broken["flags"][0] & am.KIND_MASK == am.KIND_PARSE_ERROR
                 recs = np.concatenate([stopped] * 3 + [broken if parse_errors else stopped] * 3)
                 p.upsert(sub, recs)
-                assert hold_oracle.held(p.ocols, p.since)[sub].all()
+                assert p.m.held()[sub].all()
             if k == 4:
-                fl = np.flatnonzero(p.since != NONE)
+                fl = np.flatnonzero(p.m.since != NONE)
                 p.post(fl[::3], np.full(len(fl[::3]), am.PHASE_SUCCEEDED, np.uint8))
-            got, want = p.tick(T)
-            p.check(got, want, k)
+            got = p.tick(T)
             if k == 2:  # held, and still reported
                 acts = dict(zip(got[0].tolist(), got[1].tolist()))
                 assert all(acts.get(int(i), 0) & (am.ACT_STOPPED | am.ACT_PARSE_ERROR) for i in sub)
             nd = p.s.next_due(T)
-            oc = {kk: v.copy() for kk, v in p.ocols.items()}
-            since = p.since.copy()
+            oc = {kk: v.copy() for kk, v in p.m.cols().items()}
+            since = p.m.since.copy()
             t = T + 1
             while nd is None or t < min(nd, T + 3600):
                 assert len(hold_oracle.sweep(zmap, oc, since, t)[0]) == 0, (k, t, nd)
@@ -511,22 +388,21 @@ def test_next_due_on_the_adversarial_population(am, zmap, parse_errors):
 
 # ---- 7. full size, on the GPU only ---------------------------------------------------------------------------------
 def test_full_size_config2_against_the_oracle(am, zmap):
-    if _emulated(am):
+    if emulated(am):
         pytest.skip("10 M records: GPU only")
     n = 10_000_000
     T0 = amgen.T0_MON_0915
     cols = amgen.fill(2, 2, 0, n, T0, am.load().am_healthcheck_classify)
-    p = Pair(am, zmap, cols)
+    p = Pair(am, zmap, cols, hold=True)
     rng = np.random.default_rng(2)
     try:
         T = T0
         for k, step in enumerate([0, 1, 59, 1, 60]):
             T += step
             if k == 3:
-                fl = np.flatnonzero(p.since != NONE)
+                fl = np.flatnonzero(p.m.since != NONE)
                 sl = rng.choice(fl, min(len(fl), 50_000), replace=False)
                 p.post(sl, rng.integers(1, 3, len(sl)).astype(np.uint8))
-            got, want = p.tick(T, mode=CATCH if k == 4 else 0, entry="tick_view" if k % 2 else "tick")
-            p.check(got, want, k)
+            p.tick(T, mode=CATCH if k == 4 else 0, entry="tick_view" if k % 2 else "tick")
     finally:
         p.close()

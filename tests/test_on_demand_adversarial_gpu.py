@@ -14,8 +14,8 @@ import pytest
 import amgen
 import oracle_c
 import test_remedy_hold_gpu
-import test_workflow_timeout_gpu
 from adversarial import I32MAX, I32MIN, TS, ZoneMap, population, zones_usable
+from handle_pair import Pair
 
 pytestmark = pytest.mark.gpu
 
@@ -281,12 +281,9 @@ HOLD_VARIANTS = ["hold", "hold_timeouts", "remedy_hold", "remedy_hold_timeouts"]
 
 
 def _pair(am, zmap, cols, variant):
-    """a handle with the variant's holds on and its oracle state: the remedy-hold suite's pair for the remedy hold, the
-    timeout suite's for the hold alone (a handle that never gets a non-zero wf_timeout sweeps with the hold-only
-    variants, and the timeout oracle is then the hold oracle)"""
-    if variant.startswith("remedy"):
-        return test_remedy_hold_gpu.Pair(am, zmap, cols)
-    return test_workflow_timeout_gpu.Pair(am, zmap, cols)
+    """a handle with the variant's holds on and its model (a handle that never gets a non-zero wf_timeout sweeps with
+    the hold-only variants, and the timeout oracle is then the hold oracle)"""
+    return Pair(am, zmap, cols, hold=True, remedy=variant.startswith("remedy"))
 
 
 def _busy(am, T, k, W):
@@ -319,20 +316,20 @@ def test_next_due_with_the_hold(am, orc, zmap, variant, T):
         try:
             p.upsert(np.arange(n), recs)
             p.tick(T)
-            assert p.st.in_flight()[0] == T
+            assert p.m.in_flight()[0] == T
             failed = rng.choice(busy, (len(busy) + 1) // 2, replace=False)
             p.post(failed, np.full(len(failed), am.PHASE_FAILED, dtype=np.uint8))
             p.tick(T + 1)
             for dt in (1, 2, 9, 31, 101, 10 ** 6):
                 t = T + 1 + dt
-                runs = dict(since=p.st.since, deadline=p.st.deadline)
+                runs = dict(since=p.m.since, deadline=p.m.deadline)
                 if remedy:
-                    runs.update(rsince=p.st.rsince, rdeadline=p.st.rdeadline)
-                    remedy_deadlines += int(((p.st.rsince != NONE) & (p.st.rdeadline != NO_DEADLINE)).sum())
-                want = _next_due_want(am, lib, p.st.ocols, t, **runs)
+                    runs.update(rsince=p.m.rsince, rdeadline=p.m.rdeadline)
+                    remedy_deadlines += int(((p.m.rsince != NONE) & (p.m.rdeadline != NO_DEADLINE)).sum())
+                want = _next_due_want(am, lib, p.m.cols(), t, **runs)
                 assert p.s.next_due(t) == want, (n, t, want)
-                hold_mattered += _next_due_want(am, lib, p.st.ocols, t) != want
-                floor_mattered += _next_due_want(am, lib, p.st.ocols, t, floor=t, **runs) != want
+                hold_mattered += _next_due_want(am, lib, p.m.cols(), t) != want
+                floor_mattered += _next_due_want(am, lib, p.m.cols(), t, floor=t, **runs) != want
         finally:
             p.close()
     assert hold_mattered > 0
@@ -421,13 +418,13 @@ def test_hold_variants_at_extreme_instants(am, zmap, variant, T, mode):
                     m = min(200, n - 1)
                     p.load(int(rng.integers(1, n - m + 1)), population(rng, m, T, True, tz))
                 elif r < 0.47:
+                    p.set_hold(False)
+                    p.set_hold(True)
                     if remedy:
-                        assert p.set_hold(False) == 0 and p.set_hold(True) == 0 and p.set_remedy(True) == 0
-                    else:
-                        p.hold_off_on()
-                busy = p.st.since != NONE
+                        p.set_remedy(True)
+                busy = p.m.since != NONE
                 if remedy:
-                    busy |= p.st.rsince != NONE
+                    busy |= p.m.rsince != NONE
                 busy = np.flatnonzero(busy)
                 if len(busy) and k % 2:
                     sl = rng.choice(busy, min(len(busy), 30), replace=False)
@@ -435,7 +432,7 @@ def test_hold_variants_at_extreme_instants(am, zmap, variant, T, mode):
                     rp = np.where(rng.random(len(sl)) < 0.5, 0, rng.integers(1, 3, len(sl))).astype(np.uint8)
                     p.post(sl, ph, rp)
             T += step
-            held += int((p.st.in_flight() != NONE).sum())
+            held += int((p.m.in_flight() != NONE).sum())
             out = p.tick(T, mode)
             timed += len(out[3][0])
             if remedy:

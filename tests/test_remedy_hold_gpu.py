@@ -1,10 +1,9 @@
 """The remedy hold (am_sweep_set_hold_remedy, with the hold in flight on): a check is not submitted while its remedy
 workflow runs, and a remedy that outlives its workflow timeout is failed on the device.  Compared after every tick with
-the remedy-hold oracle (tests/remedy_hold_oracle.py) — list, statistics, all sixteen columns, am_sweep_in_flight,
+the model (tests/handle_model.py, tests/handle_pair.py) — list, statistics, all sixteen columns, am_sweep_in_flight,
 am_sweep_remedy_in_flight and both timed-out lists — through every tick entry point: the hand-derived cases, long random
 sequences on the adversarial population with sparse and dense posts, catch-up ticks on named zones, next_due against
 brute force, short buffers, launch counts, and 10 M records."""
-import os
 import zlib
 
 import numpy as np
@@ -13,8 +12,8 @@ import pytest
 import amgen
 import remedy_hold_cases
 import remedy_hold_oracle
-from adversarial import ZoneMap, first_difference, population, zones_usable
-from test_in_flight_gpu import DevOut
+from adversarial import ZoneMap, population, zones_usable
+from handle_pair import Pair, emulated
 
 pytestmark = pytest.mark.gpu
 
@@ -30,122 +29,6 @@ def zmap(am, orc):
     return ZoneMap()
 
 
-def _emulated(am):
-    return "emu" in os.path.basename(am.abi.LIB_PATH)
-
-
-class Pair:
-    """a handle with the hold and the remedy hold on and its oracle state, kept in step by every call and compared after
-    every tick; `tick` returns the handle's answer (the oracle's list for tick_shard, whose list stays on the device)"""
-
-    def __init__(self, am, zmap, cols, entry="tick", cap=None):
-        self.am, self.entry = am, entry
-        self.n = len(cols["flags"])
-        self.s = am.Sweep(capacity=self.n)
-        self.s.set_hold_in_flight(True)
-        self.s.set_hold_remedy(True)
-        self.s.load_range(0, cols)
-        self.st = remedy_hold_oracle.State(zmap, cols)
-        self.cap = cap
-        self.dev = None
-        self.hold = True
-        self.rtimed_total = 0
-        self.started = 0
-
-    def close(self):
-        self.s.close()
-
-    def upsert(self, slots, recs):
-        self.s.upsert(slots, recs)
-        self.st.upsert(slots, recs)
-
-    def remove(self, slots):
-        self.s.remove(slots)
-        self.st.remove(slots)
-
-    def post(self, slots, phase, rphase=None):
-        self.s.post_result(slots, phase, rphase)
-        self.st.post(slots, phase, rphase)
-
-    def load(self, first, cols):
-        self.s.load_range(first, cols)
-        self.st.load(first, cols)
-
-    def _rc(self, fn, on):
-        try:
-            fn(on)
-            return 0
-        except self.am.AmError as e:
-            return e.code
-
-    def set_hold(self, on):
-        rc = self._rc(self.s.set_hold_in_flight, on)
-        if rc == 0 and self.hold and not on:
-            self.st.hold_on_again()
-        self.hold = bool(on)
-        return rc
-
-    def set_remedy(self, on):
-        rc = self._rc(self.s.set_hold_remedy, on)
-        if rc == 0:
-            self.st.set_remedy(on)
-        return rc
-
-    def in_flight(self):
-        return self.s.in_flight(0, self.n)
-
-    def remedy_in_flight(self):
-        return self.s.remedy_in_flight(0, self.n)
-
-    def cols(self):
-        return self.s.read_range(0, self.n)
-
-    def tick(self, T, mode=0, entry=None):
-        am, s = self.am, self.s
-        entry = entry or self.entry
-        before = self.st.rsince.copy()
-        want = self.st.tick(T, mode)
-        self.started += int(((self.st.rsince == T) & (before != T)).sum())
-        if entry == "tick" and self.cap is not None:
-            try:
-                got = s.tick(T, mode=mode, cap=self.cap)
-            except am.AmError as e:
-                assert e.code == am.AM_E_NOSPACE
-                idx, act, left = s.last_list(0, e.needed)
-                assert left == e.needed == want[2]["n_emitted"]
-                got = (idx, act, None)
-            if got[2] is None:
-                got = (got[0], got[1], want[2])  # (an AM_E_NOSPACE tick: the statistics are not returned)
-        elif entry == "tick":
-            got = s.tick(T, mode=mode)
-        elif entry == "tick_view":
-            i, a, st = s.tick_view(T, mode=mode)
-            got = (i.astype(np.uint64), a.astype(np.uint32), st)
-        elif entry == "tick_device":
-            self.dev = self.dev or DevOut(am, self.n)
-            got = self.dev.tick(am, s, T, mode)
-        else:
-            s.tick_shard(T, mode=mode)
-            got = None
-        what = (entry, mode, T)
-        timed, rtimed = s.last_timed_out(), s.last_remedy_timed_out()
-        for k in range(2):
-            np.testing.assert_array_equal(timed[k], want[3][k], err_msg=str(what))
-            np.testing.assert_array_equal(rtimed[k], want[4][k], err_msg=str(what))
-        self.rtimed_total += len(rtimed[0])
-        dev = s.read_range(0, self.n)
-        if got is None:
-            for name in am.COLUMN_NAMES:
-                np.testing.assert_array_equal(dev[name], self.st.ocols[name], err_msg=f"{what} {name}")
-            got = want[:3]
-        else:
-            bad = first_difference(am, got, want[:3], dev, self.st.ocols)
-            assert bad is None, (what, bad)
-        np.testing.assert_array_equal(s.in_flight(0, self.n), self.st.in_flight(), err_msg=str(what))
-        np.testing.assert_array_equal(s.remedy_in_flight(0, self.n), self.st.remedy_in_flight(), err_msg=str(what))
-        return got[0], got[1], got[2], timed, rtimed
-
-
 def _empty(am, n):
     cols = am.records_to_columns(np.zeros(n, dtype=am.RECORD_DTYPE))
     cols["flags"][:] = am.F_TOMBSTONE
@@ -156,7 +39,7 @@ def _empty(am, n):
 @pytest.mark.parametrize("entry", ENTRIES)
 @pytest.mark.parametrize("case", remedy_hold_cases.CASES, ids=lambda c: c.__name__)
 def test_hand_derived_cases(am, zmap, case, entry):
-    p = Pair(am, zmap, _empty(am, 8), entry)
+    p = Pair(am, zmap, _empty(am, 8), hold=True, remedy=True, entry=entry)
     try:
         case(am, p)
     finally:
@@ -189,10 +72,13 @@ def _random_walk(am, p, rng, n, T, mode, population_of):
                 first = int(rng.integers(0, n - 200))
                 p.load(first, am.records_to_columns(population_of(200)))
             elif r < 0.44:
-                assert p.set_hold(False) == 0 and p.set_hold(True) == 0 and p.set_remedy(True) == 0
+                p.set_hold(False)
+                p.set_hold(True)
+                p.set_remedy(True)
             elif r < 0.47:
-                assert p.set_remedy(False) == 0 and p.set_remedy(True) == 0
-            busy = np.flatnonzero((p.st.since != NONE) | (p.st.rsince != NONE))
+                p.set_remedy(False)
+                p.set_remedy(True)
+            busy = np.flatnonzero((p.m.since != NONE) | (p.m.rsince != NONE))
             if len(busy) and k % 2:
                 dense = k % 5 == 3
                 sl = rng.choice(busy, min(len(busy), 2000 if dense else 30), replace=False)
@@ -212,7 +98,7 @@ def test_random_sequences_equal_the_oracle(am, zmap, entry, mode):
     rng = np.random.default_rng(zlib.crc32(f"remedy hold {entry} {mode}".encode()))
     T = T_OCT + 12 * DAY + 14 * HOUR - 3
     cols = population(rng, n, T, True, zmap.ids_of(zones_usable(T - DAY, T + 2 * DAY)))
-    p = Pair(am, zmap, cols, "tick" if entry == "short_buffer" else entry, cap=5 if entry == "short_buffer" else None)
+    p = Pair(am, zmap, cols, hold=True, remedy=True, entry="tick_short" if entry == "short_buffer" else entry, cap=5)
     try:
         _random_walk(am, p, rng, n, T, mode, lambda m: _records(am, rng, m, T, zmap, 120))
         assert p.started > 100 and p.rtimed_total > 10, (p.started, p.rtimed_total)
@@ -227,14 +113,14 @@ def test_catch_up_on_named_zones(am, zmap):
     cols = amgen.fill(22, 2, 0, n, T, am.load().am_healthcheck_classify)
     rng = np.random.default_rng(22)
     cols["flags"] |= np.where(rng.random(n) < 0.5, am.F_HAS_REMEDY, 0).astype(np.uint32)
-    p = Pair(am, zmap, cols)
+    p = Pair(am, zmap, cols, hold=True, remedy=True)
     try:
         recs = am.columns_to_records(cols)
         recs["wf_timeout"] = rng.integers(0, 400, n)
         p.upsert(np.arange(n), recs)
         for k, step in enumerate([0, 60, 1, 150, 59, 600, 1, 3600, 61, 240]):
             T += step
-            busy = np.flatnonzero((p.st.since != NONE) | (p.st.rsince != NONE))
+            busy = np.flatnonzero((p.m.since != NONE) | (p.m.rsince != NONE))
             if k and len(busy):
                 sl = rng.choice(busy, min(len(busy), 1500), replace=False)
                 p.post(sl, np.where(rng.random(len(sl)) < 0.7, 2, 0).astype(np.uint8),
@@ -254,7 +140,7 @@ def test_next_due_against_brute_force(am, zmap):
                            rec(am, 0, repeat_after_sec=300, finished_at=T - 1000, has_remedy=True),
                            rec(am, 200, cron="*/5 * * * *", has_remedy=True),
                            rec(am, 90, cron="7 * * * *")])
-    p = Pair(am, zmap, _empty(am, len(recs)))
+    p = Pair(am, zmap, _empty(am, len(recs)), hold=True, remedy=True)
     try:
         p.upsert(np.arange(len(recs)), recs)
         checked = 0
@@ -263,7 +149,7 @@ def test_next_due_against_brute_force(am, zmap):
             if post:
                 p.post(post, [2] * len(post))
             p.tick(T)
-            assert p.s.next_due(T) == p.st.next_event(T, 4000), T
+            assert p.s.next_due(T) == p.m.first_active_tick(T, 4000), T
             checked += 1
         assert checked == 7 and p.started >= 3
     finally:
@@ -305,12 +191,12 @@ def test_launch_counts(am):
 
 # ---- 6. full size, on the GPU only ----------------------------------------------------------------------------------------
 def test_full_size_config3(am, zmap):
-    if _emulated(am):
+    if emulated(am):
         pytest.skip("10 M records: GPU only")
     n = 10_000_000
     T0 = amgen.T0_MON_0915
     cols = amgen.fill(3, 3, 0, n, T0, am.load().am_healthcheck_classify)
-    p = Pair(am, zmap, cols)
+    p = Pair(am, zmap, cols, hold=True, remedy=True)
     rng = np.random.default_rng(3)
     try:
         recs = am.columns_to_records(cols)
@@ -320,7 +206,7 @@ def test_full_size_config3(am, zmap):
         for k, step in enumerate([0, 1, 59, 1, 60, 3600]):
             T += step
             if k in (1, 3):
-                fl = np.flatnonzero(p.st.since != NONE)
+                fl = np.flatnonzero(p.m.since != NONE)
                 sl = rng.choice(fl, min(len(fl), 50_000 if k == 1 else 2_000_000), replace=False)
                 p.post(sl, np.full(len(sl), 2, dtype=np.uint8))
             p.tick(T, mode=CATCH if k == 4 else 0, entry="tick_view" if k % 2 else "tick")

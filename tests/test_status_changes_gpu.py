@@ -1,9 +1,10 @@
 """Status changes (am_sweep_set_track_changes / am_sweep_last_changes): after every tick the handle's changed set must
-equal the changed-set oracle's (tests/changes_oracle.py, the column diff of the existing oracles' states), and the
-columns it returns the oracle's columns of those slots.  Through every tick entry point: the hand-derived cases, the
+equal the changed-set oracle's (tests/changes_oracle.py, the column diff of the model's states, tests/handle_model.py),
+and the columns it returns the model's columns of those slots.  Through every tick entry point: the hand-derived cases, the
 sparse and the dense result routes with reads between posts and ticks, the hold with timeouts and the remedy hold,
 catch-up ticks on named zones with AM_SWEEP_FULL_SCAN and closed loop, short buffers, refused ticks, the call contract,
-run_ticks, the switch, random call sequences through tests/sequence_model.py, launch counts and 10 M records."""
+run_ticks, the switch, random call sequences through tests/test_call_sequences_gpu.py's walk, launch counts and 10 M
+records."""
 import os
 import zlib
 
@@ -14,8 +15,8 @@ import amgen
 import changes_cases
 import changes_oracle
 from adversarial import ZoneMap, population, zones_usable
+from handle_pair import Pair, check_changes, emulated
 from test_call_sequences_gpu import WALKS, Walk
-from test_in_flight_gpu import DevOut
 from timeout_cases import M0, rec
 
 pytestmark = pytest.mark.gpu
@@ -32,88 +33,17 @@ def zmap(am, orc):
     return ZoneMap()
 
 
-def _emulated(am):
-    return "emu" in os.path.basename(am.abi.LIB_PATH)
-
-
-def check_changes(am, s, want, ocols, where, names=None):
-    """the handle's changed set against the oracle's, its columns against the oracle's columns"""
-    idx, cols = s.last_changes(names=names)
-    np.testing.assert_array_equal(idx, want, err_msg=f"{where}: changed set")
-    loc = (want - np.uint64(s.shard_base)).astype(np.int64)
-    for name, a in cols.items():
-        np.testing.assert_array_equal(a, ocols[name][loc], err_msg=f"{where}: {name}")
-    return len(idx)
-
-
-class Pair:
-    """a handle with tracking on and its oracle (changes_oracle.Model), kept in step by every call; every tick compares
-    the changed set and its columns"""
-
-    def __init__(self, am, zmap, n, hold=None, entry="tick", shard_base=0):
-        self.am, self.entry = am, entry
-        self.s = am.Sweep(capacity=n, shard_base=shard_base)
-        self.o = changes_oracle.Model(zmap, n, hold, shard_base)
-        if hold:
-            self.s.set_hold_in_flight(True)
-        if hold == "remedy":
-            self.s.set_hold_remedy(True)
-        self.s.set_track_changes(True)
-        self.dev = None
-        self.listed = 0
-
-    def close(self):
-        self.s.close()
-
-    def upsert(self, slots, recs):
-        self.s.upsert(slots, recs)
-        self.o.upsert(slots, recs)
-
-    def remove(self, slots):
-        self.s.remove(slots)
-        self.o.remove(slots)
-
-    def post(self, slots, phase, rphase=None):
-        self.s.post_result(slots, phase, rphase)
-        self.o.post(slots, phase, rphase)
-
-    def load(self, first, cols):
-        self.s.load_range(first, cols)
-        self.o.load(first, cols)
-
-    def read(self, slots):
-        self.s.read(slots)
-
-    def changes(self):
-        return self.o.changes()
-
-    def tick(self, T, mode=0, entry=None, names=None):
-        am, s = self.am, self.s
-        entry = entry or self.entry
-        want = self.o.tick(T, mode)
-        if entry == "tick":
-            s.tick(T, mode=mode)
-        elif entry == "tick_short":
-            try:
-                s.tick(T, mode=mode, cap=1)
-            except am.AmError as e:
-                assert e.code == am.AM_E_NOSPACE
-        elif entry == "tick_view":
-            s.tick_view(T, mode=mode)
-        elif entry == "tick_device":
-            self.dev = self.dev or DevOut(am, self.o.n)
-            self.dev.tick(am, s, T, mode)
-        else:
-            s.tick_shard(T, mode=mode)
-        self.listed += check_changes(am, s, self.o.changes(), self.o.cols, (entry, mode, T), names)
-        return want
+def pair(am, zmap, n, hold=None, **kw):
+    """a handle with tracking on and its model.  hold: None (off), "hold" (the hold in flight) or "remedy" (the hold,
+    workflow timeouts and the remedy hold)"""
+    return Pair(am, zmap, n, hold=hold is not None, remedy=hold == "remedy", track=True, every_slot=False, **kw)
 
 
 # ---- 1. the hand-derived cases, through every tick entry point -------------------------------------------------------
 @pytest.mark.parametrize("entry", ENTRIES)
 @pytest.mark.parametrize("case", changes_cases.CASES, ids=lambda c: c.__name__)
 def test_hand_derived_cases(am, zmap, case, entry):
-    p = Pair(am, zmap, case.n, case.hold, entry)
+    p = pair(am, zmap, case.n, case.hold, entry=entry)
     try:
         case(am, p)
     finally:
@@ -138,7 +68,7 @@ def _walk(am, zmap, hold, early, mode, seed_text, n=3000):
     old = os.environ.get("AMSWEEP_EARLY_RESULTS")
     os.environ["AMSWEEP_EARLY_RESULTS"] = str(early)
     try:
-        p = Pair(am, zmap, n, hold)
+        p = pair(am, zmap, n, hold)
     finally:
         if old is None:
             del os.environ["AMSWEEP_EARLY_RESULTS"]
@@ -186,7 +116,7 @@ def test_closed_loop(am, zmap):
     n = 4000
     rng = np.random.default_rng(5)
     T = M0 + 3
-    p = Pair(am, zmap, n)
+    p = pair(am, zmap, n)
     try:
         p.upsert(np.arange(n), am.columns_to_records(population(rng, n, T, True, zmap.ids_of(zones_usable(T - DAY, T + DAY)))))
         for k, step in enumerate([0, 1, 57, 60, 1, 3600]):
@@ -207,7 +137,7 @@ def test_catch_up_on_named_zones(am, zmap):
     cols = amgen.fill(22, 2, 0, n, T, am.load().am_healthcheck_classify)
     rng = np.random.default_rng(22)
     cols["flags"] |= np.where(rng.random(n) < 0.5, am.F_HAS_REMEDY, 0).astype(np.uint32)
-    p = Pair(am, zmap, n, "remedy")
+    p = pair(am, zmap, n, "remedy")
     try:
         recs = am.columns_to_records(cols)
         recs["wf_timeout"] = rng.integers(0, 400, n)
@@ -281,44 +211,18 @@ def test_contract(am, zmap):
 
 # ---- 5. random call sequences through the sequence model ------------------------------------------------------------------
 class ChangesWalk(Walk):
-    """tests/test_call_sequences_gpu.py's walk with tracking on: after every tick the changed set against the model's
-    column diff; run_ticks empties it; the switch is turned off and on again now and then"""
+    """tests/test_call_sequences_gpu.py's walk with tracking on (it compares the changed set after every tick and
+    run_ticks); the switch is turned off and on again now and then"""
 
-    def __init__(self, *a):
-        super().__init__(*a)
-        self.s.set_track_changes(True)
-        self.want = changes_oracle.EMPTY
+    def __init__(self, *a, details=False):
+        super().__init__(*a, track=True, details=details)
         self.checked = 0
-        tick = self.m.tick
-
-        def recorded(T, mode):
-            out = tick(T, mode)
-            self.out = out
-            return out
-
-        self.m.tick = recorded
 
     def tick(self, T, mode, every_column, entry=None):
-        before = changes_oracle.snapshot(self.m.cols)
         if self.step % 11 == 10 and self.rng.integers(0, 2):
-            self.s.set_track_changes(False)
-            self.s.set_track_changes(True)
-            self.want = changes_oracle.EMPTY
-        ok = super().tick(T, mode, every_column, entry)
-        if ok:
-            self.want = changes_oracle.changed(before, self.m.cols, self.out[0], self.out[1], self.s.shard_base)
-            check_changes(self.am, self.s, self.want, self.m.cols, self.where)
-        else:
-            np.testing.assert_array_equal(self.s.last_changes(names=[])[0], self.want, err_msg=str(self.where))
+            self.set_track()
         self.checked += 1
-        return ok
-
-    def run_ticks(self, T, every_column):
-        k = super().run_ticks(T, every_column)
-        if k:
-            self.want = changes_oracle.EMPTY
-        np.testing.assert_array_equal(self.s.last_changes(names=[])[0], self.want, err_msg=str(self.where))
-        return k
+        return super().tick(T, mode, every_column, entry)
 
 
 @pytest.mark.parametrize("k", [0, 2, 3, 5], ids=[WALKS[k][3] for k in (0, 2, 3, 5)])
@@ -359,7 +263,7 @@ def test_launch_counts(am):
 # ---- 7. full size, on the GPU only -----------------------------------------------------------------------------------------
 def test_full_size_config3(am, zmap):
     """one 10 M-record config 3 tick: 75 % of the records have a result (the dense route), compared in full"""
-    if _emulated(am):
+    if emulated(am):
         pytest.skip("10 M records: GPU only")
     n = 10_000_000
     T0 = amgen.T0_MON_0915
@@ -372,4 +276,4 @@ def test_full_size_config3(am, zmap):
         want = changes_oracle.changed(before, cols, idx, act)
         s.tick_view(T0)
         assert len(want) > 7_000_000, len(want)
-        check_changes(am, s, want, cols, "config 3", names=STATUS)
+        check_changes(s, want, cols, "config 3", names=STATUS)

@@ -1,5 +1,5 @@
-"""The workflow-timeout oracle (tests/timeout_oracle.py) reproduces the hand-derived cases of tests/timeout_cases.py, and
-with no deadline anywhere it is the hold oracle's tick."""
+"""The workflow-timeout oracle (tests/timeout_oracle.py) in tests/handle_model.py reproduces the hand-derived cases of
+tests/timeout_cases.py, and with no deadline anywhere it is the hold oracle's tick."""
 import numpy as np
 import pytest
 
@@ -7,32 +7,12 @@ import hold_oracle
 import timeout_cases
 import timeout_oracle
 from adversarial import ZoneMap, population, zones_usable
-
-
-class OracleDriver:
-    def __init__(self, am, n=8):
-        self.st = timeout_oracle.State(ZoneMap(), am.records_to_columns(np.zeros(n, dtype=am.RECORD_DTYPE)))
-        self.st.ocols["flags"][:] = am.F_TOMBSTONE
-
-    def upsert(self, slots, recs):
-        self.st.upsert(slots, recs)
-
-    def post(self, slots, phase, rphase=None):
-        self.st.post(slots, phase, rphase)
-
-    def tick(self, T, mode=0):
-        return self.st.tick(T, mode)
-
-    def in_flight(self):
-        return self.st.in_flight()
-
-    def cols(self):
-        return self.st.ocols
+from handle_model import HandleModel
 
 
 @pytest.mark.parametrize("case", timeout_cases.CASES, ids=lambda c: c.__name__)
 def test_hand_derived_cases(am, orc, case):
-    case(am, OracleDriver(am))
+    case(am, HandleModel(ZoneMap(), 8, hold=True))
 
 
 def test_without_deadlines_it_is_the_hold_oracle(am, orc):

@@ -1,9 +1,8 @@
 """Workflow timeouts (am_record_t.wf_timeout with the hold in flight on): a held run that outlives its deadline is
-treated at the first tick past it as if Failed had been posted.  Compared after every tick with the timeout oracle
-(tests/timeout_oracle.py) — list, statistics, all sixteen columns, am_sweep_in_flight and am_sweep_last_timed_out —
+treated at the first tick past it as if Failed had been posted.  Compared after every tick with the model
+(tests/handle_model.py, tests/handle_pair.py) — list, statistics, all sixteen columns, am_sweep_in_flight and am_sweep_last_timed_out —
 through every tick entry point: the hand-derived cases, long random sequences on the adversarial population, next_due
 against brute force, the refusals, the hold off, launch counts, and 10 M records."""
-import os
 import zlib
 
 import numpy as np
@@ -11,9 +10,8 @@ import pytest
 
 import amgen
 import timeout_cases
-import timeout_oracle
-from adversarial import ZoneMap, first_difference, population, zones_usable
-from test_in_flight_gpu import DevOut
+from adversarial import ZoneMap, population, zones_usable
+from handle_pair import Pair, emulated
 
 pytestmark = pytest.mark.gpu
 
@@ -29,97 +27,6 @@ def zmap(am, orc):
     return ZoneMap()
 
 
-def _emulated(am):
-    return "emu" in os.path.basename(am.abi.LIB_PATH)
-
-
-class Pair:
-    """a handle with the hold on and its timeout-oracle state, kept in step by every call and compared after every
-    tick; `tick` returns the handle's answer (the oracle's list for tick_shard, whose list stays on the device)"""
-
-    def __init__(self, am, zmap, cols, entry="tick", cap=None):
-        self.am, self.entry = am, entry
-        self.n = len(cols["flags"])
-        self.s = am.Sweep(capacity=self.n)
-        self.s.set_hold_in_flight(True)
-        self.s.load_range(0, cols)
-        self.st = timeout_oracle.State(zmap, cols)
-        self.cap = cap
-        self.dev = None
-        self.timed_total = 0
-
-    def close(self):
-        self.s.close()
-
-    def upsert(self, slots, recs):
-        self.s.upsert(slots, recs)
-        self.st.upsert(slots, recs)
-
-    def remove(self, slots):
-        self.s.remove(slots)
-        self.st.remove(slots)
-
-    def post(self, slots, phase, rphase=None):
-        self.s.post_result(slots, phase, rphase)
-        self.st.post(slots, phase, rphase)
-
-    def load(self, first, cols):
-        self.s.load_range(first, cols)
-        self.st.load(first, cols)
-
-    def hold_off_on(self):
-        self.s.set_hold_in_flight(False)
-        self.s.set_hold_in_flight(True)
-        self.st.hold_on_again()
-
-    def in_flight(self):
-        return self.s.in_flight(0, self.n)
-
-    def cols(self):
-        return self.s.read_range(0, self.n)
-
-    def tick(self, T, mode=0, entry=None):
-        am, s = self.am, self.s
-        entry = entry or self.entry
-        want = self.st.tick(T, mode)
-        if entry == "tick" and self.cap is not None:
-            try:
-                got = s.tick(T, mode=mode, cap=self.cap)
-            except am.AmError as e:
-                assert e.code == am.AM_E_NOSPACE
-                idx, act, left = s.last_list(0, e.needed)
-                assert left == e.needed == want[2]["n_emitted"]
-                got = (idx, act, None)
-            if got[2] is None:
-                got = (got[0], got[1], want[2])  # (an AM_E_NOSPACE tick: the statistics are not returned)
-        elif entry == "tick":
-            got = s.tick(T, mode=mode)
-        elif entry == "tick_view":
-            i, a, st = s.tick_view(T, mode=mode)
-            got = (i.astype(np.uint64), a.astype(np.uint32), st)
-        elif entry == "tick_device":
-            self.dev = self.dev or DevOut(am, self.n)
-            got = self.dev.tick(am, s, T, mode)
-        else:
-            s.tick_shard(T, mode=mode)
-            got = None
-        timed = s.last_timed_out()
-        what = (entry, mode, T)
-        np.testing.assert_array_equal(timed[0], want[3][0], err_msg=str(what))
-        np.testing.assert_array_equal(timed[1], want[3][1], err_msg=str(what))
-        self.timed_total += len(timed[0])
-        dev = s.read_range(0, self.n)
-        if got is None:
-            for name in am.COLUMN_NAMES:
-                np.testing.assert_array_equal(dev[name], self.st.ocols[name], err_msg=f"{what} {name}")
-            got = want[:3]
-        else:
-            bad = first_difference(am, got, want[:3], dev, self.st.ocols)
-            assert bad is None, (what, bad)
-        np.testing.assert_array_equal(s.in_flight(0, self.n), self.st.in_flight(), err_msg=str(what))
-        return got[0], got[1], got[2], timed
-
-
 def _empty(am, n):
     cols = am.records_to_columns(np.zeros(n, dtype=am.RECORD_DTYPE))
     cols["flags"][:] = am.F_TOMBSTONE
@@ -130,7 +37,7 @@ def _empty(am, n):
 @pytest.mark.parametrize("entry", ENTRIES)
 @pytest.mark.parametrize("case", timeout_cases.CASES, ids=lambda c: c.__name__)
 def test_hand_derived_cases(am, zmap, case, entry):
-    p = Pair(am, zmap, _empty(am, 8), entry)
+    p = Pair(am, zmap, _empty(am, 8), hold=True, entry=entry)
     try:
         case(am, p)
     finally:
@@ -155,7 +62,7 @@ def test_random_sequences_equal_the_oracle(am, zmap, entry, mode):
     rng = np.random.default_rng(zlib.crc32(f"timeout {entry} {mode}".encode()))
     T = T_OCT + 12 * DAY + 14 * HOUR - 3
     cols = population(rng, n, T, True, zmap.ids_of(zones_usable(T - DAY, T + 2 * DAY)))
-    p = Pair(am, zmap, cols, "tick" if entry == "short_buffer" else entry, cap=5 if entry == "short_buffer" else None)
+    p = Pair(am, zmap, cols, hold=True, entry="tick_short" if entry == "short_buffer" else entry, cap=5)
     try:
         # W on most records from the start (a load sets none: upsert them)
         sl = np.arange(n)
@@ -172,8 +79,9 @@ def test_random_sequences_equal_the_oracle(am, zmap, entry, mode):
                     first = int(rng.integers(0, n - 200))
                     p.load(first, population(rng, 200, T, True, zmap.ids_of(zones_usable(T - DAY, T + 2 * DAY))))
                 elif r < 0.53:
-                    p.hold_off_on()
-                fl = np.flatnonzero(p.st.since != NONE)
+                    p.set_hold(False)
+                    p.set_hold(True)
+                fl = np.flatnonzero(p.m.since != NONE)
                 if len(fl) and k % 2:
                     dense = k % 5 == 3
                     sl = rng.choice(fl, min(len(fl), 2000 if dense else 30), replace=False)
@@ -196,7 +104,7 @@ def test_next_due_counts_expiries(am, zmap):
                            rec(am, 0, repeat_after_sec=300, finished_at=T - 1000),
                            rec(am, 200, cron="*/5 * * * *"),
                            rec(am, 90, cron="7 * * * *")])
-    p = Pair(am, zmap, _empty(am, len(recs)))
+    p = Pair(am, zmap, _empty(am, len(recs)), hold=True)
     try:
         p.upsert(np.arange(len(recs)), recs)
         checked = 0
@@ -206,7 +114,7 @@ def test_next_due_counts_expiries(am, zmap):
                 p.post(post, [am.PHASE_SUCCEEDED] * len(post))
             p.tick(T)
             nd = p.s.next_due(T)
-            want = p.st.next_event(T, 4000)
+            want = p.m.first_active_tick(T, 4000)
             assert nd == want, (T, nd, want)
             checked += 1
         assert checked == 7
@@ -283,12 +191,12 @@ def test_launch_counts(am):
 
 # ---- 5. full size, on the GPU only --------------------------------------------------------------------------------------
 def test_full_size_config2_with_a_burst_of_expiries(am, zmap):
-    if _emulated(am):
+    if emulated(am):
         pytest.skip("10 M records: GPU only")
     n = 10_000_000
     T0 = amgen.T0_MON_0915
     cols = amgen.fill(2, 2, 0, n, T0, am.load().am_healthcheck_classify)
-    p = Pair(am, zmap, cols)
+    p = Pair(am, zmap, cols, hold=True)
     rng = np.random.default_rng(2)
     try:
         recs = am.columns_to_records(cols)
@@ -298,7 +206,7 @@ def test_full_size_config2_with_a_burst_of_expiries(am, zmap):
         for k, step in enumerate([0, 1, 59, 1, 60, 3600]):
             T += step
             if k == 3:
-                fl = np.flatnonzero(p.st.since != NONE)
+                fl = np.flatnonzero(p.m.since != NONE)
                 sl = rng.choice(fl, min(len(fl), 50_000), replace=False)
                 p.post(sl, rng.integers(1, 3, len(sl)).astype(np.uint8))
             got = p.tick(T, mode=CATCH if k == 4 else 0, entry="tick_view" if k % 2 else "tick")

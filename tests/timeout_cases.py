@@ -1,5 +1,5 @@
 """Hand-derived cases of workflow timeouts (am_record_t.wf_timeout with the hold in flight on), written against a
-`driver`: the timeout oracle alone (tests/test_timeout_oracle.py) or a handle compared with it after every tick
+`driver`: the model alone (tests/handle_model.py) or a handle compared with it after every tick
 (tests/test_workflow_timeout_gpu.py, through every tick entry point).  A driver has upsert(slots, recs),
 post(slots, phase, rphase=None), tick(T, mode=0) -> (global idx, action, stats, (timed-out idx, since)),
 in_flight() -> since per slot, and cols() -> the sixteen columns."""
