@@ -39,6 +39,49 @@ def build():
     return LIB
 
 
+def build_tsan(main_cpp, out):
+    """tests/emu/<main_cpp> with the library's own sources on the emulator, built with -fsanitize=thread into `out`
+    (the emulator tells TSan about its fibers); skips the test when the toolchain has no ThreadSanitizer runtime"""
+    import pytest
+    srcs = sources()[0] + [os.path.join(HERE, main_cpp)]
+    r = subprocess.run(["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-Wno-unknown-pragmas", "-Wno-tsan",
+                        "-pthread", "-DAMSWEEP_EMULATE", "-include", os.path.join(HERE, "cuda_emu.h"),
+                        "-include", os.path.join(HERE, "cuda_rt_emu.h"), "-x", "c++"] + srcs + ["-o", out],
+                       capture_output=True, text=True)
+    if r.returncode != 0:
+        pytest.skip("ThreadSanitizer runtime not available: " + r.stderr[-300:])
+    return out
+
+
+def _child(cmd, env, timeout):
+    return subprocess.run([sys.executable] + cmd, cwd=ROOT, env=dict(os.environ, AMSWEEP_LIB=build(), **(env or {})),
+                          capture_output=True, text=True, timeout=timeout)
+
+
+def run_script(name, args, env=None, timeout=900):
+    """tests/emu/<name> with `args` on the emulated library, in a child process: it must exit 0 and print "ok ..."
+    first; returns its stdout"""
+    out = _child([os.path.join(HERE, name)] + [str(a) for a in args], env, timeout)
+    assert out.returncode == 0 and out.stdout.strip().startswith("ok"), out.stdout[-3000:] + out.stderr[-3000:]
+    return out.stdout
+
+
+def run_suite(paths, k=None, env=None, timeout=1800, allow=()):
+    """the `-m gpu` tests of `paths` on the emulated library, in a child pytest that must pass.  Returns its summary
+    line as counts, e.g. {"passed": 61, "deselected": 2}; an outcome other than passed that is not in `allow`
+    (failed, error, skipped, xfailed, ...) fails the call."""
+    out = _child(["-m", "pytest"] + ([paths] if isinstance(paths, str) else list(paths)) +
+                 ["-m", "gpu", "-q", "-x", "-p", "no:cacheprovider"] + (["-k", k] if k else []), env, timeout)
+    tail = out.stdout[-3000:] + out.stderr[-2000:]
+    assert out.returncode == 0, tail
+    counts = {}
+    for part in out.stdout.strip().splitlines()[-1].strip("= ").split(" in ")[0].split(", "):
+        n, what = part.split()
+        counts[what.rstrip("s") if what in ("errors", "warnings") else what] = int(n)
+    assert counts.get("passed", 0) > 0 and set(counts) <= {"passed", "deselected", "warning", *allow}, tail
+    return counts
+
+
 def load():
     global _lib
     if _lib is None:

@@ -1,7 +1,4 @@
-"""Child process of the emulator tests: `world` ranks as Python threads drive the REAL C-ABI of the
-emulated library (csrc/sweep.cu + csrc/gather.cu host code, the tick and exchange kernels on
-cuda_emu.h; CUDA IPC handles carry plain pointers, cuda_rt_emu.h).  ctypes releases the GIL during
-a call, so the ranks' push kernels really run concurrently and meet through their flags.
+"""Child process of the emulator tests: `world` ranks drive the exchange through the rank harness (tests/emu/ranks.py).
 
 usage: run_gather_ranks.py tick  <world> <idx_bytes> <records in total> <ticks> [config]
        run_gather_ranks.py plain <world> <idx_bytes> <records per rank> <ticks>
@@ -16,147 +13,83 @@ tick : every rank owns an index-range shard of ONE amgen population (am.Sweep on
 plain: the round-1 list format (am_gather_push) against the concatenation of random lists.
 Prints "ok ..." and exits 0 on success."""
 import ctypes as C
-import importlib
 import os
 import sys
-import threading
 
 import numpy as np
+from ranks import Gather, Shards, abi, am, check_columns, check_list, check_view, lib, run_ranks
 
-ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tools", "amgen")):
-    sys.path.insert(0, p)
-abi = importlib.import_module("active-monitor_b200._lib")
-assert "emu" in os.path.basename(abi.LIB_PATH), "run with AMSWEEP_LIB pointing at libamsweep_emu.so"
-am = importlib.import_module("active-monitor_b200")
-gather = importlib.import_module("active-monitor_b200.gather")
-lib = abi.load()
+import amgen  # noqa: E402
+import oracle_c  # noqa: E402
 
 mode, world, idx_bytes, n_arg, ticks = sys.argv[1], int(sys.argv[2]), int(sys.argv[3]), int(sys.argv[4]), int(sys.argv[5])
 config = int(sys.argv[6]) if len(sys.argv) > 6 else 3
 T0 = 1789982100
 absent = int(os.environ.get("EMU_ABSENT_RANK", "-1"))
 use_view = os.environ.get("EMU_TICK_VIEW") == "1"  # am_gather_tick_view instead of tick_shard + exchange
-handles = [None] * world
-errors = []
-bar = threading.Barrier(world)
-
-
-def view(ptr, n, ctype, dtype):
-    """numpy copy of n elements at a raw address (np.ctypeslib.as_array on a POINTER patches the
-    ctypes type object: not safe from several rank threads at once)"""
-    if n == 0:
-        return np.zeros(0, dtype)
-    return np.frombuffer((ctype * n).from_address(ptr), dtype=dtype).copy()
-
-
-def out_views(h, total):
-    it, dt = (C.c_uint32, np.uint32) if idx_bytes == 4 else (C.c_uint64, np.uint64)
-    gi = view(lib.am_gather_out_idx(h), total, it, dt).astype(np.uint64)
-    ga = view(lib.am_gather_out_act(h), total, C.c_uint8, np.uint8)
-    return gi, ga
-
-
-def out_counts(h):
-    return view(lib.am_gather_out_counts(h), world + 1, C.c_uint32, np.uint32)
-
-
-def connect(rank, cap_total):
-    h = C.c_void_p()
-    assert lib.am_gather_create(C.byref(h), rank, rank, world, cap_total, idx_bytes) == 0
-    mine = C.create_string_buffer(abi.IPC_HANDLE_BYTES)
-    assert lib.am_gather_export(h, mine) == 0
-    handles[rank] = bytes(mine.raw)
-    bar.wait()
-    assert lib.am_gather_connect(h, b"".join(handles)) == 0
-    return h
 
 
 # ---------------------------------------------------------------- tick exchange
 if mode == "tick":
-    import amgen
-    import oracle_c
     n_total = n_arg
-    shards = [gather.shard_range(n_total, r, world) for r in range(world)]
-    bases = np.array([s[0] for s in shards], dtype=np.uint64)
-    sizes = np.array([s[1] for s in shards], dtype=np.uint64)
+    lay = Shards(n_total, world)
     whole = amgen.fill(config, 4, 0, n_total, T0, oracle_c.load().orc_classify, threads=2)
-    want = []  # per tick: (idx, act, per-shard stats)
+    want = []  # per tick: (T, idx, act)
     for k in range(ticks):
         T = T0 + 60 * k - (k % 2)  # on and off the minute
         wi, wa, _ = oracle_c.sweep(whole, T)
         want.append((T, wi, wa))
 
-    def rank_main(rank):
-        try:
-            first, cnt = shards[rank]
-            cols = amgen.fill(config, 4, first, cnt, T0, lib.am_healthcheck_classify, threads=1)
-            ocols = {k: v.copy() for k, v in cols.items()}
-            s = am.Sweep(capacity=cnt, device=rank, shard_base=first)
-            s.load_range(0, cols)
-            h = connect(rank, n_total)
-            assert lib.am_gather_set_layout(h, bases.ctypes.data, sizes.ctypes.data) == 0
-            # argument errors come back before anything a peer could observe happens
-            assert lib.am_gather_exchange(h, s._h, None, None) == abi.AM_E_INVAL  # no tick_shard yet
-            if use_view:
-                assert lib.am_gather_tick_view(h, T0, 0, C.byref(abi.AmTickView()), None) == abi.AM_E_INVAL  # not bound yet
-                assert lib.am_gather_bind(h, s._h, None, None) == 0
-            st = np.zeros(1, dtype=abi.STATS_DTYPE)
-            for k, (T, wi, wa) in enumerate(want):  # no barrier between ticks, as on a stream
-                if rank == absent:
-                    continue
-                vw = None
-                if use_view:  # the whole step in one call (am_gather_bind + am_gather_tick_view)
-                    v = abi.AmTickView()
-                    rc = lib.am_gather_tick_view(h, T, 0, C.byref(v), C.cast(st.ctypes.data, C.POINTER(abi.AmTickStats)))
-                    if absent >= 0:
-                        assert rc == abi.AM_E_DEVICE, rc  # a peer never arrived: the watchdog, reported as an error
-                    else:
-                        assert rc == 0, (rc, lib.am_gather_last_error(h))
-                        vw = (view(C.cast(v.idx_local, C.c_void_p).value, int(v.n), C.c_uint32, np.uint32),
-                              view(C.cast(v.action, C.c_void_p).value, int(v.n), C.c_uint8, np.uint8), int(v.shard_base))
+    def rank_main(rank, bar):
+        first, cnt = lay.shards[rank]
+        cols = amgen.fill(config, 4, first, cnt, T0, lib.am_healthcheck_classify, threads=1)
+        ocols = {k: v.copy() for k, v in cols.items()}
+        s = am.Sweep(capacity=cnt, device=rank, shard_base=first)
+        s.load_range(0, cols)
+        g = Gather(rank, bar, n_total, idx_bytes)
+        g.set_layout(lay)
+        # argument errors come back before anything a peer could observe happens
+        assert lib.am_gather_exchange(g.h, s._h, None, None) == abi.AM_E_INVAL  # no tick_shard yet
+        if use_view:
+            assert lib.am_gather_tick_view(g.h, T0, 0, C.byref(abi.AmTickView()), None) == abi.AM_E_INVAL  # not bound yet
+            g.bind(s)
+
+        def exchange(T):
+            s.tick_shard(T)
+            rc = lib.am_gather_exchange(g.h, s._h, g.st.ctypes.data, None)
+            assert rc == 0, (rc, lib.am_gather_last_error(g.h))
+
+        for k, (T, wi, wa) in enumerate(want if rank != absent else []):  # no barrier between ticks, as on a stream
+            if absent >= 0:  # a peer never arrives: the watchdog value, which the whole step reports as an error
+                if use_view:
+                    rc = g.tick_view(T, 0)[0]
+                    assert rc == abi.AM_E_DEVICE, rc
                 else:
-                    s.tick_shard(T)
-                    rc = lib.am_gather_exchange(h, s._h, st.ctypes.data, None)
-                    assert rc == 0, (rc, lib.am_gather_last_error(h))
-                counts = out_counts(h)
-                if absent >= 0:
-                    assert int(counts[world]) == 0xFFFFFFFF, counts
-                    break
-                total = int(counts[world])
-                assert total <= n_total, (rank, k, counts.tolist())
-                gi, ga = out_views(h, total)
-                np.testing.assert_array_equal(gi, wi, err_msg=f"rank {rank} tick {k} idx")
-                np.testing.assert_array_equal(ga.astype(np.uint32), wa, err_msg=f"rank {rank} tick {k} act")
-                oi, oa, ost = oracle_c.sweep(ocols, T, shard_base=first)  # this shard alone
-                got = {f: int(st[f][0]) for f in abi.STAT_FIELDS}
-                assert got == ost, (rank, k, got, ost)
-                if vw is not None:  # this rank's own part of the global list, as local slots
-                    assert vw[2] == first
-                    np.testing.assert_array_equal(vw[0].astype(np.uint64) + np.uint64(first), oi, err_msg=f"rank {rank} tick {k} view idx")
-                    np.testing.assert_array_equal(vw[1].astype(np.uint32), oa, err_msg=f"rank {rank} tick {k} view act")
-                assert [int(c) for c in counts[:world]] == [int(((wi >= b) & (wi < b + z)).sum()) for b, z in zip(bases, sizes)]
-            if absent < 0:
-                dev = s.read_range(0, cnt)
-                for name in abi.COLUMN_NAMES:
-                    np.testing.assert_array_equal(dev[name], ocols[name], err_msg=f"rank {rank} column {name}")
-            bar.wait()
-            lib.am_gather_destroy(h)
-            s.close()
-        except BaseException as e:  # noqa: BLE001
-            import traceback
-            errors.append((rank, repr(e), traceback.format_exc()[-1500:]))
-            try:
-                bar.abort()
-            except Exception:
-                pass
+                    exchange(T)
+                counts = g.counts()
+                assert int(counts[world]) == 0xFFFFFFFF, counts
+                break
+            if use_view:  # the whole step in one call (am_gather_bind + am_gather_tick_view)
+                gi, ga, counts, vw = g.step(T, 0)
+            else:
+                exchange(T)
+                gi, ga, counts = g.read()
+            check_list(rank, k, gi, ga, wi, wa)
+            oi, oa, ost = oracle_c.sweep(ocols, T, shard_base=first)  # this shard alone
+            got = {f: int(g.st[f][0]) for f in abi.STAT_FIELDS}
+            assert got == ost, (rank, k, got, ost)
+            if use_view:  # this rank's own part of the global list
+                check_view(rank, k, vw, oi, oa)
+            assert [int(c) for c in counts[:world]] == [int(lay.own(wi, r).sum()) for r in range(world)]
+        if absent < 0:
+            check_columns(rank, s, ocols)
+        g.close(bar, s)
 
 # ---------------------------------------------------------------- plain lists
 else:
     n_rec = n_arg
     sizes_l = [n_rec + (37 if r == world - 1 else 0) for r in range(world)]
     bases = np.concatenate([[0], np.cumsum(sizes_l)[:-1]]).astype(np.uint64)
-    cap_total = int(sum(sizes_l))
 
     def local_list(rank, tick):
         rng = np.random.default_rng(1000 * tick + rank)
@@ -167,42 +100,25 @@ else:
         act = np.where(rng.random(len(idx)) < 0.97, 0x01, rng.choice([0x08, 0x23, 0x80], len(idx))).astype(np.uint8)
         return idx, act
 
-    def rank_main(rank):
-        try:
-            h = connect(rank, cap_total)
-            for t in range(1, ticks + 1):
-                idx, act = local_list(rank, t)
-                cnt = np.array([len(idx)], dtype=np.uint32)
-                idx_buf = np.concatenate([idx, np.zeros(4, np.uint32)])  # device buffers are larger than the list
-                act_buf = np.concatenate([act, np.zeros(4, np.uint8)])
-                rc = lib.am_gather_push(h, idx_buf.ctypes.data, act_buf.ctypes.data, cnt.ctypes.data, int(bases[rank]), None)
-                assert rc == 0, (rc, lib.am_gather_last_error(h))
-                counts = out_counts(h)
-                gi, ga = out_views(h, int(counts[world]))
-                want_i, want_a = [], []
-                for r in range(world):
-                    li, la = local_list(r, t)
-                    assert int(counts[r]) == len(li), (rank, t, r, int(counts[r]), len(li))
-                    want_i.append(li.astype(np.uint64) + bases[r])
-                    want_a.append(la)
-                np.testing.assert_array_equal(gi, np.concatenate(want_i), err_msg=f"rank {rank} tick {t} idx")
-                np.testing.assert_array_equal(ga, np.concatenate(want_a), err_msg=f"rank {rank} tick {t} act")
-            bar.wait()
-            lib.am_gather_destroy(h)
-        except BaseException as e:  # noqa: BLE001
-            errors.append((rank, repr(e), ""))
-            try:
-                bar.abort()
-            except Exception:
-                pass
+    def rank_main(rank, bar):
+        g = Gather(rank, bar, int(sum(sizes_l)), idx_bytes)
+        for t in range(1, ticks + 1):
+            idx, act = local_list(rank, t)
+            cnt = np.array([len(idx)], dtype=np.uint32)
+            idx_buf = np.concatenate([idx, np.zeros(4, np.uint32)])  # device buffers are larger than the list
+            act_buf = np.concatenate([act, np.zeros(4, np.uint8)])
+            rc = lib.am_gather_push(g.h, idx_buf.ctypes.data, act_buf.ctypes.data, cnt.ctypes.data, int(bases[rank]), None)
+            assert rc == 0, (rc, lib.am_gather_last_error(g.h))
+            gi, ga, counts = g.read()
+            want_i, want_a = [], []
+            for r in range(world):
+                li, la = local_list(r, t)
+                assert int(counts[r]) == len(li), (rank, t, r, int(counts[r]), len(li))
+                want_i.append(li.astype(np.uint64) + bases[r])
+                want_a.append(la)
+            check_list(rank, t, gi, ga, np.concatenate(want_i), np.concatenate(want_a))
+        g.close(bar)
 
 
-th = [threading.Thread(target=rank_main, args=(r,)) for r in range(world)]
-for t in th:
-    t.start()
-for t in th:
-    t.join()
-if errors:
-    print("FAILED", errors)
-    sys.exit(1)
+run_ranks(world, rank_main)
 print(f"ok {mode}{' watchdog' if absent >= 0 else ''} world={world} idx_bytes={idx_bytes} n={n_arg} ticks={ticks}")

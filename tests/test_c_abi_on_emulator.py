@@ -20,15 +20,14 @@ import pytest
 
 from conftest import ROOT
 
-EMU = os.path.join(ROOT, "tests", "emu")
-CSRC = os.path.join(ROOT, "active-monitor_b200", "csrc")
-LIB = os.path.join(EMU, "libamsweep_emu.so")
+sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
+import emu_sweep  # noqa: E402
+
+EMU = emu_sweep.HERE
 
 
 @pytest.fixture(scope="module")
 def emu_lib():
-    sys.path.insert(0, EMU)
-    import emu_sweep
     return emu_sweep.build()
 
 
@@ -41,18 +40,11 @@ def test_emulated_library_exports_the_whole_abi(emu_lib):
         assert hasattr(lib, name), name
 
 
-def test_gpu_parity_suite_through_the_c_abi_on_the_emulated_library(emu_lib):
-    env = dict(os.environ, AMSWEEP_LIB=emu_lib)
-    out = subprocess.run([sys.executable, "-m", "pytest", "tests/test_sweep_gpu.py", "tests/test_golden_fixtures.py",
-                          "tests/test_timezones.py", "tests/test_sweep_adversarial_gpu.py",
-                          "tests/test_device_pipeline_gpu.py",
-                          "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider", "-k", "not tick_device and not 10m"],
-                         cwd=ROOT, env=env, capture_output=True, text=True, timeout=1800)
-    tail = out.stdout[-3000:] + out.stderr[-2000:]
-    assert out.returncode == 0, tail
-    last = out.stdout.strip().splitlines()[-1]
-    assert " passed" in last and "failed" not in last and "error" not in last, tail
-    assert int(last.split(" passed")[0].split()[-1]) >= 135, tail
+def test_gpu_parity_suite_through_the_c_abi_on_the_emulated_library():
+    got = emu_sweep.run_suite(["tests/test_sweep_gpu.py", "tests/test_golden_fixtures.py", "tests/test_timezones.py",
+                               "tests/test_sweep_adversarial_gpu.py", "tests/test_device_pipeline_gpu.py"],
+                              k="not tick_device and not 10m", allow=("skipped",))
+    assert got["passed"] >= 135, got
 
 
 def test_reconciler_cpp_mirror_on_the_emulated_library(emu_lib):
@@ -66,31 +58,19 @@ def test_reconciler_cpp_mirror_on_the_emulated_library(emu_lib):
     assert out.returncode == 0 and out.stdout.strip().endswith("ok"), out.stdout + out.stderr
 
 
-def test_random_call_sequences_against_a_sequential_model(emu_lib):
+def test_random_call_sequences_against_a_sequential_model():
     """tests/emu/fuzz_c_abi.py: random upsert / remove / post_result / read / tick sequences (duplicate
     slots, results before and after upserts, removes of absent slots, short output buffers, open and
     closed loop, a shard base) through am.Sweep on the emulated library; every tick and every read must
     equal the sequential model (calls take effect in call order; a tick is the oracle's sweep)."""
-    env = dict(os.environ, AMSWEEP_LIB=emu_lib)
-    out = subprocess.run([sys.executable, os.path.join(EMU, "fuzz_c_abi.py"), "60", "30", "3000"], cwd=ROOT, env=env,
-                         capture_output=True, text=True, timeout=900)
-    assert out.returncode == 0 and out.stdout.strip().startswith("ok"), out.stdout[-2000:] + out.stderr[-3000:]
+    emu_sweep.run_script("fuzz_c_abi.py", [60, 30, 3000])
 
 
 def test_threading_contract_under_threadsanitizer(tmp_path):
     """tests/emu/tsan_c_abi.cpp: four threads stage upserts / removes / results while one thread ticks
     and reads (the contract of SURVEY 8b), built with -fsanitize=thread from the library's own sources
     on the emulator.  No ThreadSanitizer report = the host runtime's locking covers every shared access."""
-    exe = str(tmp_path / "tsan_c_abi.bin")
-    sys.path.insert(0, EMU)
-    import emu_sweep
-    srcs = emu_sweep.sources()[0] + [os.path.join(EMU, "tsan_c_abi.cpp")]
-    r = subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-Wno-unknown-pragmas", "-Wno-tsan",
-                        "-pthread", "-DAMSWEEP_EMULATE", "-include", os.path.join(EMU, "cuda_emu.h"),
-                        "-include", os.path.join(EMU, "cuda_rt_emu.h"), "-x", "c++"] + srcs + ["-o", exe],
-                       capture_output=True, text=True)
-    if r.returncode != 0:
-        pytest.skip("ThreadSanitizer runtime not available: " + r.stderr[-300:])
+    exe = emu_sweep.build_tsan("tsan_c_abi.cpp", str(tmp_path / "tsan_c_abi.bin"))
     out = subprocess.run([exe], capture_output=True, text=True, timeout=900,
                          env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0"))
     assert "ThreadSanitizer" not in out.stderr, out.stderr[-3000:]

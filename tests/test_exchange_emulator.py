@@ -16,25 +16,12 @@ import sys
 
 import pytest
 
-from conftest import ROOT
-
-EMU = os.path.join(ROOT, "tests", "emu")
-
-
-@pytest.fixture(scope="module")
-def emu_lib():
-    sys.path.insert(0, EMU)
-    import emu_sweep
-    return emu_sweep.build()
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
+import emu_sweep  # noqa: E402
 
 
-def _run(emu_lib, args, env=None, timeout=900):
-    e = dict(os.environ, AMSWEEP_LIB=emu_lib)
-    e.update(env or {})
-    out = subprocess.run([sys.executable, os.path.join(EMU, "run_gather_ranks.py")] + [str(a) for a in args],
-                         cwd=ROOT, env=e, capture_output=True, text=True, timeout=timeout)
-    assert out.returncode == 0 and out.stdout.strip().startswith("ok"), out.stdout[-3000:] + out.stderr[-3000:]
-    return out.stdout
+def _run(args, env=None, timeout=900):
+    return emu_sweep.run_script("run_gather_ranks.py", args, env, timeout)
 
 
 # world, idx_bytes, records in total, ticks, population
@@ -51,56 +38,56 @@ CASES = [
 
 
 @pytest.mark.parametrize("case", CASES, ids=lambda c: "w{}_b{}_n{}_t{}_c{}".format(*c))
-def test_exchanged_ticks_equal_the_unsharded_oracle(emu_lib, case):
-    _run(emu_lib, ["tick"] + list(case))
+def test_exchanged_ticks_equal_the_unsharded_oracle(case):
+    _run(["tick"] + list(case))
 
 
 @pytest.mark.parametrize("case", [(2, 4, 40_000, 4, 3), (3, 8, 30_011, 4, 2), (8, 4, 65_536, 3, 3), (5, 4, 5, 2, 2)],
                          ids=lambda c: "w{}_b{}_n{}_t{}_c{}".format(*c))
-def test_whole_step_in_one_call_returns_the_ranks_own_part_as_local_slots(emu_lib, case):
+def test_whole_step_in_one_call_returns_the_ranks_own_part_as_local_slots(case):
     """am_gather_bind + am_gather_tick_view: tick_shard + exchange + extraction of the rank's own part of the
     global list into pinned host memory, one synchronisation; the global list, the shard statistics and the view
     must all equal the oracle's."""
-    _run(emu_lib, ["tick"] + list(case), env={"EMU_TICK_VIEW": "1"})
+    _run(["tick"] + list(case), env={"EMU_TICK_VIEW": "1"})
 
 
-def test_whole_step_reports_an_absent_peer_as_an_error(emu_lib):
-    out = _run(emu_lib, ["tick", 3, 4, 30_000, 3], env={"EMU_ABSENT_RANK": "1", "AMSWEEP_PUSH_TIMEOUT_MS": "300",
+def test_whole_step_reports_an_absent_peer_as_an_error():
+    out = _run(["tick", 3, 4, 30_000, 3], env={"EMU_ABSENT_RANK": "1", "AMSWEEP_PUSH_TIMEOUT_MS": "300",
                                                          "EMU_TICK_VIEW": "1"}, timeout=120)
     assert "watchdog" in out
 
 
 @pytest.mark.parametrize("ctas", [1, 3, 40])
-def test_any_push_grid_size(emu_lib, ctas):
-    _run(emu_lib, ["tick", 3, 4, 50_000, 3, 3], env={"AMSWEEP_PUSH_CTAS": str(ctas)})
+def test_any_push_grid_size(ctas):
+    _run(["tick", 3, 4, 50_000, 3, 3], env={"AMSWEEP_PUSH_CTAS": str(ctas)})
 
 
-def test_protocol_survives_skew_between_ranks(emu_lib):
+def test_protocol_survives_skew_between_ranks():
     """EMU_JITTER: random pauses at launches and system-scope stores let ranks drift apart by whole
     kernels over 25 back-to-back ticks; the epoch / done-flag / two-slot-set protocol must still
     deliver the oracle's list on every rank."""
-    _run(emu_lib, ["tick", 4, 4, 48_000, 25, 2], env={"EMU_JITTER": "1"})
+    _run(["tick", 4, 4, 48_000, 25, 2], env={"EMU_JITTER": "1"})
 
 
-def test_a_fast_rank_may_finish_its_next_push_before_a_slow_one_has_seen_this_one(emu_lib):
+def test_a_fast_rank_may_finish_its_next_push_before_a_slow_one_has_seen_this_one():
     """Tiny shards, 8 ranks, 40 ticks, skew: a rank regularly raises done(e+1) while a peer still waits
     for its done(e) — the wait must accept ">= e" (round-2 bug found here: waiting for "== e" let the
     slow rank run into the watchdog)."""
-    _run(emu_lib, ["tick", 8, 8, 9_000, 40, 2], env={"EMU_JITTER": "1", "AMSWEEP_PUSH_TIMEOUT_MS": "20000"})
-    _run(emu_lib, ["tick", 8, 4, 9_000, 40, 3])
+    _run(["tick", 8, 8, 9_000, 40, 2], env={"EMU_JITTER": "1", "AMSWEEP_PUSH_TIMEOUT_MS": "20000"})
+    _run(["tick", 8, 4, 9_000, 40, 3])
 
 
-def test_watchdog_gives_up_on_an_absent_peer(emu_lib):
+def test_watchdog_gives_up_on_an_absent_peer():
     """The device-side wait for the peers' done flags is bounded (AMSWEEP_PUSH_TIMEOUT_MS): a rank that
     never exchanges makes the others report 0xFFFFFFFF in out_counts[world] instead of hanging the GPU."""
-    out = _run(emu_lib, ["tick", 3, 4, 30_000, 3], env={"EMU_ABSENT_RANK": "1", "AMSWEEP_PUSH_TIMEOUT_MS": "300"},
+    out = _run(["tick", 3, 4, 30_000, 3], env={"EMU_ABSENT_RANK": "1", "AMSWEEP_PUSH_TIMEOUT_MS": "300"},
                timeout=120)
     assert "watchdog" in out
 
 
 @pytest.mark.parametrize("world,idx_bytes,records", [(2, 4, 20_000), (3, 8, 30_011), (8, 4, 9_000)])
-def test_round1_plain_list_format_still_equals_the_concatenation(emu_lib, world, idx_bytes, records):
-    _run(emu_lib, ["plain", world, idx_bytes, records, 5])
+def test_round1_plain_list_format_still_equals_the_concatenation(world, idx_bytes, records):
+    _run(["plain", world, idx_bytes, records, 5])
 
 
 def test_flag_protocol_orders_every_cross_rank_access_under_threadsanitizer(tmp_path):
@@ -110,16 +97,7 @@ def test_flag_protocol_orders_every_cross_rank_access_under_threadsanitizer(tmp_
     System-scope release/acquire are atomics there, everything else — peer payload stores, slot reads
     by the list rebuild — plain memory accesses: a report would mean some cross-rank data is not
     ordered by the done-flag protocol."""
-    sys.path.insert(0, EMU)
-    import emu_sweep
-    exe = str(tmp_path / "tsan_exchange.bin")
-    srcs = emu_sweep.sources()[0] + [os.path.join(EMU, "tsan_exchange.cpp")]
-    r = subprocess.run(["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-Wno-unknown-pragmas", "-Wno-tsan",
-                        "-pthread", "-DAMSWEEP_EMULATE", "-include", os.path.join(EMU, "cuda_emu.h"),
-                        "-include", os.path.join(EMU, "cuda_rt_emu.h"), "-x", "c++"] + srcs + ["-o", exe],
-                       capture_output=True, text=True)
-    if r.returncode != 0:
-        pytest.skip("ThreadSanitizer runtime not available: " + r.stderr[-300:])
+    exe = emu_sweep.build_tsan("tsan_exchange.cpp", str(tmp_path / "tsan_exchange.bin"))
     out = subprocess.run([exe], capture_output=True, text=True, timeout=900,
                          env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
     assert "ThreadSanitizer" not in out.stderr, out.stderr[-3000:]

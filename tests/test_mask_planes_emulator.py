@@ -2,22 +2,12 @@
 host sources) behind the real C-ABI, in a child process, as tests/test_c_abi_on_emulator.py does for the
 rest of the GPU parity suite."""
 import os
-import subprocess
 import sys
 
-from conftest import ROOT
-
-EMU = os.path.join(ROOT, "tests", "emu")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
+import emu_sweep  # noqa: E402
 
 
 def test_mask_planes_suite_on_the_emulated_library():
-    sys.path.insert(0, EMU)
-    import emu_sweep
-    env = dict(os.environ, AMSWEEP_LIB=emu_sweep.build())
-    out = subprocess.run([sys.executable, "-m", "pytest", "tests/test_mask_planes_gpu.py", "-m", "gpu", "-q", "-x",
-                          "-p", "no:cacheprovider"], cwd=ROOT, env=env, capture_output=True, text=True, timeout=1800)
-    tail = out.stdout[-3000:] + out.stderr[-2000:]
-    assert out.returncode == 0, tail
-    last = out.stdout.strip().splitlines()[-1]
-    assert " passed" in last and "failed" not in last and "skipped" not in last, tail
-    assert int(last.split(" passed")[0].split()[-1]) >= 5, tail
+    got = emu_sweep.run_suite("tests/test_mask_planes_gpu.py")
+    assert got["passed"] >= 5, got

@@ -2,28 +2,17 @@
 behind the real C-ABI, in a child process, as tests/test_workflow_timeout_emulator.py does for workflow timeouts.  The
 10 M-record comparison stays on the GPU."""
 import os
-import subprocess
 import sys
 
 import pytest
 
-from conftest import ROOT
-
-EMU = os.path.join(ROOT, "tests", "emu")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
+import emu_sweep  # noqa: E402
 
 
 def test_remedy_hold_suite_on_the_emulated_library():
-    sys.path.insert(0, EMU)
-    import emu_sweep
-    env = dict(os.environ, AMSWEEP_LIB=emu_sweep.build())
-    out = subprocess.run([sys.executable, "-m", "pytest", "tests/test_remedy_hold_gpu.py", "-m", "gpu", "-q", "-x",
-                          "-p", "no:cacheprovider", "-k", "not full_size"], cwd=ROOT, env=env, capture_output=True,
-                         text=True, timeout=1800)
-    tail = out.stdout[-3000:] + out.stderr[-2000:]
-    assert out.returncode == 0, tail
-    last = out.stdout.strip().splitlines()[-1]
-    assert " passed" in last and "failed" not in last and "skipped" not in last, tail
-    assert int(last.split(" passed")[0].split()[-1]) >= 59, tail
+    got = emu_sweep.run_suite("tests/test_remedy_hold_gpu.py", k="not full_size")
+    assert got["passed"] >= 59, got
 
 
 # world, idx_bytes, records in total, amgen config (22: named time zones, 3: remedy actions)
@@ -31,9 +20,4 @@ def test_remedy_hold_suite_on_the_emulated_library():
 def test_each_shard_holds_and_times_out_its_own_remedies_through_am_gather_tick_view(case):
     """tests/emu/run_gather_remedy_hold.py: every rank's global list against the remedy-hold oracle of the unsharded
     population, and its am_sweep_last_remedy_timed_out the part it owns (every rank times out remedy runs)"""
-    sys.path.insert(0, EMU)
-    import emu_sweep
-    out = subprocess.run([sys.executable, os.path.join(EMU, "run_gather_remedy_hold.py")] + [str(a) for a in case],
-                         cwd=ROOT, env=dict(os.environ, AMSWEEP_LIB=emu_sweep.build()), capture_output=True, text=True,
-                         timeout=900)
-    assert out.returncode == 0 and out.stdout.strip().startswith("ok"), out.stdout[-3000:] + out.stderr[-3000:]
+    emu_sweep.run_script("run_gather_remedy_hold.py", case)
