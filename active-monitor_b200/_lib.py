@@ -118,6 +118,14 @@ class AmTickStats(C.Structure):
 STATS_DTYPE = np.dtype([(n, "<u8") for n in STAT_FIELDS])
 assert STATS_DTYPE.itemsize == C.sizeof(AmTickStats) == 128
 
+
+class AmSimParams(C.Structure):
+    _fields_ = [("wf_min", i32), ("wf_max", i32), ("remedy_min", i32), ("remedy_max", i32)]
+
+
+SIM_FIELDS = ["n_in_flight", "n_remedy_in_flight", "n_timed_out", "n_remedy_timed_out"]
+SIM_DTYPE = np.dtype([(n, "<u8") for n in SIM_FIELDS])
+
 # every symbol include/amsweep.h declares: name -> (restype, argtypes)
 P = C.POINTER
 SYMBOLS = {
@@ -145,6 +153,7 @@ SYMBOLS = {
     "am_sweep_tick_device": (C.c_int, [C.c_void_p, i64, u32, C.c_void_p, C.c_void_p, u64,
                                        C.c_void_p, C.c_void_p, C.c_void_p]),
     "am_sweep_run_ticks": (C.c_int, [C.c_void_p, i64, u64, u32, u64, C.c_void_p]),
+    "am_sweep_simulate": (C.c_int, [C.c_void_p, i64, u64, u32, u64, P(AmSimParams), C.c_void_p, C.c_void_p]),
     "am_sweep_repeat_after_sec": (C.c_int, [C.c_void_p, i64, u64, u64, C.c_void_p]),
     "am_sweep_next_due": (C.c_int, [C.c_void_p, i64, P(i64)]),
     "am_sweep_read": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, P(AmRecordCols)]),

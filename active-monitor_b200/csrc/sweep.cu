@@ -202,6 +202,9 @@ struct am_sweep {
   bool to_fetched = false;  // ... and has been copied to to_host / rto_host, sorted
   std::vector<std::pair<uint32_t, int64_t>> to_host;   // health-check runs: (slot, since)
   std::vector<std::pair<uint32_t, int64_t>> rto_host;  // remedy runs: (slot, start)
+  // simulated workflows (am_sweep_simulate), allocated at the first call: per warp segment a lower bound of its held
+  // runs' simulated ends (biased key), for the tick-by-tick completion pass
+  unsigned long long* sim_end = nullptr;
   // status changes (am_sweep_set_track_changes), allocated at the first enable: one bit per slot that the coming tick
   // changes ([n_groups * kGroupWords], drains and the tick add to it, the list kernel clears it), the last tick's
   // ascending slot list ([cap_padded]), and the per-group counts, offsets and total of the compaction
@@ -1568,6 +1571,139 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
   }
   cudaFree(d_stats);
   if (h->track) {  // the run applied what its drain noted: start again from the flags
+    const int rs = seed_changes(h, h->stream, 0, h->cap_padded);
+    if (rc == AM_OK) rc = rs;
+  }
+  return rc;
+}
+
+int am_sweep_simulate(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint32_t mode, uint64_t seed,
+                      const am_sim_params_t* params, am_tick_stats_t* stats_out, am_sim_tick_t* sim_out) {
+  if (!h || !stats_out || !params || (mode & ~(AM_SWEEP_BLOCKED | AM_SWEEP_FULL_SCAN))) return AM_E_INVAL;
+  if (params->wf_min < 1 || params->wf_max < params->wf_min || params->remedy_min < 1 ||
+      params->remedy_max < params->remedy_min || n_ticks > (1ull << 24))
+    return AM_E_INVAL;
+  if (!time_ok(unix_sec0) || !time_ok(unix_sec0 + (int64_t)n_ticks)) return AM_E_RANGE;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if (!h->hold || !h->remedy) {  // (only the configuration with both holds is simulated: refused, nothing happens)
+    h->last_error = "am_sweep_simulate needs the hold in flight and the remedy hold on";
+    return AM_E_INVAL;
+  }
+  if (n_ticks == 0) return AM_OK;
+  int rc = set_stream(h, h->stream);
+  if (rc != AM_OK) return rc;
+  h->to_ran = false;  // (the timed-out lists and the list of status changes are empty afterwards)
+  h->chg_listed = h->chg_fetched = false;
+  // The staged calls come first; their results stay pending in the flags for the first tick (after its simulated posts,
+  // which only ever replace a slot's bit group, as a later post_result would).
+  rc = drain_staged(h, h->stream);
+  if (rc != AM_OK) return rc;
+  h->seed = seed;
+  const SimDraw q{seed, params->wf_min, params->wf_max - params->wf_min + 1, params->remedy_min,
+                  params->remedy_max - params->remedy_min + 1};
+  const bool blocked = (mode & AM_SWEEP_BLOCKED) != 0;
+  const uint64_t n_seg = (h->n_records + kRecPerWarp - 1) / kRecPerWarp;
+  if (!blocked && !h->sim_end) AM_CUDA(h, dev_array(h, &h->sim_end, h->cap_padded / kRecPerWarp * 8, h->stream, false));
+  am_tick_stats_t* d_stats = nullptr;
+  AM_CUDA(h, cudaMalloc((void**)&d_stats, n_ticks * (sizeof(am_tick_stats_t) + sizeof(am_sim_tick_t))));
+  unsigned long long* d_sim = reinterpret_cast<unsigned long long*>(d_stats + n_ticks);
+  if (cudaError_t e = cudaMemsetAsync(d_stats, 0, n_ticks * (sizeof(am_tick_stats_t) + sizeof(am_sim_tick_t)), h->stream);
+      e != cudaSuccess) {
+    h->last_error = cudaGetErrorString(e);
+    cudaFree(d_stats);
+    return AM_E_DEVICE;
+  }
+  if (cudaError_t e = cudaEventRecord(h->ev0, h->stream); e != cudaSuccess) {
+    h->last_error = cudaGetErrorString(e);
+    rc = AM_E_DEVICE;
+  }
+  auto launched = [&]() {
+    h->launches++;
+    if (cudaError_t e = cudaGetLastError(); e != cudaSuccess) { h->last_error = cudaGetErrorString(e); rc = AM_E_DEVICE; }
+  };
+  // Blocked: sweep_block_kernel<false, true>, blocks cut as in am_sweep_run_ticks.
+  uint64_t block_ticks = kDefaultBlockTicks;
+  if (const char* e = getenv("AMSWEEP_BLOCK_TICKS")) { long v = atol(e); if (v >= 1 && v <= kMaxBlockTicks) block_ticks = (uint64_t)v; }
+  for (uint64_t k = 0; blocked && h->n_records && k < n_ticks && rc == AM_OK;) {
+    const int64_t T = unix_sec0 + (int64_t)k;
+    rc = refresh_zones(h, T, h->stream);
+    if (rc != AM_OK) break;
+    uint64_t K = n_ticks - k < block_ticks ? n_ticks - k : block_ticks;
+    if (h->tz_n > 1 && h->tz_hi < T + (int64_t)K) K = (uint64_t)(h->tz_hi - T);  // (tz_hi > T after the refresh)
+    SimBlockParams b{};
+    b.c = h->cols;
+    b.n_records = h->n_records;
+    b.shard_base = h->shard_base;
+    b.seed = h->seed;
+    b.T0 = T;
+    b.K = (uint32_t)K;
+    b.tz_off = h->tz_n > 1 ? (const int32_t*)h->tz_off.dev : nullptr;
+    b.stats = reinterpret_cast<unsigned long long*>(d_stats + k);
+    b.since = h->since;
+    if (h->wf_timeout) {
+      b.deadline = h->deadline;
+      b.wf_timeout = h->wf_timeout;
+      b.seg_deadline = h->seg_deadline;
+    }
+    b.q = q;
+    b.sim = d_sim + k * 4;
+    const unsigned grid = (unsigned)((h->n_records + kBlockRecords - 1) / kBlockRecords);
+    void (*const block_fn)(const SimBlockParams) = sweep_block_kernel<false, true>;
+    AM_LAUNCH(block_fn, grid, kBlockThreads, h->stream, b);
+    launched();
+    k += K;
+  }
+  // Tick by tick: the completion pass, then the tick (expiry pass and sweep), then the bounds of the runs it started
+  // and the tick's counts.
+  if (!blocked && rc == AM_OK) {
+    AM_CUDA(h, cudaMemsetAsync(h->sim_end, 0xFF, h->cap_padded / kRecPerWarp * 8, h->stream));
+    if (h->n_records) {
+      AM_LAUNCH(sim_bounds_kernel, (unsigned)((h->n_records + 255) / 256), 256, h->stream, h->cols, (const int64_t*)h->since,
+                h->sim_end, h->n_records, q, h->shard_base);
+      launched();
+    }
+  }
+  const int64_t earliest = params->wf_min < params->remedy_min ? params->wf_min : params->remedy_min;
+  for (uint64_t k = 0; !blocked && k < n_ticks && rc == AM_OK; ++k) {
+    const int64_t T = unix_sec0 + (int64_t)k;
+    if (n_seg) {
+      AM_LAUNCH_PDL(sim_complete_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream, h->cols, h->since, h->sim_end,
+                    (uint32_t)n_seg, T, q, h->shard_base);
+      launched();
+    }
+    if (rc == AM_OK) rc = expire_runs(h, h->stream, T);
+    const int parity = (int)h->parity;
+    const ListOut o{h->due_idx[k & 1], h->due_action[k & 1], h->cap_padded, nullptr, d_stats + k};
+    if (rc == AM_OK) rc = launch_tick(h, T, mode & AM_SWEEP_FULL_SCAN, o, h->stream);
+    if (rc == AM_OK && n_seg) {
+      AM_LAUNCH_PDL(sim_note_starts_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream,
+                    (const uint32_t*)h->set[parity].out.bitmap, h->sim_end, (uint32_t)n_seg, T + earliest);
+      launched();
+    }
+    if (rc == AM_OK) {
+      AM_LAUNCH_PDL(sim_count_kernel, h->sms * 8, 256, h->stream, h->cols, (const int64_t*)h->since, h->n_records,
+                    (const int64_t*)(h->to_ran ? h->to_since : nullptr), (const uint32_t*)(h->to_ran ? h->to_count : nullptr),
+                    d_sim + k * 4);
+      launched();
+    }
+  }
+  h->to_ran = false;
+  if (rc == AM_OK) {
+    cudaError_t e = cudaEventRecord(h->ev1, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e == cudaSuccess) e = cudaMemcpy(stats_out, d_stats, n_ticks * sizeof(am_tick_stats_t), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && sim_out) e = cudaMemcpy(sim_out, d_sim, n_ticks * sizeof(am_sim_tick_t), cudaMemcpyDeviceToHost);
+    float ms = 0;
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+    if (e != cudaSuccess) { h->last_error = cudaGetErrorString(e); rc = AM_E_DEVICE; }
+    else h->last_ms = ms;
+    if (rc == AM_OK)
+      for (uint64_t k = 0; k < n_ticks; ++k) stats_out[k].n_records = h->n_records;
+    if (rc == AM_OK) { h->has_prev = true; h->prev_T = unix_sec0 + (int64_t)n_ticks - 1; }
+  }
+  cudaFree(d_stats);
+  if (h->track) {  // the ticks applied what the drains noted: start again from the flags
     const int rs = seed_changes(h, h->stream, 0, h->cap_padded);
     if (rc == AM_OK) rc = rs;
   }

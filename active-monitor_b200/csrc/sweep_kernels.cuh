@@ -1477,6 +1477,130 @@ __global__ void expire_runs_kernel(DevCols c, int64_t* since, int64_t* deadline,
   }
 }
 
+// ---- simulated workflows (am_sweep_simulate) ----------------------------------------------------------------------
+// The durations of the two kinds of run: min and max - min + 1, in seconds.
+struct SimDraw {
+  uint64_t seed;
+  int32_t wf_min, wf_span, remedy_min, remedy_span;
+};
+
+// The simulated end of the run a since word holds (either kind), and the phase bits its end posts (*bits: a workflow
+// phase for a health-check run, a remedy phase for a remedy run).  A pure function of the run's start: the keyed
+// splitmix64 of the closed loop (outcome_key) decides both, the outcome from its low bytes as the closed loop does
+// (the record's fail_p8 for a health check, 179/256 for a remedy), the duration from its high word.
+__device__ __forceinline__ int64_t sim_run_end(const SimDraw& q, uint64_t g, int64_t since, uint32_t flags, uint32_t* bits) {
+  const bool remedy = is_remedy_run(since);
+  const int64_t start = run_start(since);
+  const uint64_t k = outcome_key(q.seed, g, (uint64_t)start);
+  if (remedy) {
+    *bits = AM_F_REMEDY_PENDING | ((uint32_t)((k >> 8) & 0xFF) < 179u ? AM_F_REMEDY_OUTCOME_OK : 0u);
+    return start + q.remedy_min + (int64_t)((k >> 32) % (uint64_t)q.remedy_span);
+  }
+  *bits = (uint32_t)(k & 0xFF) < ((flags >> AM_F_FAILP_SHIFT) & 0xFFu) ? AM_F_PENDING_FAIL : AM_F_PENDING_OK;
+  return start + q.wf_min + (int64_t)((k >> 32) % (uint64_t)q.wf_span);
+}
+
+// The simulated post of a run that ends: its phase replaces its bit group, as am_sweep_post_result stages it.
+__device__ __forceinline__ uint32_t sim_post(uint32_t f, uint32_t bits) {
+  return (f & ~((bits & kHcBits) ? kHcBits : kRemedyBits)) | bits;
+}
+
+// The completion pass of a simulated tick at T, ahead of its expiry pass: every held run (held_run, either kind) whose
+// simulated end is <= T posts its phase into the flags and clears since, as the drain of a posted phase does
+// (apply_result_ops_kernel, clear_since_kernel).  Shaped like expire_runs_kernel: lane L of a warp reads the bound of
+// segment 32 w + L (`seg_end`, a lower bound of the segment's simulated ends); a segment whose bound is <= T is visited
+// by the whole warp and gets the exact minimum of what is left.  A segment's bound is lowered when a tick starts a run
+// in it (sim_note_starts_kernel).
+__global__ void sim_complete_kernel(DevCols c, int64_t* since, unsigned long long* seg_end, uint32_t n_seg, int64_t T,
+                                    SimDraw q, uint64_t shard_base) {
+  pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const uint32_t seg0 = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 32u;
+  if (seg0 >= n_seg) return;  // warp-uniform
+  const unsigned long long tkey = biased_key(T);
+  uint32_t due = __ballot_sync(kFull, seg0 + (uint32_t)lane < n_seg && seg_end[seg0 + lane] <= tkey);
+  while (due) {  // warp-uniform
+    const uint32_t seg = seg0 + (uint32_t)(__ffs((int)due) - 1);
+    due &= due - 1;
+    unsigned long long left = ~0ull;
+#pragma unroll
+    for (int q4 = 0; q4 < 4; ++q4) {
+      const uint32_t i = seg * (uint32_t)kRecPerWarp + 32u * q4 + (uint32_t)lane;
+      const int64_t s = since[i];
+      if (s == kNotInFlight) continue;
+      const uint32_t f = c.flags[i];
+      if (!held_run(s, [&] { return c.finished_at[i]; }, [&] { return f; })) continue;
+      uint32_t bits;
+      const int64_t end = sim_run_end(q, shard_base + i, s, f, &bits);
+      if (end <= T) {
+        c.flags[i] = sim_post(f, bits);
+        since[i] = kNotInFlight;
+      } else if (biased_key(end) < left) {
+        left = biased_key(end);
+      }
+    }
+    left = warp_min(left);
+    if (lane == 0) seg_end[seg] = left;
+  }
+}
+
+// The bounds of sim_complete_kernel from the since words as they stand: every held run's simulated end, per segment
+// (`seg_end` all ones on entry).  One thread per slot; a warp's 32 slots lie in one segment.
+__global__ void sim_bounds_kernel(DevCols c, const int64_t* __restrict__ since, unsigned long long* seg_end, uint64_t n,
+                                  SimDraw q, uint64_t shard_base) {
+  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  unsigned long long key = ~0ull;
+  if (i < n) {
+    const int64_t s = since[i];
+    if (s != kNotInFlight) {
+      const uint32_t f = c.flags[i];
+      uint32_t bits;
+      if (held_run(s, [&] { return c.finished_at[i]; }, [&] { return f; }))
+        key = biased_key(sim_run_end(q, shard_base + i, s, f, &bits));
+    }
+  }
+  key = warp_min(key);
+  if ((threadIdx.x & 31) == 0 && key != ~0ull) atomicMin(seg_end + i / (uint64_t)kRecPerWarp, key);
+}
+
+// After a simulated tick's sweep: every run it started is a record it emitted (SUBMIT_HC, or RUN_REMEDY for a remedy
+// run), and no run ends before T + the shorter minimum duration (`earliest`).  So a segment with an emitted record in
+// the tick's bitmap gets its bound lowered to that.  One thread per segment (four bitmap words).
+__global__ void sim_note_starts_kernel(const uint32_t* __restrict__ bitmap, unsigned long long* seg_end, uint32_t n_seg,
+                                       int64_t earliest) {
+  pdl_wait();
+  const uint32_t seg = blockIdx.x * blockDim.x + threadIdx.x;
+  if (seg >= n_seg) return;
+  const uint4 w = *reinterpret_cast<const uint4*>(bitmap + 4ull * seg);
+  if ((w.x | w.y | w.z | w.w) && biased_key(earliest) < seg_end[seg]) seg_end[seg] = biased_key(earliest);
+}
+
+// The counts of a simulated tick's row (am_sim_tick_t, zero on entry) after its sweep: the held runs of either kind, as
+// am_sweep_in_flight / am_sweep_remedy_in_flight report them, and the tick's timed-out list split by kind (`to_count`
+// NULL when the tick ran no expiry pass).  Grid-stride.
+__global__ void sim_count_kernel(DevCols c, const int64_t* __restrict__ since, uint64_t n, const int64_t* __restrict__ to_since,
+                                 const uint32_t* __restrict__ to_count, unsigned long long* row) {
+  pdl_wait();
+  uint32_t hc = 0, rm = 0, to = 0, rto = 0;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int64_t s = since[i];
+    if (s != kNotInFlight && held_run(s, [&] { return c.finished_at[i]; }, [&] { return c.flags[i]; })) {
+      if (is_remedy_run(s)) ++rm; else ++hc;
+    }
+  }
+  const uint32_t m = to_count ? *to_count : 0u;
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < m; k += stride) {
+    if (is_remedy_run(to_since[k])) ++rto; else ++to;
+  }
+  const uint32_t v[4] = {hc, rm, to, rto};
+#pragma unroll
+  for (int f = 0; f < 4; ++f) {
+    const uint32_t t = __reduce_add_sync(kFull, v[f]);
+    if ((threadIdx.x & 31) == 0 && t) atomicAdd(row + f, (unsigned long long)t);
+  }
+}
+
 __global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;

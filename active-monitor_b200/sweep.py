@@ -293,6 +293,16 @@ class Sweep:
                                                  out.ctypes.data), "am_sweep_run_ticks")
         return out
 
+    def simulate(self, unix_sec0: int, n_ticks: int, mode: int = 0, seed: int = 0, params=(1, 1, 1, 1)):
+        """n_ticks ticks with the held workflows simulated (am_sweep_simulate); params = (wf_min, wf_max, remedy_min,
+        remedy_max) in seconds.  Returns (stats rows STATS_DTYPE[n], sim rows SIM_DTYPE[n])."""
+        out = np.zeros(n_ticks, dtype=L.STATS_DTYPE)
+        sim = np.zeros(n_ticks, dtype=L.SIM_DTYPE)
+        p = L.AmSimParams(*params)
+        self._check(self._lib.am_sweep_simulate(self._h, unix_sec0, n_ticks, mode, seed, C.byref(p), out.ctypes.data,
+                                                sim.ctypes.data), "am_sweep_simulate")
+        return out, sim
+
     def repeat_after_sec(self, unix_sec: int, first: int, n: int) -> np.ndarray:
         """hcc.go:262 for every record of [first, first+n): Next() evaluated on the device."""
         out = np.zeros(n, dtype=np.int64)

@@ -371,6 +371,46 @@ int am_sweep_tick_shard(am_sweep_t*, int64_t unix_sec, uint32_t mode, void* cuda
 int am_sweep_run_ticks(am_sweep_t*, int64_t unix_sec0, uint64_t n_ticks, uint32_t mode,
                        uint64_t seed, am_tick_stats_t* stats_out);
 
+/* Simulated workflow durations of am_sweep_simulate, in seconds: 1 <= min <= max for both kinds. */
+typedef struct am_sim_params {
+  int32_t wf_min, wf_max;          /* health-check workflow duration */
+  int32_t remedy_min, remedy_max;  /* remedy workflow duration       */
+} am_sim_params_t;
+
+typedef struct am_sim_tick {       /* one row per simulated tick */
+  uint64_t n_in_flight;            /* slots am_sweep_in_flight would report after the tick        */
+  uint64_t n_remedy_in_flight;     /* slots am_sweep_remedy_in_flight would report after the tick */
+  uint64_t n_timed_out;            /* entries am_sweep_last_timed_out would list for the tick     */
+  uint64_t n_remedy_timed_out;     /* entries am_sweep_last_remedy_timed_out would list           */
+} am_sim_tick_t;
+
+/* A run of n_ticks one-second ticks with the workflows the ticks submit simulated on the device: the
+ * hold in flight, the remedy hold and workflow timeouts (INTEGRATION.md §3) over a simulated day.
+ * Every draw is a pure function of the run's start second: with g the global index and
+ * k = the closed loop's outcome key of (seed, g, start), a health-check run started at S ends Failed iff
+ * (k & 0xFF) < the record's fail_p8 (flags bits 16..23), else Succeeded, after
+ * wf_min + (k >> 32) % (wf_max - wf_min + 1) seconds; a remedy run started at R ends Succeeded iff
+ * ((k >> 8) & 0xFF) < 179 after remedy_min + (k >> 32) % (remedy_max - remedy_min + 1) seconds.
+ * For T = unix_sec0 .. unix_sec0 + n_ticks - 1 the call leaves the handle and stats_out[k] exactly as
+ *   1. am_sweep_post_result(slot, phase(S), AM_PHASE_NONE) for every slot whose health-check run is held
+ *      with start S and S + d(S) <= T, and am_sweep_post_result(slot, AM_PHASE_NONE, rphase(R)) for every
+ *      slot whose remedy run is held with start R and R + dr(R) <= T (runs overdue at the first tick
+ *      included, whoever started them);
+ *   2. am_sweep_tick(h, T, mode & AM_SWEEP_FULL_SCAN, ...), its statistics into stats_out[k] and the
+ *      counts above into sim_out[k] (sim_out may be NULL)
+ * would, after the calls staged before this one.  So a run whose end equals its deadline completes, and
+ * one whose deadline comes first times out and never posts its phase.  Like am_sweep_run_ticks it
+ * produces no per-tick lists: afterwards the timed-out lists and the change list are empty, and with
+ * tracking on the bits are re-seeded from the flags.  P becomes the last second; runs still in flight
+ * stay held for later ticks, am_sweep_in_flight and am_sweep_next_due.  AM_SWEEP_BLOCKED runs the
+ * temporal-blocking kernel (blocks as in am_sweep_run_ticks) with the same results.  The seed becomes
+ * the handle's (am_sweep_set_seed).  Refused before anything happens (nothing drained, P unchanged):
+ * AM_E_INVAL while the hold in flight or the remedy hold is off, for params NULL or out of bounds,
+ * stats_out NULL, n_ticks > 2^24 or a mode bit other than AM_SWEEP_BLOCKED | AM_SWEEP_FULL_SCAN;
+ * AM_E_RANGE for times out of range. */
+int am_sweep_simulate(am_sweep_t*, int64_t unix_sec0, uint64_t n_ticks, uint32_t mode, uint64_t seed,
+                      const am_sim_params_t* params, am_tick_stats_t* stats_out, am_sim_tick_t* sim_out);
+
 /* RepeatAfterSec of records [first, first+n) as the reference derives it at
  * reconcile time (hcc.go:259-262): Next(unix_sec) - unix_sec for a 5-field
  * schedule (robfig SpecSchedule.Next evaluated on the device; -9223372035 when
