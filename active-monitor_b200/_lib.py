@@ -123,6 +123,18 @@ class AmSimParams(C.Structure):
     _fields_ = [("wf_min", i32), ("wf_max", i32), ("remedy_min", i32), ("remedy_max", i32)]
 
 
+CHECKPOINT_VERSION = 1
+CKPT_HOLD, CKPT_REMEDY, CKPT_TRACK, CKPT_DETAILS, CKPT_TIMEOUTS = 0x1, 0x2, 0x4, 0x8, 0x10
+
+
+class AmCheckpointInfo(C.Structure):
+    _fields_ = [("first_global", u64), ("n", u64), ("swept_end", u64), ("prev_tick", i64), ("seed", u64),
+                ("switches", u32), ("n_zones", u32), ("version", u32), ("reserved", u32), ("bytes", u64)]
+
+    def as_dict(self) -> dict:
+        return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "reserved"}
+
+
 SIM_FIELDS = ["n_in_flight", "n_remedy_in_flight", "n_timed_out", "n_remedy_timed_out"]
 SIM_DTYPE = np.dtype([(n, "<u8") for n in SIM_FIELDS])
 
@@ -167,6 +179,9 @@ SYMBOLS = {
     "am_sweep_last_changes": (C.c_int, [C.c_void_p, u64, C.c_void_p, P(AmRecordCols), u64, P(u64)]),
     "am_sweep_set_change_details": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_last_change_details": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
+    "am_sweep_checkpoint": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, u64, P(u64)]),
+    "am_checkpoint_info": (C.c_int, [C.c_void_p, u64, P(AmCheckpointInfo)]),
+    "am_sweep_restore": (C.c_int, [C.c_void_p, C.c_void_p, u64]),
     "am_sweep_size": (u64, [C.c_void_p]),
     "am_sweep_capacity": (u64, [C.c_void_p]),
     "am_sweep_device": (C.c_int, [C.c_void_p]),

@@ -39,6 +39,7 @@
 #include <utility>
 #include <vector>
 
+#include "checkpoint_kernels.cuh"
 #include "sweep_internal.h"
 #include "sweep_kernels.cuh"
 #include "tz.h"
@@ -238,6 +239,20 @@ struct am_sweep {
   Staging* pend_clear = nullptr;  // a host tick's drain leaves clear_marks_kernel for after the tick's kernels
   size_t pend_clear_n = 0;
   std::vector<Owned> owned;
+  // checkpoints (am_sweep_checkpoint / am_sweep_restore), allocated at the first one and serialised by ck_mu (they share
+  // it all): the blob's sections in HBM (room for every section of every slot of capacity), the pass's checksum sum and
+  // zone marks (device and pinned), the stream that copies blobs to and from the caller while ticks go on, and two
+  // pinned chunks that a restore's upload alternates between.  Freed by am_sweep_destroy itself (not in `owned`:
+  // a restore allocates them outside the tick guard).
+  std::mutex ck_mu;
+  char* ck_dev = nullptr;
+  unsigned long long* ck_meta = nullptr;    // [0] checksum sum, then 8 words of zone marks
+  unsigned long long* ck_meta_h = nullptr;  // pinned copy
+  cudaStream_t ck_stream = nullptr;
+  cudaEvent_t ck_ev = nullptr;  // the pass is done (and its meta copied)
+  char* ck_pin[2] = {nullptr, nullptr};
+  cudaEvent_t ck_pin_ev[2] = {nullptr, nullptr};
+  bool ck_pin_pending[2] = {false, false};
 };
 
 namespace {
@@ -1119,6 +1134,15 @@ void am_sweep_destroy(am_sweep_t* h) {
   }
   h->host_out.release();
   h->pin_in.release(); h->dev_in.release();
+  if (h->ck_dev) cudaFree(h->ck_dev);
+  if (h->ck_meta) cudaFree(h->ck_meta);
+  if (h->ck_meta_h) cudaFreeHost(h->ck_meta_h);
+  for (int k = 0; k < 2; ++k) {
+    if (h->ck_pin[k]) cudaFreeHost(h->ck_pin[k]);
+    if (h->ck_pin_ev[k]) cudaEventDestroy(h->ck_pin_ev[k]);
+  }
+  if (h->ck_ev) cudaEventDestroy(h->ck_ev);
+  if (h->ck_stream) cudaStreamDestroy(h->ck_stream);
   if (h->stream) cudaStreamDestroy(h->stream);
   if (h->cstream) cudaStreamDestroy(h->cstream);
   delete h;
@@ -2017,6 +2041,339 @@ static int read_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* 
     if (out->remedy_total) out->remedy_total[k] = r[k].remedy_total;
     if (out->remedy_finished_at) out->remedy_finished_at[k] = r[k].remedy_finished_at;
   }
+  return AM_OK;
+}
+
+}  // extern "C"
+
+// ---- checkpoints (DESIGN.md "Checkpoint format") ----------------------------------------------------------------------
+namespace {
+
+constexpr uint64_t kCkMagic = 0x54504B4357534D41ull;  // "AMSWCKPT"
+constexpr uint64_t kCkHeader = 128;
+constexpr uint32_t kCkAllSwitches = AM_CKPT_HOLD | AM_CKPT_REMEDY | AM_CKPT_TRACK | AM_CKPT_DETAILS | AM_CKPT_TIMEOUTS;
+constexpr size_t kCkChunk = 32u << 20;  // bytes per pinned chunk of a restore's upload
+
+struct CkptHeader {
+  uint64_t magic;
+  uint32_t version, switches;
+  uint64_t bytes, checksum, first_global, n, swept_end;
+  int64_t prev_tick;
+  uint64_t seed;
+  uint32_t n_zones, reserved32;
+  uint64_t reserved[6];
+};
+static_assert(sizeof(CkptHeader) == kCkHeader, "checkpoint header: 16 words");
+
+struct CkptLayout {
+  uint64_t off[kCkSections] = {};
+  uint64_t sections_end = kCkHeader;
+};
+
+// The sections a blob of n slots with `switches` has, in order, each at an 8-B aligned offset.
+CkptLayout ckpt_layout(uint64_t n, uint32_t switches) {
+  CkptLayout L;
+  auto put = [&](int s, uint64_t bytes) {
+    L.off[s] = L.sections_end;
+    L.sections_end += (bytes + 7) / 8 * 8;
+  };
+  for (int k = 0; k < 16; ++k) put(k, n * ck_elem(k));
+  if (switches & AM_CKPT_TIMEOUTS) { put(kCkSecWfTimeout, n * 4); put(kCkSecDeadline, n * 8); }
+  if (switches & AM_CKPT_HOLD) put(kCkSecSince, n * 8);
+  if (switches & AM_CKPT_TRACK) put(kCkSecChanged, (n + 31) / 32 * 4);
+  if (switches & AM_CKPT_DETAILS) { put(kCkSecDetApplied, n); put(kCkSecDetStart, n * 8); }
+  return L;
+}
+
+uint64_t ckpt_zone_entry_bytes(size_t name_len) { return 8 + (name_len + 7) / 8 * 8; }
+
+// The checksum's terms of the words in [a, b) of a blob (the header, whose checksum word counts as 0, and the zone table).
+uint64_t ckpt_host_sum(const char* buf, uint64_t a, uint64_t b) {
+  uint64_t s = 0;
+  for (uint64_t o = a; o < b; o += 8) {
+    uint64_t w;
+    memcpy(&w, buf + o, 8);
+    if (o == offsetof(CkptHeader, checksum)) w = 0;
+    s += ckpt_mix(o * 8, w);
+  }
+  return s;
+}
+
+struct CkptZone {
+  uint32_t id;
+  std::string name;
+};
+
+// A blob's header, layout and zone table, checked for consistency (not the checksum: that is a device pass).
+int ckpt_parse(const void* buf, uint64_t len, CkptHeader* hd, CkptLayout* L, std::vector<CkptZone>* zones) {
+  if (!buf || len < kCkHeader) return AM_E_INVAL;
+  const char* p = (const char*)buf;
+  memcpy(hd, p, kCkHeader);
+  if (hd->magic != kCkMagic || hd->version != AM_CHECKPOINT_VERSION) return AM_E_INVAL;
+  if ((hd->switches & ~kCkAllSwitches) || ((hd->switches & AM_CKPT_REMEDY) && !(hd->switches & AM_CKPT_HOLD)) ||
+      ((hd->switches & AM_CKPT_DETAILS) && !(hd->switches & AM_CKPT_TRACK)))
+    return AM_E_INVAL;
+  if (hd->bytes > len || hd->bytes % 8 || hd->n > 0xFFFFFFFFull || hd->first_global + hd->n < hd->first_global ||
+      hd->swept_end < hd->first_global || hd->swept_end > hd->first_global + hd->n || hd->n_zones > 255)
+    return AM_E_INVAL;
+  *L = ckpt_layout(hd->n, hd->switches);
+  uint64_t at = L->sections_end;
+  bool seen[256] = {};
+  zones->clear();
+  for (uint32_t k = 0; k < hd->n_zones; ++k) {
+    if (at + 8 > hd->bytes) return AM_E_INVAL;
+    uint32_t id, nl;
+    memcpy(&id, p + at, 4);
+    memcpy(&nl, p + at + 4, 4);
+    if (id < 1 || id > 255 || seen[id] || nl < 1 || nl > 255 || at + ckpt_zone_entry_bytes(nl) > hd->bytes)
+      return AM_E_INVAL;
+    seen[id] = true;
+    zones->push_back({id, std::string(p + at + 8, nl)});
+    at += ckpt_zone_entry_bytes(nl);
+  }
+  return at == hd->bytes ? AM_OK : AM_E_INVAL;
+}
+
+uint32_t ckpt_switches(const am_sweep* h) {
+  return (h->hold ? AM_CKPT_HOLD : 0u) | (h->remedy ? AM_CKPT_REMEDY : 0u) | (h->track ? AM_CKPT_TRACK : 0u) |
+         (h->details ? AM_CKPT_DETAILS : 0u) | (h->wf_timeout ? AM_CKPT_TIMEOUTS : 0u);
+}
+
+// The checkpoint state of a handle, at the first checkpoint or restore (ck_mu held).
+int ckpt_alloc(am_sweep* h) {
+  AM_CUDA(h, cudaSetDevice(h->device));
+  if (h->ck_dev) return AM_OK;
+  AM_CUDA(h, cudaStreamCreateWithFlags(&h->ck_stream, cudaStreamNonBlocking));
+  AM_CUDA(h, cudaEventCreateWithFlags(&h->ck_ev, cudaEventDisableTiming));
+  for (int k = 0; k < 2; ++k) {
+    AM_CUDA(h, cudaEventCreateWithFlags(&h->ck_pin_ev[k], cudaEventDisableTiming));
+    AM_CUDA(h, cudaHostAlloc((void**)&h->ck_pin[k], kCkChunk, cudaHostAllocDefault));
+  }
+  AM_CUDA(h, cudaHostAlloc((void**)&h->ck_meta_h, 5 * 8, cudaHostAllocDefault));
+  AM_CUDA(h, cudaMalloc((void**)&h->ck_meta, 5 * 8));
+  AM_CUDA(h, cudaMalloc((void**)&h->ck_dev, ckpt_layout(h->cap_padded, kCkAllSwitches).sections_end));  // (the last)
+  return AM_OK;
+}
+
+CkptBlob ckpt_blob(const am_sweep* h, const CkptLayout& L, uint64_t n) {
+  CkptBlob b{};
+  b.p = h->ck_dev;
+  memcpy(b.off, L.off, sizeof b.off);
+  b.n = n;
+  return b;
+}
+
+CkptState ckpt_state(am_sweep* h) {
+  CkptState s{};
+  for (int k = 0; k < 16; ++k) s.col[k] = *col_slot(h->cols, k);
+  if (h->wf_timeout) {
+    s.wf_timeout = h->wf_timeout;
+    s.deadline = h->deadline;
+    s.seg_deadline = h->seg_deadline;
+  }
+  if (h->hold) s.since = h->since;
+  if (h->track) s.changed = h->chg_bits;
+  if (h->details) {
+    s.det_applied = h->det_applied;
+    s.det_start = h->det_start;
+  }
+  return s;
+}
+
+}  // namespace
+
+extern "C" {
+
+int am_sweep_checkpoint(am_sweep_t* h, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out) {
+  if (!h || !len_out || (cap && !buf)) return AM_E_INVAL;
+  if (first + n > h->capacity || first + n < first) return AM_E_INVAL;
+  std::lock_guard<std::mutex> ck(h->ck_mu);
+  CkptHeader hd{};
+  CkptLayout L;
+  {  // the pass, with the tick guard held: the drain, then one kernel over the range on the handle's stream
+    TickGuard g(h);
+    if (!g.ok) return AM_E_BUSY;
+    int rc = begin_call(h);  // (first: the drain may allocate the timeout state, a section of the blob)
+    if (rc != AM_OK) return rc;
+    hd.switches = ckpt_switches(h);
+    L = ckpt_layout(n, hd.switches);
+    uint64_t bound = L.sections_end;  // (room for the names of every registered zone)
+    std::string name;
+    for (int32_t id = 1; amsweep_tz::name_of(id, &name); ++id) bound += ckpt_zone_entry_bytes(name.size());
+    if (cap < bound) {
+      *len_out = bound;
+      return AM_E_NOSPACE;
+    }
+    rc = ckpt_alloc(h);
+    if (rc != AM_OK) return rc;
+    hd.magic = kCkMagic;
+    hd.version = AM_CHECKPOINT_VERSION;
+    hd.first_global = h->shard_base + first;
+    hd.n = n;
+    hd.swept_end = h->shard_base + std::min(std::max(h->n_records, first), first + n);
+    hd.prev_tick = h->has_prev ? h->prev_T : INT64_MIN;
+    hd.seed = h->seed;
+    AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->stream));
+    if (n) {
+      AM_LAUNCH(checkpoint_pack_kernel, (unsigned)((n + 255) / 256), 256, h->stream, ckpt_state(h), ckpt_blob(h, L, n),
+                first, h->ck_meta, (uint32_t*)(h->ck_meta + 1));
+      h->launches++;
+      AM_CUDA(h, cudaGetLastError());
+    }
+    AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaEventRecord(h->ck_ev, h->stream));
+  }
+  // Ticks may run from here on: the copy to the caller waits for the pass only, on the checkpoint stream.
+  AM_CUDA(h, cudaEventSynchronize(h->ck_ev));
+  char* p = (char*)buf;
+  uint64_t at = L.sections_end;
+  const uint32_t* marks = (const uint32_t*)(h->ck_meta_h + 1);
+  for (uint32_t id = 1; id < 256; ++id) {
+    if (!((marks[id >> 5] >> (id & 31)) & 1u)) continue;
+    std::string name;
+    if (!amsweep_tz::name_of((int32_t)id, &name)) {  // (upserts and loads refuse ids that are not registered)
+      h->last_error = "am_sweep_checkpoint: a record carries a zone id that is not registered";
+      return AM_E_DEVICE;
+    }
+    const uint32_t nl = (uint32_t)name.size();
+    memset(p + at, 0, ckpt_zone_entry_bytes(nl));
+    memcpy(p + at, &id, 4);
+    memcpy(p + at + 4, &nl, 4);
+    memcpy(p + at + 8, name.data(), nl);
+    at += ckpt_zone_entry_bytes(nl);
+    ++hd.n_zones;
+  }
+  hd.bytes = at;
+  memcpy(p, &hd, kCkHeader);
+  AM_CUDA(h, cudaStreamWaitEvent(h->ck_stream, h->ck_ev, 0));
+  if (L.sections_end > kCkHeader)
+    AM_CUDA(h, cudaMemcpyAsync(p + kCkHeader, h->ck_dev + kCkHeader, L.sections_end - kCkHeader, cudaMemcpyDeviceToHost,
+                               h->ck_stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  hd.checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, at);
+  memcpy(p + offsetof(CkptHeader, checksum), &hd.checksum, 8);
+  *len_out = at;
+  return AM_OK;
+}
+
+int am_checkpoint_info(const void* buf, uint64_t len, am_checkpoint_info_t* info) {
+  if (!info) return AM_E_INVAL;
+  CkptHeader hd;
+  CkptLayout L;
+  std::vector<CkptZone> zones;
+  const int rc = ckpt_parse(buf, len, &hd, &L, &zones);
+  if (rc != AM_OK) return rc;
+  *info = am_checkpoint_info_t{};
+  info->first_global = hd.first_global;
+  info->n = hd.n;
+  info->swept_end = hd.swept_end;
+  info->prev_tick = hd.prev_tick;
+  info->seed = hd.seed;
+  info->switches = hd.switches;
+  info->n_zones = hd.n_zones;
+  info->version = hd.version;
+  info->bytes = hd.bytes;
+  return AM_OK;
+}
+
+int am_sweep_restore(am_sweep_t* h, const void* buf, uint64_t len) {
+  if (!h || !buf) return AM_E_INVAL;
+  CkptHeader hd;
+  CkptLayout L;
+  std::vector<CkptZone> zones;
+  int rc = ckpt_parse(buf, len, &hd, &L, &zones);
+  if (rc != AM_OK) {
+    h->last_error = "am_sweep_restore: not a checkpoint of this format version, or truncated";
+    return rc;
+  }
+  if (hd.first_global < h->shard_base || hd.first_global - h->shard_base + hd.n > h->capacity) {
+    h->last_error = "am_sweep_restore: the blob's slots are not all inside this shard";
+    return AM_E_RANGE;
+  }
+  const uint64_t first = hd.first_global - h->shard_base;
+  ZoneLut lut{};  // (id 0 stays 0)
+  for (const CkptZone& z : zones) {
+    int32_t id = 0;
+    rc = am_tz_lookup(z.name.data(), z.name.size(), &id);
+    if (rc != AM_OK) {
+      h->last_error = "am_sweep_restore: time zone " + z.name + (rc == AM_E_PARSE ? " is unknown here" : " does not fit the registry");
+      return rc;
+    }
+    lut.id[z.id] = (uint8_t)id;
+  }
+  std::lock_guard<std::mutex> ck(h->ck_mu);
+  rc = ckpt_alloc(h);
+  if (rc != AM_OK) return rc;
+  // Up in chunks through two pinned buffers (the host fills one while the other crosses), then the device pass that
+  // verifies the checksum: all before anything of the handle changes.
+  const char* p = (const char*)buf;
+  for (uint64_t off = kCkHeader, k = 0; off < L.sections_end; off += kCkChunk, ++k) {
+    const size_t m = (size_t)std::min<uint64_t>(kCkChunk, L.sections_end - off);
+    const int b = (int)(k & 1);
+    if (h->ck_pin_pending[b]) AM_CUDA(h, cudaEventSynchronize(h->ck_pin_ev[b]));
+    memcpy(h->ck_pin[b], p + off, m);
+    AM_CUDA(h, cudaMemcpyAsync(h->ck_dev + off, h->ck_pin[b], m, cudaMemcpyHostToDevice, h->ck_stream));
+    AM_CUDA(h, cudaEventRecord(h->ck_pin_ev[b], h->ck_stream));
+    h->ck_pin_pending[b] = true;
+  }
+  AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->ck_stream));
+  if (hd.n) {
+    AM_LAUNCH(checkpoint_verify_kernel, (unsigned)((hd.n + 255) / 256), 256, h->ck_stream, ckpt_blob(h, L, hd.n),
+              h->ck_meta, (uint32_t*)(h->ck_meta + 1));
+    AM_CUDA(h, cudaGetLastError());
+  }
+  AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  h->ck_pin_pending[0] = h->ck_pin_pending[1] = false;
+  const uint64_t sum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, hd.bytes);
+  if (sum != hd.checksum) {
+    h->last_error = "am_sweep_restore: checksum mismatch";
+    return AM_E_INVAL;
+  }
+  const uint32_t* marks = (const uint32_t*)(h->ck_meta_h + 1);
+  for (uint32_t id = 1; id < 256; ++id)
+    if (((marks[id >> 5] >> (id & 31)) & 1u) && !lut.id[id]) {
+      h->last_error = "am_sweep_restore: a record names a zone the blob's table does not";
+      return AM_E_INVAL;
+    }
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if ((hd.switches & ~AM_CKPT_TIMEOUTS) != (ckpt_switches(h) & ~AM_CKPT_TIMEOUTS)) {
+    h->last_error = "am_sweep_restore: set the handle's switches to the blob's first (am_checkpoint_info)";
+    return AM_E_INVAL;
+  }
+  if (h->has_prev && (hd.prev_tick == INT64_MIN || hd.prev_tick != h->prev_T)) {
+    h->last_error = "am_sweep_restore: the handle's previous tick differs from the blob's";
+    return AM_E_INVAL;
+  }
+  // a restore is a call in the per-slot order: the calls staged before it are applied first, and it replaces them
+  rc = begin_call(h);
+  if (rc != AM_OK) return rc;
+  if ((hd.switches & AM_CKPT_TIMEOUTS) && !h->wf_timeout) {
+    rc = alloc_timeouts(h, h->stream);
+    if (rc != AM_OK) return rc;
+  }
+  if (hd.n) {
+    AM_LAUNCH(checkpoint_scatter_kernel, (unsigned)((hd.n + 255) / 256), 256, h->stream, ckpt_state(h), ckpt_blob(h, L, hd.n),
+              first, lut);
+    const uint64_t seg0 = first / kRecPerWarp, n_seg = (first + hd.n + kRecPerWarp - 1) / kRecPerWarp - seg0;
+    AM_LAUNCH(build_planes_range_kernel, (unsigned)((n_seg + kWarps - 1) / kWarps), kBlock, h->stream, h->cols, h->planes,
+              (uint32_t)seg0, (uint32_t)n_seg);
+    h->launches += 2;
+    AM_CUDA(h, cudaGetLastError());
+  }
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  const uint64_t hwm = hd.swept_end - h->shard_base;
+  if (hwm > h->n_records) h->n_records = hwm;
+  if (hd.prev_tick != INT64_MIN) {
+    h->has_prev = true;
+    h->prev_T = hd.prev_tick;
+  }
+  h->seed = hd.seed;
+  // the previous tick's lists are not carried: empty until the next tick
+  h->host_n = 0;
+  h->to_ran = h->to_fetched = false;
+  h->chg_listed = h->chg_fetched = false;
   return AM_OK;
 }
 

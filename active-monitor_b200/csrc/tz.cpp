@@ -250,6 +250,13 @@ int count() {
   return (int)g_zones.size();
 }
 
+bool name_of(int32_t id, std::string* name) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (id < 1 || (size_t)id > g_zones.size()) return false;
+  *name = g_zones[(size_t)id - 1]->name;
+  return true;
+}
+
 namespace {
 // the next instant after `utc` at which zone_offset(z, .) may change (never later than the true one)
 int64_t next_change(const Zone& z, int64_t utc) {

@@ -16,6 +16,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <string>
 #include <vector>
 
 #include "civil.h"
@@ -31,6 +32,8 @@ int lookup(const char* name, size_t len, int32_t* id_out);
 // UTC offset (seconds east) of zone `id` at a UTC instant.  false: unknown id.
 bool offset_at(int32_t id, int64_t utc, int32_t* utoff);
 int count();
+// The name zone `id` was registered under.  false: unknown id (0 included).
+bool name_of(int32_t id, std::string* name);
 // Flattened copy of the registry for the device (entry 0 = UTC) and its version (bumped on every
 // registration); descs == nullptr: the version only.
 uint64_t snapshot(std::vector<ZoneDesc>* descs, std::vector<int64_t>* trans, std::vector<int32_t>* off);

@@ -131,6 +131,20 @@ def classify(*, repeat_after_sec=0, cron="", has_resource=True, has_remedy=False
     return rc, arr
 
 
+def checkpoint_info(blob) -> dict:
+    """the header of a checkpoint blob (am_checkpoint_info): first_global, n, swept_end, prev_tick (None: no previous
+    tick), seed, switches (CKPT_*), n_zones, version, bytes.  Raises AmError(AM_E_INVAL) for anything else."""
+    a = np.frombuffer(blob, dtype=np.uint8)
+    info = L.AmCheckpointInfo()
+    rc = L.load().am_checkpoint_info(a.ctypes.data if len(a) else None, len(a), C.byref(info))
+    if rc != L.AM_OK:
+        raise AmError(rc, "am_checkpoint_info")
+    d = info.as_dict()
+    if d["prev_tick"] == -(1 << 63):
+        d["prev_tick"] = None
+    return d
+
+
 # ---- SoA helpers -------------------------------------------------------------
 def alloc_columns(n: int) -> dict:
     return {name: np.zeros(n, dtype=dt) for name, dt in L.COLUMNS}
@@ -331,6 +345,26 @@ class Sweep:
         self._check(self._lib.am_sweep_read(self._h, 0, len(idx), idx.ctypes.data, C.byref(cs)),
                     "am_sweep_read")
         return cols
+
+    # -- checkpoints
+    def checkpoint(self, first: int = 0, n: int | None = None) -> bytes:
+        """the state of local slots [first, first+n) (n None: to the capacity) as one blob (am_sweep_checkpoint)"""
+        n = self.capacity - first if n is None else n
+        need = L.u64(0)
+        buf = np.zeros(0, np.uint8)
+        while True:  # (a zone registered between the calls can make the first size too small)
+            rc = self._lib.am_sweep_checkpoint(self._h, first, n, buf.ctypes.data if len(buf) else None, len(buf),
+                                               C.byref(need))
+            if rc != L.AM_E_NOSPACE:
+                break
+            buf = np.zeros(need.value, np.uint8)
+        self._check(rc, "am_sweep_checkpoint")
+        return buf[:need.value].tobytes()
+
+    def restore(self, blob):
+        """place a checkpoint blob's slots into this handle (am_sweep_restore); set the switches first"""
+        a = np.frombuffer(blob, dtype=np.uint8)
+        self._check(self._lib.am_sweep_restore(self._h, a.ctypes.data if len(a) else None, len(a)), "am_sweep_restore")
 
     # -- hold in flight
     def set_hold_in_flight(self, on: bool):

@@ -612,6 +612,69 @@ int am_sweep_set_change_details(am_sweep_t*, int on);
 int am_sweep_last_change_details(am_sweep_t*, uint64_t offset, uint64_t* idx, am_change_detail_t* out, uint64_t cap,
                                  uint64_t* n_out);
 
+/* Checkpoints: a handle's whole state for a range of slots as one self-describing byte blob (DESIGN.md section 6
+ * item 19, "Checkpoint format"), so that a restarted or resharded controller goes on tick for tick.  A blob carries,
+ * per slot, the sixteen columns (flags bits raw), wf_timeout and the running workflow's deadline when the handle has
+ * the timeout state, `since` (remedy runs included) while the hold is on, the change bit while tracking is on and the
+ * detail capture while details are on, all as they stand; and the previous tick's second P, the seed, the switches,
+ * the names of the time zones its 5-field records use and a 64-bit checksum (against accidental damage, not
+ * tampering).  92 B per slot with no switch on, up to 121.125 B with all of them.  Not carried: the previous tick's
+ * lists (am_sweep_last_list, both timed-out lists, the changes and their details: empty on the restored handle until
+ * its next tick), profiling state and the launch count.
+ * EQUIVALENCE: restore the blobs of one checkpoint of a handle H, all taken between the same two ticks, into handles
+ * whose shards cover H's swept slots; from then on the same calls, split by slot, return what they return on H (every
+ * tick entry point with its list and statistics except n_records, which is per shard; am_sweep_simulate; read,
+ * in_flight, remedy_in_flight, repeat_after_sec, next_due; the timed-out lists, the changes and the details).  With one
+ * handle of the same shard that includes n_records. */
+#define AM_CHECKPOINT_VERSION 1
+#define AM_CKPT_HOLD 0x1u     /* the hold in flight was on                   */
+#define AM_CKPT_REMEDY 0x2u   /* ... and the remedy hold                      */
+#define AM_CKPT_TRACK 0x4u    /* status changes were tracked                  */
+#define AM_CKPT_DETAILS 0x8u  /* ... with change details                      */
+#define AM_CKPT_TIMEOUTS 0x10u /* the handle had the workflow-timeout state   */
+typedef struct am_checkpoint_info {
+  uint64_t first_global, n; /* the slots it holds, by GLOBAL index: [first_global, first_global + n)    */
+  uint64_t swept_end;       /* global end of the source's swept slots (high-water mark) within the range */
+  int64_t prev_tick;        /* P, INT64_MIN when the source had none                                   */
+  uint64_t seed;
+  uint32_t switches;        /* AM_CKPT_*                                                                */
+  uint32_t n_zones;         /* named zones its records use                                              */
+  uint32_t version;         /* AM_CHECKPOINT_VERSION                                                    */
+  uint32_t reserved;
+  uint64_t bytes;           /* the blob's length                                                        */
+} am_checkpoint_info_t;
+
+/* Checkpoint of local slots [first, first+n) into buf[0..cap).  A call in the per-slot order: staged calls are drained
+ * as am_sweep_read drains them (a result the drain leaves pending is carried pending).  The tick guard is held only
+ * while the drain and one device pass over the range are issued on the handle's stream (a tick in that time
+ * returns AM_E_BUSY; later ticks queue behind the pass).  The pass packs the sections into a staging area in HBM
+ * (allocated at the first checkpoint or restore, about 122 B per slot of capacity, kept until am_sweep_destroy), marks
+ * the zones in use and sums the checksum; the copy into buf follows on a stream of its own, while ticks run.
+ * Checkpoints and restores of one handle are serialised.
+ * *len_out = the blob's length.  AM_E_NOSPACE (after the drain, nothing else done): cap is below what the call needs,
+ * returned in *len_out (room for the names of every registered zone; the blob itself may be shorter). */
+int am_sweep_checkpoint(am_sweep_t*, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out);
+/* The header of a blob, checked for consistency (format version, sizes, zone table); no handle, no GPU.  The checksum
+ * is verified by am_sweep_restore.  AM_E_INVAL: not a blob of this format version, or truncated. */
+int am_checkpoint_info(const void* buf, uint64_t len, am_checkpoint_info_t* info);
+/* Restore a blob into this handle: slot g of the blob goes to local slot g - shard_base.  A call in the per-slot order:
+ * the calls staged before it are drained first and it replaces them for its slots.  The blob is copied up in chunks,
+ * verified on the device (checksum) and its zone names resolved with am_tz_lookup before anything changes; then one
+ * pass scatters every section (zone ids rewritten to this process's), the mask planes of the slots are rebuilt, the
+ * timeout state is allocated if the blob has it and the handle not (a handle with it restoring a blob without it gets
+ * no timeouts and no deadlines for the slots), and the high-water mark is raised to swept_end - shard_base.  P and the
+ * seed become the blob's.  Set the switches first, from am_checkpoint_info (am_sweep_set_hold_in_flight, ...).
+ * Refused before anything changes (nothing drained, nothing written, P unchanged):
+ *   AM_E_INVAL        truncated blob, bad checksum, unknown format version; switches (AM_CKPT_TIMEOUTS aside) that
+ *                     differ from the handle's; a handle whose previous tick differs from the blob's P (blobs taken
+ *                     at different ticks disagree on P);
+ *   AM_E_PARSE        a zone name this process cannot load;
+ *   AM_E_UNSUPPORTED  a 256th distinct zone;
+ *   AM_E_RANGE        slots outside this shard.
+ * Zones registered while resolving the names before a refusal stay registered: the registry is process-wide and only
+ * grows, which is harmless. */
+int am_sweep_restore(am_sweep_t*, const void* buf, uint64_t len);
+
 /* Introspection */
 uint64_t am_sweep_size(const am_sweep_t*);     /* high-water mark (slots swept) */
 uint64_t am_sweep_capacity(const am_sweep_t*);
