@@ -22,8 +22,10 @@
 //   * am_sweep_tick, _tick_view, _tick_device and _tick_shard run one path (run_tick): the
 //     refusals, the drain, the sweep and the commit of the previous tick's second; the sweep
 //     variant comes from one table (sweep_variant);
-//   * fixed-size device arrays, pinned host arrays and events are recorded on the handle as
-//     they are made (dev_array, host_array, new_event): am_sweep_destroy frees that list.
+//   * am_sweep_run_ticks and am_sweep_simulate run one path for runs of ticks (begin_run, run_rows, run_blocks) around
+//     their own tick loops;
+//   * fixed-size device arrays, pinned host arrays, events and streams are recorded on the handle as they are made
+//     (dev_array, host_array, new_event, new_stream): am_sweep_destroy frees that list.
 //
 // There is deliberately no CPU path in this file: without a CUDA device
 // am_sweep_create fails with AM_E_DEVICE.
@@ -91,9 +93,9 @@ struct Upload {
   bool pending = false;
 };
 
-// What am_sweep_destroy frees: every fixed-size allocation and every event of a handle, recorded as it is made.
+// What am_sweep_destroy frees: every fixed-size allocation, event and stream of a handle, recorded as it is made.
 struct Owned {
-  enum Kind { kDevice, kPinned, kEvent } kind;
+  enum Kind { kDevice, kPinned, kEvent, kStream } kind;
   void* p;
 };
 
@@ -239,11 +241,11 @@ struct am_sweep {
   Staging* pend_clear = nullptr;  // a host tick's drain leaves clear_marks_kernel for after the tick's kernels
   size_t pend_clear_n = 0;
   std::vector<Owned> owned;
+  std::mutex owned_mu;  // guards appends to `owned` (a restore allocates outside the tick guard)
   // checkpoints (am_sweep_checkpoint / am_sweep_restore), allocated at the first one and serialised by ck_mu (they share
   // it all): the blob's sections in HBM (room for every section of every slot of capacity), the pass's checksum sum and
   // zone marks (device and pinned), the stream that copies blobs to and from the caller while ticks go on, and two
-  // pinned chunks that a restore's upload alternates between.  Freed by am_sweep_destroy itself (not in `owned`:
-  // a restore allocates them outside the tick guard).
+  // pinned chunks that a restore's upload alternates between.
   std::mutex ck_mu;
   char* ck_dev = nullptr;
   unsigned long long* ck_meta = nullptr;    // [0] checksum sum, then 8 words of zone marks
@@ -317,13 +319,18 @@ int set_stream(am_sweep* h, cudaStream_t s) {
   return order_on(h, s);
 }
 
+void own(am_sweep* h, Owned::Kind kind, void* p) {
+  std::lock_guard<std::mutex> lk(h->owned_mu);
+  h->owned.push_back({kind, p});
+}
+
 // A fixed-size device array owned by the handle until am_sweep_destroy; zeroed on `s` when `zero`.
 template <class T>
 cudaError_t dev_array(am_sweep* h, T** p, size_t bytes, cudaStream_t s, bool zero = true) {
   void* q = nullptr;
   cudaError_t e = cudaMalloc(&q, bytes);
   if (e != cudaSuccess) return e;
-  h->owned.push_back({Owned::kDevice, q});
+  own(h, Owned::kDevice, q);
   *p = (T*)q;
   return zero ? cudaMemsetAsync(q, 0, bytes, s) : cudaSuccess;
 }
@@ -332,13 +339,18 @@ cudaError_t host_array(am_sweep* h, T** p, size_t bytes, unsigned flags = cudaHo
   void* q = nullptr;
   cudaError_t e = cudaHostAlloc(&q, bytes, flags);
   if (e != cudaSuccess) return e;
-  h->owned.push_back({Owned::kPinned, q});
+  own(h, Owned::kPinned, q);
   *p = (T*)q;
   return cudaSuccess;
 }
 cudaError_t new_event(am_sweep* h, cudaEvent_t* ev, bool timed = false) {
   cudaError_t e = timed ? cudaEventCreate(ev) : cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) h->owned.push_back({Owned::kEvent, (void*)*ev});
+  if (e == cudaSuccess) own(h, Owned::kEvent, (void*)*ev);
+  return e;
+}
+cudaError_t new_stream(am_sweep* h, cudaStream_t* s) {
+  cudaError_t e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
+  if (e == cudaSuccess) own(h, Owned::kStream, (void*)*s);
   return e;
 }
 
@@ -998,6 +1010,109 @@ int run_tick(am_sweep* h, int64_t T, uint32_t mode, cudaStream_t s, TickKind kin
   return AM_OK;
 }
 
+// The prologue of a run of ticks (am_sweep_run_ticks, am_sweep_simulate; tick guard held, refusals made): on the
+// handle's stream, the staged calls drained (as tick *tick_T's drain when given), the run's seed.  A run's ticks list
+// no timed-out runs and no status changes.
+int begin_run(am_sweep* h, const int64_t* tick_T, uint64_t seed) {
+  int rc = set_stream(h, h->stream);
+  if (rc != AM_OK) return rc;
+  h->to_ran = false;
+  h->chg_listed = h->chg_fetched = false;
+  rc = drain_staged(h, h->stream, tick_T);
+  if (rc != AM_OK) return rc;
+  h->seed = seed;
+  return AM_OK;
+}
+
+// The device rows of a run of n ticks: n am_tick_stats_t and, for a simulation, n am_sim_tick_t (4 accumulators each)
+// after them.  One allocation, freed on every return.
+struct RunRows {
+  am_tick_stats_t* stats = nullptr;
+  unsigned long long* sim = nullptr;
+  size_t bytes = 0;
+  ~RunRows() { cudaFree(stats); }
+  cudaError_t alloc(uint64_t n, bool with_sim) {
+    bytes = n * (sizeof(am_tick_stats_t) + (with_sim ? sizeof(am_sim_tick_t) : 0));
+    const cudaError_t e = cudaMalloc((void**)&stats, bytes);
+    if (e == cudaSuccess && with_sim) sim = reinterpret_cast<unsigned long long*>(stats + n);
+    return e;
+  }
+};
+
+// Ticks per pass of a blocked run: AMSWEEP_BLOCK_TICKS in [1, kMaxBlockTicks], else kDefaultBlockTicks.
+uint64_t block_ticks() {
+  if (const char* e = getenv("AMSWEEP_BLOCK_TICKS")) {
+    const long v = atol(e);
+    if (v >= 1 && v <= kMaxBlockTicks) return (uint64_t)v;
+  }
+  return kDefaultBlockTicks;
+}
+
+// Temporal blocking (sweep_block.cuh): the n ticks from T0 in blocks of up to block_ticks() ticks, one pass over the
+// columns each.  A block never spans an instant at which a registered zone changes its UTC offset (the kernel holds one
+// offset per zone for the whole block).  Per block, `b`'s BlockParams part is filled in and launch(b, k, grid) launches
+// the caller's instantiation for the block that starts at tick k.
+template <class P, class Launch>
+int run_blocks(am_sweep* h, int64_t T0, uint64_t n, am_tick_stats_t* stats, P b, Launch&& launch) {
+  const uint64_t per_block = block_ticks();
+  const unsigned grid = (unsigned)((h->n_records + kBlockRecords - 1) / kBlockRecords);
+  for (uint64_t k = 0; k < n;) {
+    const int64_t T = T0 + (int64_t)k;
+    const int rc = refresh_zones(h, T, h->stream);
+    if (rc != AM_OK) return rc;
+    uint64_t K = n - k < per_block ? n - k : per_block;
+    if (h->tz_n > 1 && h->tz_hi < T + (int64_t)K) K = (uint64_t)(h->tz_hi - T);  // (tz_hi > T after the refresh)
+    b.c = h->cols;
+    b.n_records = h->n_records;
+    b.shard_base = h->shard_base;
+    b.seed = h->seed;
+    b.T0 = T;
+    b.K = (uint32_t)K;
+    b.tz_off = h->tz_n > 1 ? (const int32_t*)h->tz_off.dev : nullptr;
+    b.stats = reinterpret_cast<unsigned long long*>(stats + k);
+    launch(b, k, grid);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
+    k += K;
+  }
+  return AM_OK;
+}
+
+// A run of n ticks from T0 once begin_run is done: its rows (zeroed when blocked or simulated: the kernels accumulate
+// into them), ev0, ticks(rows) (the entry's own ticks), ev1, one synchronisation, the rows copied out (the sim rows
+// when sim_out is given), last_ms, n_records in every row of a blocked run, and P committed on success.  With
+// tracking on, a run that got as far as its rows seeds the change bits again from the flags whatever happened: its
+// ticks applied what its drain noted.
+template <class Ticks>
+int run_rows(am_sweep* h, int64_t T0, uint64_t n, bool blocked, bool with_sim, am_tick_stats_t* stats_out,
+             am_sim_tick_t* sim_out, Ticks&& ticks) {
+  RunRows rows;
+  AM_CUDA(h, rows.alloc(n, with_sim));
+  int rc = [&]() -> int {
+    if (blocked || with_sim) AM_CUDA(h, cudaMemsetAsync(rows.stats, 0, rows.bytes, h->stream));
+    AM_CUDA(h, cudaEventRecord(h->ev0, h->stream));
+    const int trc = ticks(rows);
+    if (trc != AM_OK) return trc;
+    AM_CUDA(h, cudaEventRecord(h->ev1, h->stream));
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    AM_CUDA(h, cudaMemcpy(stats_out, rows.stats, n * sizeof(am_tick_stats_t), cudaMemcpyDeviceToHost));
+    if (sim_out) AM_CUDA(h, cudaMemcpy(sim_out, rows.sim, n * sizeof(am_sim_tick_t), cudaMemcpyDeviceToHost));
+    float ms = 0;
+    AM_CUDA(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+    h->last_ms = ms;
+    if (blocked)  // (a tick's publish_kernel writes its row's n_records)
+      for (uint64_t k = 0; k < n; ++k) stats_out[k].n_records = h->n_records;
+    h->has_prev = true;
+    h->prev_T = T0 + (int64_t)n - 1;
+    return AM_OK;
+  }();
+  if (h->track) {
+    const int rs = seed_changes(h, h->stream, 0, h->cap_padded);
+    if (rc == AM_OK) rc = rs;
+  }
+  return rc;
+}
+
 }  // namespace
 
 namespace amsweep {
@@ -1073,8 +1188,8 @@ int am_sweep_create(am_sweep_t** out, int device_id, uint64_t capacity, uint64_t
   if (const char* e = getenv("AMSWEEP_EARLY_RESULTS")) h->early_results = atoi(e) != 0;  // (A/B of the two result paths)
   int rc = [&]() -> int {
     AM_CUDA(h, cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, device_id));
-    AM_CUDA(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    AM_CUDA(h, cudaStreamCreateWithFlags(&h->cstream, cudaStreamNonBlocking));
+    AM_CUDA(h, new_stream(h, &h->stream));
+    AM_CUDA(h, new_stream(h, &h->cstream));
     for (cudaEvent_t* e : {&h->ev_last, &h->stage[0].copied, &h->stage[0].drained, &h->stage[1].copied,
                            &h->stage[1].drained, &h->set[0].consumed, &h->set[1].consumed})
       AM_CUDA(h, new_event(h, e));
@@ -1126,7 +1241,8 @@ void am_sweep_destroy(am_sweep_t* h) {
   for (const Owned& o : h->owned) {
     if (o.kind == Owned::kDevice) cudaFree(o.p);
     else if (o.kind == Owned::kPinned) cudaFreeHost(o.p);
-    else cudaEventDestroy((cudaEvent_t)o.p);
+    else if (o.kind == Owned::kEvent) cudaEventDestroy((cudaEvent_t)o.p);
+    else cudaStreamDestroy((cudaStream_t)o.p);
   }
   for (Staging& st : h->stage) {
     st.ops.release(); st.recs.release();
@@ -1134,17 +1250,6 @@ void am_sweep_destroy(am_sweep_t* h) {
   }
   h->host_out.release();
   h->pin_in.release(); h->dev_in.release();
-  if (h->ck_dev) cudaFree(h->ck_dev);
-  if (h->ck_meta) cudaFree(h->ck_meta);
-  if (h->ck_meta_h) cudaFreeHost(h->ck_meta_h);
-  for (int k = 0; k < 2; ++k) {
-    if (h->ck_pin[k]) cudaFreeHost(h->ck_pin[k]);
-    if (h->ck_pin_ev[k]) cudaEventDestroy(h->ck_pin_ev[k]);
-  }
-  if (h->ck_ev) cudaEventDestroy(h->ck_ev);
-  if (h->ck_stream) cudaStreamDestroy(h->ck_stream);
-  if (h->stream) cudaStreamDestroy(h->stream);
-  if (h->cstream) cudaStreamDestroy(h->cstream);
   delete h;
 }
 
@@ -1527,78 +1632,24 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
     h->last_error = "am_sweep_run_ticks while the hold in flight is on";
     return AM_E_INVAL;
   }
-  int rc = set_stream(h, h->stream);
-  if (rc != AM_OK) return rc;
-  h->to_ran = false;  // (ticks: the timed-out list is reset; with the hold off nothing times out)
-  h->chg_listed = h->chg_fetched = false;  // (and the list of status changes: a run's ticks are not tracked)
   // A blocked run publishes no tick's accumulators: its drain leaves posted results pending in the flags,
   // and the block kernel applies them at its first tick (and counts them in that tick's row).
-  rc = drain_staged(h, h->stream, (mode & AM_SWEEP_BLOCKED) ? nullptr : &unix_sec0);
+  const int rc = begin_run(h, (mode & AM_SWEEP_BLOCKED) ? nullptr : &unix_sec0, seed);
   if (rc != AM_OK) return rc;
-  h->seed = seed;
-  am_tick_stats_t* d_stats = nullptr;
-  AM_CUDA(h, cudaMalloc((void**)&d_stats, n_ticks * sizeof(am_tick_stats_t)));
-  const bool blocked = (mode & AM_SWEEP_BLOCKED) != 0 && h->n_records != 0;
-  if (blocked) {  // the block kernel accumulates into the rows
-    if (cudaError_t e = cudaMemsetAsync(d_stats, 0, n_ticks * sizeof(am_tick_stats_t), h->stream); e != cudaSuccess) {
-      h->last_error = cudaGetErrorString(e);
-      cudaFree(d_stats);
-      return AM_E_DEVICE;
+  const bool blocked = (mode & AM_SWEEP_BLOCKED) != 0 && h->n_records != 0;  // (an empty shard runs tick by tick)
+  return run_rows(h, unix_sec0, n_ticks, blocked, false, stats_out, nullptr, [&](const RunRows& rows) -> int {
+    if (blocked)
+      return run_blocks(h, unix_sec0, n_ticks, rows.stats, BlockParams{}, [&](const BlockParams& b, uint64_t, unsigned grid) {
+        if (mode & AM_SWEEP_CLOSED_LOOP) AM_LAUNCH(sweep_block_kernel<true>, grid, kBlockThreads, h->stream, b);
+        else AM_LAUNCH(sweep_block_kernel<false>, grid, kBlockThreads, h->stream, b);
+      });
+    for (uint64_t k = 0; k < n_ticks; ++k) {
+      const ListOut o{h->due_idx[k & 1], h->due_action[k & 1], h->cap_padded, nullptr, rows.stats + k};
+      const int trc = launch_tick(h, unix_sec0 + (int64_t)k, mode, o, h->stream);
+      if (trc != AM_OK) return trc;
     }
-  }
-  if (cudaError_t e = cudaEventRecord(h->ev0, h->stream); e != cudaSuccess) {
-    h->last_error = cudaGetErrorString(e);
-    rc = AM_E_DEVICE;
-  }
-  // Temporal blocking (sweep_block.cuh): up to kMaxBlockTicks ticks per pass over the columns.  A block
-  // never spans an instant at which a registered zone changes its UTC offset (the kernel holds one
-  // offset per zone for the whole block).
-  uint64_t block_ticks = kDefaultBlockTicks;
-  if (const char* e = getenv("AMSWEEP_BLOCK_TICKS")) { long v = atol(e); if (v >= 1 && v <= kMaxBlockTicks) block_ticks = (uint64_t)v; }
-  for (uint64_t k = 0; blocked && k < n_ticks && rc == AM_OK;) {
-    const int64_t T = unix_sec0 + (int64_t)k;
-    rc = refresh_zones(h, T, h->stream);
-    if (rc != AM_OK) break;
-    uint64_t K = n_ticks - k < block_ticks ? n_ticks - k : block_ticks;
-    if (h->tz_n > 1 && h->tz_hi < T + (int64_t)K) K = (uint64_t)(h->tz_hi - T);  // (tz_hi > T after the refresh)
-    BlockParams b{};
-    b.c = h->cols;
-    b.n_records = h->n_records;
-    b.shard_base = h->shard_base;
-    b.seed = h->seed;
-    b.T0 = T;
-    b.K = (uint32_t)K;
-    b.tz_off = h->tz_n > 1 ? (const int32_t*)h->tz_off.dev : nullptr;
-    b.stats = reinterpret_cast<unsigned long long*>(d_stats + k);
-    const unsigned grid = (unsigned)((h->n_records + kBlockRecords - 1) / kBlockRecords);
-    if (mode & AM_SWEEP_CLOSED_LOOP) AM_LAUNCH(sweep_block_kernel<true>, grid, kBlockThreads, h->stream, b);
-    else AM_LAUNCH(sweep_block_kernel<false>, grid, kBlockThreads, h->stream, b);
-    h->launches++;
-    if (cudaError_t e = cudaGetLastError(); e != cudaSuccess) { h->last_error = cudaGetErrorString(e); rc = AM_E_DEVICE; }
-    k += K;
-  }
-  for (uint64_t k = 0; !blocked && k < n_ticks && rc == AM_OK; ++k) {
-    const ListOut o{h->due_idx[k & 1], h->due_action[k & 1], h->cap_padded, nullptr, d_stats + k};
-    rc = launch_tick(h, unix_sec0 + (int64_t)k, mode, o, h->stream);
-  }
-  if (rc == AM_OK) {
-    cudaError_t e = cudaEventRecord(h->ev1, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e == cudaSuccess) e = cudaMemcpy(stats_out, d_stats, n_ticks * sizeof(am_tick_stats_t), cudaMemcpyDeviceToHost);
-    float ms = 0;
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-    if (e != cudaSuccess) { h->last_error = cudaGetErrorString(e); rc = AM_E_DEVICE; }
-    else h->last_ms = ms;
-    if (blocked && rc == AM_OK)
-      for (uint64_t k = 0; k < n_ticks; ++k) stats_out[k].n_records = h->n_records;
-    if (rc == AM_OK) { h->has_prev = true; h->prev_T = unix_sec0 + (int64_t)n_ticks - 1; }
-  }
-  cudaFree(d_stats);
-  if (h->track) {  // the run applied what its drain noted: start again from the flags
-    const int rs = seed_changes(h, h->stream, 0, h->cap_padded);
-    if (rc == AM_OK) rc = rs;
-  }
-  return rc;
+    return AM_OK;
+  });
 }
 
 int am_sweep_simulate(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint32_t mode, uint64_t seed,
@@ -1615,122 +1666,71 @@ int am_sweep_simulate(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint32
     return AM_E_INVAL;
   }
   if (n_ticks == 0) return AM_OK;
-  int rc = set_stream(h, h->stream);
-  if (rc != AM_OK) return rc;
-  h->to_ran = false;  // (the timed-out lists and the list of status changes are empty afterwards)
-  h->chg_listed = h->chg_fetched = false;
   // The staged calls come first; their results stay pending in the flags for the first tick (after its simulated posts,
   // which only ever replace a slot's bit group, as a later post_result would).
-  rc = drain_staged(h, h->stream);
+  int rc = begin_run(h, nullptr, seed);
   if (rc != AM_OK) return rc;
-  h->seed = seed;
   const SimDraw q{seed, params->wf_min, params->wf_max - params->wf_min + 1, params->remedy_min,
                   params->remedy_max - params->remedy_min + 1};
   const bool blocked = (mode & AM_SWEEP_BLOCKED) != 0;
-  const uint64_t n_seg = (h->n_records + kRecPerWarp - 1) / kRecPerWarp;
   if (!blocked && !h->sim_end) AM_CUDA(h, dev_array(h, &h->sim_end, h->cap_padded / kRecPerWarp * 8, h->stream, false));
-  am_tick_stats_t* d_stats = nullptr;
-  AM_CUDA(h, cudaMalloc((void**)&d_stats, n_ticks * (sizeof(am_tick_stats_t) + sizeof(am_sim_tick_t))));
-  unsigned long long* d_sim = reinterpret_cast<unsigned long long*>(d_stats + n_ticks);
-  if (cudaError_t e = cudaMemsetAsync(d_stats, 0, n_ticks * (sizeof(am_tick_stats_t) + sizeof(am_sim_tick_t)), h->stream);
-      e != cudaSuccess) {
-    h->last_error = cudaGetErrorString(e);
-    cudaFree(d_stats);
-    return AM_E_DEVICE;
-  }
-  if (cudaError_t e = cudaEventRecord(h->ev0, h->stream); e != cudaSuccess) {
-    h->last_error = cudaGetErrorString(e);
-    rc = AM_E_DEVICE;
-  }
-  auto launched = [&]() {
-    h->launches++;
-    if (cudaError_t e = cudaGetLastError(); e != cudaSuccess) { h->last_error = cudaGetErrorString(e); rc = AM_E_DEVICE; }
-  };
-  // Blocked: sweep_block_kernel<false, true>, blocks cut as in am_sweep_run_ticks.
-  uint64_t block_ticks = kDefaultBlockTicks;
-  if (const char* e = getenv("AMSWEEP_BLOCK_TICKS")) { long v = atol(e); if (v >= 1 && v <= kMaxBlockTicks) block_ticks = (uint64_t)v; }
-  for (uint64_t k = 0; blocked && h->n_records && k < n_ticks && rc == AM_OK;) {
-    const int64_t T = unix_sec0 + (int64_t)k;
-    rc = refresh_zones(h, T, h->stream);
-    if (rc != AM_OK) break;
-    uint64_t K = n_ticks - k < block_ticks ? n_ticks - k : block_ticks;
-    if (h->tz_n > 1 && h->tz_hi < T + (int64_t)K) K = (uint64_t)(h->tz_hi - T);  // (tz_hi > T after the refresh)
-    SimBlockParams b{};
-    b.c = h->cols;
-    b.n_records = h->n_records;
-    b.shard_base = h->shard_base;
-    b.seed = h->seed;
-    b.T0 = T;
-    b.K = (uint32_t)K;
-    b.tz_off = h->tz_n > 1 ? (const int32_t*)h->tz_off.dev : nullptr;
-    b.stats = reinterpret_cast<unsigned long long*>(d_stats + k);
-    b.since = h->since;
-    if (h->wf_timeout) {
-      b.deadline = h->deadline;
-      b.wf_timeout = h->wf_timeout;
-      b.seg_deadline = h->seg_deadline;
+  rc = run_rows(h, unix_sec0, n_ticks, blocked, true, stats_out, sim_out, [&](const RunRows& rows) -> int {
+    if (blocked) {  // sweep_block_kernel<false, true>; an empty shard launches nothing
+      if (h->n_records == 0) return AM_OK;
+      SimBlockParams sb{};
+      sb.since = h->since;
+      if (h->wf_timeout) {
+        sb.deadline = h->deadline;
+        sb.wf_timeout = h->wf_timeout;
+        sb.seg_deadline = h->seg_deadline;
+      }
+      sb.q = q;
+      return run_blocks(h, unix_sec0, n_ticks, rows.stats, sb, [&](SimBlockParams& b, uint64_t k, unsigned grid) {
+        b.sim = rows.sim + k * 4;
+        void (*const block_fn)(const SimBlockParams) = sweep_block_kernel<false, true>;
+        AM_LAUNCH(block_fn, grid, kBlockThreads, h->stream, b);
+      });
     }
-    b.q = q;
-    b.sim = d_sim + k * 4;
-    const unsigned grid = (unsigned)((h->n_records + kBlockRecords - 1) / kBlockRecords);
-    void (*const block_fn)(const SimBlockParams) = sweep_block_kernel<false, true>;
-    AM_LAUNCH(block_fn, grid, kBlockThreads, h->stream, b);
-    launched();
-    k += K;
-  }
-  // Tick by tick: the completion pass, then the tick (expiry pass and sweep), then the bounds of the runs it started
-  // and the tick's counts.
-  if (!blocked && rc == AM_OK) {
+    // Tick by tick: the completion pass, then the tick (expiry pass and sweep), then the bounds of the runs it started
+    // and the tick's counts.
+    const uint64_t n_seg = (h->n_records + kRecPerWarp - 1) / kRecPerWarp;
+    const int64_t earliest = params->wf_min < params->remedy_min ? params->wf_min : params->remedy_min;
     AM_CUDA(h, cudaMemsetAsync(h->sim_end, 0xFF, h->cap_padded / kRecPerWarp * 8, h->stream));
     if (h->n_records) {
       AM_LAUNCH(sim_bounds_kernel, (unsigned)((h->n_records + 255) / 256), 256, h->stream, h->cols, (const int64_t*)h->since,
                 h->sim_end, h->n_records, q, h->shard_base);
-      launched();
+      h->launches++;
+      AM_CUDA(h, cudaGetLastError());
     }
-  }
-  const int64_t earliest = params->wf_min < params->remedy_min ? params->wf_min : params->remedy_min;
-  for (uint64_t k = 0; !blocked && k < n_ticks && rc == AM_OK; ++k) {
-    const int64_t T = unix_sec0 + (int64_t)k;
-    if (n_seg) {
-      AM_LAUNCH_PDL(sim_complete_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream, h->cols, h->since, h->sim_end,
-                    (uint32_t)n_seg, T, q, h->shard_base);
-      launched();
-    }
-    if (rc == AM_OK) rc = expire_runs(h, h->stream, T);
-    const int parity = (int)h->parity;
-    const ListOut o{h->due_idx[k & 1], h->due_action[k & 1], h->cap_padded, nullptr, d_stats + k};
-    if (rc == AM_OK) rc = launch_tick(h, T, mode & AM_SWEEP_FULL_SCAN, o, h->stream);
-    if (rc == AM_OK && n_seg) {
-      AM_LAUNCH_PDL(sim_note_starts_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream,
-                    (const uint32_t*)h->set[parity].out.bitmap, h->sim_end, (uint32_t)n_seg, T + earliest);
-      launched();
-    }
-    if (rc == AM_OK) {
+    for (uint64_t k = 0; k < n_ticks; ++k) {
+      const int64_t T = unix_sec0 + (int64_t)k;
+      if (n_seg) {
+        AM_LAUNCH_PDL(sim_complete_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream, h->cols, h->since, h->sim_end,
+                      (uint32_t)n_seg, T, q, h->shard_base);
+        h->launches++;
+        AM_CUDA(h, cudaGetLastError());
+      }
+      int trc = expire_runs(h, h->stream, T);
+      if (trc != AM_OK) return trc;
+      const int parity = (int)h->parity;
+      const ListOut o{h->due_idx[k & 1], h->due_action[k & 1], h->cap_padded, nullptr, rows.stats + k};
+      trc = launch_tick(h, T, mode & AM_SWEEP_FULL_SCAN, o, h->stream);
+      if (trc != AM_OK) return trc;
+      if (n_seg) {
+        AM_LAUNCH_PDL(sim_note_starts_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream,
+                      (const uint32_t*)h->set[parity].out.bitmap, h->sim_end, (uint32_t)n_seg, T + earliest);
+        h->launches++;
+        AM_CUDA(h, cudaGetLastError());
+      }
       AM_LAUNCH_PDL(sim_count_kernel, h->sms * 8, 256, h->stream, h->cols, (const int64_t*)h->since, h->n_records,
                     (const int64_t*)(h->to_ran ? h->to_since : nullptr), (const uint32_t*)(h->to_ran ? h->to_count : nullptr),
-                    d_sim + k * 4);
-      launched();
+                    rows.sim + k * 4);
+      h->launches++;
+      AM_CUDA(h, cudaGetLastError());
     }
-  }
-  h->to_ran = false;
-  if (rc == AM_OK) {
-    cudaError_t e = cudaEventRecord(h->ev1, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e == cudaSuccess) e = cudaMemcpy(stats_out, d_stats, n_ticks * sizeof(am_tick_stats_t), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && sim_out) e = cudaMemcpy(sim_out, d_sim, n_ticks * sizeof(am_sim_tick_t), cudaMemcpyDeviceToHost);
-    float ms = 0;
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-    if (e != cudaSuccess) { h->last_error = cudaGetErrorString(e); rc = AM_E_DEVICE; }
-    else h->last_ms = ms;
-    if (rc == AM_OK)
-      for (uint64_t k = 0; k < n_ticks; ++k) stats_out[k].n_records = h->n_records;
-    if (rc == AM_OK) { h->has_prev = true; h->prev_T = unix_sec0 + (int64_t)n_ticks - 1; }
-  }
-  cudaFree(d_stats);
-  if (h->track) {  // the ticks applied what the drains noted: start again from the flags
-    const int rs = seed_changes(h, h->stream, 0, h->cap_padded);
-    if (rc == AM_OK) rc = rs;
-  }
+    return AM_OK;
+  });
+  h->to_ran = false;  // (the timed-out lists are empty afterwards, as the list of status changes is)
   return rc;
 }
 
@@ -1901,6 +1901,42 @@ static int change_page(am_sweep_t* h, bool listed, uint64_t offset, uint64_t cap
   return list_page(listed ? h->chg_n : 0, offset, cap, n_out, ncopy);
 }
 
+// The bytes gather_cols fills for n slots: each requested column of `cols` (may be NULL), 8-B aligned.
+static size_t gather_bytes(uint64_t n, const am_record_cols_t* cols) {
+  size_t bytes = 0;
+  for (int k = 0; k < 16; ++k)
+    if (cols && *cols_member(cols, k)) bytes += (n * kColElem[k] + 7) / 8 * 8;
+  return bytes;
+}
+
+// The requested columns of `cols` (may be NULL) at the n slots d_idx[0..n) (device memory), into the caller's arrays:
+// gathered column by column into dev_in, copied to pin_in (both at least gather_bytes(n, cols) already, and what the
+// caller keeps there lies past that), one synchronisation, then scattered.
+static int gather_cols(am_sweep_t* h, const uint32_t* d_idx, uint64_t n, am_record_cols_t* cols) {
+  GatherCols gc{};
+  size_t at[16], bytes = 0;
+  unsigned nc = 0;
+  for (int k = 0; k < 16; ++k) {
+    if (!cols || !*cols_member(cols, k)) continue;
+    at[nc] = bytes;
+    gc.src[nc] = *col_slot(h->cols, k);
+    gc.dst[nc] = (char*)h->dev_in.p + bytes;
+    gc.elem[nc] = (uint32_t)kColElem[k];
+    bytes += (n * kColElem[k] + 7) / 8 * 8;
+    ++nc;
+  }
+  if (nc) {
+    AM_LAUNCH(gather_columns_kernel, dim3((unsigned)((n + 255) / 256), nc), 256, h->stream, gc, d_idx, (uint32_t)n);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, bytes, cudaMemcpyDeviceToHost, h->stream));
+  }
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  for (int k = 0, c = 0; k < 16; ++k)
+    if (cols && *cols_member(cols, k)) memcpy(*cols_member(cols, k), (const char*)h->pin_in.p + at[c++], n * kColElem[k]);
+  return AM_OK;
+}
+
 int am_sweep_last_timed_out(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t* since, uint64_t cap, uint64_t* n_out) {
   return timed_out_impl(h, offset, idx, since, cap, n_out, false);
 }
@@ -1925,38 +1961,16 @@ int am_sweep_last_changes(am_sweep_t* h, uint64_t offset, uint64_t* idx, am_reco
   const int page = change_page(h, h->chg_listed, offset, cap, n_out, &ncopy);
   if (page != AM_OK && page != AM_E_NOSPACE) return page;
   if (ncopy) {
-    // pin_in / dev_in: the list's entries, then each requested column (8-B aligned), gathered on the device
-    GatherCols gc{};
-    size_t at[16], bytes = (ncopy * 4 + 7) / 8 * 8;
-    unsigned nc = 0;
-    for (int k = 0; k < 16; ++k) {
-      if (!cols || !*cols_member(cols, k)) continue;
-      at[nc] = bytes;
-      gc.src[nc] = *col_slot(h->cols, k);
-      gc.elem[nc] = (uint32_t)kColElem[k];
-      bytes += (ncopy * kColElem[k] + 7) / 8 * 8;
-      ++nc;
-    }
-    AM_CUDA(h, h->pin_in.reserve(bytes));
-    AM_CUDA(h, h->dev_in.reserve(bytes));
+    // pin_in / dev_in: the requested columns, then (pin_in only) the list's entries
+    const size_t at = gather_bytes(ncopy, cols);
+    AM_CUDA(h, h->pin_in.reserve(at + ncopy * 4));
+    AM_CUDA(h, h->dev_in.reserve(at));
     const uint32_t* d_idx = h->chg_list + offset;
-    for (unsigned c = 0; c < nc; ++c) gc.dst[c] = (char*)h->dev_in.p + at[c];
-    if (nc) {
-      AM_LAUNCH(gather_columns_kernel, dim3((unsigned)((ncopy + 255) / 256), nc), 256, h->stream, gc, d_idx, (uint32_t)ncopy);
-      h->launches++;
-      AM_CUDA(h, cudaGetLastError());
-      AM_CUDA(h, cudaMemcpyAsync((char*)h->pin_in.p + at[0], (char*)h->dev_in.p + at[0], bytes - at[0],
-                                 cudaMemcpyDeviceToHost, h->stream));
-    }
-    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, d_idx, ncopy * 4, cudaMemcpyDeviceToHost, h->stream));
-    AM_CUDA(h, cudaStreamSynchronize(h->stream));
-    const uint32_t* li = (const uint32_t*)h->pin_in.p;
+    AM_CUDA(h, cudaMemcpyAsync((char*)h->pin_in.p + at, d_idx, ncopy * 4, cudaMemcpyDeviceToHost, h->stream));
+    rc = gather_cols(h, d_idx, ncopy, cols);  // (synchronises)
+    if (rc != AM_OK) return rc;
+    const uint32_t* li = (const uint32_t*)((const char*)h->pin_in.p + at);
     for (uint64_t k = 0; k < ncopy; ++k) idx[k] = h->shard_base + li[k];
-    for (int k = 0, c = 0; k < 16; ++k) {
-      void* dst = cols ? *cols_member(cols, k) : nullptr;
-      if (!dst) continue;
-      memcpy(dst, (const char*)h->pin_in.p + at[c++], ncopy * kColElem[k]);
-    }
   }
   return page;
 }
@@ -2014,34 +2028,8 @@ static int read_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* 
   for (uint64_t k = 0; k < n; ++k)
     if (idx[k] >= h->capacity) return AM_E_RANGE;
   const uint32_t* d_idx;
-  const int rc = stage_indices(h, n * sizeof(am_record_t), n, idx, &d_idx);
-  if (rc != AM_OK) return rc;
-  AM_LAUNCH(gather_records_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols, d_idx, (am_record_t*)h->dev_in.p,
-            (uint32_t)n);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * sizeof(am_record_t), cudaMemcpyDeviceToHost, h->stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  const am_record_t* r = (const am_record_t*)h->pin_in.p;
-  for (uint64_t k = 0; k < n; ++k) {
-    if (out->minute) out->minute[k] = r[k].minute;
-    if (out->hour) out->hour[k] = r[k].hour;
-    if (out->dom) out->dom[k] = r[k].dom;
-    if (out->month) out->month[k] = r[k].month;
-    if (out->dow) out->dow[k] = r[k].dow;
-    if (out->ras) out->ras[k] = r[k].ras;
-    if (out->flags) out->flags[k] = r[k].flags;
-    if (out->finished_at) out->finished_at[k] = r[k].finished_at;
-    if (out->runs_limit) out->runs_limit[k] = r[k].runs_limit;
-    if (out->reset_interval) out->reset_interval[k] = r[k].reset_interval;
-    if (out->success) out->success[k] = r[k].success;
-    if (out->failed) out->failed[k] = r[k].failed;
-    if (out->remedy_success) out->remedy_success[k] = r[k].remedy_success;
-    if (out->remedy_failed) out->remedy_failed[k] = r[k].remedy_failed;
-    if (out->remedy_total) out->remedy_total[k] = r[k].remedy_total;
-    if (out->remedy_finished_at) out->remedy_finished_at[k] = r[k].remedy_finished_at;
-  }
-  return AM_OK;
+  const int rc = stage_indices(h, gather_bytes(n, out), n, idx, &d_idx);
+  return rc != AM_OK ? rc : gather_cols(h, d_idx, n, out);
 }
 
 }  // extern "C"
@@ -2143,15 +2131,16 @@ uint32_t ckpt_switches(const am_sweep* h) {
 int ckpt_alloc(am_sweep* h) {
   AM_CUDA(h, cudaSetDevice(h->device));
   if (h->ck_dev) return AM_OK;
-  AM_CUDA(h, cudaStreamCreateWithFlags(&h->ck_stream, cudaStreamNonBlocking));
-  AM_CUDA(h, cudaEventCreateWithFlags(&h->ck_ev, cudaEventDisableTiming));
+  AM_CUDA(h, new_stream(h, &h->ck_stream));
+  AM_CUDA(h, new_event(h, &h->ck_ev));
   for (int k = 0; k < 2; ++k) {
-    AM_CUDA(h, cudaEventCreateWithFlags(&h->ck_pin_ev[k], cudaEventDisableTiming));
-    AM_CUDA(h, cudaHostAlloc((void**)&h->ck_pin[k], kCkChunk, cudaHostAllocDefault));
+    AM_CUDA(h, new_event(h, &h->ck_pin_ev[k]));
+    AM_CUDA(h, host_array(h, &h->ck_pin[k], kCkChunk));
   }
-  AM_CUDA(h, cudaHostAlloc((void**)&h->ck_meta_h, 5 * 8, cudaHostAllocDefault));
-  AM_CUDA(h, cudaMalloc((void**)&h->ck_meta, 5 * 8));
-  AM_CUDA(h, cudaMalloc((void**)&h->ck_dev, ckpt_layout(h->cap_padded, kCkAllSwitches).sections_end));  // (the last)
+  AM_CUDA(h, host_array(h, &h->ck_meta_h, 5 * 8));
+  AM_CUDA(h, dev_array(h, &h->ck_meta, 5 * 8, h->ck_stream, false));
+  const uint64_t blob = ckpt_layout(h->cap_padded, kCkAllSwitches).sections_end;
+  AM_CUDA(h, dev_array(h, &h->ck_dev, blob, h->ck_stream, false));  // (the last)
   return AM_OK;
 }
 

@@ -1926,7 +1926,8 @@ __global__ void gather_details_kernel(const uint32_t* __restrict__ idx, uint32_t
   dst[k] = d;
 }
 
-// am_sweep_last_changes: the requested columns of the listed slots idx[0..n), column-major into dst[c] (blockIdx.y = c).
+// am_sweep_read by index and am_sweep_last_changes: the requested columns of the listed slots idx[0..n), column-major
+// into dst[c] (blockIdx.y = c).
 struct GatherCols {
   const void* src[16];
   void* dst[16];
@@ -1938,22 +1939,6 @@ __global__ void gather_columns_kernel(const GatherCols g, const uint32_t* __rest
   const uint32_t c = blockIdx.y, i = idx[k];
   if (g.elem[c] == 8u) ((uint64_t*)g.dst[c])[k] = ((const uint64_t*)g.src[c])[i];
   else ((uint32_t*)g.dst[c])[k] = ((const uint32_t*)g.src[c])[i];
-}
-
-__global__ void gather_records_kernel(DevCols c, const uint32_t* __restrict__ idx, am_record_t* out,
-                                      uint32_t n) {
-  uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= n) return;
-  const uint32_t i = idx[k];
-  am_record_t r;
-  r.minute = c.minute[i]; r.hour = c.hour[i]; r.dom = c.dom[i]; r.month = c.month[i]; r.dow = c.dow[i];
-  r.finished_at = c.finished_at[i]; r.remedy_finished_at = c.remedy_finished_at[i];
-  r.ras = c.ras[i]; r.flags = c.flags[i];
-  r.runs_limit = c.runs_limit[i]; r.reset_interval = c.reset_interval[i];
-  r.success = c.success[i]; r.failed = c.failed[i]; r.remedy_success = c.remedy_success[i];
-  r.remedy_failed = c.remedy_failed[i]; r.remedy_total = c.remedy_total[i];
-  r.wf_timeout = 0;  // (not returned by am_sweep_read)
-  out[k] = r;
 }
 
 }  // namespace amsweep
