@@ -125,6 +125,7 @@ class AmSimParams(C.Structure):
 
 CHECKPOINT_VERSION = 1
 CKPT_HOLD, CKPT_REMEDY, CKPT_TRACK, CKPT_DETAILS, CKPT_TIMEOUTS = 0x1, 0x2, 0x4, 0x8, 0x10
+CKPT_ADMISSION = 0x20
 
 
 class AmCheckpointInfo(C.Structure):
@@ -134,6 +135,12 @@ class AmCheckpointInfo(C.Structure):
     def as_dict(self) -> dict:
         return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "reserved"}
 
+
+class AmAdmission(C.Structure):
+    _fields_ = [("n_candidates", u64), ("n_admitted", u64), ("n_deferred", u64), ("oldest_deferred", i64)]
+
+
+UNLIMITED = (1 << 64) - 1  # am_sweep_set_submit_budget: no budget
 
 SIM_FIELDS = ["n_in_flight", "n_remedy_in_flight", "n_timed_out", "n_remedy_timed_out"]
 SIM_DTYPE = np.dtype([(n, "<u8") for n in SIM_FIELDS])
@@ -174,6 +181,9 @@ SYMBOLS = {
     "am_sweep_last_timed_out": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
     "am_sweep_set_hold_remedy": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_remedy_in_flight": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, C.c_void_p]),
+    "am_sweep_set_submit_budget": (C.c_int, [C.c_void_p, u64]),
+    "am_sweep_last_admission": (C.c_int, [C.c_void_p, P(AmAdmission)]),
+    "am_sweep_deferred": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, C.c_void_p]),
     "am_sweep_last_remedy_timed_out": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
     "am_sweep_set_track_changes": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_last_changes": (C.c_int, [C.c_void_p, u64, C.c_void_p, P(AmRecordCols), u64, P(u64)]),

@@ -22,11 +22,13 @@ enum CkptSection : int {
   kCkSecChanged,         // 1 bit per slot in u32 words, while tracking is on
   kCkSecDetApplied,      // u8, while details are on
   kCkSecDetStart,        // i64, while details are on
+  kCkSecWait,            // i64, with the submit budget's admission state: the second since which the slot waits
   kCkSections
 };
 // element bytes per section (0: the bit section)
 AM_HD constexpr uint32_t ck_elem(int s) {
-  return (s < 5 || s == 7 || s == 15 || s == kCkSecDeadline || s == kCkSecSince || s == kCkSecDetStart) ? 8
+  return (s < 5 || s == 7 || s == 15 || s == kCkSecDeadline || s == kCkSecSince || s == kCkSecDetStart ||
+          s == kCkSecWait) ? 8
          : s == kCkSecChanged ? 0 : s == kCkSecDetApplied ? 1 : 4;
 }
 
@@ -53,6 +55,7 @@ struct CkptState {
   uint32_t* changed;
   uint8_t* det_applied;
   int64_t* det_start;
+  int64_t* wait;  // the submit budget's waiting seconds
 };
 
 template <class T>
@@ -130,6 +133,11 @@ __global__ void __launch_bounds__(256) checkpoint_pack_kernel(const CkptState s,
       reinterpret_cast<int64_t*>(b.p + b.off[kCkSecDetStart])[j] = t;
       acc += ckpt_mix((b.off[kCkSecDetApplied] + j) * 8, a) + ck_term(b, kCkSecDetStart, j, t);
     }
+    if (b.off[kCkSecWait]) {
+      const int64_t v = s.wait[i];
+      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecWait])[j] = v;
+      acc += ck_term(b, kCkSecWait, j, v);
+    }
   }
   if (b.off[kCkSecChanged]) {  // (warp-uniform)
     const uint32_t bit = in ? (s.changed[i >> 5] >> (i & 31)) & 1u : 0u;
@@ -205,6 +213,7 @@ __global__ void __launch_bounds__(256) checkpoint_scatter_kernel(const CkptState
     s.det_applied[i] = ck_blob_get<uint8_t>(b, kCkSecDetApplied, j);
     s.det_start[i] = ck_blob_get<int64_t>(b, kCkSecDetStart, j);
   }
+  if (s.wait) s.wait[i] = ck_blob_get<int64_t>(b, kCkSecWait, j);
 }
 
 }  // namespace amsweep

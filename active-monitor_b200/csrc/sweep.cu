@@ -41,6 +41,7 @@
 #include <utility>
 #include <vector>
 
+#include "admission_kernels.cuh"
 #include "checkpoint_kernels.cuh"
 #include "sweep_internal.h"
 #include "sweep_kernels.cuh"
@@ -255,6 +256,20 @@ struct am_sweep {
   char* ck_pin[2] = {nullptr, nullptr};
   cudaEvent_t ck_pin_ev[2] = {nullptr, nullptr};
   bool ck_pin_pending[2] = {false, false};
+  // submit budget (am_sweep_set_submit_budget, only with the hold): the most SUBMIT_HC entries a tick emits, and the
+  // admission state, allocated at the first finite budget (admission_kernels.cuh): per slot the second since which it
+  // waits, the FIFO of waiting slots and this tick's kept and new ones, a byte per FIFO entry, one bit per slot of
+  // fresh submissions, the per-group and per-chunk counts and the counters
+  uint64_t budget = UINT64_MAX;
+  int64_t* adm_wait = nullptr;
+  uint32_t* adm_fifo = nullptr;
+  uint32_t* adm_keep = nullptr;
+  uint32_t* adm_fresh = nullptr;
+  uint8_t* adm_cand = nullptr;
+  uint32_t* adm_sub = nullptr;
+  uint32_t* adm_group_sub = nullptr;
+  uint32_t* adm_chunk = nullptr;
+  AdmCtl* adm_ctl = nullptr;
 };
 
 namespace {
@@ -481,6 +496,110 @@ int alloc_timeouts(am_sweep* h, cudaStream_t s) {
   return drop_deadlines(h, s, 0, cap, true);
 }
 
+// Submit budget: the admission passes run while the hold is on and the admission state exists.
+bool admission_on(const am_sweep* h) { return h->hold && h->adm_ctl; }
+
+// No slot waits for admission, the FIFO is empty, the last tick's numbers are zero (the oldest second INT64_MAX).
+int reset_admission(am_sweep* h, cudaStream_t s) {
+  AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, s, h->adm_wait, kNotWaiting, h->cap_padded);
+  h->launches++;
+  AM_CUDA(h, cudaGetLastError());
+  AdmCtl z{};
+  z.oldest = INT64_MAX;
+  AM_CUDA(h, cudaMemcpyAsync(h->adm_ctl, &z, sizeof z, cudaMemcpyHostToDevice, s));  // (pageable: copied before the return)
+  return AM_OK;
+}
+
+// The admission state, allocated at the first finite budget: 21.14 B per slot of capacity (the waiting second 8, the FIFO
+// and a tick's kept and new slots 12, a byte per FIFO entry, a bit of fresh submissions, 4 B per FIFO chunk).
+int alloc_admission(am_sweep* h, cudaStream_t s) {
+  const size_t cap = h->cap_padded, ngroups = groups_of(cap);
+  AM_CUDA(h, dev_array(h, &h->adm_wait, cap * 8, s, false));
+  AM_CUDA(h, dev_array(h, &h->adm_fifo, cap * 4, s, false));
+  AM_CUDA(h, dev_array(h, &h->adm_keep, cap * 4, s, false));
+  AM_CUDA(h, dev_array(h, &h->adm_fresh, cap * 4, s, false));
+  AM_CUDA(h, dev_array(h, &h->adm_cand, cap, s, false));
+  AM_CUDA(h, dev_array(h, &h->adm_sub, ngroups * kGroupWords * 4, s, false));
+  AM_CUDA(h, dev_array(h, &h->adm_group_sub, ngroups * 4, s, false));
+  AM_CUDA(h, dev_array(h, &h->adm_chunk, (cap / kAdmBlock + 1) * 4, s, false));
+  AM_CUDA(h, dev_array(h, &h->adm_ctl, sizeof(AdmCtl), s, false));
+  return reset_admission(h, s);
+}
+
+// Whether a slot waits for admission, as the waits stand after the last drain (FIFO entries whose slot stopped waiting
+// do not count): one pass over the FIFO and one read-back.
+int admission_waiting(am_sweep* h, bool* out) {
+  *out = false;
+  if (!admission_on(h)) return AM_OK;
+  const int rc = set_stream(h, h->stream);
+  if (rc != AM_OK) return rc;
+  AM_CUDA(h, h->dev_in.reserve(8));
+  AM_CUDA(h, h->pin_in.reserve(8));
+  AM_CUDA(h, cudaMemsetAsync(h->dev_in.p, 0xFF, 8, h->stream));
+  AM_LAUNCH(adm_next_due_kernel, h->sms * 4, 256, h->stream, (const uint32_t*)h->adm_fifo, (const int64_t*)h->adm_wait,
+            (const AdmCtl*)h->adm_ctl, (int64_t)0, (unsigned long long*)h->dev_in.p);
+  h->launches++;
+  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, 8, cudaMemcpyDeviceToHost, h->stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  *out = *(const unsigned long long*)h->pin_in.p != ~0ull;
+  return AM_OK;
+}
+
+// The FIFO rebuilt from the waiting seconds of the swept slots, in admission order (second, then slot), on the host: a
+// restore places waits anywhere in the order.  The last tick's counts become those of an empty tick with this backlog.
+int rebuild_admission_fifo(am_sweep* h) {
+  std::vector<int64_t> wait(h->n_records);
+  if (h->n_records)
+    AM_CUDA(h, cudaMemcpy(wait.data(), h->adm_wait, h->n_records * 8, cudaMemcpyDeviceToHost));
+  std::vector<uint32_t> fifo;
+  for (uint64_t i = 0; i < h->n_records; ++i)
+    if (wait[i] != kNotWaiting) fifo.push_back((uint32_t)i);
+  std::stable_sort(fifo.begin(), fifo.end(), [&](uint32_t a, uint32_t b) { return wait[a] < wait[b]; });
+  if (!fifo.empty()) AM_CUDA(h, cudaMemcpy(h->adm_fifo, fifo.data(), fifo.size() * 4, cudaMemcpyHostToDevice));
+  AdmCtl q{};
+  q.n_fifo = q.n_deferred = fifo.size();
+  q.oldest = fifo.empty() ? INT64_MAX : wait[fifo[0]];
+  AM_CUDA(h, cudaMemcpy(h->adm_ctl, &q, sizeof q, cudaMemcpyHostToDevice));
+  return AM_OK;
+}
+
+// A tick's admission passes, between its sweep and scan_groups_kernel, over buffer set `ts` (admission_kernels.cuh).
+int launch_admission(am_sweep* h, int64_t T, const TickSet& ts, cudaStream_t s) {
+  AdmParams a{};
+  a.out = ts.out;
+  a.n_groups = groups_of(h->n_records);
+  a.n_tiles = tiles_of(h->n_records);
+  a.c = h->cols;
+  a.since = h->since;
+  if (h->wf_timeout) {
+    a.deadline = h->deadline;
+    a.wf_timeout = h->wf_timeout;
+    a.seg_deadline = h->seg_deadline;
+  }
+  a.wait = h->adm_wait;
+  a.fifo = h->adm_fifo;
+  a.keep = h->adm_keep;
+  a.fresh = h->adm_fresh;
+  a.cand = h->adm_cand;
+  a.sub = h->adm_sub;
+  a.group_sub = h->adm_group_sub;
+  a.chunk = h->adm_chunk;
+  a.ctl = h->adm_ctl;
+  a.budget = h->budget;
+  a.T = T;
+  const unsigned grid = (unsigned)h->sms * 4;  // (the per-entry passes loop over the backlog's chunks)
+  AM_LAUNCH(adm_masks_kernel, a.n_groups, kGroupWords, s, a);
+  AM_LAUNCH(adm_check_kernel, grid, kAdmBlock, s, a);
+  AM_LAUNCH(adm_plan_kernel, 1, 1024, s, a);
+  AM_LAUNCH(adm_fifo_kernel, grid, kAdmBlock, s, a);
+  AM_LAUNCH(adm_fresh_kernel, a.n_groups, kGroupWords, s, a);
+  AM_LAUNCH(adm_merge_kernel, grid, 256, s, a);
+  h->launches += 6;
+  AM_CUDA(h, cudaGetLastError());
+  return AM_OK;
+}
+
 // A tick's expiry pass (expire_runs_kernel), while the hold is on and the timeout state exists.  Every tick that gets
 // as far as its drain resets the timed-out list.
 int expire_runs(am_sweep* h, cudaStream_t s, int64_t T) {
@@ -643,6 +762,10 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   }
   if (h->hold) {  // a posted workflow phase or a remove ends the slot's run (an upsert keeps the hold)
     AM_LAUNCH_PDL(clear_since_kernel, G, B, s, h->since, d_ops, (uint32_t)n);
+    h->launches++;
+  }
+  if (admission_on(h)) {  // ... and ends the slot's wait for admission (its FIFO entry is dropped at the next tick)
+    AM_LAUNCH_PDL(clear_since_kernel, G, B, s, h->adm_wait, d_ops, (uint32_t)n);
     h->launches++;
   }
   // Workflow timeouts expire here, ahead of the result kernels: a remedy phase posted alone in this drain is then
@@ -887,6 +1010,10 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   if (o.expand) AM_LAUNCH_PDL(sweep, p.n_tiles, kBlock, s, p);
   else AM_LAUNCH(sweep, p.n_tiles, kBlock, s, p);
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[1], s));
+  if (admission_on(h)) {  // the submit budget cuts the sweep's output in place (profiling: counted in the rest)
+    const int rc = launch_admission(h, T, ts, s);
+    if (rc != AM_OK) return rc;
+  }
   ScanParams sc{};
   sc.group_count = ts.out.group_count;
   sc.group_prefix = ts.out.group_prefix;
@@ -1315,6 +1442,11 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
     h->launches++;
     AM_CUDA(h, cudaGetLastError());
   }
+  if (admission_on(h)) {  // ... and wait for nothing
+    AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, h->stream, h->adm_wait + first, kNotWaiting, n);
+    h->launches++;
+    AM_CUDA(h, cudaGetLastError());
+  }
   if (h->wf_timeout) {  // am_record_cols_t has no timeout column: loaded slots have none, and no deadline
     AM_CUDA(h, cudaMemsetAsync(h->wf_timeout + first, 0, n * 4, h->stream));
     rc = drop_deadlines(h, h->stream, first, n, false);
@@ -1346,8 +1478,51 @@ int am_sweep_set_hold_in_flight(am_sweep_t* h, int on) {
       if (rc != AM_OK) return rc;
     }
   }
+  if (h->adm_ctl) {  // every wait for admission ends
+    int rc = set_stream(h, h->stream);
+    if (rc == AM_OK) rc = reset_admission(h, h->stream);
+    if (rc != AM_OK) return rc;
+  }
+  h->budget = UINT64_MAX;
   h->hold = on != 0;
   if (!on) h->remedy = false;  // (the since words are refilled when the hold is turned on again)
+  return AM_OK;
+}
+
+int am_sweep_set_submit_budget(am_sweep_t* h, uint64_t per_tick) {
+  if (!h) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if (!h->hold) {
+    h->last_error = "am_sweep_set_submit_budget while the hold in flight is off";
+    return AM_E_INVAL;
+  }
+  if (per_tick != UINT64_MAX && !h->adm_ctl) {
+    int rc = set_stream(h, h->stream);
+    if (rc == AM_OK) rc = alloc_admission(h, h->stream);
+    if (rc != AM_OK) return rc;
+  }
+  h->budget = per_tick;
+  return AM_OK;
+}
+
+int am_sweep_last_admission(am_sweep_t* h, am_admission_t* out) {
+  if (!h || !out) return AM_E_INVAL;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  if (!h->adm_ctl) {
+    h->last_error = "am_sweep_last_admission: the handle never had a finite submit budget";
+    return AM_E_INVAL;
+  }
+  int rc = set_stream(h, h->stream);  // (after a device tick: waits for it)
+  if (rc != AM_OK) return rc;
+  AdmCtl q{};
+  AM_CUDA(h, cudaMemcpyAsync(&q, h->adm_ctl, sizeof q, cudaMemcpyDeviceToHost, h->stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  out->n_candidates = q.n_candidates;
+  out->n_admitted = q.n_admitted;
+  out->n_deferred = q.n_deferred;
+  out->oldest_deferred = q.oldest;
   return AM_OK;
 }
 
@@ -1665,6 +1840,15 @@ int am_sweep_simulate(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint32
     h->last_error = "am_sweep_simulate needs the hold in flight and the remedy hold on";
     return AM_E_INVAL;
   }
+  if (mode & AM_SWEEP_BLOCKED) {  // (the blocked kernel has no admission)
+    bool waiting = false;
+    const int brc = admission_waiting(h, &waiting);
+    if (brc != AM_OK) return brc;
+    if (waiting || h->budget != UINT64_MAX) {
+      h->last_error = "am_sweep_simulate: AM_SWEEP_BLOCKED with a finite submit budget or checks waiting for admission";
+      return AM_E_INVAL;
+    }
+  }
   if (n_ticks == 0) return AM_OK;
   // The staged calls come first; their results stay pending in the flags for the first tick (after its simulated posts,
   // which only ever replace a slot's bit group, as a later post_result would).
@@ -1796,6 +1980,11 @@ int am_sweep_next_due(am_sweep_t* h, int64_t unix_sec, int64_t* next_out) {
             (const int64_t*)(h->hold ? h->deadline : nullptr), h->n_records, unix_sec, zone_due,
             (unsigned long long*)h->dev_in.p);
   h->launches++;
+  if (admission_on(h)) {  // a check still waiting for admission is due at the next second
+    AM_LAUNCH(adm_next_due_kernel, h->sms * 4, 256, h->stream, (const uint32_t*)h->adm_fifo, (const int64_t*)h->adm_wait,
+              (const AdmCtl*)h->adm_ctl, unix_sec, (unsigned long long*)h->dev_in.p);
+    h->launches++;
+  }
   AM_CUDA(h, cudaGetLastError());
   AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, 8, cudaMemcpyDeviceToHost, h->stream));
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -1848,6 +2037,34 @@ int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t
 
 int am_sweep_remedy_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* started_out) {
   return in_flight_impl(h, first, n, idx, started_out, true);
+}
+
+int am_sweep_deferred(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
+  if (!h || (n && !since_out)) return AM_E_INVAL;
+  if (n == 0) return AM_OK;
+  if (n > 0xFFFFFFFFull || (!idx && (first + n > h->capacity || first + n < first))) return AM_E_INVAL;
+  if (idx)
+    for (uint64_t k = 0; k < n; ++k)
+      if (idx[k] >= h->capacity) return AM_E_RANGE;
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  int rc = begin_call(h);  // removes, loads and posted phases by now end their slots' waits
+  if (rc != AM_OK) return rc;
+  if (!admission_on(h)) {
+    for (uint64_t k = 0; k < n; ++k) since_out[k] = kNotWaiting;
+    return AM_OK;
+  }
+  const uint32_t* d_idx;
+  rc = stage_indices(h, n * 8, n, idx, &d_idx);
+  if (rc != AM_OK) return rc;
+  AM_LAUNCH(adm_gather_kernel, (unsigned)((n + 255) / 256), 256, h->stream, (const int64_t*)h->adm_wait, (uint32_t)first,
+            d_idx, (uint32_t)n, (int64_t*)h->dev_in.p);
+  h->launches++;
+  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * 8, cudaMemcpyDeviceToHost, h->stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  memcpy(since_out, h->pin_in.p, n * 8);
+  return AM_OK;
 }
 
 // One of the last tick's two timed-out lists, entries [offset, ...) as global indices: the health-check runs, or the
@@ -2039,7 +2256,8 @@ namespace {
 
 constexpr uint64_t kCkMagic = 0x54504B4357534D41ull;  // "AMSWCKPT"
 constexpr uint64_t kCkHeader = 128;
-constexpr uint32_t kCkAllSwitches = AM_CKPT_HOLD | AM_CKPT_REMEDY | AM_CKPT_TRACK | AM_CKPT_DETAILS | AM_CKPT_TIMEOUTS;
+constexpr uint32_t kCkAllSwitches =
+    AM_CKPT_HOLD | AM_CKPT_REMEDY | AM_CKPT_TRACK | AM_CKPT_DETAILS | AM_CKPT_TIMEOUTS | AM_CKPT_ADMISSION;
 constexpr size_t kCkChunk = 32u << 20;  // bytes per pinned chunk of a restore's upload
 
 struct CkptHeader {
@@ -2070,6 +2288,7 @@ CkptLayout ckpt_layout(uint64_t n, uint32_t switches) {
   if (switches & AM_CKPT_HOLD) put(kCkSecSince, n * 8);
   if (switches & AM_CKPT_TRACK) put(kCkSecChanged, (n + 31) / 32 * 4);
   if (switches & AM_CKPT_DETAILS) { put(kCkSecDetApplied, n); put(kCkSecDetStart, n * 8); }
+  if (switches & AM_CKPT_ADMISSION) put(kCkSecWait, n * 8);
   return L;
 }
 
@@ -2099,7 +2318,8 @@ int ckpt_parse(const void* buf, uint64_t len, CkptHeader* hd, CkptLayout* L, std
   memcpy(hd, p, kCkHeader);
   if (hd->magic != kCkMagic || hd->version != AM_CHECKPOINT_VERSION) return AM_E_INVAL;
   if ((hd->switches & ~kCkAllSwitches) || ((hd->switches & AM_CKPT_REMEDY) && !(hd->switches & AM_CKPT_HOLD)) ||
-      ((hd->switches & AM_CKPT_DETAILS) && !(hd->switches & AM_CKPT_TRACK)))
+      ((hd->switches & AM_CKPT_DETAILS) && !(hd->switches & AM_CKPT_TRACK)) ||
+      ((hd->switches & AM_CKPT_ADMISSION) && !(hd->switches & AM_CKPT_HOLD)))
     return AM_E_INVAL;
   if (hd->bytes > len || hd->bytes % 8 || hd->n > 0xFFFFFFFFull || hd->first_global + hd->n < hd->first_global ||
       hd->swept_end < hd->first_global || hd->swept_end > hd->first_global + hd->n || hd->n_zones > 255)
@@ -2124,7 +2344,8 @@ int ckpt_parse(const void* buf, uint64_t len, CkptHeader* hd, CkptLayout* L, std
 
 uint32_t ckpt_switches(const am_sweep* h) {
   return (h->hold ? AM_CKPT_HOLD : 0u) | (h->remedy ? AM_CKPT_REMEDY : 0u) | (h->track ? AM_CKPT_TRACK : 0u) |
-         (h->details ? AM_CKPT_DETAILS : 0u) | (h->wf_timeout ? AM_CKPT_TIMEOUTS : 0u);
+         (h->details ? AM_CKPT_DETAILS : 0u) | (h->wf_timeout ? AM_CKPT_TIMEOUTS : 0u) |
+         (admission_on(h) ? AM_CKPT_ADMISSION : 0u);
 }
 
 // The checkpoint state of a handle, at the first checkpoint or restore (ck_mu held).
@@ -2166,6 +2387,7 @@ CkptState ckpt_state(am_sweep* h) {
     s.det_applied = h->det_applied;
     s.det_start = h->det_start;
   }
+  if (admission_on(h)) s.wait = h->adm_wait;
   return s;
 }
 
@@ -2354,6 +2576,10 @@ int am_sweep_restore(am_sweep_t* h, const void* buf, uint64_t len) {
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   const uint64_t hwm = hd.swept_end - h->shard_base;
   if (hwm > h->n_records) h->n_records = hwm;
+  if (admission_on(h)) {  // the admission order of every waiting slot of the handle, from the waits as they now stand
+    rc = rebuild_admission_fifo(h);
+    if (rc != AM_OK) return rc;
+  }
   if (hd.prev_tick != INT64_MIN) {
     h->has_prev = true;
     h->prev_T = hd.prev_tick;

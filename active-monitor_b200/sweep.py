@@ -395,6 +395,24 @@ class Sweep:
         am_sweep_remedy_in_flight), INT64_MIN elsewhere; arguments as in_flight"""
         return self._per_slot("am_sweep_remedy_in_flight", first, n, idx)
 
+    # -- submit budget
+    def set_submit_budget(self, per_tick: int | None):
+        """the most SUBMIT_HC entries every later tick emits (am_sweep_set_submit_budget; needs the hold); None is
+        unlimited"""
+        v = L.UNLIMITED if per_tick is None else int(per_tick)
+        self._check(self._lib.am_sweep_set_submit_budget(self._h, v), "am_sweep_set_submit_budget")
+
+    def last_admission(self) -> dict:
+        """the last tick's n_candidates, n_admitted, n_deferred and oldest_deferred (am_sweep_last_admission)"""
+        a = L.AmAdmission()
+        self._check(self._lib.am_sweep_last_admission(self._h, C.byref(a)), "am_sweep_last_admission")
+        return {n: int(getattr(a, n)) for n, _ in a._fields_}
+
+    def deferred(self, first: int = 0, n: int | None = None, idx=None) -> np.ndarray:
+        """i64 second since which each slot waits for admission, INT64_MIN for the others (am_sweep_deferred);
+        arguments as in_flight"""
+        return self._per_slot("am_sweep_deferred", first, n, idx)
+
     def _timed_out(self, fn: str, offset: int, cap: int | None):
         n = L.u64(0)
         call = getattr(self._lib, fn)

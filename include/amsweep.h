@@ -518,6 +518,51 @@ int am_sweep_last_remedy_timed_out(am_sweep_t*, uint64_t offset, uint64_t* idx, 
  * of them while the remedy hold is off).  Drains staged calls like am_sweep_read. */
 int am_sweep_remedy_in_flight(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* started_out);
 
+/* Submit budget: the most AM_ACT_SUBMIT_HC entries a tick submits, so that a controller never starts more workflows than
+ * it can hand off (DESIGN.md section 6 item 19).  per_tick is the budget of every later tick of every entry point
+ * (am_sweep_tick, _tick_view, _tick_device, _tick_shard and so am_gather_exchange / am_gather_tick_view, and each tick
+ * of am_sweep_simulate) until it is set again; UINT64_MAX, the default, is unlimited.  AM_E_INVAL, changing nothing,
+ * while the hold in flight is off; turning the hold off or on makes it unlimited again and ends every wait below.  The
+ * first finite budget allocates about 21.2 B per slot of capacity on the device; a handle that never sets one launches
+ * nothing for it.  At a tick T:
+ *  - a CANDIDATE is a record the tick would emit with AM_ACT_SUBMIT_HC with an unlimited budget if every record that
+ *    waits for admission were due: live, INTERVAL / CRON_EVERY / CRON_SPEC, not held (either hold), and due by its
+ *    usual rule (catch-up windows and named zones included) or waiting;
+ *  - candidates are admitted in this order: waiting ones by waiting second, then index, then fresh ones by index.  The
+ *    first min(budget, candidates) are ADMITTED and get what a submission gets (SUBMIT_HC, since = T, the deadline
+ *    T + W), so StartedAt and the workflow timeout count from admission;
+ *  - every other candidate is DEFERRED: SUBMIT_HC leaves its entry (an entry left with no action leaves the list; no
+ *    other action is budgeted), its since and deadline are none, and it waits from T on unless it already waited.  A
+ *    5-field check waiting across several activations is submitted once;
+ *  - a wait ends at admission, at a tick at which the record is not a candidate (stopped, parse error, no resource,
+ *    removed, held by a remedy run), at a remove, a load, a restore of the slot, a posted workflow phase, and when the
+ *    hold is toggled; an upsert keeps it.  A waiting check is admitted after at most ceil(checks ahead / budget) ticks
+ *    with a non-zero budget.
+ * The tick's list, am_tick_stats_t, n_emitted, the device and shard lists and the exchange are the admitted list's;
+ * the result counters are not budgeted.  am_sweep_next_due counts a waiting check as due at unix_sec + 1,
+ * am_sweep_in_flight reads INT64_MIN for it, change tracking never lists admission by itself and the details report the
+ * action of the admitted list.  The budget is per handle, so per shard.  Refused (AM_E_INVAL, before anything happens):
+ * am_sweep_simulate with AM_SWEEP_BLOCKED under a finite budget or while a check waits (as the waits stand after the
+ * last drain: calls staged since are not applied by a refused call).  Checkpoints carry the waits (AM_CKPT_ADMISSION)
+ * and a restore puts its slots back into the admission order by (waiting second, index); the budget itself is not
+ * carried: set it, as the other switches, before restoring. */
+int am_sweep_set_submit_budget(am_sweep_t*, uint64_t per_tick);
+
+typedef struct am_admission {
+  uint64_t n_candidates;   /* candidates of the last tick                                      */
+  uint64_t n_admitted;     /* ... admitted: min(budget, n_candidates)                          */
+  uint64_t n_deferred;     /* slots still waiting after it                                     */
+  int64_t oldest_deferred; /* the least waiting second among them, INT64_MAX when none waits  */
+} am_admission_t;
+
+/* The admission of the last tick of any entry point (after am_sweep_tick_device / am_sweep_tick_shard: waits for it).
+ * AM_E_INVAL when the handle never had a finite budget; zero counts after the hold was toggled. */
+int am_sweep_last_admission(am_sweep_t*, am_admission_t* out);
+
+/* For each slot of [first, first+n) (idx == NULL) or idx[0..n): the second since which the check waits for admission,
+ * INT64_MIN when it does not.  Drains staged calls like am_sweep_in_flight. */
+int am_sweep_deferred(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out);
+
 /* The runs the last tick (of any entry point) timed out, ascending by global index, from entry
  * `offset` on: idx[k] the global index, since[k] the run's Status.StartedAt (hcc.go:609/665), for
  * the status and the "Workflow timed out" event (hcc.go:631) the caller writes.  *n_out = entries
@@ -618,7 +663,8 @@ int am_sweep_last_change_details(am_sweep_t*, uint64_t offset, uint64_t* idx, am
  * the timeout state, `since` (remedy runs included) while the hold is on, the change bit while tracking is on and the
  * detail capture while details are on, all as they stand; and the previous tick's second P, the seed, the switches,
  * the names of the time zones its 5-field records use and a 64-bit checksum (against accidental damage, not
- * tampering).  92 B per slot with no switch on, up to 121.125 B with all of them.  Not carried: the previous tick's
+ * tampering).  92 B per slot with no switch on, up to 129.125 B with all of them (the waits for admission, 8 B, with
+ * AM_CKPT_ADMISSION).  Not carried: the previous tick's
  * lists (am_sweep_last_list, both timed-out lists, the changes and their details: empty on the restored handle until
  * its next tick), profiling state and the launch count.
  * EQUIVALENCE: restore the blobs of one checkpoint of a handle H, all taken between the same two ticks, into handles
@@ -632,6 +678,8 @@ int am_sweep_last_change_details(am_sweep_t*, uint64_t offset, uint64_t* idx, am
 #define AM_CKPT_TRACK 0x4u    /* status changes were tracked                  */
 #define AM_CKPT_DETAILS 0x8u  /* ... with change details                      */
 #define AM_CKPT_TIMEOUTS 0x10u /* the handle had the workflow-timeout state   */
+#define AM_CKPT_ADMISSION 0x20u /* the hold was on and the handle had the submit budget's admission state (a finite
+                                   budget was ever set): each slot's waiting second for admission             */
 typedef struct am_checkpoint_info {
   uint64_t first_global, n; /* the slots it holds, by GLOBAL index: [first_global, first_global + n)    */
   uint64_t swept_end;       /* global end of the source's swept slots (high-water mark) within the range */
@@ -648,7 +696,7 @@ typedef struct am_checkpoint_info {
  * as am_sweep_read drains them (a result the drain leaves pending is carried pending).  The tick guard is held only
  * while the drain and one device pass over the range are issued on the handle's stream (a tick in that time
  * returns AM_E_BUSY; later ticks queue behind the pass).  The pass packs the sections into a staging area in HBM
- * (allocated at the first checkpoint or restore, about 122 B per slot of capacity, kept until am_sweep_destroy), marks
+ * (allocated at the first checkpoint or restore, about 130 B per slot of capacity, kept until am_sweep_destroy), marks
  * the zones in use and sums the checksum; the copy into buf follows on a stream of its own, while ticks run.
  * Checkpoints and restores of one handle are serialised.
  * *len_out = the blob's length.  AM_E_NOSPACE (after the drain, nothing else done): cap is below what the call needs,
@@ -684,7 +732,8 @@ int am_sweep_device(const am_sweep_t*);
 double am_sweep_last_kernel_ms(const am_sweep_t*);
 /* Per-kernel device timing: when on, every tick records CUDA events on the
  * launching stream before and after sweep_tick_kernel and after the rest of the
- * tick (scan + expand + publish).  am_sweep_last_profile waits for the last tick and
+ * tick (scan + expand + publish, and before them the submit budget's admission passes
+ * when the handle has them).  am_sweep_last_profile waits for the last tick and
  * returns the two durations in milliseconds.  Off by default (the extra events
  * break the programmatic launch chain: do not time a step with it on). */
 int am_sweep_set_profiling(am_sweep_t*, int on);
