@@ -162,6 +162,7 @@ SYMBOLS = {
     "am_sweep_destroy": (None, [C.c_void_p]),
     "am_sweep_load_range": (C.c_int, [C.c_void_p, u64, u64, P(AmRecordCols)]),
     "am_sweep_upsert": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p]),
+    "am_sweep_update_spec": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p]),
     "am_sweep_remove": (C.c_int, [C.c_void_p, u64, C.c_void_p]),
     "am_sweep_post_result": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "am_sweep_tick": (C.c_int, [C.c_void_p, i64, u32, C.c_void_p, C.c_void_p, u64, P(u64),

@@ -107,8 +107,8 @@ struct Staging {
   DevBuf d_ops, d_recs;
   size_t n_ops = 0, n_recs = 0;
   size_t flushed_ops = 0, flushed_recs = 0;  // already enqueued for copy to the device twins
-  uint32_t n_state = 0, n_result = 0;
-  bool any_wf = false;  // an upsert staged here carries a non-zero wf_timeout
+  uint32_t n_state = 0, n_result = 0, n_spec = 0;
+  bool any_wf = false;  // an upsert or spec update staged here carries a non-zero wf_timeout
   // am_sweep_post_result calls that have reserved a range of the op arrays and are filling it
   // OUTSIDE the lock (the controller's workers post concurrently, hcc.go:170-188): while there are
   // any, the arrays may not move, nothing past `flushed_ops` is known complete, and the drain waits
@@ -171,6 +171,7 @@ struct am_sweep {
   Staging stage[2];
   int cur = 0;                // the staging area callers append to
   uint32_t* marks = nullptr;  // [3 * cap_padded] per-slot {latest state op, latest phase, latest remedy phase}
+  uint32_t* spec_marks = nullptr;  // [cap_padded] per-slot latest spec update, allocated by the first drain that has one
   PinnedBuf pin_in;
   DevBuf dev_in;
   // named time zones: one UTC offset per registered zone (tz.h) on the device, refreshed when the
@@ -241,6 +242,7 @@ struct am_sweep {
   bool early_results = true;  // AMSWEEP_EARLY_RESULTS=0: every posted result is applied inside the sweep
   Staging* pend_clear = nullptr;  // a host tick's drain leaves clear_marks_kernel for after the tick's kernels
   size_t pend_clear_n = 0;
+  bool pend_clear_spec = false;   // ... and that drain had spec updates
   std::vector<Owned> owned;
   std::mutex owned_mu;  // guards appends to `owned` (a restore allocates outside the tick guard)
   // checkpoints (am_sweep_checkpoint / am_sweep_restore), allocated at the first one and serialised by ck_mu (they share
@@ -465,7 +467,10 @@ int finish_deferred_clear(am_sweep* h, cudaStream_t s) {
   h->pend_clear = nullptr;
   const size_t n = h->pend_clear_n;
   const unsigned B = 256, G = (unsigned)((n + B - 1) / B);
-  AM_LAUNCH_PDL(clear_marks_kernel, G, B, s, h->marks, (const uint2*)st->d_ops.p, (uint32_t)n);
+  if (h->pend_clear_spec)
+    AM_LAUNCH_PDL(clear_marks_kernel<true>, G, B, s, h->marks, (const uint2*)st->d_ops.p, (uint32_t)n, h->spec_marks);
+  else
+    AM_LAUNCH_PDL(clear_marks_kernel<false>, G, B, s, h->marks, (const uint2*)st->d_ops.p, (uint32_t)n, (uint32_t*)nullptr);
   h->launches++;
   AM_CUDA(h, cudaGetLastError());
   AM_CUDA(h, cudaEventRecord(st->drained, s));
@@ -732,15 +737,40 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   const uint2* d_ops = (const uint2*)st->d_ops.p;
   const am_record_t* d_recs = (const am_record_t*)st->d_recs.p;
   const unsigned B = 256, G = (unsigned)((n + B - 1) / B);
-  AM_LAUNCH(mark_ops_kernel, G, B, s, h->marks, d_ops, (uint32_t)n);
+  const bool spec = st->n_spec != 0;
+  if (spec && !h->spec_marks) AM_CUDA(h, dev_array(h, &h->spec_marks, h->cap_padded * 4, s));
+  if (spec)
+    AM_LAUNCH(mark_ops_kernel<true>, G, B, s, h->marks, d_ops, (uint32_t)n, h->spec_marks);
+  else
+    AM_LAUNCH(mark_ops_kernel<false>, G, B, s, h->marks, d_ops, (uint32_t)n, (uint32_t*)nullptr);
   h->launches++;
   if (st->n_state) {
     AM_LAUNCH_PDL(apply_state_ops_kernel, G, B, s, h->cols, h->marks, d_ops, d_recs, (uint32_t)n, h->seg_dirty);
-    // upserts and removes may change kinds, zones and masks: rebuild the plane words of the segments they
-    // touched (every drain, so a later tick sees them whichever call drained)
-    AM_LAUNCH_PDL(build_planes_dirty_kernel, (unsigned)((n + kWarps - 1) / kWarps), kBlock, s, h->cols, h->planes,
-                  h->seg_dirty, d_ops, (uint32_t)n);
-    h->launches += 2;
+    h->launches++;
+  }
+  if (spec) {  // spec updates on top of the upserts: their W after the upserts' W, so a later spec update's wins
+    if (st->any_wf && !h->wf_timeout) {
+      const int rc = alloc_timeouts(h, s);
+      if (rc != AM_OK) return rc;
+    }
+    if (h->wf_timeout && st->n_state) {
+      AM_LAUNCH_PDL(store_wf_timeout_kernel, G, B, s, h->wf_timeout, h->marks, d_ops, d_recs, (uint32_t)n);
+      h->launches++;
+    }
+    AM_LAUNCH_PDL(apply_spec_ops_kernel, G, B, s, h->cols, h->marks, (const uint32_t*)h->spec_marks, d_ops, d_recs,
+                  (uint32_t)n, h->seg_dirty, h->wf_timeout, h->track ? h->chg_bits : nullptr,
+                  h->details ? h->det_applied : nullptr, h->details ? h->det_start : nullptr);
+    h->launches++;
+  }
+  if (st->n_state || spec) {
+    // upserts, removes and spec updates may change kinds, zones and masks: rebuild the plane words of the segments
+    // they touched (every drain, so a later tick sees them whichever call drained)
+    const unsigned Gp = (unsigned)((n + kWarps - 1) / kWarps);
+    if (spec)
+      AM_LAUNCH_PDL(build_planes_dirty_kernel<true>, Gp, kBlock, s, h->cols, h->planes, h->seg_dirty, d_ops, (uint32_t)n);
+    else
+      AM_LAUNCH_PDL(build_planes_dirty_kernel<false>, Gp, kBlock, s, h->cols, h->planes, h->seg_dirty, d_ops, (uint32_t)n);
+    h->launches++;
   }
   if (h->track) {  // status changes: the phases of this drain that survive, and what its upserts and removes overwrote
     AM_LAUNCH_PDL(note_ops_kernel, G, B, s, h->chg_bits, (const uint32_t*)h->cols.flags, h->marks, d_ops, (uint32_t)n);
@@ -749,14 +779,17 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   if (h->details) {  // change details: what the surviving phases apply and the runs they end (since not yet cleared)
     AM_LAUNCH_PDL(capture_ops_kernel, G, B, s, h->det_applied, h->det_start, h->cols,
                   (const int64_t*)(h->hold ? h->since : nullptr), (const uint32_t*)h->marks, d_ops, (uint32_t)n);
-    AM_LAUNCH_PDL(capture_superseded_kernel, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n);
+    if (spec)
+      AM_LAUNCH_PDL(capture_superseded_kernel<true>, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n);
+    else
+      AM_LAUNCH_PDL(capture_superseded_kernel<false>, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n);
     h->launches += 2;
   }
   if (st->any_wf && !h->wf_timeout) {
     const int rc = alloc_timeouts(h, s);
     if (rc != AM_OK) return rc;
   }
-  if (h->wf_timeout && st->n_state) {  // (upserts with W = 0 overwrite an older W as well)
+  if (h->wf_timeout && st->n_state && !spec) {  // (upserts with W = 0 overwrite an older W as well)
     AM_LAUNCH_PDL(store_wf_timeout_kernel, G, B, s, h->wf_timeout, h->marks, d_ops, d_recs, (uint32_t)n);
     h->launches++;
   }
@@ -795,9 +828,13 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   if (defer_clear) {  // (the caller runs finish_deferred_clear on the same stream before anything else touches the handle)
     h->pend_clear = st;
     h->pend_clear_n = n;
+    h->pend_clear_spec = spec;
     AM_CUDA(h, cudaGetLastError());
   } else {
-    AM_LAUNCH_PDL(clear_marks_kernel, G, B, s, h->marks, d_ops, (uint32_t)n);
+    if (spec)
+      AM_LAUNCH_PDL(clear_marks_kernel<true>, G, B, s, h->marks, d_ops, (uint32_t)n, h->spec_marks);
+    else
+      AM_LAUNCH_PDL(clear_marks_kernel<false>, G, B, s, h->marks, d_ops, (uint32_t)n, (uint32_t*)nullptr);
     h->launches++;
     AM_CUDA(h, cudaGetLastError());
     AM_CUDA(h, cudaEventRecord(st->drained, s));
@@ -806,7 +843,7 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   st->n_ops = st->n_recs = st->flushed_ops = st->flushed_recs = 0;
   st->done_ops = 0;
   st->done_ranges.clear();
-  st->n_state = st->n_result = 0;
+  st->n_state = st->n_result = st->n_spec = 0;
   st->any_wf = false;
   st->hwm = 0;
   return AM_OK;
@@ -1598,7 +1635,10 @@ int am_sweep_set_change_details(am_sweep_t* h, int on) {
   return AM_OK;
 }
 
-int am_sweep_upsert(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_record_t* recs) {
+namespace {
+// am_sweep_upsert (kind kOpUpsert: the swept range grows to the highest slot) and am_sweep_update_spec (kOpSpec): n
+// records for slots idx, staged as one op each and a copy of the record.  A refusal stages nothing.
+int stage_records(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_record_t* recs, uint32_t kind) {
   if (!h || (n && (!idx || !recs))) return AM_E_INVAL;
   if (n == 0) return AM_OK;
   if (amsweep_host::unknown_zones(n, &recs[0].flags, sizeof(am_record_t) / sizeof(uint32_t), (uint32_t)amsweep_tz::count()))
@@ -1614,7 +1654,7 @@ int am_sweep_upsert(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_rec
   Staging& st = *stp;
   AM_CUDA(h, cudaSetDevice(h->device));
   // nothing is committed (counters unchanged) when a slot is out of range
-  if (amsweep_host::stage_slots(n, idx, h->capacity, kOpUpsert | (uint32_t)st.n_recs, 1u, (uint64_t*)st.ops.p + st.n_ops))
+  if (amsweep_host::stage_slots(n, idx, h->capacity, kind | (uint32_t)st.n_recs, 1u, (uint64_t*)st.ops.p + st.n_ops))
     return AM_E_RANGE;
   am_record_t* dst = (am_record_t*)st.recs.p + st.n_recs;
   uint64_t hwm = st.hwm;
@@ -1623,13 +1663,22 @@ int am_sweep_upsert(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_rec
     dst[k].flags &= ~AM_F_TOMBSTONE;
     if (idx[k] + 1 > hwm) hwm = idx[k] + 1;
   }
-  st.hwm = hwm;
+  if (kind == kOpUpsert) st.hwm = hwm;  // (a spec update of a slot that was never upserted does nothing)
   st.any_wf |= any_wf;
   complete_range(st, st.n_ops, st.n_ops + n);
   st.n_ops += n; st.n_recs += n;
-  st.n_state += (uint32_t)n;
+  (kind == kOpUpsert ? st.n_state : st.n_spec) += (uint32_t)n;
   AM_CUDA(h, flush_staging(h, st, false));
   return AM_OK;
+}
+}  // namespace
+
+int am_sweep_upsert(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_record_t* recs) {
+  return stage_records(h, n, idx, recs, kOpUpsert);
+}
+
+int am_sweep_update_spec(am_sweep_t* h, uint64_t n, const uint64_t* idx, const am_record_t* recs) {
+  return stage_records(h, n, idx, recs, kOpSpec);
 }
 
 int am_sweep_remove(am_sweep_t* h, uint64_t n, const uint64_t* idx) {

@@ -1136,8 +1136,12 @@ __global__ void next_due_kernel(DevCols c, const int64_t* __restrict__ since, co
 // "Failed" and a remedy "Succeeded" posted by two calls before one tick must both
 // survive.  clear: marks back to zero.  No host-side hashing or sorting.
 // A staged op is a uint2 (slot, arg): arg = kind in the top 2 bits; low 30 bits: record index
-// (upsert) or flag bits (result).
-constexpr uint32_t kOpUpsert = 0u << 30, kOpRemove = 1u << 30, kOpResult = 2u << 30, kOpKindMask = 3u << 30;
+// (upsert, spec update) or flag bits (result).
+// A spec update (am_sweep_update_spec) marks its own word, the slot's latest-spec mark ([cap_padded], allocated at the
+// first one): the kernels that take it, and build_planes_dirty_kernel, are instantiated with true for a drain with spec
+// updates; a drain without them launches the false instances, which are the kernels of a handle that never stages one.
+constexpr uint32_t kOpUpsert = 0u << 30, kOpRemove = 1u << 30, kOpResult = 2u << 30, kOpSpec = 3u << 30;
+constexpr uint32_t kOpKindMask = 3u << 30;
 
 // The mark triple of slot i: word x (kMarkState, kMarkHc, kMarkRm) is the 1-based sequence (op k: k + 1) of the slot's
 // latest state op (upsert / remove), workflow phase and remedy phase in this drain, 0 for none.  The winner rule below
@@ -1165,12 +1169,14 @@ __device__ __forceinline__ uint32_t merge_phases(uint32_t f, bool hc_valid, HcAr
   return f;
 }
 
-__global__ void mark_ops_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n) {
+template <bool SPEC>
+__global__ void mark_ops_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n, uint32_t* spec_marks) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const uint2 op = ops[k];
   const uint32_t i = op.x, arg = op.y;
+  if (SPEC && (arg & kOpKindMask) == kOpSpec) { atomicMax(&spec_marks[i], k + 1u); return; }
   if ((arg & kOpKindMask) != kOpResult) { atomicMax(&mark(marks, i, kMarkState), k + 1u); return; }
   if (arg & kHcBits) atomicMax(&mark(marks, i, kMarkHc), k + 1u);
   if (arg & AM_F_REMEDY_PENDING) atomicMax(&mark(marks, i, kMarkRm), k + 1u);
@@ -1242,7 +1248,10 @@ __global__ void build_planes_range_kernel(DevCols c, MaskPlanes pl, uint32_t seg
 }
 
 // After apply_state_ops_kernel: one warp per staged op.  The first warp that claims a segment marked
-// there rebuilds it, so the cost is one claim per op plus one rebuild per segment touched.
+// there rebuilds it, so the cost is one claim per op plus one rebuild per segment touched.  PEEK (drains with spec
+// updates, which mark only the segments whose masks, kinds or zones changed): the claim is tried only where a plain
+// load finds the mark, so the ops of clean segments, up to 128 per segment, do not queue on its word's atomic.
+template <bool PEEK>
 __global__ void build_planes_dirty_kernel(DevCols c, MaskPlanes pl, uint32_t* seg_dirty, const uint2* __restrict__ ops,
                                           uint32_t n) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
@@ -1250,7 +1259,8 @@ __global__ void build_planes_dirty_kernel(DevCols c, MaskPlanes pl, uint32_t* se
   if (k >= n) return;  // warp-uniform
   const int lane = (int)(threadIdx.x & 31);
   const uint32_t seg = ops[k].x / (uint32_t)kRecPerWarp;
-  const bool won = lane == 0 && atomicAnd(&seg_dirty[seg], 0u) != 0u;  // (an exchange with 0)
+  const bool won =
+      lane == 0 && (!PEEK || seg_dirty[seg] != 0u) && atomicAnd(&seg_dirty[seg], 0u) != 0u;  // (an exchange with 0)
   if (__ballot_sync(kFull, won)) build_segment_planes(c, pl, seg, lane);
 }
 
@@ -1601,13 +1611,15 @@ __global__ void sim_count_kernel(DevCols c, const int64_t* __restrict__ since, u
   }
 }
 
-__global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n) {
+template <bool SPEC>
+__global__ void clear_marks_kernel(uint32_t* marks, const uint2* __restrict__ ops, uint32_t n, uint32_t* spec_marks) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const uint32_t i = ops[k].x;
 #pragma unroll
   for (uint32_t x = kMarkState; x <= kMarkRm; ++x) mark(marks, i, x) = 0;
+  if (SPEC) spec_marks[i] = 0;
 }
 
 // ---- status changes (am_sweep_set_track_changes) --------------------------------------------------------------
@@ -1803,7 +1815,9 @@ __global__ void capture_ops_kernel(uint8_t* applied, int64_t* start, const DevCo
 }
 
 // After capture_ops_kernel, one thread per op: an op that ended the captured run before the winner's call did (a
-// remove; a workflow phase; for a remedy run any phase) leaves the winner's call nothing in flight.
+// remove; a workflow phase; for a remedy run any phase) leaves the winner's call nothing in flight.  A spec update ends
+// nothing.
+template <bool SPEC>
 __global__ void capture_superseded_kernel(int64_t* start, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops,
                                           uint32_t n) {
   pdl_wait();  // (launched with programmatic stream serialisation: capture_ops_kernel writes start)
@@ -1811,7 +1825,7 @@ __global__ void capture_superseded_kernel(int64_t* start, const uint32_t* __rest
   if (k >= n) return;
   const uint2 op = ops[k];
   const uint32_t i = op.x, arg = op.y, kind = arg & kOpKindMask;
-  if (kind == kOpUpsert) return;
+  if (kind == kOpUpsert || (SPEC && kind == kOpSpec)) return;
   const int64_t w = start[i];
   if (w == kNotInFlight) return;
   const bool rem = is_remedy_run(w);
@@ -1822,6 +1836,52 @@ __global__ void capture_superseded_kernel(int64_t* start, const uint32_t* __rest
     if (((arg ^ ops[win - 1u].y) & kCallTagMask) == 0u) return;  // an entry of the winner's own call
   }
   start[i] = kNotInFlight;
+}
+
+// Spec updates (am_sweep_update_spec), after apply_state_ops_kernel and store_wf_timeout_kernel: the slot's latest one,
+// unless a later upsert or remove replaced the record, rewrites the spec columns of a live slot on top of whatever that
+// upsert left, and keeps its status.  Only columns that change are stored, and only a change of masks, kind or zone marks
+// the segment for build_planes_dirty_kernel: a status echo with an unchanged spec costs the gathers alone.  `wf` (the
+// timeout state, NULL without it) takes the record's wf_timeout for the slot's next run.  Status changes (`chg` NULL
+// without tracking): an update that makes a slot with posted results live (NO_RESOURCE or HOST_FALLBACK -> a kind the
+// sweep evaluates) hands them to the coming tick, which applies them; if its bit is clear (a list dropped it while the
+// slot was not live) it is set, with the pair a pass that finds the bit clear starts from (`det_*` NULL without
+// details).  Otherwise the bits and the pairs are left alone.
+__global__ void apply_spec_ops_kernel(DevCols c, const uint32_t* __restrict__ marks, const uint32_t* __restrict__ spec_marks,
+                                      const uint2* __restrict__ ops, const am_record_t* __restrict__ recs, uint32_t n,
+                                      uint32_t* seg_dirty, int32_t* wf, uint32_t* chg, uint8_t* det_applied,
+                                      int64_t* det_start) {
+  pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint2 op = ops[k];
+  const uint32_t i = op.x, arg = op.y;
+  if ((arg & kOpKindMask) != kOpSpec || spec_marks[i] != k + 1u || mark(marks, i, kMarkState) > k + 1u) return;
+  const uint32_t f = c.flags[i];
+  if (f & AM_F_TOMBSTONE) return;
+  const am_record_t& r = recs[arg & ~kOpKindMask];
+  uint32_t g = (f & ~(uint32_t)AM_F_SPEC_MASK) | (r.flags & (uint32_t)AM_F_SPEC_MASK);
+  if ((f & AM_KIND_MASK) != AM_KIND_STOPPED || (g & AM_KIND_MASK) != AM_KIND_STOPPED) g &= ~AM_F_STOPPED_REPORTED;
+  bool planes = ((f ^ g) & (AM_KIND_MASK | AM_F_TZ_MASK)) != 0;
+  if (g != f) c.flags[i] = g;
+  const uint64_t m[5] = {r.minute, r.hour, r.dom, r.month, r.dow};
+  uint64_t* col[5] = {c.minute, c.hour, c.dom, c.month, c.dow};
+#pragma unroll
+  for (int x = 0; x < 5; ++x)
+    if (col[x][i] != m[x]) { col[x][i] = m[x]; planes = true; }
+  if (c.ras[i] != r.ras) c.ras[i] = r.ras;
+  if (c.runs_limit[i] != r.runs_limit) c.runs_limit[i] = r.runs_limit;
+  if (c.reset_interval[i] != r.reset_interval) c.reset_interval[i] = r.reset_interval;
+  if (wf && wf[i] != r.wf_timeout) wf[i] = r.wf_timeout;
+  if (planes) seg_dirty[i / kRecPerWarp] = 1u;
+  const uint32_t b = 1u << (i & 31u);
+  if (chg && is_live(g) && (g & kPendBits) && !(chg[i / 32u] & b)) {  // (this thread alone owns slot i's bit here)
+    if (det_applied) {
+      det_applied[i] = (uint8_t)applied_of(g);
+      det_start[i] = kNotInFlight;
+    }
+    atomicOr(chg + i / 32u, b);
+  }
 }
 
 // The expiry pass's timed-out runs (before note_slots_kernel sets their bits): the timeout's Failed and its run's start.

@@ -227,6 +227,14 @@ class Sweep:
         self._check(self._lib.am_sweep_upsert(self._h, len(idx), idx.ctypes.data, recs.ctypes.data),
                     "am_sweep_upsert")
 
+    def update_spec(self, idx, recs: np.ndarray):
+        """the spec of `recs` for slots `idx`, keeping each slot's status (am_sweep_update_spec)"""
+        idx = np.ascontiguousarray(idx, dtype=np.uint64)
+        recs = np.ascontiguousarray(recs, dtype=L.RECORD_DTYPE)
+        assert len(idx) == len(recs)
+        self._check(self._lib.am_sweep_update_spec(self._h, len(idx), idx.ctypes.data, recs.ctypes.data),
+                    "am_sweep_update_spec")
+
     def remove(self, idx):
         idx = np.ascontiguousarray(idx, dtype=np.uint64)
         self._check(self._lib.am_sweep_remove(self._h, len(idx), idx.ctypes.data), "am_sweep_remove")

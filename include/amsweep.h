@@ -123,6 +123,8 @@ int64_t am_cron_repeat_after_sec(const am_cron_t* c, int64_t unix_sec);
 #define AM_F_TZ_MASK (0xFFu << AM_F_TZ_SHIFT)
 #define AM_F_FAILP_SHIFT 16              /* closed-loop harness: P(fail)*256   */
 #define AM_F_FAILP_MASK (0xFFu << AM_F_FAILP_SHIFT)
+/* the flags bits that are the CR's spec: what am_sweep_update_spec takes from its records */
+#define AM_F_SPEC_MASK (AM_KIND_MASK | AM_F_HAS_REMEDY | AM_F_FAILP_MASK | AM_F_TZ_MASK)
 
 /* action byte emitted per record per tick (0 = nothing to do) */
 #define AM_ACT_SUBMIT_HC 0x01u         /* hcc.go:269-288 submit the workflow   */
@@ -285,6 +287,20 @@ int am_sweep_load_range(am_sweep_t*, uint64_t first, uint64_t n, const am_record
 /* Reconcile of created/updated CRs (hcc.go:170-188): scatter n records to
  * local slots idx[i].  Thread-safe; staged and applied by the next tick. */
 int am_sweep_upsert(am_sweep_t*, uint64_t n, const uint64_t* idx, const am_record_t* recs);
+
+/* A spec edit of CRs already placed (hcc.go:170-188 Reconcile after a spec change): the spec of n records
+ * (am_healthcheck_classify's am_record_t) for local slots idx[i], WITHOUT the CR's status.  Thread-safe; staged
+ * like am_sweep_upsert, in the same per-slot call order, and drained wherever upserts are.
+ *   taken from recs[i]: minute..dow, ras, runs_limit, reset_interval, wf_timeout and flags & AM_F_SPEC_MASK;
+ *   kept from the slot: finished_at, remedy_finished_at, the five counters, the pending, remedy and timer bits,
+ *     the run in flight and its deadline, the wait for admission, the status-change bit and its details;
+ *   AM_F_STOPPED_REPORTED stays only while the kind stays AM_KIND_STOPPED (a check the edit pauses is reported once).
+ * Per slot, let U be its latest upsert or remove of the drain and S its latest spec update: S after U (or no U)
+ * applies on top of U; S before U has no effect.  S on a tombstone (removed, or never upserted or loaded) does
+ * nothing and never extends the swept range.  Results posted after U stay valid whatever S does: a spec update
+ * never supersedes a result, never ends a hold, and the timeout of a running workflow stays the one it started with.
+ * Refusals, with nothing staged: as am_sweep_upsert (AM_E_INVAL, AM_E_RANGE). */
+int am_sweep_update_spec(am_sweep_t*, uint64_t n, const uint64_t* idx, const am_record_t* recs);
 
 /* CR deleted (hcc.go:175-186: Stop() its timer): tombstone the slots.  A removed
  * slot reads back as flags == AM_F_TOMBSTONE; its other columns are unspecified

@@ -7,6 +7,8 @@
 //
 //     NewHealthCheckReconciler           hcc.go:152
 //     (*HealthCheckReconciler).Reconcile hcc.go:170   (CR present -> process; gone -> stop timer :175-186)
+//     ProcessSpec                        the spec path of a Reconcile for a check already placed: the
+//                                                     library keeps its status (am_sweep_update_spec)
 //     processHealthCheck                 hcc.go:225   (ladder :227/:238/:251/:264, error on bad cron :254-257,
 //                                                      Spec.RepeatAfterSec set from the cron schedule :262)
 //     GetTimerByName                     hcc.go:1480  (the armed re-run timer of a check)
@@ -102,25 +104,28 @@ class HealthCheckReconciler {
   // (:238) and a check without Workflow.Resource (:227) are not errors.
   std::optional<std::string> ProcessHealthCheck(HealthCheck* hc, int64_t now) {
     am_record_t rec;
-    std::string perr;
     // r.GetTimerByName(name) != nil (hcc.go:264): a timer exists once a result of this check was
     // applied (hcc.go:745-752) and survives re-Reconciles of the same process; a fresh reconciler
     // (restart, hcc.go:161) has none
     bool armed = false;
     am_record_t cur;
     if (slots_.count(hc->Key()) && ReadRecord(hc->Key(), &cur)) armed = (cur.flags & AM_F_TIMER_ARMED) != 0;
-    int rc = Classify(*hc, armed, &rec, &perr);
-    if (rc == AM_E_UNSUPPORTED) return std::string("unsupported on the device path: ") + perr;
-    if (rc != AM_OK) return std::string(am_strerror(rc));
-    const uint32_t kind = rec.flags & AM_KIND_MASK;
-    if (kind == AM_KIND_PARSE_ERROR) return perr.empty() ? std::string("fail to parse cron") : perr;
-    if (kind == AM_KIND_CRON_SPEC || kind == AM_KIND_CRON_EVERY) {
-      am_cron_t c;
-      am_cron_parse(hc->Spec.Schedule.Cron.data(), hc->Spec.Schedule.Cron.size(), &c, nullptr, 0);
-      hc->Spec.RepeatAfterSec = am_cron_repeat_after_sec(&c, now);  // hcc.go:262
-    }
+    if (auto err = Record(hc, armed, now, &rec)) return err;
     const uint64_t slot = SlotFor(hc->Key());
     am_sweep_upsert(h_, 1, &slot, &rec);
+    return std::nullopt;
+  }
+
+  // The spec path of a Reconcile (am_sweep_update_spec) for a check already placed: only hc->Spec is taken, the
+  // library keeps the check's status.  A Reconcile that a status write enqueued, or a restart's re-list with the
+  // status etcd holds, then rolls back no result the library applied or has staged since.  Reads nothing from the
+  // device.  A check not placed yet goes through ProcessHealthCheck.  Errors and RepeatAfterSec as there.
+  std::optional<std::string> ProcessSpec(HealthCheck* hc, int64_t now) {
+    auto it = slots_.find(hc->Key());
+    if (it == slots_.end()) return ProcessHealthCheck(hc, now);
+    am_record_t rec;
+    if (auto err = Record(hc, false, now, &rec)) return err;
+    am_sweep_update_spec(h_, 1, &it->second, &rec);
     return std::nullopt;
   }
 
@@ -260,6 +265,22 @@ class HealthCheckReconciler {
 
  private:
   HealthCheckReconciler(am_sweep_t* h, uint64_t cap) : h_(h), capacity_(cap) { names_.resize(cap); }
+
+  // processHealthCheck's ladder on the host: the record of *hc, or the error the reference returns.
+  static std::optional<std::string> Record(HealthCheck* hc, bool armed, int64_t now, am_record_t* rec) {
+    std::string perr;
+    int rc = Classify(*hc, armed, rec, &perr);
+    if (rc == AM_E_UNSUPPORTED) return std::string("unsupported on the device path: ") + perr;
+    if (rc != AM_OK) return std::string(am_strerror(rc));
+    const uint32_t kind = rec->flags & AM_KIND_MASK;
+    if (kind == AM_KIND_PARSE_ERROR) return perr.empty() ? std::string("fail to parse cron") : perr;
+    if (kind == AM_KIND_CRON_SPEC || kind == AM_KIND_CRON_EVERY) {
+      am_cron_t c;
+      am_cron_parse(hc->Spec.Schedule.Cron.data(), hc->Spec.Schedule.Cron.size(), &c, nullptr, 0);
+      hc->Spec.RepeatAfterSec = am_cron_repeat_after_sec(&c, now);  // hcc.go:262
+    }
+    return std::nullopt;
+  }
 
   static int Classify(const HealthCheck& hc, bool timer_armed, am_record_t* rec, std::string* perr) {
     am_healthcheck_t in{};
