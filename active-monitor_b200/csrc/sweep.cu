@@ -105,6 +105,10 @@ struct Owned {
 struct Staging {
   PinnedBuf ops, recs;   // an op = one 64-bit word: slot | arg << 32
   DevBuf d_ops, d_recs;
+  // the first op index of every post call, ascending (reservation order), and its device copy: a drain of more ops than
+  // a call tag spans tells two post calls apart by it (capture_superseded_kernel)
+  std::vector<uint32_t> calls;
+  DevBuf d_calls;
   size_t n_ops = 0, n_recs = 0;
   size_t flushed_ops = 0, flushed_recs = 0;  // already enqueued for copy to the device twins
   uint32_t n_state = 0, n_result = 0, n_spec = 0;
@@ -731,6 +735,18 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
     st->flushed_ops = st->flushed_recs = 0;
   }
   AM_CUDA(h, flush_staging(h, *st, true));
+  // Change details of a drain longer than a call tag's span: two post calls may carry one tag, and
+  // capture_superseded_kernel tells them apart by their first op indices (pageable: copied before the return)
+  const uint32_t* d_calls = nullptr;
+  const uint32_t n_calls = (uint32_t)st->calls.size();
+  if (h->details && n > kCallTagSpan && n_calls > 1) {
+    if (st->d_calls.cap < n_calls * 4ull) {
+      AM_CUDA(h, cudaStreamSynchronize(h->cstream));  // (frees synchronise)
+      AM_CUDA(h, st->d_calls.reserve(n_calls * 4ull));
+    }
+    AM_CUDA(h, cudaMemcpyAsync(st->d_calls.p, st->calls.data(), n_calls * 4ull, cudaMemcpyHostToDevice, h->cstream));
+    d_calls = (const uint32_t*)st->d_calls.p;
+  }
   AM_CUDA(h, cudaEventRecord(st->copied, h->cstream));
   st->copy_pending = true;
   AM_CUDA(h, cudaStreamWaitEvent(s, st->copied, 0));
@@ -780,9 +796,11 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
     AM_LAUNCH_PDL(capture_ops_kernel, G, B, s, h->det_applied, h->det_start, h->cols,
                   (const int64_t*)(h->hold ? h->since : nullptr), (const uint32_t*)h->marks, d_ops, (uint32_t)n);
     if (spec)
-      AM_LAUNCH_PDL(capture_superseded_kernel<true>, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n);
+      AM_LAUNCH_PDL(capture_superseded_kernel<true>, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n,
+                    d_calls, n_calls);
     else
-      AM_LAUNCH_PDL(capture_superseded_kernel<false>, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n);
+      AM_LAUNCH_PDL(capture_superseded_kernel<false>, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n,
+                    d_calls, n_calls);
     h->launches += 2;
   }
   if (st->any_wf && !h->wf_timeout) {
@@ -843,6 +861,7 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   st->n_ops = st->n_recs = st->flushed_ops = st->flushed_recs = 0;
   st->done_ops = 0;
   st->done_ranges.clear();
+  st->calls.clear();
   st->n_state = st->n_result = st->n_spec = 0;
   st->any_wf = false;
   st->hwm = 0;
@@ -1410,7 +1429,7 @@ void am_sweep_destroy(am_sweep_t* h) {
   }
   for (Staging& st : h->stage) {
     st.ops.release(); st.recs.release();
-    st.d_ops.release(); st.d_recs.release();
+    st.d_ops.release(); st.d_recs.release(); st.d_calls.release();
   }
   h->host_out.release();
   h->pin_in.release(); h->dev_in.release();
@@ -1709,6 +1728,7 @@ int am_sweep_post_result(am_sweep_t* h, uint64_t n, const uint64_t* idx, const u
   if (int rc = reserve_staging(h, lk, n, 0, &stp)) return rc;
   Staging& st = *stp;
   const size_t a = st.n_ops;
+  st.calls.push_back((uint32_t)a);
   st.n_ops += n;
   st.n_result += (uint32_t)n;
   ++st.writers;  // the drain and any growth of the arrays now wait for this call
@@ -1718,7 +1738,7 @@ int am_sweep_post_result(am_sweep_t* h, uint64_t n, const uint64_t* idx, const u
   // finished chunk to the copy stream before staging the next (when no other call is staging).
   // phase -> flag bits: {none, Succeeded, Failed} -> {0, PENDING_OK, PENDING_FAIL}
   // Every entry carries the call's tag (its first op index, mod 2^22; capture_superseded_kernel): the entries of one
-  // call see the in-flight state from before the call.
+  // call see the in-flight state from before the call.  (A drain of more than 2^22 ops also uploads st.calls.)
   const uint32_t kind = kOpResult | (((uint32_t)a << kCallTagShift) & kCallTagMask);
   unsigned bad = 0;
   cudaError_t ce = cudaSuccess;

@@ -1771,7 +1771,9 @@ __global__ void __launch_bounds__(kGroupWords) list_changes_kernel(uint32_t* bit
 // copies the pairs of its list, by entry, into a second pair of arrays (snapshot_details_kernel).
 // A result op carries its post call's tag in arg bits 8..29 (am_sweep_post_result: the call's first op index, mod
 // 2^22), which no other kernel reads: two entries of one call see the same in-flight state, as they do in call order.
-constexpr uint32_t kCallTagShift = 8, kCallTagMask = 0x3FFFFFu << kCallTagShift;
+// Within a drain of at most kCallTagSpan ops equal tags mean one call; a longer drain also hands the kernel the first
+// op index of every post call.
+constexpr uint32_t kCallTagShift = 8, kCallTagSpan = 1u << 22, kCallTagMask = (kCallTagSpan - 1u) << kCallTagShift;
 static_assert((kCallTagMask & (kOpKindMask | kHcBits | kRemedyBits)) == 0, "call tag bits");
 
 // The AM_CHG_* bits of a flags word's posted-result bits.
@@ -1816,10 +1818,11 @@ __global__ void capture_ops_kernel(uint8_t* applied, int64_t* start, const DevCo
 
 // After capture_ops_kernel, one thread per op: an op that ended the captured run before the winner's call did (a
 // remove; a workflow phase; for a remedy run any phase) leaves the winner's call nothing in flight.  A spec update ends
-// nothing.
+// nothing.  `calls` (NULL when the drain has at most kCallTagSpan ops): the n_calls first op indices of the drain's post
+// calls, ascending; two result ops with equal tags are of one call iff no call starts after the first, up to the second.
 template <bool SPEC>
 __global__ void capture_superseded_kernel(int64_t* start, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops,
-                                          uint32_t n) {
+                                          uint32_t n, const uint32_t* __restrict__ calls, uint32_t n_calls) {
   pdl_wait();  // (launched with programmatic stream serialisation: capture_ops_kernel writes start)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
@@ -1833,7 +1836,16 @@ __global__ void capture_superseded_kernel(int64_t* start, const uint32_t* __rest
   if (k + 1u >= win) return;  // (win == 0: an earlier drain's capture, which this drain does not replace)
   if (kind == kOpResult) {
     if (!((arg & kHcBits) || (rem && (arg & AM_F_REMEDY_PENDING)))) return;
-    if (((arg ^ ops[win - 1u].y) & kCallTagMask) == 0u) return;  // an entry of the winner's own call
+    if (((arg ^ ops[win - 1u].y) & kCallTagMask) == 0u) {  // an entry of the winner's own call, or one 2^22·m ops before
+      if (!calls) return;
+      uint32_t lo = 0, hi = n_calls;  // the first call that starts after op k
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (calls[mid] <= k) lo = mid + 1u;
+        else hi = mid;
+      }
+      if (lo == n_calls || calls[lo] >= win) return;  // (the winner is op win - 1)
+    }
   }
   start[i] = kNotInFlight;
 }
