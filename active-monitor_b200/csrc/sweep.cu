@@ -25,7 +25,8 @@
 //   * am_sweep_run_ticks and am_sweep_simulate run one path for runs of ticks (begin_run, run_rows, run_blocks) around
 //     their own tick loops;
 //   * fixed-size device arrays, pinned host arrays, events and streams are recorded on the handle as they are made
-//     (dev_array, host_array, new_event, new_stream): am_sweep_destroy frees that list.
+//     (dev_array, host_array, new_event, new_stream): am_sweep_destroy frees that list;
+//   * every kernel is launched through launch / launch_pdl, which count it and return its launch error.
 //
 // There is deliberately no CPU path in this file: without a CUDA device
 // am_sweep_create fails with AM_E_DEVICE.
@@ -240,7 +241,7 @@ struct am_sweep {
   bool chg_closed = false;
   bool det_listed = false;  // the last list was built with details on (a list from before they were on has none)
   std::string last_error;
-  uint64_t launches = 0;
+  std::atomic<uint64_t> launches{0};  // (a restore launches outside the tick guard)
   double last_ms = -1.0;
   uint64_t seed = 0;
   bool early_results = true;  // AMSWEEP_EARLY_RESULTS=0: every posted result is applied inside the sweep
@@ -291,6 +292,21 @@ namespace {
     }                                                                                 \
   } while (0)
 
+// Every kernel launch of the handle: counted for am_sweep_launch_count, and its launch error returned (for AM_CUDA).
+template <class... P, class... A>
+cudaError_t launch(am_sweep* h, void (*k)(P...), dim3 grid, dim3 block, cudaStream_t s, const A&... args) {
+  AM_LAUNCH(k, grid, block, s, args...);
+  h->launches.fetch_add(1, std::memory_order_relaxed);
+  return cudaGetLastError();
+}
+// ... with programmatic dependent launch (AM_LAUNCH_PDL)
+template <class... P, class... A>
+cudaError_t launch_pdl(am_sweep* h, void (*k)(P...), dim3 grid, dim3 block, cudaStream_t s, const A&... args) {
+  AM_LAUNCH_PDL(k, grid, block, s, args...);
+  h->launches.fetch_add(1, std::memory_order_relaxed);
+  return cudaGetLastError();
+}
+
 constexpr size_t kColElem[16] = {8, 8, 8, 8, 8, 4, 4, 8, 4, 4, 4, 4, 4, 4, 4, 8};
 
 void** col_slot(DevCols& c, int k) {
@@ -323,12 +339,17 @@ struct TickGuard {
 
 // Every device operation of a handle is ordered after the previous one.  They normally
 // share a stream; when the stream changes (am_sweep_tick_device on a caller stream, then a
-// read on the handle's own, ...) the new stream waits for an event recorded on the old one.
-int order_on(am_sweep* h, cudaStream_t s) {
+// read on the handle's own, ...) the new stream waits for an event recorded on the old one.  wait_last only makes
+// `s` wait; order_on also makes `s` the stream of the handle's last operation.
+int wait_last(am_sweep* h, cudaStream_t s) {
   if (h->has_last && h->last_stream != s) {
     AM_CUDA(h, cudaEventRecord(h->ev_last, h->last_stream));
     AM_CUDA(h, cudaStreamWaitEvent(s, h->ev_last, 0));
   }
+  return AM_OK;
+}
+int order_on(am_sweep* h, cudaStream_t s) {
+  if (int rc = wait_last(h, s)) return rc;
   h->last_stream = s;
   h->has_last = true;
   return AM_OK;
@@ -373,6 +394,26 @@ cudaError_t new_stream(am_sweep* h, cudaStream_t* s) {
   cudaError_t e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
   if (e == cudaSuccess) own(h, Owned::kStream, (void*)*s);
   return e;
+}
+
+// `bytes` of device memory at `src` into host memory at `dst`, after everything on the handle's stream: through pin_in,
+// one synchronisation.
+int read_back(am_sweep* h, void* dst, const void* src, size_t bytes) {
+  AM_CUDA(h, h->pin_in.reserve(bytes));
+  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, src, bytes, cudaMemcpyDeviceToHost, h->stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  memcpy(dst, h->pin_in.p, bytes);
+  return AM_OK;
+}
+
+// The least key (~0 = none) that reduce(key) — min-reductions launched on the handle's stream — leaves in a word of
+// dev_in that starts at ~0.
+template <class Reduce>
+int min_key(am_sweep* h, Reduce&& reduce, unsigned long long* out) {
+  AM_CUDA(h, h->dev_in.reserve(8));
+  AM_CUDA(h, cudaMemsetAsync(h->dev_in.p, 0xFF, 8, h->stream));
+  AM_CUDA(h, reduce((unsigned long long*)h->dev_in.p));
+  return read_back(h, out, h->dev_in.p, 8);
 }
 
 // The seconds the calendar arithmetic takes: |unix_sec| < 2^55.
@@ -461,34 +502,32 @@ int reserve_staging(am_sweep* h, std::unique_lock<std::mutex>& lk, size_t n, siz
   }
 }
 
-// Apply staged upserts / removes / results on stream `s` (called with the tick guard held).
-// The staging lock is held only for the buffer swap.
-// clear_marks_kernel of a drain that deferred it (host ticks: the sweep does not touch the marks, and the
+// The end of a drain of n ops from `st` (with spec updates among them when `spec`): its marks cleared, and the point
+// after which the device twins of `st` may be overwritten recorded.
+int clear_marks(am_sweep* h, Staging& st, size_t n, bool spec, cudaStream_t s) {
+  const unsigned B = 256, G = (unsigned)((n + B - 1) / B);
+  auto* k = spec ? clear_marks_kernel<true> : clear_marks_kernel<false>;
+  AM_CUDA(h, launch_pdl(h, k, G, B, s, h->marks, (const uint2*)st.d_ops.p, (uint32_t)n,
+                        spec ? h->spec_marks : nullptr));
+  AM_CUDA(h, cudaEventRecord(st.drained, s));
+  st.drain_pending = true;
+  return AM_OK;
+}
+
+// clear_marks of a drain that deferred it (host ticks: the sweep does not touch the marks, and the
 // host waits for an event recorded BEFORE this launch — the clear is off the tick's latency)
 int finish_deferred_clear(am_sweep* h, cudaStream_t s) {
   Staging* st = h->pend_clear;
   if (!st) return AM_OK;
   h->pend_clear = nullptr;
-  const size_t n = h->pend_clear_n;
-  const unsigned B = 256, G = (unsigned)((n + B - 1) / B);
-  if (h->pend_clear_spec)
-    AM_LAUNCH_PDL(clear_marks_kernel<true>, G, B, s, h->marks, (const uint2*)st->d_ops.p, (uint32_t)n, h->spec_marks);
-  else
-    AM_LAUNCH_PDL(clear_marks_kernel<false>, G, B, s, h->marks, (const uint2*)st->d_ops.p, (uint32_t)n, (uint32_t*)nullptr);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaEventRecord(st->drained, s));
-  st->drain_pending = true;
-  return AM_OK;
+  return clear_marks(h, *st, h->pend_clear_n, h->pend_clear_spec, s);
 }
 
 // Workflow timeouts: no deadline in [first, first + n) (the segment bounds stay lower bounds: a segment reached by its
 // bound finds nothing and gets its exact minimum); `all` also resets every bound.
 int drop_deadlines(am_sweep* h, cudaStream_t s, uint64_t first, uint64_t n, bool all) {
-  AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, s, h->deadline + first, kNoDeadline, n);
-  h->launches++;
+  AM_CUDA(h, launch(h, fill_i64_kernel, h->sms * 8, 256, s, h->deadline + first, kNoDeadline, n));
   if (all) AM_CUDA(h, cudaMemsetAsync(h->seg_deadline, 0xFF, h->cap_padded / kRecPerWarp * 8, s));
-  AM_CUDA(h, cudaGetLastError());
   return AM_OK;
 }
 
@@ -510,9 +549,7 @@ bool admission_on(const am_sweep* h) { return h->hold && h->adm_ctl; }
 
 // No slot waits for admission, the FIFO is empty, the last tick's numbers are zero (the oldest second INT64_MAX).
 int reset_admission(am_sweep* h, cudaStream_t s) {
-  AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, s, h->adm_wait, kNotWaiting, h->cap_padded);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, launch(h, fill_i64_kernel, h->sms * 8, 256, s, h->adm_wait, kNotWaiting, h->cap_padded));
   AdmCtl z{};
   z.oldest = INT64_MAX;
   AM_CUDA(h, cudaMemcpyAsync(h->adm_ctl, &z, sizeof z, cudaMemcpyHostToDevice, s));  // (pageable: copied before the return)
@@ -540,19 +577,15 @@ int alloc_admission(am_sweep* h, cudaStream_t s) {
 int admission_waiting(am_sweep* h, bool* out) {
   *out = false;
   if (!admission_on(h)) return AM_OK;
-  const int rc = set_stream(h, h->stream);
+  int rc = set_stream(h, h->stream);
   if (rc != AM_OK) return rc;
-  AM_CUDA(h, h->dev_in.reserve(8));
-  AM_CUDA(h, h->pin_in.reserve(8));
-  AM_CUDA(h, cudaMemsetAsync(h->dev_in.p, 0xFF, 8, h->stream));
-  AM_LAUNCH(adm_next_due_kernel, h->sms * 4, 256, h->stream, (const uint32_t*)h->adm_fifo, (const int64_t*)h->adm_wait,
-            (const AdmCtl*)h->adm_ctl, (int64_t)0, (unsigned long long*)h->dev_in.p);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, 8, cudaMemcpyDeviceToHost, h->stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  *out = *(const unsigned long long*)h->pin_in.p != ~0ull;
-  return AM_OK;
+  unsigned long long key;
+  rc = min_key(h, [&](unsigned long long* k) {
+    return launch(h, adm_next_due_kernel, h->sms * 4, 256, h->stream, (const uint32_t*)h->adm_fifo,
+                  (const int64_t*)h->adm_wait, (const AdmCtl*)h->adm_ctl, (int64_t)0, k);
+  }, &key);
+  if (rc == AM_OK) *out = key != ~0ull;
+  return rc;
 }
 
 // The FIFO rebuilt from the waiting seconds of the swept slots, in admission order (second, then slot), on the host: a
@@ -598,14 +631,12 @@ int launch_admission(am_sweep* h, int64_t T, const TickSet& ts, cudaStream_t s) 
   a.budget = h->budget;
   a.T = T;
   const unsigned grid = (unsigned)h->sms * 4;  // (the per-entry passes loop over the backlog's chunks)
-  AM_LAUNCH(adm_masks_kernel, a.n_groups, kGroupWords, s, a);
-  AM_LAUNCH(adm_check_kernel, grid, kAdmBlock, s, a);
-  AM_LAUNCH(adm_plan_kernel, 1, 1024, s, a);
-  AM_LAUNCH(adm_fifo_kernel, grid, kAdmBlock, s, a);
-  AM_LAUNCH(adm_fresh_kernel, a.n_groups, kGroupWords, s, a);
-  AM_LAUNCH(adm_merge_kernel, grid, 256, s, a);
-  h->launches += 6;
-  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, launch(h, adm_masks_kernel, a.n_groups, kGroupWords, s, a));
+  AM_CUDA(h, launch(h, adm_check_kernel, grid, kAdmBlock, s, a));
+  AM_CUDA(h, launch(h, adm_plan_kernel, 1, 1024, s, a));
+  AM_CUDA(h, launch(h, adm_fifo_kernel, grid, kAdmBlock, s, a));
+  AM_CUDA(h, launch(h, adm_fresh_kernel, a.n_groups, kGroupWords, s, a));
+  AM_CUDA(h, launch(h, adm_merge_kernel, grid, 256, s, a));
   return AM_OK;
 }
 
@@ -618,33 +649,35 @@ int expire_runs(am_sweep* h, cudaStream_t s, int64_t T) {
   AM_CUDA(h, cudaMemsetAsync(h->to_count, 0, 4, s));
   const uint64_t n_seg = (h->n_records + kRecPerWarp - 1) / kRecPerWarp;
   if (n_seg) {  // one lane per segment bound, one warp per 32 of them
-    AM_LAUNCH_PDL(expire_runs_kernel, (unsigned)((n_seg + 255) / 256), 256, s, h->cols, h->since, h->deadline,
-                  h->seg_deadline, (uint32_t)n_seg, T, h->to_idx, h->to_since, h->to_count);
-    h->launches++;
-    if (h->details) {  // (before note_slots_kernel: a clear bit means the slot's pair is stale)
-      AM_LAUNCH_PDL(capture_timeouts_kernel, h->sms, 256, s, h->det_applied, h->det_start, (const uint32_t*)h->chg_bits,
-                    (const uint32_t*)h->to_idx, (const int64_t*)h->to_since, (const uint32_t*)h->to_count);
-      h->launches++;
-    }
-    if (h->track) {  // status changes: every timed-out run gets its Failed applied by this tick
-      AM_LAUNCH_PDL(note_slots_kernel, h->sms, 256, s, h->chg_bits, (const uint32_t*)h->to_idx, (const uint32_t*)h->to_count);
-      h->launches++;
-    }
+    AM_CUDA(h, launch_pdl(h, expire_runs_kernel, (unsigned)((n_seg + 255) / 256), 256, s, h->cols, h->since,
+                          h->deadline, h->seg_deadline, (uint32_t)n_seg, T, h->to_idx, h->to_since, h->to_count));
+    if (h->details)  // (before note_slots_kernel: a clear bit means the slot's pair is stale)
+      AM_CUDA(h, launch_pdl(h, capture_timeouts_kernel, h->sms, 256, s, h->det_applied, h->det_start,
+                            (const uint32_t*)h->chg_bits, (const uint32_t*)h->to_idx, (const int64_t*)h->to_since,
+                            (const uint32_t*)h->to_count));
+    if (h->track)  // status changes: every timed-out run gets its Failed applied by this tick
+      AM_CUDA(h, launch_pdl(h, note_slots_kernel, h->sms, 256, s, h->chg_bits, (const uint32_t*)h->to_idx,
+                            (const uint32_t*)h->to_count));
   }
-  AM_CUDA(h, cudaGetLastError());
   return AM_OK;
 }
 
 // Status changes: the bits of slots [first, first + n) from the flags as they stand (a live record with a pending result
 // is changed by the next tick), for turning tracking on and for am_sweep_load_range.
 int seed_changes(am_sweep* h, cudaStream_t s, uint64_t first, uint64_t n) {
-  AM_LAUNCH(seed_changes_kernel, h->sms * 8, 256, s, h->chg_bits, (const uint32_t*)h->cols.flags, first, n);
-  h->launches++;
-  if (h->details) {
-    AM_LAUNCH(seed_details_kernel, h->sms * 8, 256, s, h->det_applied, h->det_start, (const uint32_t*)h->cols.flags, first, n);
-    h->launches++;
-  }
-  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, launch(h, seed_changes_kernel, h->sms * 8, 256, s, h->chg_bits, (const uint32_t*)h->cols.flags, first, n));
+  if (h->details)
+    AM_CUDA(h, launch(h, seed_details_kernel, h->sms * 8, 256, s, h->det_applied, h->det_start,
+                      (const uint32_t*)h->cols.flags, first, n));
+  return AM_OK;
+}
+
+// The plane words of every segment that overlaps slots [first, first + n), the partial ones at either end included (a
+// load or a restore of the range), on the handle's stream.
+int rebuild_planes(am_sweep* h, uint64_t first, uint64_t n) {
+  const uint64_t seg0 = first / kRecPerWarp, n_seg = (first + n + kRecPerWarp - 1) / kRecPerWarp - seg0;
+  AM_CUDA(h, launch(h, build_planes_range_kernel, (unsigned)((n_seg + kWarps - 1) / kWarps), kBlock, h->stream, h->cols,
+                    h->planes, (uint32_t)seg0, (uint32_t)n_seg));
   return AM_OK;
 }
 
@@ -659,29 +692,26 @@ int list_changes(am_sweep* h, cudaStream_t s, int parity, bool closed, int64_t T
   if (h->n_records == 0) return AM_OK;  // (nothing swept: the list stays empty)
   const TickSet& ts = h->set[parity];
   const uint32_t n_tiles = tiles_of(h->n_records), n_groups = groups_of(h->n_records);
-  if (h->details) {
-    AM_LAUNCH_PDL(capture_sweep_kernel, (n_tiles + kWarps - 1) / kWarps, kBlock, s, h->det_applied, h->det_start,
-                  (const uint32_t*)h->chg_bits, ts.out, n_tiles, closed);
-    h->launches++;
-  }
-  AM_LAUNCH_PDL(note_exceptions_kernel, (n_tiles + kWarps - 1) / kWarps, kBlock, s, h->chg_bits, ts.out, n_tiles, closed);
-  AM_LAUNCH_PDL(count_changes_kernel, n_groups, kGroupWords, s, h->chg_bits, (const uint32_t*)h->cols.flags, h->chg_group);
+  if (h->details)
+    AM_CUDA(h, launch_pdl(h, capture_sweep_kernel, (n_tiles + kWarps - 1) / kWarps, kBlock, s, h->det_applied,
+                          h->det_start, (const uint32_t*)h->chg_bits, ts.out, n_tiles, closed));
+  AM_CUDA(h, launch_pdl(h, note_exceptions_kernel, (n_tiles + kWarps - 1) / kWarps, kBlock, s, h->chg_bits, ts.out,
+                        n_tiles, closed));
+  AM_CUDA(h, launch_pdl(h, count_changes_kernel, n_groups, kGroupWords, s, h->chg_bits, (const uint32_t*)h->cols.flags,
+                        h->chg_group));
   ScanParams sc{};
   sc.group_count = h->chg_group;
   sc.group_prefix = h->chg_prefix;
   sc.acc = h->chg_acc;
   sc.n_groups = n_groups;
   sc.cap = 0xFFFFFFFFu;
-  AM_LAUNCH_PDL(scan_groups_kernel, 1, 1024, s, sc);
-  AM_LAUNCH_PDL(list_changes_kernel, n_groups, kGroupWords, s, h->chg_bits, (const uint32_t*)h->chg_prefix, h->chg_list);
-  h->launches += 4;
-  if (h->details) {
-    AM_LAUNCH_PDL(snapshot_details_kernel, h->sms * 4, 256, s, (const uint32_t*)h->chg_list,
-                  (const unsigned long long*)(h->chg_acc + 1), (const uint8_t*)h->det_applied, (const int64_t*)h->det_start,
-                  h->det_e_applied, h->det_e_start);
-    h->launches++;
-  }
-  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, launch_pdl(h, scan_groups_kernel, 1, 1024, s, sc));
+  AM_CUDA(h, launch_pdl(h, list_changes_kernel, n_groups, kGroupWords, s, h->chg_bits, (const uint32_t*)h->chg_prefix,
+                        h->chg_list));
+  if (h->details)
+    AM_CUDA(h, launch_pdl(h, snapshot_details_kernel, h->sms * 4, 256, s, (const uint32_t*)h->chg_list,
+                          (const unsigned long long*)(h->chg_acc + 1), (const uint8_t*)h->det_applied,
+                          (const int64_t*)h->det_start, h->det_e_applied, h->det_e_start));
   h->chg_listed = true;
   return AM_OK;
 }
@@ -700,6 +730,8 @@ int claim_set(am_sweep* h, TickSet& ts, cudaStream_t s) {
   return AM_OK;
 }
 
+// Apply staged upserts / removes / results on stream `s` (called with the tick guard held).
+// The staging lock is held only for the buffer swap.
 int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, bool defer_clear = false) {
   Staging* st;
   {
@@ -755,70 +787,50 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   const unsigned B = 256, G = (unsigned)((n + B - 1) / B);
   const bool spec = st->n_spec != 0;
   if (spec && !h->spec_marks) AM_CUDA(h, dev_array(h, &h->spec_marks, h->cap_padded * 4, s));
-  if (spec)
-    AM_LAUNCH(mark_ops_kernel<true>, G, B, s, h->marks, d_ops, (uint32_t)n, h->spec_marks);
-  else
-    AM_LAUNCH(mark_ops_kernel<false>, G, B, s, h->marks, d_ops, (uint32_t)n, (uint32_t*)nullptr);
-  h->launches++;
-  if (st->n_state) {
-    AM_LAUNCH_PDL(apply_state_ops_kernel, G, B, s, h->cols, h->marks, d_ops, d_recs, (uint32_t)n, h->seg_dirty);
-    h->launches++;
-  }
+  auto* mark_ops = spec ? mark_ops_kernel<true> : mark_ops_kernel<false>;
+  AM_CUDA(h, launch(h, mark_ops, G, B, s, h->marks, d_ops, (uint32_t)n, spec ? h->spec_marks : nullptr));
+  if (st->n_state)
+    AM_CUDA(h, launch_pdl(h, apply_state_ops_kernel, G, B, s, h->cols, h->marks, d_ops, d_recs, (uint32_t)n,
+                          h->seg_dirty));
   if (spec) {  // spec updates on top of the upserts: their W after the upserts' W, so a later spec update's wins
     if (st->any_wf && !h->wf_timeout) {
       const int rc = alloc_timeouts(h, s);
       if (rc != AM_OK) return rc;
     }
-    if (h->wf_timeout && st->n_state) {
-      AM_LAUNCH_PDL(store_wf_timeout_kernel, G, B, s, h->wf_timeout, h->marks, d_ops, d_recs, (uint32_t)n);
-      h->launches++;
-    }
-    AM_LAUNCH_PDL(apply_spec_ops_kernel, G, B, s, h->cols, h->marks, (const uint32_t*)h->spec_marks, d_ops, d_recs,
-                  (uint32_t)n, h->seg_dirty, h->wf_timeout, h->track ? h->chg_bits : nullptr,
-                  h->details ? h->det_applied : nullptr, h->details ? h->det_start : nullptr);
-    h->launches++;
+    if (h->wf_timeout && st->n_state)
+      AM_CUDA(h, launch_pdl(h, store_wf_timeout_kernel, G, B, s, h->wf_timeout, h->marks, d_ops, d_recs, (uint32_t)n));
+    AM_CUDA(h, launch_pdl(h, apply_spec_ops_kernel, G, B, s, h->cols, h->marks, (const uint32_t*)h->spec_marks, d_ops,
+                          d_recs, (uint32_t)n, h->seg_dirty, h->wf_timeout, h->track ? h->chg_bits : nullptr,
+                          h->details ? h->det_applied : nullptr, h->details ? h->det_start : nullptr));
   }
   if (st->n_state || spec) {
     // upserts, removes and spec updates may change kinds, zones and masks: rebuild the plane words of the segments
     // they touched (every drain, so a later tick sees them whichever call drained)
-    const unsigned Gp = (unsigned)((n + kWarps - 1) / kWarps);
-    if (spec)
-      AM_LAUNCH_PDL(build_planes_dirty_kernel<true>, Gp, kBlock, s, h->cols, h->planes, h->seg_dirty, d_ops, (uint32_t)n);
-    else
-      AM_LAUNCH_PDL(build_planes_dirty_kernel<false>, Gp, kBlock, s, h->cols, h->planes, h->seg_dirty, d_ops, (uint32_t)n);
-    h->launches++;
+    auto* build_planes = spec ? build_planes_dirty_kernel<true> : build_planes_dirty_kernel<false>;
+    AM_CUDA(h, launch_pdl(h, build_planes, (unsigned)((n + kWarps - 1) / kWarps), kBlock, s, h->cols, h->planes,
+                          h->seg_dirty, d_ops, (uint32_t)n));
   }
-  if (h->track) {  // status changes: the phases of this drain that survive, and what its upserts and removes overwrote
-    AM_LAUNCH_PDL(note_ops_kernel, G, B, s, h->chg_bits, (const uint32_t*)h->cols.flags, h->marks, d_ops, (uint32_t)n);
-    h->launches++;
-  }
+  if (h->track)  // status changes: the phases of this drain that survive, and what its upserts and removes overwrote
+    AM_CUDA(h, launch_pdl(h, note_ops_kernel, G, B, s, h->chg_bits, (const uint32_t*)h->cols.flags, h->marks, d_ops,
+                          (uint32_t)n));
   if (h->details) {  // change details: what the surviving phases apply and the runs they end (since not yet cleared)
-    AM_LAUNCH_PDL(capture_ops_kernel, G, B, s, h->det_applied, h->det_start, h->cols,
-                  (const int64_t*)(h->hold ? h->since : nullptr), (const uint32_t*)h->marks, d_ops, (uint32_t)n);
-    if (spec)
-      AM_LAUNCH_PDL(capture_superseded_kernel<true>, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n,
-                    d_calls, n_calls);
-    else
-      AM_LAUNCH_PDL(capture_superseded_kernel<false>, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n,
-                    d_calls, n_calls);
-    h->launches += 2;
+    AM_CUDA(h, launch_pdl(h, capture_ops_kernel, G, B, s, h->det_applied, h->det_start, h->cols,
+                          (const int64_t*)(h->hold ? h->since : nullptr), (const uint32_t*)h->marks, d_ops,
+                          (uint32_t)n));
+    auto* superseded = spec ? capture_superseded_kernel<true> : capture_superseded_kernel<false>;
+    AM_CUDA(h, launch_pdl(h, superseded, G, B, s, h->det_start, (const uint32_t*)h->marks, d_ops, (uint32_t)n, d_calls,
+                          n_calls));
   }
   if (st->any_wf && !h->wf_timeout) {
     const int rc = alloc_timeouts(h, s);
     if (rc != AM_OK) return rc;
   }
-  if (h->wf_timeout && st->n_state && !spec) {  // (upserts with W = 0 overwrite an older W as well)
-    AM_LAUNCH_PDL(store_wf_timeout_kernel, G, B, s, h->wf_timeout, h->marks, d_ops, d_recs, (uint32_t)n);
-    h->launches++;
-  }
-  if (h->hold) {  // a posted workflow phase or a remove ends the slot's run (an upsert keeps the hold)
-    AM_LAUNCH_PDL(clear_since_kernel, G, B, s, h->since, d_ops, (uint32_t)n);
-    h->launches++;
-  }
-  if (admission_on(h)) {  // ... and ends the slot's wait for admission (its FIFO entry is dropped at the next tick)
-    AM_LAUNCH_PDL(clear_since_kernel, G, B, s, h->adm_wait, d_ops, (uint32_t)n);
-    h->launches++;
-  }
+  if (h->wf_timeout && st->n_state && !spec)  // (upserts with W = 0 overwrite an older W as well)
+    AM_CUDA(h, launch_pdl(h, store_wf_timeout_kernel, G, B, s, h->wf_timeout, h->marks, d_ops, d_recs, (uint32_t)n));
+  if (h->hold)  // a posted workflow phase or a remove ends the slot's run (an upsert keeps the hold)
+    AM_CUDA(h, launch_pdl(h, clear_since_kernel, G, B, s, h->since, d_ops, (uint32_t)n));
+  if (admission_on(h))  // ... and ends the slot's wait for admission (its FIFO entry is dropped at the next tick)
+    AM_CUDA(h, launch_pdl(h, clear_since_kernel, G, B, s, h->adm_wait, d_ops, (uint32_t)n));
   // Workflow timeouts expire here, ahead of the result kernels: a remedy phase posted alone in this drain is then
   // applied together with the synthetic Failed, as it is behind a Failed posted after it (the remedy gate sees both).
   if (tick_T) {
@@ -832,31 +844,21 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   if (tick_T && st->n_result && h->early_results && (uint64_t)st->n_result * 8 <= h->n_records) {
     TickSet& ts = h->set[h->parity];  // the buffer set of the tick being prepared
     if (int rc = claim_set(h, ts, s)) return rc;
-    if (h->remedy)  // (remedy runs start here; the deadline words exist with the timeout state)
-      AM_LAUNCH_PDL(apply_results_now_kernel<true>, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc, h->since,
-                    h->deadline, (const int32_t*)h->wf_timeout, h->seg_deadline);
-    else
-      AM_LAUNCH_PDL(apply_results_now_kernel<false>, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc,
-                    (int64_t*)nullptr, (int64_t*)nullptr, (const int32_t*)nullptr, (unsigned long long*)nullptr);
-    h->launches++;
+    const bool r = h->remedy;  // (remedy runs start here; the deadline words exist with the timeout state)
+    auto* apply_now = r ? apply_results_now_kernel<true> : apply_results_now_kernel<false>;
+    AM_CUDA(h, launch_pdl(h, apply_now, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc,
+                          r ? h->since : nullptr, r ? h->deadline : nullptr,
+                          r ? (const int32_t*)h->wf_timeout : nullptr, r ? h->seg_deadline : nullptr));
   } else if (st->n_result) {
-    AM_LAUNCH_PDL(apply_result_ops_kernel, G, B, s, h->cols.flags, h->marks, d_ops, (uint32_t)n);
-    h->launches++;
+    AM_CUDA(h, launch_pdl(h, apply_result_ops_kernel, G, B, s, h->cols.flags, h->marks, d_ops, (uint32_t)n));
   }
   if (defer_clear) {  // (the caller runs finish_deferred_clear on the same stream before anything else touches the handle)
     h->pend_clear = st;
     h->pend_clear_n = n;
     h->pend_clear_spec = spec;
-    AM_CUDA(h, cudaGetLastError());
   } else {
-    if (spec)
-      AM_LAUNCH_PDL(clear_marks_kernel<true>, G, B, s, h->marks, d_ops, (uint32_t)n, h->spec_marks);
-    else
-      AM_LAUNCH_PDL(clear_marks_kernel<false>, G, B, s, h->marks, d_ops, (uint32_t)n, (uint32_t*)nullptr);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
-    AM_CUDA(h, cudaEventRecord(st->drained, s));
-    st->drain_pending = true;
+    const int rc = clear_marks(h, *st, n, spec, s);
+    if (rc != AM_OK) return rc;
   }
   st->n_ops = st->n_recs = st->flushed_ops = st->flushed_recs = 0;
   st->done_ops = 0;
@@ -1036,8 +1038,8 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
     p.tz_table = (const TickWords*)h->win_boxes.dev;
   }
   if (masks && h->tz_n > 1) {  // the tick's wall clock per zone, from the cached offsets
-    AM_LAUNCH_PDL(tz_words_kernel, (h->tz_n + 63) / 64, 64, s, (const int32_t*)h->tz_off.dev, h->tz_table, T, h->tz_n);
-    h->launches++;
+    AM_CUDA(h, launch_pdl(h, tz_words_kernel, (h->tz_n + 63) / 64, 64, s, (const int32_t*)h->tz_off.dev, h->tz_table, T,
+                          h->tz_n));
     p.tz_table = h->tz_table;
   }
   if (masks) {  // the six planes of T's UTC fields
@@ -1063,8 +1065,7 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   // drain).  am_sweep_tick_shard's is a plain launch: an early-launched sweep could park its CTAs on every SM ahead
   // of the previous tick's exchange on the other stream; measured at two GPUs it made no difference to the step, so
   // the simpler form stays.
-  if (o.expand) AM_LAUNCH_PDL(sweep, p.n_tiles, kBlock, s, p);
-  else AM_LAUNCH(sweep, p.n_tiles, kBlock, s, p);
+  AM_CUDA(h, o.expand ? launch_pdl(h, sweep, p.n_tiles, kBlock, s, p) : launch(h, sweep, p.n_tiles, kBlock, s, p));
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[1], s));
   if (admission_on(h)) {  // the submit budget cuts the sweep's output in place (profiling: counted in the rest)
     const int rc = launch_admission(h, T, ts, s);
@@ -1077,8 +1078,7 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
   sc.out_count = o.count;
   sc.n_groups = groups_of(h->n_records);
   sc.cap = (uint32_t)(o.cap > 0xFFFFFFFFull ? 0xFFFFFFFFull : o.cap);
-  AM_LAUNCH_PDL(scan_groups_kernel, 1, 1024, s, sc);
-  h->launches += 2;
+  AM_CUDA(h, launch_pdl(h, scan_groups_kernel, 1, 1024, s, sc));
   if (o.expand) {
     ExpandParams e{};
     e.src[0].bitmap = ts.out.bitmap;
@@ -1096,13 +1096,11 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
     e.world = 1;
     e.stats_rank = 0;
     e.idx_bytes = 4;
-    AM_LAUNCH_PDL(expand_kernel, dim3(sc.n_groups, 1), kExpandThreads, s, e);
-    AM_LAUNCH_PDL(publish_kernel, 1, 32, s, ts.acc, o.stats, h->n_records);
-    h->launches += 2;
+    AM_CUDA(h, launch_pdl(h, expand_kernel, dim3(sc.n_groups, 1), kExpandThreads, s, e));
+    AM_CUDA(h, launch_pdl(h, publish_kernel, 1, 32, s, ts.acc, o.stats, h->n_records));
   }
   if (h->profiling) { AM_CUDA(h, cudaEventRecord(h->evp[2], s)); h->profiled = true; }
   h->parity ^= 1;
-  AM_CUDA(h, cudaGetLastError());
   return AM_OK;
 }
 
@@ -1233,10 +1231,10 @@ uint64_t block_ticks() {
 
 // Temporal blocking (sweep_block.cuh): the n ticks from T0 in blocks of up to block_ticks() ticks, one pass over the
 // columns each.  A block never spans an instant at which a registered zone changes its UTC offset (the kernel holds one
-// offset per zone for the whole block).  Per block, `b`'s BlockParams part is filled in and launch(b, k, grid) launches
-// the caller's instantiation for the block that starts at tick k.
+// offset per zone for the whole block).  Per block, `b`'s BlockParams part is filled in and launch_block(b, k, grid)
+// launches the caller's instantiation for the block that starts at tick k, returning the launch error.
 template <class P, class Launch>
-int run_blocks(am_sweep* h, int64_t T0, uint64_t n, am_tick_stats_t* stats, P b, Launch&& launch) {
+int run_blocks(am_sweep* h, int64_t T0, uint64_t n, am_tick_stats_t* stats, P b, Launch&& launch_block) {
   const uint64_t per_block = block_ticks();
   const unsigned grid = (unsigned)((h->n_records + kBlockRecords - 1) / kBlockRecords);
   for (uint64_t k = 0; k < n;) {
@@ -1253,9 +1251,7 @@ int run_blocks(am_sweep* h, int64_t T0, uint64_t n, am_tick_stats_t* stats, P b,
     b.K = (uint32_t)K;
     b.tz_off = h->tz_n > 1 ? (const int32_t*)h->tz_off.dev : nullptr;
     b.stats = reinterpret_cast<unsigned long long*>(stats + k);
-    launch(b, k, grid);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, launch_block(b, k, grid));
     k += K;
   }
   return AM_OK;
@@ -1312,24 +1308,14 @@ bool shard_last_tick(am_sweep* h, ShardTick* out) {
   out->device = h->device;
   return true;
 }
-int shard_order_consumer(am_sweep* h, cudaStream_t s) {
-  if (h->has_last && h->last_stream != s) {
-    AM_CUDA(h, cudaEventRecord(h->ev_last, h->last_stream));
-    AM_CUDA(h, cudaStreamWaitEvent(s, h->ev_last, 0));
-  }
-  return AM_OK;
-}
+int shard_order_consumer(am_sweep* h, cudaStream_t s) { return wait_last(h, s); }
 int shard_launch_expand(am_sweep* h, const ExpandParams& e, uint32_t groups_x, uint32_t world_y, cudaStream_t s) {
-  AM_LAUNCH(expand_kernel, dim3(groups_x, world_y), kExpandThreads, s, e);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, launch(h, expand_kernel, dim3(groups_x, world_y), kExpandThreads, s, e));
   return AM_OK;
 }
 int shard_launch_publish(am_sweep* h, unsigned long long* acc, am_tick_stats_t* out_stats, uint64_t n_records,
                          cudaStream_t s) {
-  AM_LAUNCH(publish_kernel, 1, 32, s, acc, out_stats, n_records);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
+  AM_CUDA(h, launch(h, publish_kernel, 1, 32, s, acc, out_stats, n_records));
   return AM_OK;
 }
 int shard_mark_consumed(am_sweep* h, int parity, cudaStream_t s) {
@@ -1378,8 +1364,7 @@ int am_sweep_create(am_sweep_t** out, int device_id, uint64_t capacity, uint64_t
       AM_CUDA(h, new_event(h, e));
     for (cudaEvent_t* e : {&h->ev0, &h->ev1, &h->evp[0], &h->evp[1], &h->evp[2]}) AM_CUDA(h, new_event(h, e, true));
     for (int k = 0; k < 16; ++k) AM_CUDA(h, dev_array(h, col_slot(h->cols, k), h->cap_padded * kColElem[k], h->stream));
-    AM_LAUNCH(fill_u32_kernel, h->sms * 8, 256, h->stream, h->cols.flags, AM_F_TOMBSTONE, h->cap_padded);
-    h->launches++;
+    AM_CUDA(h, launch(h, fill_u32_kernel, h->sms * 8, 256, h->stream, h->cols.flags, AM_F_TOMBSTONE, h->cap_padded));
     // the mask planes: every slot is a tombstone, no record has a plane bit
     h->planes.words = h->cap_padded / 32;
     AM_CUDA(h, dev_array(h, &h->planes.w, kPlanes * h->planes.words * 4, h->stream));
@@ -1404,7 +1389,6 @@ int am_sweep_create(am_sweep_t** out, int device_id, uint64_t capacity, uint64_t
     AM_CUDA(h, host_array(h, &h->h_stats, sizeof(am_tick_stats_t), cudaHostAllocMapped));
     memset(h->h_stats, 0, sizeof(am_tick_stats_t));
     AM_CUDA(h, cudaHostGetDevicePointer((void**)&h->d_stats_mapped, h->h_stats, 0));
-    AM_CUDA(h, cudaGetLastError());
     AM_CUDA(h, cudaStreamSynchronize(h->stream));
     return AM_OK;
   }();
@@ -1440,7 +1424,7 @@ uint64_t am_sweep_size(const am_sweep_t* h) { return h ? h->n_records : 0; }
 uint64_t am_sweep_capacity(const am_sweep_t* h) { return h ? h->capacity : 0; }
 int am_sweep_device(const am_sweep_t* h) { return h ? h->device : -1; }
 double am_sweep_last_kernel_ms(const am_sweep_t* h) { return h ? h->last_ms : -1.0; }
-uint64_t am_sweep_launch_count(const am_sweep_t* h) { return h ? h->launches : 0; }
+uint64_t am_sweep_launch_count(const am_sweep_t* h) { return h ? h->launches.load(std::memory_order_relaxed) : 0; }
 void* am_sweep_column_ptr(am_sweep_t* h, int column) {
   return (h && column >= 0 && column < 16) ? *col_slot(h->cols, column) : nullptr;
 }
@@ -1485,24 +1469,12 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
     if (src) AM_CUDA(h, cudaMemcpyAsync(dst, src, n * kColElem[k], cudaMemcpyHostToDevice, h->stream));
     else AM_CUDA(h, cudaMemsetAsync(dst, 0, n * kColElem[k], h->stream));
   }
-  {  // rebuild the planes of every segment that overlaps the range, the partial ones at either end included
-    const uint64_t seg0 = first / kRecPerWarp, seg1 = (first + n + kRecPerWarp - 1) / kRecPerWarp;
-    const uint64_t n_seg = seg1 - seg0;
-    AM_LAUNCH(build_planes_range_kernel, (unsigned)((n_seg + kWarps - 1) / kWarps), kBlock, h->stream, h->cols, h->planes,
-              (uint32_t)seg0, (uint32_t)n_seg);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
-  }
-  if (h->hold) {  // loaded records have nothing in flight
-    AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, h->stream, h->since + first, kNotInFlight, n);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
-  }
-  if (admission_on(h)) {  // ... and wait for nothing
-    AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, h->stream, h->adm_wait + first, kNotWaiting, n);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
-  }
+  rc = rebuild_planes(h, first, n);
+  if (rc != AM_OK) return rc;
+  if (h->hold)  // loaded records have nothing in flight
+    AM_CUDA(h, launch(h, fill_i64_kernel, h->sms * 8, 256, h->stream, h->since + first, kNotInFlight, n));
+  if (admission_on(h))  // ... and wait for nothing
+    AM_CUDA(h, launch(h, fill_i64_kernel, h->sms * 8, 256, h->stream, h->adm_wait + first, kNotWaiting, n));
   if (h->wf_timeout) {  // am_record_cols_t has no timeout column: loaded slots have none, and no deadline
     AM_CUDA(h, cudaMemsetAsync(h->wf_timeout + first, 0, n * 4, h->stream));
     rc = drop_deadlines(h, h->stream, first, n, false);
@@ -1526,9 +1498,7 @@ int am_sweep_set_hold_in_flight(am_sweep_t* h, int on) {
     int rc = set_stream(h, h->stream);
     if (rc != AM_OK) return rc;
     if (!h->since) AM_CUDA(h, dev_array(h, &h->since, h->cap_padded * sizeof(int64_t), h->stream, false));
-    AM_LAUNCH(fill_i64_kernel, h->sms * 8, 256, h->stream, h->since, kNotInFlight, h->cap_padded);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, launch(h, fill_i64_kernel, h->sms * 8, 256, h->stream, h->since, kNotInFlight, h->cap_padded));
     if (h->wf_timeout) {  // (the deadlines of runs from before the hold was turned off)
       rc = drop_deadlines(h, h->stream, 0, h->cap_padded, true);
       if (rc != AM_OK) return rc;
@@ -1594,9 +1564,7 @@ int am_sweep_set_hold_remedy(am_sweep_t* h, int on) {
   if (!on) {  // every remedy run ends (the segment bounds stay lower bounds)
     int rc = set_stream(h, h->stream);
     if (rc != AM_OK) return rc;
-    AM_LAUNCH(release_remedy_runs_kernel, h->sms * 8, 256, h->stream, h->since, h->deadline, h->cap_padded);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, launch(h, release_remedy_runs_kernel, h->sms * 8, 256, h->stream, h->since, h->deadline, h->cap_padded));
   }
   h->remedy = on != 0;
   return AM_OK;
@@ -1645,10 +1613,8 @@ int am_sweep_set_change_details(am_sweep_t* h, int on) {
       AM_CUDA(h, dev_array(h, &h->det_e_applied, h->cap_padded, h->stream, false));
       AM_CUDA(h, dev_array(h, &h->det_e_start, h->cap_padded * 8, h->stream, false));
     }
-    AM_LAUNCH(seed_details_kernel, h->sms * 8, 256, h->stream, h->det_applied, h->det_start, (const uint32_t*)h->cols.flags,
-              (uint64_t)0, h->cap_padded);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, launch(h, seed_details_kernel, h->sms * 8, 256, h->stream, h->det_applied, h->det_start,
+                      (const uint32_t*)h->cols.flags, (uint64_t)0, h->cap_padded));
   }
   h->details = on != 0;
   return AM_OK;
@@ -1884,8 +1850,8 @@ int am_sweep_run_ticks(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint3
   return run_rows(h, unix_sec0, n_ticks, blocked, false, stats_out, nullptr, [&](const RunRows& rows) -> int {
     if (blocked)
       return run_blocks(h, unix_sec0, n_ticks, rows.stats, BlockParams{}, [&](const BlockParams& b, uint64_t, unsigned grid) {
-        if (mode & AM_SWEEP_CLOSED_LOOP) AM_LAUNCH(sweep_block_kernel<true>, grid, kBlockThreads, h->stream, b);
-        else AM_LAUNCH(sweep_block_kernel<false>, grid, kBlockThreads, h->stream, b);
+        auto* k = (mode & AM_SWEEP_CLOSED_LOOP) ? sweep_block_kernel<true> : sweep_block_kernel<false>;
+        return launch(h, k, grid, kBlockThreads, h->stream, b);
       });
     for (uint64_t k = 0; k < n_ticks; ++k) {
       const ListOut o{h->due_idx[k & 1], h->due_action[k & 1], h->cap_padded, nullptr, rows.stats + k};
@@ -1940,8 +1906,7 @@ int am_sweep_simulate(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint32
       sb.q = q;
       return run_blocks(h, unix_sec0, n_ticks, rows.stats, sb, [&](SimBlockParams& b, uint64_t k, unsigned grid) {
         b.sim = rows.sim + k * 4;
-        void (*const block_fn)(const SimBlockParams) = sweep_block_kernel<false, true>;
-        AM_LAUNCH(block_fn, grid, kBlockThreads, h->stream, b);
+        return launch(h, sweep_block_kernel<false, true>, grid, kBlockThreads, h->stream, b);
       });
     }
     // Tick by tick: the completion pass, then the tick (expiry pass and sweep), then the bounds of the runs it started
@@ -1949,37 +1914,26 @@ int am_sweep_simulate(am_sweep_t* h, int64_t unix_sec0, uint64_t n_ticks, uint32
     const uint64_t n_seg = (h->n_records + kRecPerWarp - 1) / kRecPerWarp;
     const int64_t earliest = params->wf_min < params->remedy_min ? params->wf_min : params->remedy_min;
     AM_CUDA(h, cudaMemsetAsync(h->sim_end, 0xFF, h->cap_padded / kRecPerWarp * 8, h->stream));
-    if (h->n_records) {
-      AM_LAUNCH(sim_bounds_kernel, (unsigned)((h->n_records + 255) / 256), 256, h->stream, h->cols, (const int64_t*)h->since,
-                h->sim_end, h->n_records, q, h->shard_base);
-      h->launches++;
-      AM_CUDA(h, cudaGetLastError());
-    }
+    if (h->n_records)
+      AM_CUDA(h, launch(h, sim_bounds_kernel, (unsigned)((h->n_records + 255) / 256), 256, h->stream, h->cols,
+                        (const int64_t*)h->since, h->sim_end, h->n_records, q, h->shard_base));
     for (uint64_t k = 0; k < n_ticks; ++k) {
       const int64_t T = unix_sec0 + (int64_t)k;
-      if (n_seg) {
-        AM_LAUNCH_PDL(sim_complete_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream, h->cols, h->since, h->sim_end,
-                      (uint32_t)n_seg, T, q, h->shard_base);
-        h->launches++;
-        AM_CUDA(h, cudaGetLastError());
-      }
+      if (n_seg)
+        AM_CUDA(h, launch_pdl(h, sim_complete_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream, h->cols,
+                              h->since, h->sim_end, (uint32_t)n_seg, T, q, h->shard_base));
       int trc = expire_runs(h, h->stream, T);
       if (trc != AM_OK) return trc;
       const int parity = (int)h->parity;
       const ListOut o{h->due_idx[k & 1], h->due_action[k & 1], h->cap_padded, nullptr, rows.stats + k};
       trc = launch_tick(h, T, mode & AM_SWEEP_FULL_SCAN, o, h->stream);
       if (trc != AM_OK) return trc;
-      if (n_seg) {
-        AM_LAUNCH_PDL(sim_note_starts_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream,
-                      (const uint32_t*)h->set[parity].out.bitmap, h->sim_end, (uint32_t)n_seg, T + earliest);
-        h->launches++;
-        AM_CUDA(h, cudaGetLastError());
-      }
-      AM_LAUNCH_PDL(sim_count_kernel, h->sms * 8, 256, h->stream, h->cols, (const int64_t*)h->since, h->n_records,
-                    (const int64_t*)(h->to_ran ? h->to_since : nullptr), (const uint32_t*)(h->to_ran ? h->to_count : nullptr),
-                    rows.sim + k * 4);
-      h->launches++;
-      AM_CUDA(h, cudaGetLastError());
+      if (n_seg)
+        AM_CUDA(h, launch_pdl(h, sim_note_starts_kernel, (unsigned)((n_seg + 255) / 256), 256, h->stream,
+                              (const uint32_t*)h->set[parity].out.bitmap, h->sim_end, (uint32_t)n_seg, T + earliest));
+      AM_CUDA(h, launch_pdl(h, sim_count_kernel, h->sms * 8, 256, h->stream, h->cols, (const int64_t*)h->since,
+                            h->n_records, (const int64_t*)(h->to_ran ? h->to_since : nullptr),
+                            (const uint32_t*)(h->to_ran ? h->to_count : nullptr), rows.sim + k * 4));
     }
     return AM_OK;
   });
@@ -1999,14 +1953,10 @@ int am_sweep_repeat_after_sec(am_sweep_t* h, int64_t unix_sec, uint64_t first, u
   int rc = begin_call(h);
   if (rc != AM_OK) return rc;
   AM_CUDA(h, h->dev_in.reserve(n * 8));
-  AM_CUDA(h, h->pin_in.reserve(n * 8));
-  AM_LAUNCH(next_fire_kernel, (unsigned)((n + 127) / 128), 128, h->stream, h->cols, (uint32_t)first, (uint32_t)n,
-            unix_sec, (int64_t*)h->dev_in.p);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * 8, cudaMemcpyDeviceToHost, h->stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  memcpy(out, h->pin_in.p, n * 8);
+  AM_CUDA(h, launch(h, next_fire_kernel, (unsigned)((n + 127) / 128), 128, h->stream, h->cols, (uint32_t)first,
+                    (uint32_t)n, unix_sec, (int64_t*)h->dev_in.p));
+  rc = read_back(h, out, h->dev_in.p, n * 8);
+  if (rc != AM_OK) return rc;
   {  // schedules bound to a named time zone (marked kZoneBoundMark): Next() on the host
     std::vector<uint64_t> zi;
     for (uint64_t k = 0; k < n; ++k) if (out[k] == kZoneBoundMark) zi.push_back(first + k);
@@ -2042,22 +1992,17 @@ int am_sweep_next_due(am_sweep_t* h, int64_t unix_sec, int64_t* next_out) {
   if (rc != AM_OK) return rc;
   const int64_t next_minute = unix_sec + 60 - ((unix_sec % 60) + 60) % 60;
   const int64_t zone_due = (h->tz_aligned && h->tz_hi >= next_minute) ? next_minute : unix_sec + 1;
-  AM_CUDA(h, h->dev_in.reserve(8));
-  AM_CUDA(h, h->pin_in.reserve(8));
-  AM_CUDA(h, cudaMemsetAsync(h->dev_in.p, 0xFF, 8, h->stream));
-  AM_LAUNCH(next_due_kernel, h->sms * 8, 256, h->stream, h->cols, (const int64_t*)(h->hold ? h->since : nullptr),
-            (const int64_t*)(h->hold ? h->deadline : nullptr), h->n_records, unix_sec, zone_due,
-            (unsigned long long*)h->dev_in.p);
-  h->launches++;
-  if (admission_on(h)) {  // a check still waiting for admission is due at the next second
-    AM_LAUNCH(adm_next_due_kernel, h->sms * 4, 256, h->stream, (const uint32_t*)h->adm_fifo, (const int64_t*)h->adm_wait,
-              (const AdmCtl*)h->adm_ctl, unix_sec, (unsigned long long*)h->dev_in.p);
-    h->launches++;
-  }
-  AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, 8, cudaMemcpyDeviceToHost, h->stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  const unsigned long long key = *(const unsigned long long*)h->pin_in.p;
+  unsigned long long key;
+  rc = min_key(h, [&](unsigned long long* k) {
+    cudaError_t e = launch(h, next_due_kernel, h->sms * 8, 256, h->stream, h->cols,
+                           (const int64_t*)(h->hold ? h->since : nullptr),
+                           (const int64_t*)(h->hold ? h->deadline : nullptr), h->n_records, unix_sec, zone_due, k);
+    if (e == cudaSuccess && admission_on(h))  // a check still waiting for admission is due at the next second
+      e = launch(h, adm_next_due_kernel, h->sms * 4, 256, h->stream, (const uint32_t*)h->adm_fifo,
+                 (const int64_t*)h->adm_wait, (const AdmCtl*)h->adm_ctl, unix_sec, k);
+    return e;
+  }, &key);
+  if (rc != AM_OK) return rc;
   if (key != ~0ull) *next_out = (int64_t)(key ^ (1ull << 63));
   return AM_OK;
 }
@@ -2072,33 +2017,54 @@ int am_sweep_read(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx
   return rc != AM_OK ? rc : read_impl(h, first, n, idx, out);
 }
 
-static int in_flight_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out, bool remedy) {
-  if (!h || (n && !since_out)) return AM_E_INVAL;
-  if (n == 0) return AM_OK;
+}  // extern "C"
+
+namespace {
+// The slots of a per-slot call: [first, first + n) inside the capacity without `idx`, else every idx[k] (AM_E_RANGE
+// for one past it); at most 2^32 - 1 of them either way.
+int check_slots(const am_sweep* h, uint64_t first, uint64_t n, const uint64_t* idx) {
   if (n > 0xFFFFFFFFull || (!idx && (first + n > h->capacity || first + n < first))) return AM_E_INVAL;
   if (idx)
     for (uint64_t k = 0; k < n; ++k)
       if (idx[k] >= h->capacity) return AM_E_RANGE;
+  return AM_OK;
+}
+
+// am_sweep_in_flight, _remedy_in_flight and _deferred: one i64 per slot, refused before the tick guard, after the
+// staged calls; `off` everywhere while on() is false, else what gather(d_idx, d_out) — a kernel over the slots as
+// stage_indices left them, on the handle's stream — writes to d_out.
+template <class On, class Gather>
+int query_slots(am_sweep* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* out, On&& on, int64_t off,
+                Gather&& gather) {
+  if (!h || (n && !out)) return AM_E_INVAL;
+  if (n == 0) return AM_OK;
+  int rc = check_slots(h, first, n, idx);
+  if (rc != AM_OK) return rc;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  int rc = begin_call(h);  // results posted by now release their holds (left pending for the next tick)
+  rc = begin_call(h);  // posted results, removes and loads by now release holds and end waits
   if (rc != AM_OK) return rc;
-  if (!h->hold || (remedy && !h->remedy)) {
-    for (uint64_t k = 0; k < n; ++k) since_out[k] = kNotInFlight;
+  if (!on()) {
+    for (uint64_t k = 0; k < n; ++k) out[k] = off;
     return AM_OK;
   }
   const uint32_t* d_idx;
   rc = stage_indices(h, n * 8, n, idx, &d_idx);
   if (rc != AM_OK) return rc;
-  AM_LAUNCH(in_flight_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols, (const int64_t*)h->since, (uint32_t)first,
-            d_idx, (uint32_t)n, (int64_t*)h->dev_in.p, remedy);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * 8, cudaMemcpyDeviceToHost, h->stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  memcpy(since_out, h->pin_in.p, n * 8);
-  return AM_OK;
+  AM_CUDA(h, gather(d_idx, (int64_t*)h->dev_in.p));
+  return read_back(h, out, h->dev_in.p, n * 8);
 }
+
+int in_flight_impl(am_sweep* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* out, bool remedy) {
+  return query_slots(h, first, n, idx, out, [&] { return h->hold && (!remedy || h->remedy); }, kNotInFlight,
+                     [&](const uint32_t* d_idx, int64_t* d_out) {
+                       return launch(h, in_flight_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols,
+                                     (const int64_t*)h->since, (uint32_t)first, d_idx, (uint32_t)n, d_out, remedy);
+                     });
+}
+}  // namespace
+
+extern "C" {
 
 int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
   return in_flight_impl(h, first, n, idx, since_out, false);
@@ -2109,31 +2075,11 @@ int am_sweep_remedy_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const u
 }
 
 int am_sweep_deferred(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
-  if (!h || (n && !since_out)) return AM_E_INVAL;
-  if (n == 0) return AM_OK;
-  if (n > 0xFFFFFFFFull || (!idx && (first + n > h->capacity || first + n < first))) return AM_E_INVAL;
-  if (idx)
-    for (uint64_t k = 0; k < n; ++k)
-      if (idx[k] >= h->capacity) return AM_E_RANGE;
-  TickGuard g(h);
-  if (!g.ok) return AM_E_BUSY;
-  int rc = begin_call(h);  // removes, loads and posted phases by now end their slots' waits
-  if (rc != AM_OK) return rc;
-  if (!admission_on(h)) {
-    for (uint64_t k = 0; k < n; ++k) since_out[k] = kNotWaiting;
-    return AM_OK;
-  }
-  const uint32_t* d_idx;
-  rc = stage_indices(h, n * 8, n, idx, &d_idx);
-  if (rc != AM_OK) return rc;
-  AM_LAUNCH(adm_gather_kernel, (unsigned)((n + 255) / 256), 256, h->stream, (const int64_t*)h->adm_wait, (uint32_t)first,
-            d_idx, (uint32_t)n, (int64_t*)h->dev_in.p);
-  h->launches++;
-  AM_CUDA(h, cudaGetLastError());
-  AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, n * 8, cudaMemcpyDeviceToHost, h->stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  memcpy(since_out, h->pin_in.p, n * 8);
-  return AM_OK;
+  return query_slots(h, first, n, idx, since_out, [&] { return admission_on(h); }, kNotWaiting,
+                     [&](const uint32_t* d_idx, int64_t* d_out) {
+                       return launch(h, adm_gather_kernel, (unsigned)((n + 255) / 256), 256, h->stream,
+                                     (const int64_t*)h->adm_wait, (uint32_t)first, d_idx, (uint32_t)n, d_out);
+                     });
 }
 
 // One of the last tick's two timed-out lists, entries [offset, ...) as global indices: the health-check runs, or the
@@ -2144,12 +2090,10 @@ static int timed_out_impl(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
   if (h->to_ran && !h->to_fetched) {  // the device list of the last tick, waited for (it may be on a caller stream)
-    const int rc = set_stream(h, h->stream);
+    int rc = set_stream(h, h->stream);
+    uint32_t m = 0;
+    if (rc == AM_OK) rc = read_back(h, &m, h->to_count, 4);
     if (rc != AM_OK) return rc;
-    AM_CUDA(h, h->pin_in.reserve(4));
-    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->to_count, 4, cudaMemcpyDeviceToHost, h->stream));
-    AM_CUDA(h, cudaStreamSynchronize(h->stream));
-    const uint32_t m = *(const uint32_t*)h->pin_in.p;
     std::vector<uint32_t> li(m);
     std::vector<int64_t> ls(m);
     if (m) {
@@ -2178,10 +2122,8 @@ static int timed_out_impl(am_sweep_t* h, uint64_t offset, uint64_t* idx, int64_t
 // list_page over the last tick's change list (empty unless `listed`); its length is fetched once per tick.
 static int change_page(am_sweep_t* h, bool listed, uint64_t offset, uint64_t cap, uint64_t* n_out, uint64_t* ncopy) {
   if (listed && !h->chg_fetched) {
-    AM_CUDA(h, h->pin_in.reserve(8));
-    AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->chg_acc + 1, 8, cudaMemcpyDeviceToHost, h->stream));
-    AM_CUDA(h, cudaStreamSynchronize(h->stream));
-    h->chg_n = *(const unsigned long long*)h->pin_in.p;
+    const int rc = read_back(h, &h->chg_n, h->chg_acc + 1, 8);
+    if (rc != AM_OK) return rc;
     h->chg_fetched = true;
   }
   return list_page(listed ? h->chg_n : 0, offset, cap, n_out, ncopy);
@@ -2212,9 +2154,8 @@ static int gather_cols(am_sweep_t* h, const uint32_t* d_idx, uint64_t n, am_reco
     ++nc;
   }
   if (nc) {
-    AM_LAUNCH(gather_columns_kernel, dim3((unsigned)((n + 255) / 256), nc), 256, h->stream, gc, d_idx, (uint32_t)n);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, launch(h, gather_columns_kernel, dim3((unsigned)((n + 255) / 256), nc), 256, h->stream, gc, d_idx,
+                      (uint32_t)n));
     AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, bytes, cudaMemcpyDeviceToHost, h->stream));
   }
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -2281,12 +2222,9 @@ int am_sweep_last_change_details(am_sweep_t* h, uint64_t offset, uint64_t* idx, 
     AM_CUDA(h, h->pin_in.reserve(bytes));
     AM_CUDA(h, h->dev_in.reserve(bytes));
     const uint32_t* d_idx = h->chg_list + offset;
-    AM_LAUNCH(gather_details_kernel, (unsigned)((ncopy + 255) / 256), 256, h->stream, d_idx, (uint32_t)ncopy,
-              (const uint8_t*)h->det_e_applied + offset, (const int64_t*)h->det_e_start + offset, h->set[h->chg_parity].out,
-              h->chg_closed,
-              h->chg_T, (am_change_detail_t*)h->dev_in.p);
-    h->launches++;
-    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, launch(h, gather_details_kernel, (unsigned)((ncopy + 255) / 256), 256, h->stream, d_idx, (uint32_t)ncopy,
+                      (const uint8_t*)h->det_e_applied + offset, (const int64_t*)h->det_e_start + offset,
+                      h->set[h->chg_parity].out, h->chg_closed, h->chg_T, (am_change_detail_t*)h->dev_in.p));
     AM_CUDA(h, cudaMemcpyAsync(h->pin_in.p, h->dev_in.p, at, cudaMemcpyDeviceToHost, h->stream));
     AM_CUDA(h, cudaMemcpyAsync((char*)h->pin_in.p + at, d_idx, ncopy * 4, cudaMemcpyDeviceToHost, h->stream));
     AM_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -2299,8 +2237,9 @@ int am_sweep_last_change_details(am_sweep_t* h, uint64_t offset, uint64_t* idx, 
 
 // (tick guard held, staged events drained, h->stream ordered)
 static int read_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, am_record_cols_t* out) {
+  int rc = check_slots(h, first, n, idx);
+  if (rc != AM_OK) return rc;
   if (!idx) {
-    if (first + n > h->capacity || first + n < first) return AM_E_INVAL;
     for (int k = 0; k < 16; ++k) {
       void* dst = *cols_member(out, k);
       if (!dst) continue;
@@ -2310,11 +2249,8 @@ static int read_impl(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* 
     AM_CUDA(h, cudaStreamSynchronize(h->stream));
     return AM_OK;
   }
-  if (n > 0xFFFFFFFFull) return AM_E_INVAL;
-  for (uint64_t k = 0; k < n; ++k)
-    if (idx[k] >= h->capacity) return AM_E_RANGE;
   const uint32_t* d_idx;
-  const int rc = stage_indices(h, gather_bytes(n, out), n, idx, &d_idx);
+  rc = stage_indices(h, gather_bytes(n, out), n, idx, &d_idx);
   return rc != AM_OK ? rc : gather_cols(h, d_idx, n, out);
 }
 
@@ -2494,12 +2430,9 @@ int am_sweep_checkpoint(am_sweep_t* h, uint64_t first, uint64_t n, void* buf, ui
     hd.prev_tick = h->has_prev ? h->prev_T : INT64_MIN;
     hd.seed = h->seed;
     AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->stream));
-    if (n) {
-      AM_LAUNCH(checkpoint_pack_kernel, (unsigned)((n + 255) / 256), 256, h->stream, ckpt_state(h), ckpt_blob(h, L, n),
-                first, h->ck_meta, (uint32_t*)(h->ck_meta + 1));
-      h->launches++;
-      AM_CUDA(h, cudaGetLastError());
-    }
+    if (n)
+      AM_CUDA(h, launch(h, checkpoint_pack_kernel, (unsigned)((n + 255) / 256), 256, h->stream, ckpt_state(h),
+                        ckpt_blob(h, L, n), first, h->ck_meta, (uint32_t*)(h->ck_meta + 1)));
     AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->stream));
     AM_CUDA(h, cudaEventRecord(h->ck_ev, h->stream));
   }
@@ -2597,11 +2530,9 @@ int am_sweep_restore(am_sweep_t* h, const void* buf, uint64_t len) {
     h->ck_pin_pending[b] = true;
   }
   AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->ck_stream));
-  if (hd.n) {
-    AM_LAUNCH(checkpoint_verify_kernel, (unsigned)((hd.n + 255) / 256), 256, h->ck_stream, ckpt_blob(h, L, hd.n),
-              h->ck_meta, (uint32_t*)(h->ck_meta + 1));
-    AM_CUDA(h, cudaGetLastError());
-  }
+  if (hd.n)
+    AM_CUDA(h, launch(h, checkpoint_verify_kernel, (unsigned)((hd.n + 255) / 256), 256, h->ck_stream,
+                      ckpt_blob(h, L, hd.n), h->ck_meta, (uint32_t*)(h->ck_meta + 1)));
   AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
   AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
   h->ck_pin_pending[0] = h->ck_pin_pending[1] = false;
@@ -2634,13 +2565,10 @@ int am_sweep_restore(am_sweep_t* h, const void* buf, uint64_t len) {
     if (rc != AM_OK) return rc;
   }
   if (hd.n) {
-    AM_LAUNCH(checkpoint_scatter_kernel, (unsigned)((hd.n + 255) / 256), 256, h->stream, ckpt_state(h), ckpt_blob(h, L, hd.n),
-              first, lut);
-    const uint64_t seg0 = first / kRecPerWarp, n_seg = (first + hd.n + kRecPerWarp - 1) / kRecPerWarp - seg0;
-    AM_LAUNCH(build_planes_range_kernel, (unsigned)((n_seg + kWarps - 1) / kWarps), kBlock, h->stream, h->cols, h->planes,
-              (uint32_t)seg0, (uint32_t)n_seg);
-    h->launches += 2;
-    AM_CUDA(h, cudaGetLastError());
+    AM_CUDA(h, launch(h, checkpoint_scatter_kernel, (unsigned)((hd.n + 255) / 256), 256, h->stream, ckpt_state(h),
+                      ckpt_blob(h, L, hd.n), first, lut));
+    rc = rebuild_planes(h, first, hd.n);
+    if (rc != AM_OK) return rc;
   }
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   const uint64_t hwm = hd.swept_end - h->shard_base;
