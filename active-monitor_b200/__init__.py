@@ -11,7 +11,7 @@ with ``importlib.import_module("active-monitor_b200")``.
 from . import _lib as abi  # noqa: F401
 from ._lib import *  # noqa: F401,F403  (constants + ctypes structs)
 from .sweep import (AmError, Cron, CronParseError, CronUnsupported, Sweep, alloc_columns,  # noqa: F401
-                    checkpoint_info, civil_from_unix, classify, cols_struct, columns_to_records, cron_parse,
+                    checkpoint_delta_info, checkpoint_info, civil_from_unix, classify, cols_struct, columns_to_records, cron_parse,
                     records_to_columns, remedy_is_empty, tz_lookup, tz_offset)
 
 

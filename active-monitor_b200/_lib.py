@@ -136,6 +136,16 @@ class AmCheckpointInfo(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "reserved"}
 
 
+class AmCheckpointDeltaInfo(C.Structure):
+    _fields_ = [("first_global", u64), ("n", u64), ("swept_end", u64), ("prev_tick", i64), ("seed", u64),
+                ("n_changed", u64), ("seq", u64), ("parent_prev_tick", i64), ("parent_checksum", u64),
+                ("checksum", u64), ("switches", u32), ("n_zones", u32), ("version", u32), ("reserved", u32),
+                ("bytes", u64)]
+
+    def as_dict(self) -> dict:
+        return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "reserved"}
+
+
 class AmAdmission(C.Structure):
     _fields_ = [("n_candidates", u64), ("n_admitted", u64), ("n_deferred", u64), ("oldest_deferred", i64)]
 
@@ -193,6 +203,10 @@ SYMBOLS = {
     "am_sweep_checkpoint": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, u64, P(u64)]),
     "am_checkpoint_info": (C.c_int, [C.c_void_p, u64, P(AmCheckpointInfo)]),
     "am_sweep_restore": (C.c_int, [C.c_void_p, C.c_void_p, u64]),
+    "am_sweep_checkpoint_chain": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, u64, P(u64)]),
+    "am_sweep_checkpoint_delta": (C.c_int, [C.c_void_p, C.c_void_p, u64, P(u64), P(u64)]),
+    "am_checkpoint_delta_info": (C.c_int, [C.c_void_p, u64, P(AmCheckpointDeltaInfo)]),
+    "am_sweep_restore_delta": (C.c_int, [C.c_void_p, C.c_void_p, u64]),
     "am_sweep_size": (u64, [C.c_void_p]),
     "am_sweep_capacity": (u64, [C.c_void_p]),
     "am_sweep_device": (C.c_int, [C.c_void_p]),

@@ -10,6 +10,7 @@
 #endif
 #include <stdint.h>
 
+#include "sweep_kernels.cuh"  // (build_segment_planes, for the planes of a delta's slots)
 #include "sweep_types.h"
 
 namespace amsweep {
@@ -214,6 +215,229 @@ __global__ void __launch_bounds__(256) checkpoint_scatter_kernel(const CkptState
     s.det_start[i] = ck_blob_get<int64_t>(b, kCkSecDetStart, j);
   }
   if (s.wait) s.wait[i] = ck_blob_get<int64_t>(b, kCkSecWait, j);
+}
+
+// ---- delta checkpoints (am_sweep_checkpoint_delta / am_sweep_restore_delta, DESIGN.md "Delta format") ----------------
+// A delta of m changed slots of a chain's range holds, after its 128-B header, the slots' offsets (u32, relative to the
+// range's first slot, strictly ascending) and then every section of the root, each an array over the m slots in blob
+// order.  Its checksum is the full blob's rule over that layout (the offset section's elements included).
+
+constexpr uint64_t kCkHeaderBytes = 128;
+
+// The sections of a blob of n slots with `switches`, from byte `start` on, each at an 8-B aligned offset; returns the
+// end of the last one.  A full blob starts them at the header's end, a delta of m slots at ckd_start(m).
+AM_HD uint64_t ck_layout(uint64_t n, uint32_t switches, uint64_t start, uint64_t* off) {
+  uint64_t at = start;
+  for (int s = 0; s < kCkSections; ++s) {
+    const bool on = s < 16 || ((s == kCkSecWfTimeout || s == kCkSecDeadline) && (switches & AM_CKPT_TIMEOUTS)) ||
+                    (s == kCkSecSince && (switches & AM_CKPT_HOLD)) ||
+                    (s == kCkSecChanged && (switches & AM_CKPT_TRACK)) ||
+                    ((s == kCkSecDetApplied || s == kCkSecDetStart) && (switches & AM_CKPT_DETAILS)) ||
+                    (s == kCkSecWait && (switches & AM_CKPT_ADMISSION));
+    off[s] = on ? at : 0;
+    if (on) at += ((s == kCkSecChanged ? (n + 31) / 32 * 4 : n * ck_elem(s)) + 7) / 8 * 8;
+  }
+  return at;
+}
+AM_HD uint64_t ckd_start(uint64_t m) { return kCkHeaderBytes + (m * 4 + 7) / 8 * 8; }
+
+// The diff: slot first + j of the live state against element j of the base image `b` (the previous link, in the root's
+// layout over the chain's range), one thread each.  Bit j of `bits` is set iff any element a blob carries differs; a
+// warp's 32 slots make one word, and each 8192-slot group's count goes to group_count (scan_groups_kernel's input).
+__global__ void __launch_bounds__(256) delta_diff_kernel(const CkptState s, const CkptBlob b, uint64_t first,
+                                                        uint32_t* bits, uint32_t* group_count) {
+  const uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  const bool in = j < b.n;
+  const uint64_t i = first + j;
+  bool d = false;
+  if (in) {
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      if (ck_elem(k) == 8) d |= reinterpret_cast<const uint64_t*>(s.col[k])[i] != ck_blob_get<uint64_t>(b, k, j);
+      else d |= reinterpret_cast<const uint32_t*>(s.col[k])[i] != ck_blob_get<uint32_t>(b, k, j);
+    }
+    if (b.off[kCkSecWfTimeout])
+      d |= s.wf_timeout[i] != ck_blob_get<int32_t>(b, kCkSecWfTimeout, j) ||
+           s.deadline[i] != ck_blob_get<int64_t>(b, kCkSecDeadline, j);
+    if (b.off[kCkSecSince]) d |= s.since[i] != ck_blob_get<int64_t>(b, kCkSecSince, j);
+    if (b.off[kCkSecChanged])
+      d |= ((s.changed[i >> 5] >> (i & 31)) & 1u) != ((ck_blob_get<uint32_t>(b, kCkSecChanged, j >> 5) >> (j & 31)) & 1u);
+    if (b.off[kCkSecDetApplied])
+      d |= s.det_applied[i] != ck_blob_get<uint8_t>(b, kCkSecDetApplied, j) ||
+           s.det_start[i] != ck_blob_get<int64_t>(b, kCkSecDetStart, j);
+    if (b.off[kCkSecWait]) d |= s.wait[i] != ck_blob_get<int64_t>(b, kCkSecWait, j);
+  }
+  const uint32_t word = __ballot_sync(kFull, d);
+  if ((threadIdx.x & 31) == 0 && in) {
+    bits[j >> 5] = word;
+    if (word) atomicAdd(&group_count[j / kGroupRecords], (uint32_t)__popc(word));
+  }
+}
+
+// The delta's sections: changed slot k (offs[k], as list_changes_kernel wrote it from the diff's bitmap; m = *count
+// of them) to element k of every section, one thread each, at the layout of a delta of m slots (its sections land in
+// `dev` from byte 128 on), with the checksum terms of the offsets and the sections and the zone marks (ck_reduce).
+__global__ void __launch_bounds__(256) delta_pack_kernel(const CkptState s, char* dev, uint32_t switches,
+                                                        const uint32_t* __restrict__ offs,
+                                                        const unsigned long long* __restrict__ count, uint64_t first,
+                                                        unsigned long long* sum, uint32_t* zones) {
+  __shared__ uint32_t s_zones[8];
+  __shared__ CkptBlob s_b;
+  const uint64_t m = *count;
+  if ((uint64_t)blockIdx.x * blockDim.x >= m) return;  // (block-uniform)
+  if (threadIdx.x < 8) s_zones[threadIdx.x] = 0;
+  if (threadIdx.x == 0) {
+    const uint64_t start = ckd_start(m);
+    ck_layout(m, switches, start, s_b.off);
+    s_b.p = dev + kCkHeaderBytes - start;
+    s_b.n = m;
+  }
+  __syncthreads();
+  const CkptBlob& b = s_b;
+  const uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  const bool in = k < m;
+  const uint64_t j = in ? offs[k] : 0;
+  const uint64_t i = first + j;
+  uint64_t acc = 0;
+  if (in) {
+    acc += ckpt_mix((kCkHeaderBytes + k * 4) * 8, j);
+#pragma unroll
+    for (int q = 0; q < 16; ++q) {
+      if (ck_elem(q) == 8) {
+        const uint64_t v = reinterpret_cast<const uint64_t*>(s.col[q])[i];
+        reinterpret_cast<uint64_t*>(b.p + b.off[q])[k] = v;
+        acc += ck_term(b, q, k, v);
+      } else {
+        const uint32_t v = reinterpret_cast<const uint32_t*>(s.col[q])[i];
+        reinterpret_cast<uint32_t*>(b.p + b.off[q])[k] = v;
+        acc += ck_term(b, q, k, v);
+        if (q == 6) mark_zone(s_zones, v);
+      }
+    }
+    if (b.off[kCkSecWfTimeout]) {
+      const int32_t w = s.wf_timeout[i];
+      const int64_t d = s.deadline[i];
+      reinterpret_cast<int32_t*>(b.p + b.off[kCkSecWfTimeout])[k] = w;
+      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecDeadline])[k] = d;
+      acc += ck_term(b, kCkSecWfTimeout, k, w) + ck_term(b, kCkSecDeadline, k, d);
+    }
+    if (b.off[kCkSecSince]) {
+      const int64_t v = s.since[i];
+      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecSince])[k] = v;
+      acc += ck_term(b, kCkSecSince, k, v);
+    }
+    if (b.off[kCkSecDetApplied]) {
+      const uint8_t a = s.det_applied[i];
+      const int64_t t = s.det_start[i];
+      reinterpret_cast<uint8_t*>(b.p + b.off[kCkSecDetApplied])[k] = a;
+      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecDetStart])[k] = t;
+      acc += ckpt_mix((b.off[kCkSecDetApplied] + k) * 8, a) + ck_term(b, kCkSecDetStart, k, t);
+    }
+    if (b.off[kCkSecWait]) {
+      const int64_t v = s.wait[i];
+      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecWait])[k] = v;
+      acc += ck_term(b, kCkSecWait, k, v);
+    }
+  }
+  if (b.off[kCkSecChanged]) {  // (block-uniform)
+    const uint32_t bit = in ? (s.changed[i >> 5] >> (i & 31)) & 1u : 0u;
+    const uint32_t word = __ballot_sync(kFull, bit);
+    if ((threadIdx.x & 31) == 0 && in) reinterpret_cast<uint32_t*>(b.p + b.off[kCkSecChanged])[k >> 5] = word;
+    if (in) acc += ckpt_mix(b.off[kCkSecChanged] * 8 + k, bit);
+  }
+  ck_reduce(acc, s_zones, sum, zones);
+}
+
+// Element k of every section of the compact delta `d` to element offs[k] of the same section of the full-layout image
+// `b`: the commit of a delta into the producer's base image, after the copy to the caller.
+__global__ void __launch_bounds__(256) delta_commit_kernel(const CkptBlob b, const CkptBlob d,
+                                                          const uint32_t* __restrict__ offs) {
+  const uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (k >= d.n) return;
+  const uint64_t j = offs[k];
+  for (int q = 0; q < kCkSections; ++q) {
+    if (!b.off[q]) continue;
+    switch (ck_elem(q)) {
+      case 8: reinterpret_cast<uint64_t*>(b.p + b.off[q])[j] = ck_blob_get<uint64_t>(d, q, k); break;
+      case 4: reinterpret_cast<uint32_t*>(b.p + b.off[q])[j] = ck_blob_get<uint32_t>(d, q, k); break;
+      case 1: reinterpret_cast<uint8_t*>(b.p + b.off[q])[j] = ck_blob_get<uint8_t>(d, q, k); break;
+      default: {
+        uint32_t* w = reinterpret_cast<uint32_t*>(b.p + b.off[q]) + (j >> 5);
+        const uint32_t bit = 1u << (j & 31);
+        if ((ck_blob_get<uint32_t>(d, q, k >> 5) >> (k & 31)) & 1u) atomicOr(w, bit);
+        else atomicAnd(w, ~bit);
+      }
+    }
+  }
+}
+
+// am_sweep_restore_delta, before anything changes: the checksum terms of the offset section (element k at byte
+// 128 + 4k) and whether it is strictly ascending and below n (*bad != 0 otherwise).
+__global__ void __launch_bounds__(256) delta_offsets_verify_kernel(const uint32_t* __restrict__ offs, uint64_t m,
+                                                                  uint64_t n, unsigned long long* sum,
+                                                                  uint32_t* bad) {
+  __shared__ uint32_t s_zones[8];
+  if (threadIdx.x < 8) s_zones[threadIdx.x] = 0;
+  __syncthreads();
+  const uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  uint64_t acc = 0;
+  if (k < m) {
+    const uint32_t j = offs[k];
+    acc = ckpt_mix((kCkHeaderBytes + k * 4) * 8, j);
+    if (j >= n || (k && offs[k - 1] >= j)) atomicOr(bad, 1u);
+  }
+  ck_reduce(acc, s_zones, sum, nullptr);  // (no zone marks: ck_reduce touches `zones` only for marked ids)
+}
+
+// am_sweep_restore_delta: element k of the delta to slot first + offs[k], by the rules of checkpoint_scatter_kernel,
+// and the slot's segment marked for delta_planes_kernel.
+__global__ void __launch_bounds__(256) delta_scatter_kernel(const CkptState s, const CkptBlob b,
+                                                           const uint32_t* __restrict__ offs, uint64_t first,
+                                                           const ZoneLut lut, uint32_t* seg_dirty) {
+  const uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (k >= b.n) return;
+  const uint64_t i = first + offs[k];
+#pragma unroll
+  for (int q = 0; q < 16; ++q) {
+    if (ck_elem(q) == 8) {
+      reinterpret_cast<uint64_t*>(s.col[q])[i] = ck_blob_get<uint64_t>(b, q, k);
+    } else {
+      uint32_t v = ck_blob_get<uint32_t>(b, q, k);
+      if (q == 6 && zone_bound(v)) v = (v & ~AM_F_TZ_MASK) | ((uint32_t)lut.id[v >> AM_F_TZ_SHIFT] << AM_F_TZ_SHIFT);
+      reinterpret_cast<uint32_t*>(s.col[q])[i] = v;
+    }
+  }
+  if (s.wf_timeout) {
+    const bool has = b.off[kCkSecWfTimeout] != 0;
+    const int64_t d = has ? ck_blob_get<int64_t>(b, kCkSecDeadline, k) : kNoDeadline;
+    s.wf_timeout[i] = has ? ck_blob_get<int32_t>(b, kCkSecWfTimeout, k) : 0;
+    s.deadline[i] = d;
+    if (d != kNoDeadline) atomicMin(&s.seg_deadline[i / kRecPerWarp], biased_key(d));
+  }
+  if (s.since) s.since[i] = ck_blob_get<int64_t>(b, kCkSecSince, k);
+  if (s.changed) {
+    const uint32_t m = 1u << (i & 31);
+    if ((ck_blob_get<uint32_t>(b, kCkSecChanged, k >> 5) >> (k & 31)) & 1u) atomicOr(&s.changed[i >> 5], m);
+    else atomicAnd(&s.changed[i >> 5], ~m);
+  }
+  if (s.det_applied) {
+    s.det_applied[i] = ck_blob_get<uint8_t>(b, kCkSecDetApplied, k);
+    s.det_start[i] = ck_blob_get<int64_t>(b, kCkSecDetStart, k);
+  }
+  if (s.wait) s.wait[i] = ck_blob_get<int64_t>(b, kCkSecWait, k);
+  seg_dirty[i / kRecPerWarp] = 1u;
+}
+
+// After delta_scatter_kernel: one warp per changed slot; the first that claims its segment's mark rebuilds the
+// segment's plane words (the claim of build_planes_dirty_kernel, through the offsets).
+__global__ void delta_planes_kernel(DevCols c, MaskPlanes pl, uint32_t* seg_dirty, const uint32_t* __restrict__ offs,
+                                    uint64_t first, uint32_t m) {
+  const uint64_t k = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
+  if (k >= m) return;  // warp-uniform
+  const int lane = (int)(threadIdx.x & 31);
+  const uint32_t seg = (uint32_t)((first + offs[k]) / (uint32_t)kRecPerWarp);
+  const bool won = lane == 0 && atomicAnd(&seg_dirty[seg], 0u) != 0u;  // (an exchange with 0)
+  if (__ballot_sync(kFull, won)) build_segment_planes(c, pl, seg, lane);
 }
 
 }  // namespace amsweep

@@ -139,6 +139,12 @@ struct TickSet {
   bool unpublished = false;
 };
 
+// A delta chain's range on the handle that applied its last link (am_sweep_restore_delta): that link's checksum and the
+// handle's tick count when it was applied.
+struct CkptLink {
+  uint64_t first_global, n, checksum, ticks;
+};
+
 constexpr size_t kFlushOps = 32768;   // staged ops per early host-to-device chunk
 constexpr size_t kFlushRecs = 8192;   // staged upsert records per early chunk
 }  // namespace
@@ -263,6 +269,27 @@ struct am_sweep {
   char* ck_pin[2] = {nullptr, nullptr};
   cudaEvent_t ck_pin_ev[2] = {nullptr, nullptr};
   bool ck_pin_pending[2] = {false, false};
+  // delta chains (am_sweep_checkpoint_chain / _delta / am_sweep_restore_delta), also under ck_mu.  On a producer,
+  // allocated when its first chain starts: the previous link's sections over the chain's range (the root's layout; room
+  // for a full blob of capacity), the diff's bitmap ([groups of capacity * kGroupWords]) and per-group counts and
+  // offsets.  On both sides, at the first chain or delta restore: a delta's slot offsets ([cap_padded]) and the
+  // scan's accumulators ([1] the changed slots, [2] a bad offset), device and pinned.
+  char* ckd_base = nullptr;
+  uint32_t* ckd_bits = nullptr;
+  uint32_t* ckd_group = nullptr;
+  uint32_t* ckd_prefix = nullptr;
+  uint32_t* ckd_off = nullptr;
+  unsigned long long* ckd_acc = nullptr;
+  unsigned long long* ckd_acc_h = nullptr;
+  // the producer's chain: its range, the root's switches, the last link's checksum, sequence number and P
+  bool chain = false;
+  uint64_t chain_first = 0, chain_n = 0, chain_checksum = 0, chain_seq = 0;
+  uint32_t chain_switches = 0;
+  int64_t chain_prev_tick = 0;
+  // the restorer's chains: per range the last link it applied (a full restore starts an entry), and the ticks run by
+  // any entry point (a delta applies only to a handle that has not ticked since its parent)
+  std::vector<CkptLink> links;
+  uint64_t ticks = 0;
   // submit budget (am_sweep_set_submit_budget, only with the hold): the most SUBMIT_HC entries a tick emits, and the
   // admission state, allocated at the first finite budget (admission_kernels.cuh): per slot the second since which it
   // waits, the FIFO of waiting slots and this tick's kept and new ones, a byte per FIFO entry, one bit per slot of
@@ -1188,6 +1215,7 @@ int run_tick(am_sweep* h, int64_t T, uint32_t mode, cudaStream_t s, TickKind kin
   }
   h->has_prev = true;
   h->prev_T = T;
+  ++h->ticks;
   return AM_OK;
 }
 
@@ -1283,6 +1311,7 @@ int run_rows(am_sweep* h, int64_t T0, uint64_t n, bool blocked, bool with_sim, a
       for (uint64_t k = 0; k < n; ++k) stats_out[k].n_records = h->n_records;
     h->has_prev = true;
     h->prev_T = T0 + (int64_t)n - 1;
+    h->ticks += n;
     return AM_OK;
   }();
   if (h->track) {
@@ -2274,7 +2303,26 @@ struct CkptHeader {
   uint32_t n_zones, reserved32;
   uint64_t reserved[6];
 };
-static_assert(sizeof(CkptHeader) == kCkHeader, "checkpoint header: 16 words");
+static_assert(sizeof(CkptHeader) == kCkHeader && kCkHeader == kCkHeaderBytes, "checkpoint header: 16 words");
+
+// A delta: the full header's words, the link's in its reserved words.
+constexpr uint64_t kCkdMagic = 0x4C444B4357534D41ull;  // "AMSWCKDL"
+struct CkptDeltaHeader {
+  uint64_t magic;
+  uint32_t version, switches;
+  uint64_t bytes, checksum, first_global, n, swept_end;
+  int64_t prev_tick;
+  uint64_t seed;
+  uint32_t n_zones, reserved32;
+  uint64_t n_changed, seq;
+  int64_t parent_prev_tick;
+  uint64_t parent_checksum;
+  uint64_t reserved[2];
+};
+static_assert(sizeof(CkptDeltaHeader) == kCkHeader &&
+                  offsetof(CkptDeltaHeader, checksum) == offsetof(CkptHeader, checksum) &&
+                  offsetof(CkptDeltaHeader, n_zones) == offsetof(CkptHeader, n_zones),
+              "delta header: the full header's words first");
 
 struct CkptLayout {
   uint64_t off[kCkSections] = {};
@@ -2284,16 +2332,13 @@ struct CkptLayout {
 // The sections a blob of n slots with `switches` has, in order, each at an 8-B aligned offset.
 CkptLayout ckpt_layout(uint64_t n, uint32_t switches) {
   CkptLayout L;
-  auto put = [&](int s, uint64_t bytes) {
-    L.off[s] = L.sections_end;
-    L.sections_end += (bytes + 7) / 8 * 8;
-  };
-  for (int k = 0; k < 16; ++k) put(k, n * ck_elem(k));
-  if (switches & AM_CKPT_TIMEOUTS) { put(kCkSecWfTimeout, n * 4); put(kCkSecDeadline, n * 8); }
-  if (switches & AM_CKPT_HOLD) put(kCkSecSince, n * 8);
-  if (switches & AM_CKPT_TRACK) put(kCkSecChanged, (n + 31) / 32 * 4);
-  if (switches & AM_CKPT_DETAILS) { put(kCkSecDetApplied, n); put(kCkSecDetStart, n * 8); }
-  if (switches & AM_CKPT_ADMISSION) put(kCkSecWait, n * 8);
+  L.sections_end = ck_layout(n, switches, kCkHeader, L.off);
+  return L;
+}
+// ... and of a delta of m slots (its sections after the offset section)
+CkptLayout ckd_layout(uint64_t m, uint32_t switches) {
+  CkptLayout L;
+  L.sections_end = ck_layout(m, switches, ckd_start(m), L.off);
   return L;
 }
 
@@ -2316,35 +2361,94 @@ struct CkptZone {
   std::string name;
 };
 
-// A blob's header, layout and zone table, checked for consistency (not the checksum: that is a device pass).
-int ckpt_parse(const void* buf, uint64_t len, CkptHeader* hd, CkptLayout* L, std::vector<CkptZone>* zones) {
-  if (!buf || len < kCkHeader) return AM_E_INVAL;
-  const char* p = (const char*)buf;
-  memcpy(hd, p, kCkHeader);
-  if (hd->magic != kCkMagic || hd->version != AM_CHECKPOINT_VERSION) return AM_E_INVAL;
-  if ((hd->switches & ~kCkAllSwitches) || ((hd->switches & AM_CKPT_REMEDY) && !(hd->switches & AM_CKPT_HOLD)) ||
-      ((hd->switches & AM_CKPT_DETAILS) && !(hd->switches & AM_CKPT_TRACK)) ||
-      ((hd->switches & AM_CKPT_ADMISSION) && !(hd->switches & AM_CKPT_HOLD)))
+// The header words a full blob and a delta share, and the zone table from the end of the sections to `bytes`, checked
+// for consistency (not the checksum: that is a device pass).
+template <class Header>
+int ckpt_parse_common(const char* p, uint64_t len, const Header& hd, uint64_t sections_end,
+                      std::vector<CkptZone>* zones) {
+  if (hd.version != AM_CHECKPOINT_VERSION) return AM_E_INVAL;
+  if ((hd.switches & ~kCkAllSwitches) || ((hd.switches & AM_CKPT_REMEDY) && !(hd.switches & AM_CKPT_HOLD)) ||
+      ((hd.switches & AM_CKPT_DETAILS) && !(hd.switches & AM_CKPT_TRACK)) ||
+      ((hd.switches & AM_CKPT_ADMISSION) && !(hd.switches & AM_CKPT_HOLD)))
     return AM_E_INVAL;
-  if (hd->bytes > len || hd->bytes % 8 || hd->n > 0xFFFFFFFFull || hd->first_global + hd->n < hd->first_global ||
-      hd->swept_end < hd->first_global || hd->swept_end > hd->first_global + hd->n || hd->n_zones > 255)
+  if (hd.bytes > len || hd.bytes % 8 || hd.n > 0xFFFFFFFFull || hd.first_global + hd.n < hd.first_global ||
+      hd.swept_end < hd.first_global || hd.swept_end > hd.first_global + hd.n || hd.n_zones > 255)
     return AM_E_INVAL;
-  *L = ckpt_layout(hd->n, hd->switches);
-  uint64_t at = L->sections_end;
+  uint64_t at = sections_end;
   bool seen[256] = {};
   zones->clear();
-  for (uint32_t k = 0; k < hd->n_zones; ++k) {
-    if (at + 8 > hd->bytes) return AM_E_INVAL;
+  for (uint32_t k = 0; k < hd.n_zones; ++k) {
+    if (at + 8 > hd.bytes) return AM_E_INVAL;
     uint32_t id, nl;
     memcpy(&id, p + at, 4);
     memcpy(&nl, p + at + 4, 4);
-    if (id < 1 || id > 255 || seen[id] || nl < 1 || nl > 255 || at + ckpt_zone_entry_bytes(nl) > hd->bytes)
+    if (id < 1 || id > 255 || seen[id] || nl < 1 || nl > 255 || at + ckpt_zone_entry_bytes(nl) > hd.bytes)
       return AM_E_INVAL;
     seen[id] = true;
     zones->push_back({id, std::string(p + at + 8, nl)});
     at += ckpt_zone_entry_bytes(nl);
   }
-  return at == hd->bytes ? AM_OK : AM_E_INVAL;
+  return at == hd.bytes ? AM_OK : AM_E_INVAL;
+}
+
+// A blob's header, layout and zone table.
+int ckpt_parse(const void* buf, uint64_t len, CkptHeader* hd, CkptLayout* L, std::vector<CkptZone>* zones) {
+  if (!buf || len < kCkHeader) return AM_E_INVAL;
+  memcpy(hd, buf, kCkHeader);
+  if (hd->magic != kCkMagic) return AM_E_INVAL;
+  *L = ckpt_layout(hd->n, hd->switches);
+  return ckpt_parse_common((const char*)buf, len, *hd, L->sections_end, zones);
+}
+// ... a delta's (its sections end past `bytes` when n_changed is out of range: refused there)
+int ckd_parse(const void* buf, uint64_t len, CkptDeltaHeader* hd, CkptLayout* L, std::vector<CkptZone>* zones) {
+  if (!buf || len < kCkHeader) return AM_E_INVAL;
+  memcpy(hd, buf, kCkHeader);
+  if (hd->magic != kCkdMagic || hd->n_changed > hd->n || hd->n > 0xFFFFFFFFull || hd->seq == 0) return AM_E_INVAL;
+  *L = ckd_layout(hd->n_changed, hd->switches);
+  return ckpt_parse_common((const char*)buf, len, *hd, L->sections_end, zones);
+}
+
+// The zones a pass marked (8 words of marks, one bit per id) with their names.  AM_E_DEVICE: an id that is not
+// registered (upserts and loads refuse those).
+int ckpt_marked_zones(am_sweep* h, const uint32_t* marks, const char* who, std::vector<CkptZone>* zones) {
+  zones->clear();
+  for (uint32_t id = 1; id < 256; ++id) {
+    if (!((marks[id >> 5] >> (id & 31)) & 1u)) continue;
+    std::string name;
+    if (!amsweep_tz::name_of((int32_t)id, &name)) {
+      h->last_error = std::string(who) + ": a record carries a zone id that is not registered";
+      return AM_E_DEVICE;
+    }
+    zones->push_back({id, name});
+  }
+  return AM_OK;
+}
+// ... written as a zone table at p + at; returns its end
+uint64_t ckpt_put_zones(char* p, uint64_t at, const std::vector<CkptZone>& zones) {
+  for (const CkptZone& z : zones) {
+    const uint32_t nl = (uint32_t)z.name.size();
+    memset(p + at, 0, ckpt_zone_entry_bytes(nl));
+    memcpy(p + at, &z.id, 4);
+    memcpy(p + at + 4, &nl, 4);
+    memcpy(p + at + 8, z.name.data(), nl);
+    at += ckpt_zone_entry_bytes(nl);
+  }
+  return at;
+}
+// A blob's zone table resolved to this process's ids with am_tz_lookup (id 0 stays 0).
+int ckpt_zone_lut(am_sweep* h, const std::vector<CkptZone>& zones, const char* who, ZoneLut* lut) {
+  *lut = ZoneLut{};
+  for (const CkptZone& z : zones) {
+    int32_t id = 0;
+    const int rc = am_tz_lookup(z.name.data(), z.name.size(), &id);
+    if (rc != AM_OK) {
+      h->last_error =
+          std::string(who) + ": time zone " + z.name + (rc == AM_E_PARSE ? " is unknown here" : " does not fit the registry");
+      return rc;
+    }
+    lut->id[z.id] = (uint8_t)id;
+  }
+  return AM_OK;
 }
 
 uint32_t ckpt_switches(const am_sweep* h) {
@@ -2370,14 +2474,6 @@ int ckpt_alloc(am_sweep* h) {
   return AM_OK;
 }
 
-CkptBlob ckpt_blob(const am_sweep* h, const CkptLayout& L, uint64_t n) {
-  CkptBlob b{};
-  b.p = h->ck_dev;
-  memcpy(b.off, L.off, sizeof b.off);
-  b.n = n;
-  return b;
-}
-
 CkptState ckpt_state(am_sweep* h) {
   CkptState s{};
   for (int k = 0; k < 16; ++k) s.col[k] = *col_slot(h->cols, k);
@@ -2396,14 +2492,95 @@ CkptState ckpt_state(am_sweep* h) {
   return s;
 }
 
-}  // namespace
+CkptBlob ckpt_blob(const am_sweep* h, const CkptLayout& L, uint64_t n) {
+  CkptBlob b{};
+  b.p = h->ck_dev;
+  memcpy(b.off, L.off, sizeof b.off);
+  b.n = n;
+  return b;
+}
+// The chain's base image: the previous link's sections over the chain's n slots, in the root's layout.
+CkptBlob ckd_base_blob(const am_sweep* h, uint64_t n, uint32_t switches) {
+  CkptBlob b = ckpt_blob(h, ckpt_layout(n, switches), n);
+  b.p = h->ckd_base;
+  return b;
+}
+// A delta of m slots in the staging area: its offsets in ckd_off, its sections from byte 128 of ck_dev on.
+CkptBlob ckd_blob(const am_sweep* h, const CkptLayout& L, uint64_t m) {
+  CkptBlob b = ckpt_blob(h, L, m);
+  b.p = h->ck_dev + kCkHeader - ckd_start(m);
+  return b;
+}
 
-extern "C" {
+// The delta state of a handle (ck_mu held, after ckpt_alloc): the offsets and accumulators on both sides; the base
+// image, the bitmap and the group arrays on a producer.
+int ckd_alloc(am_sweep* h, bool producer) {
+  if (!h->ckd_off) {
+    AM_CUDA(h, dev_array(h, &h->ckd_acc, 4 * 8, h->ck_stream));
+    AM_CUDA(h, host_array(h, &h->ckd_acc_h, 4 * 8));
+    AM_CUDA(h, dev_array(h, &h->ckd_off, h->cap_padded * 4, h->ck_stream, false));  // (the last)
+  }
+  if (producer && !h->ckd_base) {
+    const size_t ngroups = groups_of(h->cap_padded);
+    AM_CUDA(h, dev_array(h, &h->ckd_bits, ngroups * kGroupWords * 4, h->ck_stream));
+    AM_CUDA(h, dev_array(h, &h->ckd_group, ngroups * 4, h->ck_stream));
+    AM_CUDA(h, dev_array(h, &h->ckd_prefix, (ngroups + 1) * 4, h->ck_stream, false));
+    AM_CUDA(h, dev_array(h, &h->ckd_base, ckpt_layout(h->cap_padded, kCkAllSwitches).sections_end, h->ck_stream,
+                         false));  // (the last)
+  }
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));  // (the zeroed arrays are read on the handle's stream)
+  return AM_OK;
+}
 
-int am_sweep_checkpoint(am_sweep_t* h, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out) {
-  if (!h || !len_out || (cap && !buf)) return AM_E_INVAL;
-  if (first + n > h->capacity || first + n < first) return AM_E_INVAL;
-  std::lock_guard<std::mutex> ck(h->ck_mu);
+// `bytes` at `src` (host) to `dst` (device) on the checkpoint stream, in chunks through the two pinned buffers (the
+// host fills one while the other crosses).
+int ckpt_upload(am_sweep* h, char* dst, const char* src, uint64_t bytes) {
+  for (uint64_t off = 0, k = 0; off < bytes; off += kCkChunk, ++k) {
+    const size_t m = (size_t)std::min<uint64_t>(kCkChunk, bytes - off);
+    const int b = (int)(k & 1);
+    if (h->ck_pin_pending[b]) AM_CUDA(h, cudaEventSynchronize(h->ck_pin_ev[b]));
+    memcpy(h->ck_pin[b], src + off, m);
+    AM_CUDA(h, cudaMemcpyAsync(dst + off, h->ck_pin[b], m, cudaMemcpyHostToDevice, h->ck_stream));
+    AM_CUDA(h, cudaEventRecord(h->ck_pin_ev[b], h->ck_stream));
+    h->ck_pin_pending[b] = true;
+  }
+  return AM_OK;
+}
+
+// A restore's refusal after the checksum (tick guard held): switches, the timeout state aside, that differ from the
+// handle's.
+int ckpt_restore_switches(am_sweep* h, uint32_t switches, const char* who) {
+  if ((switches & ~AM_CKPT_TIMEOUTS) != (ckpt_switches(h) & ~AM_CKPT_TIMEOUTS)) {
+    h->last_error = std::string(who) + ": set the handle's switches to the blob's first (am_checkpoint_info)";
+    return AM_E_INVAL;
+  }
+  return AM_OK;
+}
+
+// The end of a restore after its scatter (tick guard held): the high-water mark, the admission order, P and the seed;
+// the previous tick's lists are not carried: empty until the next tick.
+int ckpt_restore_finish(am_sweep* h, uint64_t swept_end, int64_t prev_tick, uint64_t seed) {
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  const uint64_t hwm = swept_end - h->shard_base;
+  if (hwm > h->n_records) h->n_records = hwm;
+  if (admission_on(h)) {  // the admission order of every waiting slot of the handle, from the waits as they now stand
+    const int rc = rebuild_admission_fifo(h);
+    if (rc != AM_OK) return rc;
+  }
+  if (prev_tick != INT64_MIN) {
+    h->has_prev = true;
+    h->prev_T = prev_tick;
+  }
+  h->seed = seed;
+  h->host_n = 0;
+  h->to_ran = h->to_fetched = false;
+  h->chg_listed = h->chg_fetched = false;
+  return AM_OK;
+}
+
+// A full checkpoint (am_sweep_checkpoint, ck_mu held); *hd_out and *L_out = its header and layout.
+int checkpoint_locked(am_sweep* h, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out,
+                      CkptHeader* hd_out, CkptLayout* L_out) {
   CkptHeader hd{};
   CkptLayout L;
   {  // the pass, with the tick guard held: the drain, then one kernel over the range on the handle's stream
@@ -2439,23 +2616,11 @@ int am_sweep_checkpoint(am_sweep_t* h, uint64_t first, uint64_t n, void* buf, ui
   // Ticks may run from here on: the copy to the caller waits for the pass only, on the checkpoint stream.
   AM_CUDA(h, cudaEventSynchronize(h->ck_ev));
   char* p = (char*)buf;
-  uint64_t at = L.sections_end;
-  const uint32_t* marks = (const uint32_t*)(h->ck_meta_h + 1);
-  for (uint32_t id = 1; id < 256; ++id) {
-    if (!((marks[id >> 5] >> (id & 31)) & 1u)) continue;
-    std::string name;
-    if (!amsweep_tz::name_of((int32_t)id, &name)) {  // (upserts and loads refuse ids that are not registered)
-      h->last_error = "am_sweep_checkpoint: a record carries a zone id that is not registered";
-      return AM_E_DEVICE;
-    }
-    const uint32_t nl = (uint32_t)name.size();
-    memset(p + at, 0, ckpt_zone_entry_bytes(nl));
-    memcpy(p + at, &id, 4);
-    memcpy(p + at + 4, &nl, 4);
-    memcpy(p + at + 8, name.data(), nl);
-    at += ckpt_zone_entry_bytes(nl);
-    ++hd.n_zones;
-  }
+  std::vector<CkptZone> zones;
+  const int rc = ckpt_marked_zones(h, (const uint32_t*)(h->ck_meta_h + 1), "am_sweep_checkpoint", &zones);
+  if (rc != AM_OK) return rc;
+  const uint64_t at = ckpt_put_zones(p, L.sections_end, zones);
+  hd.n_zones = (uint32_t)zones.size();
   hd.bytes = at;
   memcpy(p, &hd, kCkHeader);
   AM_CUDA(h, cudaStreamWaitEvent(h->ck_stream, h->ck_ev, 0));
@@ -2466,7 +2631,34 @@ int am_sweep_checkpoint(am_sweep_t* h, uint64_t first, uint64_t n, void* buf, ui
   hd.checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, at);
   memcpy(p + offsetof(CkptHeader, checksum), &hd.checksum, 8);
   *len_out = at;
+  *hd_out = hd;
+  *L_out = L;
   return AM_OK;
+}
+
+// A restored full blob starts the handle's link entry for its range, replacing every entry that overlaps it.
+void ckpt_start_link(am_sweep* h, uint64_t first_global, uint64_t n, uint64_t checksum) {
+  auto& v = h->links;
+  v.erase(std::remove_if(v.begin(), v.end(),
+                         [&](const CkptLink& e) {
+                           return e.first_global < first_global + n && first_global < e.first_global + e.n;
+                         }),
+          v.end());
+  v.push_back({first_global, n, checksum, h->ticks});
+}
+
+
+}  // namespace
+
+extern "C" {
+
+int am_sweep_checkpoint(am_sweep_t* h, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out) {
+  if (!h || !len_out || (cap && !buf)) return AM_E_INVAL;
+  if (first + n > h->capacity || first + n < first) return AM_E_INVAL;
+  std::lock_guard<std::mutex> ck(h->ck_mu);
+  CkptHeader hd;
+  CkptLayout L;
+  return checkpoint_locked(h, first, n, buf, cap, len_out, &hd, &L);
 }
 
 int am_checkpoint_info(const void* buf, uint64_t len, am_checkpoint_info_t* info) {
@@ -2504,31 +2696,16 @@ int am_sweep_restore(am_sweep_t* h, const void* buf, uint64_t len) {
     return AM_E_RANGE;
   }
   const uint64_t first = hd.first_global - h->shard_base;
-  ZoneLut lut{};  // (id 0 stays 0)
-  for (const CkptZone& z : zones) {
-    int32_t id = 0;
-    rc = am_tz_lookup(z.name.data(), z.name.size(), &id);
-    if (rc != AM_OK) {
-      h->last_error = "am_sweep_restore: time zone " + z.name + (rc == AM_E_PARSE ? " is unknown here" : " does not fit the registry");
-      return rc;
-    }
-    lut.id[z.id] = (uint8_t)id;
-  }
+  ZoneLut lut;
+  rc = ckpt_zone_lut(h, zones, "am_sweep_restore", &lut);
+  if (rc != AM_OK) return rc;
   std::lock_guard<std::mutex> ck(h->ck_mu);
   rc = ckpt_alloc(h);
   if (rc != AM_OK) return rc;
-  // Up in chunks through two pinned buffers (the host fills one while the other crosses), then the device pass that
-  // verifies the checksum: all before anything of the handle changes.
+  // Up in chunks, then the device pass that verifies the checksum: all before anything of the handle changes.
   const char* p = (const char*)buf;
-  for (uint64_t off = kCkHeader, k = 0; off < L.sections_end; off += kCkChunk, ++k) {
-    const size_t m = (size_t)std::min<uint64_t>(kCkChunk, L.sections_end - off);
-    const int b = (int)(k & 1);
-    if (h->ck_pin_pending[b]) AM_CUDA(h, cudaEventSynchronize(h->ck_pin_ev[b]));
-    memcpy(h->ck_pin[b], p + off, m);
-    AM_CUDA(h, cudaMemcpyAsync(h->ck_dev + off, h->ck_pin[b], m, cudaMemcpyHostToDevice, h->ck_stream));
-    AM_CUDA(h, cudaEventRecord(h->ck_pin_ev[b], h->ck_stream));
-    h->ck_pin_pending[b] = true;
-  }
+  rc = ckpt_upload(h, h->ck_dev + kCkHeader, p + kCkHeader, L.sections_end - kCkHeader);
+  if (rc != AM_OK) return rc;
   AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->ck_stream));
   if (hd.n)
     AM_CUDA(h, launch(h, checkpoint_verify_kernel, (unsigned)((hd.n + 255) / 256), 256, h->ck_stream,
@@ -2549,10 +2726,8 @@ int am_sweep_restore(am_sweep_t* h, const void* buf, uint64_t len) {
     }
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  if ((hd.switches & ~AM_CKPT_TIMEOUTS) != (ckpt_switches(h) & ~AM_CKPT_TIMEOUTS)) {
-    h->last_error = "am_sweep_restore: set the handle's switches to the blob's first (am_checkpoint_info)";
-    return AM_E_INVAL;
-  }
+  rc = ckpt_restore_switches(h, hd.switches, "am_sweep_restore");
+  if (rc != AM_OK) return rc;
   if (h->has_prev && (hd.prev_tick == INT64_MIN || hd.prev_tick != h->prev_T)) {
     h->last_error = "am_sweep_restore: the handle's previous tick differs from the blob's";
     return AM_E_INVAL;
@@ -2570,22 +2745,252 @@ int am_sweep_restore(am_sweep_t* h, const void* buf, uint64_t len) {
     rc = rebuild_planes(h, first, hd.n);
     if (rc != AM_OK) return rc;
   }
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  const uint64_t hwm = hd.swept_end - h->shard_base;
-  if (hwm > h->n_records) h->n_records = hwm;
-  if (admission_on(h)) {  // the admission order of every waiting slot of the handle, from the waits as they now stand
-    rc = rebuild_admission_fifo(h);
+  rc = ckpt_restore_finish(h, hd.swept_end, hd.prev_tick, hd.seed);
+  if (rc != AM_OK) return rc;
+  ckpt_start_link(h, hd.first_global, hd.n, hd.checksum);
+  return AM_OK;
+}
+
+int am_sweep_checkpoint_chain(am_sweep_t* h, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out) {
+  if (!h || !len_out || (cap && !buf)) return AM_E_INVAL;
+  if (first + n > h->capacity || first + n < first) return AM_E_INVAL;
+  std::lock_guard<std::mutex> ck(h->ck_mu);
+  int rc = ckpt_alloc(h);
+  if (rc == AM_OK) rc = ckd_alloc(h, true);
+  if (rc != AM_OK) return rc;
+  CkptHeader hd;
+  CkptLayout L;
+  rc = checkpoint_locked(h, first, n, buf, cap, len_out, &hd, &L);
+  if (rc != AM_OK) return rc;
+  // the root's sections become the chain's base image (the staging area holds them until the next checkpoint)
+  if (L.sections_end > kCkHeader)
+    AM_CUDA(h, cudaMemcpyAsync(h->ckd_base + kCkHeader, h->ck_dev + kCkHeader, L.sections_end - kCkHeader,
+                               cudaMemcpyDeviceToDevice, h->ck_stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  h->chain = true;
+  h->chain_first = first;
+  h->chain_n = n;
+  h->chain_switches = hd.switches;
+  h->chain_checksum = hd.checksum;
+  h->chain_seq = 0;
+  h->chain_prev_tick = hd.prev_tick;
+  return AM_OK;
+}
+
+int am_sweep_checkpoint_delta(am_sweep_t* h, void* buf, uint64_t cap, uint64_t* len_out, uint64_t* n_changed) {
+  if (!h || !len_out || !n_changed || (cap && !buf)) return AM_E_INVAL;
+  std::lock_guard<std::mutex> ck(h->ck_mu);
+  if (!h->chain) {
+    h->last_error = "am_sweep_checkpoint_delta: the handle has no chain (am_sweep_checkpoint_chain)";
+    return AM_E_INVAL;
+  }
+  const uint64_t first = h->chain_first, n = h->chain_n;
+  CkptDeltaHeader hd{};
+  {  // the passes, with the tick guard held: the drain, then the diff, its compaction and the pack on the handle's stream
+    TickGuard g(h);
+    if (!g.ok) return AM_E_BUSY;
+    const int rc = begin_call(h);
+    if (rc != AM_OK) return rc;
+    if (ckpt_switches(h) != h->chain_switches) {
+      h->last_error = "am_sweep_checkpoint_delta: the switches differ from the chain root's: start a new chain";
+      return AM_E_INVAL;
+    }
+    hd.magic = kCkdMagic;
+    hd.version = AM_CHECKPOINT_VERSION;
+    hd.switches = h->chain_switches;
+    hd.first_global = h->shard_base + first;
+    hd.n = n;
+    hd.swept_end = h->shard_base + std::min(std::max(h->n_records, first), first + n);
+    hd.prev_tick = h->has_prev ? h->prev_T : INT64_MIN;
+    hd.seed = h->seed;
+    hd.seq = h->chain_seq + 1;
+    hd.parent_prev_tick = h->chain_prev_tick;
+    hd.parent_checksum = h->chain_checksum;
+    AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->stream));
+    if (n) {
+      const unsigned grid = (unsigned)((n + 255) / 256);
+      AM_CUDA(h, launch(h, delta_diff_kernel, grid, 256, h->stream, ckpt_state(h),
+                        ckd_base_blob(h, n, hd.switches), first, h->ckd_bits, h->ckd_group));
+      ScanParams sc{};
+      sc.group_count = h->ckd_group;
+      sc.group_prefix = h->ckd_prefix;
+      sc.acc = h->ckd_acc;
+      sc.n_groups = groups_of(n);
+      sc.cap = 0xFFFFFFFFu;
+      AM_CUDA(h, launch(h, scan_groups_kernel, 1, 1024, h->stream, sc));
+      AM_CUDA(h, launch(h, list_changes_kernel, sc.n_groups, kGroupWords, h->stream, h->ckd_bits,
+                        (const uint32_t*)h->ckd_prefix, h->ckd_off));
+      AM_CUDA(h, launch(h, delta_pack_kernel, grid, 256, h->stream, ckpt_state(h), h->ck_dev, hd.switches,
+                        (const uint32_t*)h->ckd_off, (const unsigned long long*)(h->ckd_acc + 1), first, h->ck_meta,
+                        (uint32_t*)(h->ck_meta + 1)));
+      AM_CUDA(h, cudaMemcpyAsync(h->ckd_acc_h, h->ckd_acc, 4 * 8, cudaMemcpyDeviceToHost, h->stream));
+    }
+    AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->stream));
+    AM_CUDA(h, cudaEventRecord(h->ck_ev, h->stream));
+  }
+  // Ticks may run from here on: the copy to the caller and the commit wait for the passes only, on the checkpoint stream.
+  AM_CUDA(h, cudaEventSynchronize(h->ck_ev));
+  const uint64_t m = n ? h->ckd_acc_h[1] : 0;
+  const CkptLayout L = ckd_layout(m, hd.switches);
+  std::vector<CkptZone> zones;
+  int rc = ckpt_marked_zones(h, (const uint32_t*)(h->ck_meta_h + 1), "am_sweep_checkpoint_delta", &zones);
+  if (rc != AM_OK) return rc;
+  uint64_t need = L.sections_end;
+  for (const CkptZone& z : zones) need += ckpt_zone_entry_bytes(z.name.size());
+  if (cap < need) {  // (nothing committed: the next delta carries these slots again)
+    *len_out = need;
+    return AM_E_NOSPACE;
+  }
+  char* p = (char*)buf;
+  ckpt_put_zones(p, L.sections_end, zones);
+  hd.n_changed = m;
+  hd.n_zones = (uint32_t)zones.size();
+  hd.bytes = need;
+  memcpy(p, &hd, kCkHeader);
+  const uint64_t start = ckd_start(m);
+  memset(p + kCkHeader + m * 4, 0, start - kCkHeader - m * 4);  // (the offset section's padding)
+  AM_CUDA(h, cudaStreamWaitEvent(h->ck_stream, h->ck_ev, 0));
+  if (m) {
+    AM_CUDA(h, cudaMemcpyAsync(p + kCkHeader, h->ckd_off, m * 4, cudaMemcpyDeviceToHost, h->ck_stream));
+    AM_CUDA(h, cudaMemcpyAsync(p + start, h->ck_dev + kCkHeader, L.sections_end - start, cudaMemcpyDeviceToHost,
+                               h->ck_stream));
+  }
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  hd.checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, need);
+  memcpy(p + offsetof(CkptDeltaHeader, checksum), &hd.checksum, 8);
+  // the blob is the caller's: the base image advances to it
+  if (m) {
+    AM_CUDA(h, launch(h, delta_commit_kernel, (unsigned)((m + 255) / 256), 256, h->ck_stream,
+                      ckd_base_blob(h, n, hd.switches), ckd_blob(h, L, m), (const uint32_t*)h->ckd_off));
+    AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  }
+  h->chain_checksum = hd.checksum;
+  h->chain_seq = hd.seq;
+  h->chain_prev_tick = hd.prev_tick;
+  *len_out = need;
+  *n_changed = m;
+  return AM_OK;
+}
+
+int am_checkpoint_delta_info(const void* buf, uint64_t len, am_checkpoint_delta_info_t* info) {
+  if (!info) return AM_E_INVAL;
+  CkptDeltaHeader hd;
+  CkptLayout L;
+  std::vector<CkptZone> zones;
+  const int rc = ckd_parse(buf, len, &hd, &L, &zones);
+  if (rc != AM_OK) return rc;
+  *info = am_checkpoint_delta_info_t{};
+  info->first_global = hd.first_global;
+  info->n = hd.n;
+  info->swept_end = hd.swept_end;
+  info->prev_tick = hd.prev_tick;
+  info->seed = hd.seed;
+  info->n_changed = hd.n_changed;
+  info->seq = hd.seq;
+  info->parent_prev_tick = hd.parent_prev_tick;
+  info->parent_checksum = hd.parent_checksum;
+  info->checksum = hd.checksum;
+  info->switches = hd.switches;
+  info->n_zones = hd.n_zones;
+  info->version = hd.version;
+  info->bytes = hd.bytes;
+  return AM_OK;
+}
+
+int am_sweep_restore_delta(am_sweep_t* h, const void* buf, uint64_t len) {
+  if (!h || !buf) return AM_E_INVAL;
+  CkptDeltaHeader hd;
+  CkptLayout L;
+  std::vector<CkptZone> zones;
+  int rc = ckd_parse(buf, len, &hd, &L, &zones);
+  if (rc != AM_OK) {
+    h->last_error = "am_sweep_restore_delta: not a delta of this format version, or truncated";
+    return rc;
+  }
+  if (hd.first_global < h->shard_base || hd.first_global - h->shard_base + hd.n > h->capacity) {
+    h->last_error = "am_sweep_restore_delta: the delta's slots are not all inside this shard";
+    return AM_E_RANGE;
+  }
+  const uint64_t first = hd.first_global - h->shard_base, m = hd.n_changed;
+  ZoneLut lut;
+  rc = ckpt_zone_lut(h, zones, "am_sweep_restore_delta", &lut);
+  if (rc != AM_OK) return rc;
+  std::lock_guard<std::mutex> ck(h->ck_mu);
+  rc = ckpt_alloc(h);
+  if (rc == AM_OK) rc = ckd_alloc(h, false);
+  if (rc != AM_OK) return rc;
+  // Up in chunks (the offsets to ckd_off, the sections to the staging area), then the device passes that verify the
+  // checksum and the offsets: all before anything of the handle changes.
+  const char* p = (const char*)buf;
+  const uint64_t start = ckd_start(m);
+  rc = ckpt_upload(h, (char*)h->ckd_off, p + kCkHeader, m * 4);
+  if (rc == AM_OK) rc = ckpt_upload(h, h->ck_dev + kCkHeader, p + start, L.sections_end - start);
+  if (rc != AM_OK) return rc;
+  AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->ck_stream));
+  AM_CUDA(h, cudaMemsetAsync(h->ckd_acc, 0, 4 * 8, h->ck_stream));
+  if (m) {
+    const unsigned grid = (unsigned)((m + 255) / 256);
+    AM_CUDA(h, launch(h, delta_offsets_verify_kernel, grid, 256, h->ck_stream, (const uint32_t*)h->ckd_off, m, hd.n,
+                      h->ck_meta, (uint32_t*)(h->ckd_acc + 2)));
+    AM_CUDA(h, launch(h, checkpoint_verify_kernel, grid, 256, h->ck_stream, ckd_blob(h, L, m), h->ck_meta,
+                      (uint32_t*)(h->ck_meta + 1)));
+  }
+  AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
+  AM_CUDA(h, cudaMemcpyAsync(h->ckd_acc_h, h->ckd_acc, 4 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  h->ck_pin_pending[0] = h->ck_pin_pending[1] = false;
+  const uint64_t sum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, hd.bytes);
+  if (sum != hd.checksum) {
+    h->last_error = "am_sweep_restore_delta: checksum mismatch";
+    return AM_E_INVAL;
+  }
+  if (h->ckd_acc_h[2]) {
+    h->last_error = "am_sweep_restore_delta: the slot offsets are not strictly ascending inside the range";
+    return AM_E_INVAL;
+  }
+  const uint32_t* marks = (const uint32_t*)(h->ck_meta_h + 1);
+  for (uint32_t id = 1; id < 256; ++id)
+    if (((marks[id >> 5] >> (id & 31)) & 1u) && !lut.id[id]) {
+      h->last_error = "am_sweep_restore_delta: a record names a zone the delta's table does not";
+      return AM_E_INVAL;
+    }
+  TickGuard g(h);
+  if (!g.ok) return AM_E_BUSY;
+  CkptLink* link = nullptr;
+  for (CkptLink& e : h->links)
+    if (e.first_global == hd.first_global && e.n == hd.n) link = &e;
+  if (!link || link->checksum != hd.parent_checksum) {
+    h->last_error = "am_sweep_restore_delta: the delta's parent is not the last link this handle applied for its range";
+    return AM_E_INVAL;
+  }
+  if (link->ticks != h->ticks) {
+    h->last_error = "am_sweep_restore_delta: the handle ticked since it applied the delta's parent";
+    return AM_E_INVAL;
+  }
+  rc = ckpt_restore_switches(h, hd.switches, "am_sweep_restore_delta");
+  if (rc != AM_OK) return rc;
+  const int64_t P = h->has_prev ? h->prev_T : INT64_MIN;
+  if (P != hd.parent_prev_tick && P != hd.prev_tick) {
+    h->last_error = "am_sweep_restore_delta: the handle's previous tick is neither the delta's nor its parent's";
+    return AM_E_INVAL;
+  }
+  // a call in the per-slot order: the calls staged before it are applied first
+  rc = begin_call(h);
+  if (rc != AM_OK) return rc;
+  if ((hd.switches & AM_CKPT_TIMEOUTS) && !h->wf_timeout) {
+    rc = alloc_timeouts(h, h->stream);
     if (rc != AM_OK) return rc;
   }
-  if (hd.prev_tick != INT64_MIN) {
-    h->has_prev = true;
-    h->prev_T = hd.prev_tick;
+  if (m) {
+    AM_CUDA(h, launch(h, delta_scatter_kernel, (unsigned)((m + 255) / 256), 256, h->stream, ckpt_state(h),
+                      ckd_blob(h, L, m), (const uint32_t*)h->ckd_off, first, lut, h->seg_dirty));
+    AM_CUDA(h, launch(h, delta_planes_kernel, (unsigned)((m + kWarps - 1) / kWarps), kBlock, h->stream, h->cols,
+                      h->planes, h->seg_dirty, (const uint32_t*)h->ckd_off, first, (uint32_t)m));
   }
-  h->seed = hd.seed;
-  // the previous tick's lists are not carried: empty until the next tick
-  h->host_n = 0;
-  h->to_ran = h->to_fetched = false;
-  h->chg_listed = h->chg_fetched = false;
+  rc = ckpt_restore_finish(h, hd.swept_end, hd.prev_tick, hd.seed);
+  if (rc != AM_OK) return rc;
+  link->checksum = hd.checksum;
+  link->ticks = h->ticks;
   return AM_OK;
 }
 

@@ -739,6 +739,77 @@ int am_checkpoint_info(const void* buf, uint64_t len, am_checkpoint_info_t* info
  * grows, which is harmless. */
 int am_sweep_restore(am_sweep_t*, const void* buf, uint64_t len);
 
+/* Delta checkpoints (DESIGN.md section 6 item 21, "Delta format"): a chain over a range of slots is one full blob, its
+ * root, then links that carry only the slots whose state changed since the link before.  A standby handle restores the
+ * root with am_sweep_restore and applies each delta in order with am_sweep_restore_delta; it then answers as a
+ * restore of a full checkpoint taken on the source at the last delta would (EQUIVALENCE above), so a full checkpoint
+ * of the range on it is byte for byte the source's.  "Changed" is state-based: a slot is in a delta iff any element a
+ * full blob carries for it (the sixteen columns with the flags bits raw, wf_timeout and deadline, since, the change
+ * bit, the detail capture, the waiting second) differs from the previous link's, whichever call or tick wrote it.
+ * A delta's header holds the chain's range, swept_end, P and the seed at the delta, the switches, n_changed, the
+ * link's sequence number (the root is 0), the parent's P and the parent link's checksum; then the n_changed slot
+ * offsets (u32, relative to the range's first slot, strictly ascending), every section of the root as an array over
+ * those slots only (the change bit packed as bits), and the zone table of their records.  Its magic differs from a
+ * full blob's: am_checkpoint_info and am_sweep_restore refuse it (AM_E_INVAL).
+ * Memory: a producer reserves, when its first chain starts, a base image of a full blob's sections over its capacity
+ * (the previous link's state, up to 129.125 B per slot), the diff's bitmap (1 bit per slot) and the offsets of a
+ * delta with every slot changed (4 B per slot); a standby reserves the offsets (4 B per slot) at its first
+ * am_sweep_restore_delta.  All are kept until am_sweep_destroy; a handle that never starts a chain or applies a delta
+ * allocates nothing and launches nothing for them. */
+typedef struct am_checkpoint_delta_info {
+  uint64_t first_global, n; /* the chain's range, by GLOBAL index                                     */
+  uint64_t swept_end;       /* global end of the source's swept slots within the range, at the delta */
+  int64_t prev_tick;        /* P at the delta, INT64_MIN when the source had none                     */
+  uint64_t seed;
+  uint64_t n_changed;       /* slots it carries                                                       */
+  uint64_t seq;             /* the link's sequence number: 1 for the first delta after the root       */
+  int64_t parent_prev_tick; /* P of the link before it                                                */
+  uint64_t parent_checksum; /* checksum of the link before it (a root's header checksum for seq 1)    */
+  uint64_t checksum;        /* its own checksum: the next delta's parent_checksum                     */
+  uint32_t switches;        /* AM_CKPT_*, the root's                                                  */
+  uint32_t n_zones;
+  uint32_t version;         /* AM_CHECKPOINT_VERSION                                                  */
+  uint32_t reserved;
+  uint64_t bytes;           /* the blob's length                                                      */
+} am_checkpoint_delta_info_t;
+/* A full checkpoint of local slots [first, first+n) that also starts (or restarts) the handle's delta chain over that
+ * range: the blob is byte for byte what am_sweep_checkpoint(first, n) returns at the same point, and its sections stay
+ * in HBM as the chain's base.  Same contract and refusals as am_sweep_checkpoint; a refused call leaves the previous
+ * chain as it was.  Launches: those of am_sweep_checkpoint (its drain's, and 1 over a non-empty range). */
+int am_sweep_checkpoint_chain(am_sweep_t*, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out);
+/* The chain's next link: the slots of its range whose state differs from the previous link's, into buf[0..cap).  A call
+ * in the per-slot order that drains as am_sweep_checkpoint does; the tick guard is held only while the drain and the
+ * device passes are issued on the handle's stream (the diff against the base image, the compaction and the pack).
+ * The copy into buf and the commit of the delta into the base image follow on the checkpoint stream while ticks run;
+ * the base advances only once buf holds the blob.  Serialised with checkpoints and restores of the handle.
+ * *len_out = the blob's length, *n_changed = the slots it carries.  Launches over a non-empty range: 4 (diff,
+ * group scan, compaction, pack) and 1 more (commit) when n_changed > 0, besides its drain's.
+ *   AM_E_NOSPACE  (after the drain and the passes) cap is below the blob's length, returned in *len_out; nothing is
+ *                 committed: the next delta carries the same slots and whatever changed since;
+ *   AM_E_INVAL    the handle has no chain, or its switches (the timeout state included, which a later upsert may
+ *                 allocate) differ from the root's: start a new chain. */
+int am_sweep_checkpoint_delta(am_sweep_t*, void* buf, uint64_t cap, uint64_t* len_out, uint64_t* n_changed);
+/* The header of a delta, checked for consistency (format version, sizes, zone table); no handle, no GPU.  AM_E_INVAL:
+ * not a delta of this format version, or truncated. */
+int am_checkpoint_delta_info(const void* buf, uint64_t len, am_checkpoint_delta_info_t* info);
+/* Apply a delta to this handle.  The handle keeps, per chain range, the checksum of the last link it applied: a full
+ * blob restored with am_sweep_restore starts the entry of its range (and drops every entry whose range overlaps it).
+ * A delta applies only when an entry exists for its exact range, that entry's checksum is the delta's parent checksum,
+ * no tick of any entry point ran on the handle since the entry was last updated, and the handle's P is the delta's
+ * parent P or its own P (so several chains taken at the same ticks apply to one handle in any order).  A call in the
+ * per-slot order: the calls staged before it are drained first.  Then its slots are scattered (zone ids rewritten to
+ * this process's), the mask planes of their segments rebuilt, the high-water mark raised to swept_end - shard_base,
+ * the admission order rebuilt when the handle has the admission state, P and the seed set to the delta's and the
+ * previous tick's lists emptied, as am_sweep_restore does.  Launches: 4 when n_changed > 0 (offsets and sections
+ * verified, scatter, plane rebuild), none otherwise, besides those of its drain, of the allocation of the timeout
+ * state when the delta has it and the handle not, and of the admission order's rebuild when the handle has the
+ * admission state.  Refused before anything changes, with am_sweep_restore's codes
+ * (header, checksum and offsets verified on the device, zone names, switches, slots outside the shard), and:
+ *   AM_E_INVAL  offsets that are not strictly ascending below n; no entry for the range, a parent checksum that is
+ *               not the entry's (a skipped, repeated or foreign link), a tick since the parent, or a P that is neither
+ *               the delta's nor its parent's.  A caller that loses a delta has broken its chain: it starts a new one. */
+int am_sweep_restore_delta(am_sweep_t*, const void* buf, uint64_t len);
+
 /* Introspection */
 uint64_t am_sweep_size(const am_sweep_t*);     /* high-water mark (slots swept) */
 uint64_t am_sweep_capacity(const am_sweep_t*);
