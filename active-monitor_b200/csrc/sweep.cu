@@ -357,6 +357,9 @@ void* const* cols_member(const am_record_cols_t* c, int k) {
   return slots[k];
 }
 
+// The high-water mark moves under the tick guard; am_sweep_size reads it from any thread without taking the guard.
+void set_hwm(am_sweep* h, uint64_t v) { __atomic_store_n(&h->n_records, v, __ATOMIC_RELAXED); }
+
 struct TickGuard {
   am_sweep* h;
   bool ok;
@@ -785,7 +788,7 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   }
   // from here on `st` is private to this (single) ticking thread
   const size_t n = st->n_ops, nrec = st->n_recs;
-  if (st->hwm > h->n_records) h->n_records = st->hwm;  // every upserted slot extends the swept range
+  if (st->hwm > h->n_records) set_hwm(h, st->hwm);  // every upserted slot extends the swept range
   if (st->d_ops.cap < n * 8 || st->d_recs.cap < nrec * sizeof(am_record_t)) {
     // grow the device twins (frees synchronise) and copy everything again
     AM_CUDA(h, cudaStreamSynchronize(h->cstream));
@@ -1449,7 +1452,7 @@ void am_sweep_destroy(am_sweep_t* h) {
   delete h;
 }
 
-uint64_t am_sweep_size(const am_sweep_t* h) { return h ? h->n_records : 0; }
+uint64_t am_sweep_size(const am_sweep_t* h) { return h ? __atomic_load_n(&h->n_records, __ATOMIC_RELAXED) : 0; }
 uint64_t am_sweep_capacity(const am_sweep_t* h) { return h ? h->capacity : 0; }
 int am_sweep_device(const am_sweep_t* h) { return h ? h->device : -1; }
 double am_sweep_last_kernel_ms(const am_sweep_t* h) { return h ? h->last_ms : -1.0; }
@@ -1514,7 +1517,7 @@ int am_sweep_load_range(am_sweep_t* h, uint64_t first, uint64_t n, const am_reco
     if (rc != AM_OK) return rc;
   }
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  if (first + n > h->n_records) h->n_records = first + n;
+  if (first + n > h->n_records) set_hwm(h, first + n);
   return AM_OK;
 }
 
@@ -2344,6 +2347,17 @@ CkptLayout ckd_layout(uint64_t m, uint32_t switches) {
 
 uint64_t ckpt_zone_entry_bytes(size_t name_len) { return 8 + (name_len + 7) / 8 * 8; }
 
+// Zeroes the bytes between each section's last element and the next 8-B boundary in the host copy `p` of a blob with
+// n slots per section (layout L).  The staging area they are copied from keeps whatever an earlier blob with another
+// layout left there, and blobs of one state must be equal byte for byte.
+void ckpt_zero_padding(char* p, const CkptLayout& L, uint64_t n) {
+  for (int s = 0; s < kCkSections; ++s) {
+    if (!L.off[s]) continue;
+    const uint64_t used = s == kCkSecChanged ? (n + 31) / 32 * 4 : n * ck_elem(s);
+    memset(p + L.off[s] + used, 0, (used + 7) / 8 * 8 - used);
+  }
+}
+
 // The checksum's terms of the words in [a, b) of a blob (the header, whose checksum word counts as 0, and the zone table).
 uint64_t ckpt_host_sum(const char* buf, uint64_t a, uint64_t b) {
   uint64_t s = 0;
@@ -2562,7 +2576,7 @@ int ckpt_restore_switches(am_sweep* h, uint32_t switches, const char* who) {
 int ckpt_restore_finish(am_sweep* h, uint64_t swept_end, int64_t prev_tick, uint64_t seed) {
   AM_CUDA(h, cudaStreamSynchronize(h->stream));
   const uint64_t hwm = swept_end - h->shard_base;
-  if (hwm > h->n_records) h->n_records = hwm;
+  if (hwm > h->n_records) set_hwm(h, hwm);
   if (admission_on(h)) {  // the admission order of every waiting slot of the handle, from the waits as they now stand
     const int rc = rebuild_admission_fifo(h);
     if (rc != AM_OK) return rc;
@@ -2628,6 +2642,7 @@ int checkpoint_locked(am_sweep* h, uint64_t first, uint64_t n, void* buf, uint64
     AM_CUDA(h, cudaMemcpyAsync(p + kCkHeader, h->ck_dev + kCkHeader, L.sections_end - kCkHeader, cudaMemcpyDeviceToHost,
                                h->ck_stream));
   AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  ckpt_zero_padding(p, L, n);
   hd.checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, at);
   memcpy(p + offsetof(CkptHeader, checksum), &hd.checksum, 8);
   *len_out = at;
@@ -2856,6 +2871,7 @@ int am_sweep_checkpoint_delta(am_sweep_t* h, void* buf, uint64_t cap, uint64_t* 
                                h->ck_stream));
   }
   AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  ckpt_zero_padding(p, L, m);
   hd.checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, need);
   memcpy(p + offsetof(CkptDeltaHeader, checksum), &hd.checksum, 8);
   // the blob is the caller's: the base image advances to it
