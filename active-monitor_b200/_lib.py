@@ -152,6 +152,9 @@ class AmAdmission(C.Structure):
 
 UNLIMITED = (1 << 64) - 1  # am_sweep_set_submit_budget: no budget
 
+# am_sweep_select states: the dense query whose values it selects from
+SEL_IN_FLIGHT, SEL_REMEDY_IN_FLIGHT, SEL_WAITING = 1, 2, 3
+
 SIM_FIELDS = ["n_in_flight", "n_remedy_in_flight", "n_timed_out", "n_remedy_timed_out"]
 SIM_DTYPE = np.dtype([(n, "<u8") for n in SIM_FIELDS])
 
@@ -189,6 +192,7 @@ SYMBOLS = {
     "am_sweep_read": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, P(AmRecordCols)]),
     "am_sweep_set_hold_in_flight": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_in_flight": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, C.c_void_p]),
+    "am_sweep_select": (C.c_int, [C.c_void_p, u32, u64, u64, i64, C.c_void_p, C.c_void_p, u64, P(u64), P(i64)]),
     "am_sweep_last_timed_out": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
     "am_sweep_set_hold_remedy": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_remedy_in_flight": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, C.c_void_p]),

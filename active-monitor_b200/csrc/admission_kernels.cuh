@@ -29,6 +29,7 @@
 namespace amsweep {
 
 constexpr int64_t kNotWaiting = INT64_MIN;
+static_assert(kNotWaiting == kNotInFlight, "one 'not in the state' value for every AM_SEL_* state");
 constexpr int kAdmBlock = 256;  // threads per CTA of the per-entry passes = FIFO entries per chunk
 static_assert(kGroupWords == kAdmBlock, "adm_block_scan serves the per-group passes (one word per thread) as well");
 
@@ -337,11 +338,68 @@ __global__ void adm_next_due_kernel(const uint32_t* __restrict__ fifo, const int
   if (any) atomicMin(out, biased_key(T + 1));
 }
 
-// am_sweep_deferred: wait[] of the slots [first, first + n) or idx[0..n).
+// What am_sweep_deferred reports for slot i: the second since which it waits for admission, kNotWaiting when it does
+// not.  The one definition of the value: the dense query and am_sweep_select's mark pass call it.
+__device__ __forceinline__ int64_t adm_wait(const int64_t* __restrict__ wait, uint32_t i) { return wait[i]; }
+
+// am_sweep_deferred: adm_wait of the slots first + k (idx == NULL) or first + idx[k], k < n.
 __global__ void adm_gather_kernel(const int64_t* __restrict__ wait, uint32_t first, const uint32_t* __restrict__ idx,
                                   uint32_t n, int64_t* out) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < n) out[k] = wait[idx ? idx[k] : first + k];
+  if (k < n) out[k] = adm_wait(wait, first + (idx ? idx[k] : k));
+}
+
+// am_sweep_select's mark pass over the slots [first, first + n): one CTA per 8192-slot group of the range (slot
+// first + j is in group j / 8192), one slot per thread and step.  Slot first + j matches when its value v — adm_wait
+// when `wait` is given (AM_SEL_WAITING), else held_run_start on `since` — is set (not INT64_MIN) and v <= before.  Bit
+// j of `bits` is set iff it matches (every word of the CTA's group is written), group_count[g] = the group's matches
+// (scan_groups_kernel's input), acc[1] += them and acc[0] = min(acc[0], biased_key(least match)) with one atomic each
+// per CTA.  Reads 8 B per slot (since or wait); finishedAt and the flags only where since is set.
+__global__ void __launch_bounds__(kGroupWords) select_mark_kernel(DevCols c, const int64_t* __restrict__ since,
+                                                                  const int64_t* __restrict__ wait, bool remedy,
+                                                                  uint32_t first, uint32_t n, int64_t before,
+                                                                  uint32_t* bits, uint32_t* group_count,
+                                                                  unsigned long long* acc) {
+  __shared__ uint32_t s_cnt[kGroupWords / 32];
+  __shared__ unsigned long long s_min[kGroupWords / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t g = blockIdx.x;
+  uint32_t cnt = 0;
+  unsigned long long best = ~0ull;
+#pragma unroll 4
+  for (uint32_t r = 0; r < kGroupRecords / kGroupWords; ++r) {  // step r: slots j0 .. j0 + 255, words j0 / 32 + warp
+    const uint32_t j0 = g * kGroupRecords + r * kGroupWords;
+    const uint32_t j = j0 + threadIdx.x;
+    bool m = false;
+    if (j < n) {
+      const int64_t v = wait ? adm_wait(wait, first + j) : held_run_start(c, since, first + j, remedy);
+      m = v != kNotWaiting && v <= before;
+      if (m && biased_key(v) < best) best = biased_key(v);
+    }
+    const uint32_t word = __ballot_sync(kFull, m);
+    if (lane == 0) {
+      bits[j0 / 32u + warp] = word;
+      cnt += (uint32_t)__popc(word);
+    }
+  }
+  best = warp_min(best);
+  if (lane == 0) {
+    s_cnt[warp] = cnt;
+    s_min[warp] = best;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t t = 0;
+    for (uint32_t k = 0; k < kGroupWords / 32; ++k) {
+      t += s_cnt[k];
+      best = s_min[k] < best ? s_min[k] : best;
+    }
+    group_count[g] = t;
+    if (t) {
+      atomicAdd(acc + 1, (unsigned long long)t);
+      atomicMin(acc, best);
+    }
+  }
 }
 
 }  // namespace amsweep

@@ -304,6 +304,14 @@ struct am_sweep {
   uint32_t* adm_group_sub = nullptr;
   uint32_t* adm_chunk = nullptr;
   AdmCtl* adm_ctl = nullptr;
+  // sparse state queries (am_sweep_select), allocated at the first call that reaches the device: the mark pass's bitmap
+  // ([groups of capacity * kGroupWords]), per-group counts and offsets, the matches' slots relative to the call's first
+  // ([cap_padded]) and the accumulators ([0] the least match as a biased key, [1] the matches)
+  uint32_t* sel_bits = nullptr;
+  uint32_t* sel_group = nullptr;
+  uint32_t* sel_prefix = nullptr;
+  uint32_t* sel_list = nullptr;
+  unsigned long long* sel_acc = nullptr;
 };
 
 namespace {
@@ -2062,56 +2070,135 @@ int check_slots(const am_sweep* h, uint64_t first, uint64_t n, const uint64_t* i
   return AM_OK;
 }
 
-// am_sweep_in_flight, _remedy_in_flight and _deferred: one i64 per slot, refused before the tick guard, after the
-// staged calls; `off` everywhere while on() is false, else what gather(d_idx, d_out) — a kernel over the slots as
-// stage_indices left them, on the handle's stream — writes to d_out.
-template <class On, class Gather>
-int query_slots(am_sweep* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* out, On&& on, int64_t off,
-                Gather&& gather) {
-  if (!h || (n && !out)) return AM_E_INVAL;
+// The per-slot states (AM_SEL_*) behind am_sweep_in_flight, _remedy_in_flight, _deferred and am_sweep_select: whether
+// the handle has the state on (every slot reads INT64_MIN while it is off) ...
+bool state_on(const am_sweep* h, uint32_t state) {
+  return state == AM_SEL_WAITING ? admission_on(h) : h->hold && (state == AM_SEL_IN_FLIGHT || h->remedy);
+}
+// ... and the values of the slots first + k (d_idx NULL) or first + d_idx[k], k < n, into d_out on the handle's stream.
+cudaError_t launch_values(am_sweep* h, uint32_t state, uint64_t first, const uint32_t* d_idx, uint64_t n, int64_t* d_out) {
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  if (state == AM_SEL_WAITING)
+    return launch(h, adm_gather_kernel, grid, 256, h->stream, (const int64_t*)h->adm_wait, (uint32_t)first, d_idx,
+                  (uint32_t)n, d_out);
+  return launch(h, in_flight_kernel, grid, 256, h->stream, h->cols, (const int64_t*)h->since, (uint32_t)first, d_idx,
+                (uint32_t)n, d_out, state == AM_SEL_REMEDY_IN_FLIGHT);
+}
+
+// The path of every per-slot query: nothing for n == 0, the slots refused before the tick guard, then the guard and
+// the drain (posted results, removes and loads by now release holds and end waits), then run(state_on(h, state)).
+template <class Run>
+int slot_query(am_sweep* h, uint32_t state, uint64_t first, uint64_t n, const uint64_t* idx, Run&& run) {
   if (n == 0) return AM_OK;
   int rc = check_slots(h, first, n, idx);
   if (rc != AM_OK) return rc;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  rc = begin_call(h);  // posted results, removes and loads by now release holds and end waits
-  if (rc != AM_OK) return rc;
-  if (!on()) {
-    for (uint64_t k = 0; k < n; ++k) out[k] = off;
-    return AM_OK;
-  }
-  const uint32_t* d_idx;
-  rc = stage_indices(h, n * 8, n, idx, &d_idx);
-  if (rc != AM_OK) return rc;
-  AM_CUDA(h, gather(d_idx, (int64_t*)h->dev_in.p));
-  return read_back(h, out, h->dev_in.p, n * 8);
+  rc = begin_call(h);
+  return rc != AM_OK ? rc : run(state_on(h, state));
 }
 
-int in_flight_impl(am_sweep* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* out, bool remedy) {
-  return query_slots(h, first, n, idx, out, [&] { return h->hold && (!remedy || h->remedy); }, kNotInFlight,
-                     [&](const uint32_t* d_idx, int64_t* d_out) {
-                       return launch(h, in_flight_kernel, (unsigned)((n + 255) / 256), 256, h->stream, h->cols,
-                                     (const int64_t*)h->since, (uint32_t)first, d_idx, (uint32_t)n, d_out, remedy);
-                     });
+// am_sweep_in_flight, _remedy_in_flight and _deferred: one i64 per slot, INT64_MIN everywhere while the state is off.
+int query_slots(am_sweep* h, uint32_t state, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* out) {
+  if (!h || (n && !out)) return AM_E_INVAL;
+  return slot_query(h, state, first, n, idx, [&](bool on) {
+    if (!on) {
+      for (uint64_t k = 0; k < n; ++k) out[k] = INT64_MIN;
+      return AM_OK;
+    }
+    const uint32_t* d_idx;
+    int rc = stage_indices(h, n * 8, n, idx, &d_idx);
+    if (rc != AM_OK) return rc;
+    AM_CUDA(h, launch_values(h, state, idx ? 0 : first, d_idx, n, (int64_t*)h->dev_in.p));
+    return read_back(h, out, h->dev_in.p, n * 8);
+  });
+}
+
+int sel_alloc(am_sweep* h) {
+  if (h->sel_acc) return AM_OK;
+  const size_t ngroups = groups_of(h->cap_padded);
+  AM_CUDA(h, dev_array(h, &h->sel_bits, ngroups * kGroupWords * 4, h->stream, false));
+  AM_CUDA(h, dev_array(h, &h->sel_group, ngroups * 4, h->stream, false));
+  AM_CUDA(h, dev_array(h, &h->sel_prefix, (ngroups + 1) * 4, h->stream, false));
+  AM_CUDA(h, dev_array(h, &h->sel_list, h->cap_padded * 4, h->stream, false));
+  AM_CUDA(h, dev_array(h, &h->sel_acc, 2 * 8, h->stream, false));  // (the last: the others exist once it does)
+  return AM_OK;
 }
 }  // namespace
 
 extern "C" {
 
 int am_sweep_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
-  return in_flight_impl(h, first, n, idx, since_out, false);
+  return query_slots(h, AM_SEL_IN_FLIGHT, first, n, idx, since_out);
 }
 
 int am_sweep_remedy_in_flight(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* started_out) {
-  return in_flight_impl(h, first, n, idx, started_out, true);
+  return query_slots(h, AM_SEL_REMEDY_IN_FLIGHT, first, n, idx, started_out);
 }
 
 int am_sweep_deferred(am_sweep_t* h, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out) {
-  return query_slots(h, first, n, idx, since_out, [&] { return admission_on(h); }, kNotWaiting,
-                     [&](const uint32_t* d_idx, int64_t* d_out) {
-                       return launch(h, adm_gather_kernel, (unsigned)((n + 255) / 256), 256, h->stream,
-                                     (const int64_t*)h->adm_wait, (uint32_t)first, d_idx, (uint32_t)n, d_out);
-                     });
+  return query_slots(h, AM_SEL_WAITING, first, n, idx, since_out);
+}
+
+// The mark pass writes the range's bitmap, group counts and accumulators; with cap > 0 the scan and the compaction
+// list every match (relative to first) and the values of the first m = min(cap, n) list entries are gathered.  The
+// entries past the matches are zeroed first, so that the gather reads slot `first` for them.  One synchronisation
+// brings back the accumulators and m entries of the list and the values.
+int am_sweep_select(am_sweep_t* h, uint32_t state, uint64_t first, uint64_t n, int64_t before, uint64_t* idx,
+                    int64_t* value, uint64_t cap, uint64_t* n_match, int64_t* oldest) {
+  if (!h || state < AM_SEL_IN_FLIGHT || state > AM_SEL_WAITING || !n_match || !oldest || (cap && (!idx || !value)))
+    return AM_E_INVAL;
+  *n_match = 0;
+  *oldest = INT64_MAX;
+  return slot_query(h, state, first, n, nullptr, [&](bool on) {
+    if (!on) return AM_OK;
+    int rc = sel_alloc(h);
+    if (rc != AM_OK) return rc;
+    const uint32_t n_groups = groups_of(n);
+    const uint64_t m = std::min(cap, n);
+    AM_CUDA(h, cudaMemsetAsync(h->sel_acc, 0xFF, 8, h->stream));
+    AM_CUDA(h, cudaMemsetAsync(h->sel_acc + 1, 0, 8, h->stream));
+    const bool waiting = state == AM_SEL_WAITING;
+    AM_CUDA(h, launch(h, select_mark_kernel, n_groups, kGroupWords, h->stream, h->cols,
+                      (const int64_t*)(waiting ? nullptr : h->since), (const int64_t*)(waiting ? h->adm_wait : nullptr),
+                      state == AM_SEL_REMEDY_IN_FLIGHT, (uint32_t)first, (uint32_t)n, before, h->sel_bits,
+                      h->sel_group, h->sel_acc));
+    if (m) {
+      ScanParams sc{};
+      sc.group_count = h->sel_group;
+      sc.group_prefix = h->sel_prefix;
+      sc.acc = h->sel_acc;
+      sc.n_groups = n_groups;
+      sc.cap = 0xFFFFFFFFu;
+      AM_CUDA(h, cudaMemsetAsync(h->sel_list, 0, m * 4, h->stream));
+      AM_CUDA(h, launch(h, scan_groups_kernel, 1, 1024, h->stream, sc));
+      AM_CUDA(h, launch(h, list_changes_kernel, n_groups, kGroupWords, h->stream, h->sel_bits,
+                        (const uint32_t*)h->sel_prefix, h->sel_list));
+      AM_CUDA(h, h->dev_in.reserve(m * 8));
+      AM_CUDA(h, launch_values(h, state, first, h->sel_list, m, (int64_t*)h->dev_in.p));
+    }
+    // pin_in: the accumulators, m values, m list entries
+    AM_CUDA(h, h->pin_in.reserve(16 + m * 12));
+    char* p = (char*)h->pin_in.p;
+    AM_CUDA(h, cudaMemcpyAsync(p, h->sel_acc, 16, cudaMemcpyDeviceToHost, h->stream));
+    if (m) {
+      AM_CUDA(h, cudaMemcpyAsync(p + 16, h->dev_in.p, m * 8, cudaMemcpyDeviceToHost, h->stream));
+      AM_CUDA(h, cudaMemcpyAsync(p + 16 + m * 8, h->sel_list, m * 4, cudaMemcpyDeviceToHost, h->stream));
+    }
+    AM_CUDA(h, cudaStreamSynchronize(h->stream));
+    const unsigned long long* acc = (const unsigned long long*)p;
+    const uint64_t nm = acc[1];
+    *n_match = nm;
+    if (nm) *oldest = (int64_t)(acc[0] ^ (1ull << 63));
+    const uint64_t k = std::min(cap, nm);
+    const int64_t* vals = (const int64_t*)(p + 16);
+    const uint32_t* list = (const uint32_t*)(p + 16 + m * 8);
+    for (uint64_t j = 0; j < k; ++j) {
+      idx[j] = h->shard_base + first + list[j];
+      value[j] = vals[j];
+    }
+    return nm > cap ? AM_E_NOSPACE : AM_OK;
+  });
 }
 
 // One of the last tick's two timed-out lists, entries [offset, ...) as global indices: the health-check runs, or the

@@ -1395,17 +1395,24 @@ __global__ void fill_i64_kernel(int64_t* p, int64_t v, uint64_t n) {
   for (; i < n; i += stride) p[i] = v;
 }
 
-// am_sweep_in_flight: since of the slots the next tick would hold (the sweep's rule, on the drained state) for a
-// health-check run, else kNotInFlight.  `remedy` (am_sweep_remedy_in_flight): the start of a held remedy run instead.
-// idx == NULL: the range [first, first + n).
+// What am_sweep_in_flight reports for slot i: since of a slot the next tick would hold (the sweep's rule, on the drained
+// state) for a health-check run, else kNotInFlight.  `remedy` (am_sweep_remedy_in_flight): the start of a held remedy
+// run instead.  finishedAt and the flags are read only for a slot whose since is set.  The one definition of both
+// values: the dense queries and am_sweep_select's mark pass call it.
+__device__ __forceinline__ int64_t held_run_start(const DevCols& c, const int64_t* __restrict__ since, uint32_t i,
+                                                  bool remedy) {
+  const int64_t s = since[i];
+  const bool held = held_run(s, [&] { return c.finished_at[i]; }, [&] { return c.flags[i]; });
+  return held && is_remedy_run(s) == remedy ? run_start(s) : kNotInFlight;
+}
+
+// am_sweep_in_flight / am_sweep_remedy_in_flight: held_run_start of the slots first + k (idx == NULL) or first + idx[k],
+// k < n.
 __global__ void in_flight_kernel(DevCols c, const int64_t* __restrict__ since, uint32_t first, const uint32_t* __restrict__ idx,
                                  uint32_t n, int64_t* out, bool remedy) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
-  const uint32_t i = idx ? idx[k] : first + k;
-  const int64_t s = since[i];
-  const bool held = held_run(s, [&] { return c.finished_at[i]; }, [&] { return c.flags[i]; });
-  out[k] = held && is_remedy_run(s) == remedy ? run_start(s) : kNotInFlight;
+  out[k] = held_run_start(c, since, first + (idx ? idx[k] : k), remedy);
 }
 
 // Workflow timeouts: the drain's winning upserts (the marks decide, as in apply_state_ops_kernel) store their record's

@@ -469,6 +469,40 @@ class Sweep:
         arguments as in_flight"""
         return self._per_slot("am_sweep_deferred", first, n, idx)
 
+    def select(self, state: int, first: int = 0, n: int | None = None, before: int | None = None,
+               cap: int | None = None):
+        """the slots of [first, first+n) in `state` (SEL_IN_FLIGHT, SEL_REMEDY_IN_FLIGHT or SEL_WAITING) whose value,
+        what in_flight / remedy_in_flight / deferred returns for them, is <= before (None: any), found on the device
+        (am_sweep_select): (global idx u64 ascending, value i64, n_match, oldest).  n defaults as in in_flight.  cap
+        None: every match (a counting call first); else at most cap of them, n_match and oldest still over the whole
+        range; cap 0 is the counting form.  oldest is INT64_MAX when nothing matches."""
+        if n is None:
+            n = max(self.size - first, 0)
+        before = (1 << 63) - 1 if before is None else int(before)
+        nm, old = L.u64(0), L.i64(0)
+
+        def call(k):
+            idx, value = np.empty(k, dtype=np.uint64), np.empty(k, dtype=np.int64)
+            rc = self._lib.am_sweep_select(self._h, state, first, n, before, idx.ctypes.data if k else None,
+                                           value.ctypes.data if k else None, k, C.byref(nm), C.byref(old))
+            if rc not in (L.AM_OK, L.AM_E_NOSPACE):
+                self._check(rc, "am_sweep_select")
+            return rc, idx, value
+
+        if cap is None:  # count, then fetch; again if calls staged in between added matches
+            while True:
+                rc, idx, value = call(0)
+                cap = int(nm.value)
+                if cap == 0:
+                    break
+                rc, idx, value = call(cap)
+                if rc == L.AM_OK:
+                    break
+        else:
+            rc, idx, value = call(cap)
+        k = min(int(nm.value), cap)
+        return idx[:k], value[:k], int(nm.value), int(old.value)
+
     def _timed_out(self, fn: str, offset: int, cap: int | None):
         n = L.u64(0)
         call = getattr(self._lib, fn)

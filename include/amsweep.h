@@ -595,6 +595,34 @@ int am_sweep_last_timed_out(am_sweep_t*, uint64_t offset, uint64_t* idx, int64_t
  * hcc.go:609/638/665), which the caller can write back with the result. */
 int am_sweep_in_flight(am_sweep_t*, uint64_t first, uint64_t n, const uint64_t* idx, int64_t* since_out);
 
+/* Sparse state queries: the slots of [first, first+n) in one state, with their value, their count and the least value,
+ * found on the device (DESIGN.md section 6 item 22), so that a restart, a stuck-run alert or a gauge need not copy a
+ * dense read of every slot to the host.
+ *  - A STATE names one dense per-slot query; the value of a slot is what that query returns for it at this point:   */
+#define AM_SEL_IN_FLIGHT 1u        /* value = what am_sweep_in_flight returns for the slot        */
+#define AM_SEL_REMEDY_IN_FLIGHT 2u /* value = what am_sweep_remedy_in_flight returns for the slot */
+#define AM_SEL_WAITING 3u          /* value = what am_sweep_deferred returns for the slot         */
+/*  - Slot i of [first, first+n) MATCHES when its value v is not INT64_MIN and v <= before (INT64_MAX: every slot in
+ *    the state; T - X: in it since before T - X).
+ *  - idx[k] (global index, shard_base added, ascending) and value[k] of the first min(cap, *n_match) matches are
+ *    written; *n_match = the matches of the whole range and *oldest = their least value (INT64_MAX when none), also
+ *    when the list is cut short.  AM_E_NOSPACE when *n_match > cap (the first cap entries are valid).  With cap == 0,
+ *    idx and value may be NULL: the counting form.  Page with a cursor: call again with first = the last returned
+ *    local slot + 1 (the call keeps nothing between calls).
+ *  - Refused with AM_E_INVAL before the tick guard, nothing drained: an unknown state, n_match or oldest NULL, cap > 0
+ *    with idx or value NULL, or a range am_sweep_in_flight refuses.  Otherwise it behaves as am_sweep_in_flight does:
+ *    n == 0 returns at once, AM_E_BUSY during a tick, staged calls are drained first, and a tick of
+ *    am_sweep_tick_device / am_sweep_tick_shard on a caller stream is waited for.
+ *  - While the state is off (the hold, the remedy hold, or the hold with the admission state of a finite budget) the
+ *    call returns AM_OK with *n_match = 0 and *oldest = INT64_MAX, and launches nothing beyond its drain.
+ *  - Kernel launches of a call that reaches the device: 4 with cap > 0 (the mark pass, the group scan, the
+ *    compaction and the gather of min(cap, n) values, whether or not anything matches), 1 with cap == 0.  One
+ *    synchronisation.  The first such call allocates about 4.13 B per slot of capacity on the device (a 1-bit mask,
+ *    per-group counts and offsets, the list), kept until am_sweep_destroy; a handle that never calls it allocates and
+ *    launches nothing for it. */
+int am_sweep_select(am_sweep_t*, uint32_t state, uint64_t first, uint64_t n, int64_t before, uint64_t* idx,
+                    int64_t* value, uint64_t cap, uint64_t* n_match, int64_t* oldest);
+
 /* Status changes: which checks need their status written back after a tick (the reference writes
  * the status subresource after every phase it applies, updateHealthCheckStatus, hcc.go:734 and
  * :1445-1462).  Off by default.  While on, every tick of every entry point (am_sweep_tick,
@@ -686,8 +714,8 @@ int am_sweep_last_change_details(am_sweep_t*, uint64_t offset, uint64_t* idx, am
  * EQUIVALENCE: restore the blobs of one checkpoint of a handle H, all taken between the same two ticks, into handles
  * whose shards cover H's swept slots; from then on the same calls, split by slot, return what they return on H (every
  * tick entry point with its list and statistics except n_records, which is per shard; am_sweep_simulate; read,
- * in_flight, remedy_in_flight, repeat_after_sec, next_due; the timed-out lists, the changes and the details).  With one
- * handle of the same shard that includes n_records. */
+ * in_flight, remedy_in_flight, select, repeat_after_sec, next_due; the timed-out lists, the changes and the details).
+ * With one handle of the same shard that includes n_records. */
 #define AM_CHECKPOINT_VERSION 1
 #define AM_CKPT_HOLD 0x1u     /* the hold in flight was on                   */
 #define AM_CKPT_REMEDY 0x2u   /* ... and the remedy hold                      */

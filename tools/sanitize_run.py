@@ -1,5 +1,5 @@
 """Small driver for compute-sanitizer: every kernel variant (open/closed loop, on/off
-minute), staged upsert/remove/post_result, read-by-index, on-device Next()."""
+minute), staged upsert/remove/post_result, read-by-index, on-device Next(), and one sparse state query per state."""
 import importlib, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, "tools", "amgen")):
@@ -23,4 +23,10 @@ with am.Sweep(capacity=n + 500) as s:
     s.read(np.arange(0, n, 97))
     s.repeat_after_sec(T0, 0, 5000)
     s.run_ticks(T0 + 100, 5, mode=1, seed=3)
+    s.set_hold_in_flight(True)
+    s.set_hold_remedy(True)
+    s.set_submit_budget(100)
+    s.tick(T0 + 200)
+    for state in (am.SEL_IN_FLIGHT, am.SEL_REMEDY_IN_FLIGHT, am.SEL_WAITING):
+        s.select(state, 3, n - 10, T0 + 200, cap=1000)
 print("sanitize_run ok", tot)
