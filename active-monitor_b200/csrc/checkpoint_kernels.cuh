@@ -390,10 +390,12 @@ __global__ void __launch_bounds__(256) delta_offsets_verify_kernel(const uint32_
 }
 
 // am_sweep_restore_delta: element k of the delta to slot first + offs[k], by the rules of checkpoint_scatter_kernel,
-// and the slot's segment marked for delta_planes_kernel.
+// and the slot's segment marked for delta_planes_kernel; the slot's due word as well while the handle keeps them (`due`
+// NULL otherwise).
 __global__ void __launch_bounds__(256) delta_scatter_kernel(const CkptState s, const CkptBlob b,
                                                            const uint32_t* __restrict__ offs, uint64_t first,
-                                                           const ZoneLut lut, uint32_t* seg_dirty) {
+                                                           const ZoneLut lut, uint32_t* seg_dirty, uint32_t* due,
+                                                           int64_t due_epoch) {
   const uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (k >= b.n) return;
   const uint64_t i = first + offs[k];
@@ -425,6 +427,7 @@ __global__ void __launch_bounds__(256) delta_scatter_kernel(const CkptState s, c
     s.det_start[i] = ck_blob_get<int64_t>(b, kCkSecDetStart, k);
   }
   if (s.wait) s.wait[i] = ck_blob_get<int64_t>(b, kCkSecWait, k);
+  if (due) due[i] = due_word(ck_blob_get<int32_t>(b, 5, k), ck_blob_get<int64_t>(b, 7, k), due_epoch);
   seg_dirty[i / kRecPerWarp] = 1u;
 }
 

@@ -312,6 +312,17 @@ struct am_sweep {
   uint32_t* sel_prefix = nullptr;
   uint32_t* sel_list = nullptr;
   unsigned long long* sel_acc = nullptr;
+  // due words (due_word, sweep_kernels.cuh) of the open-loop plain ticks, allocated at the first one ([cap_padded]): exact
+  // for slots [0, due_end) against the epoch due_epoch while due_valid.  The few writers of ras and finishedAt the common
+  // flows run keep them (the DUE sweep variants, the drain's upserts, spec updates and results, delta restores); every
+  // other one clears due_valid, and the next such tick rebuilds them (due_tick).  A caller handed ras or finishedAt by
+  // am_sweep_column_ptr may write them unseen: due_exposed, never cleared, keeps the handle on the variants that read
+  // both columns.
+  uint32_t* due = nullptr;
+  int64_t due_epoch = 0;
+  uint64_t due_end = 0;
+  bool due_valid = false;
+  std::atomic<bool> due_exposed{false};
 };
 
 namespace {
@@ -716,6 +727,7 @@ int rebuild_planes(am_sweep* h, uint64_t first, uint64_t n) {
   const uint64_t seg0 = first / kRecPerWarp, n_seg = (first + n + kRecPerWarp - 1) / kRecPerWarp - seg0;
   AM_CUDA(h, launch(h, build_planes_range_kernel, (unsigned)((n_seg + kWarps - 1) / kWarps), kBlock, h->stream, h->cols,
                     h->planes, (uint32_t)seg0, (uint32_t)n_seg));
+  h->due_valid = false;  // (the range's ras and finishedAt were replaced: the next plain tick rebuilds the due words)
   return AM_OK;
 }
 
@@ -767,6 +779,9 @@ int claim_set(am_sweep* h, TickSet& ts, cudaStream_t s) {
   }
   return AM_OK;
 }
+
+// The due words for a kernel that writes ras or finishedAt to keep, NULL when there is nothing exact to keep.
+uint32_t* due_kept(const am_sweep* h) { return h->due_valid ? h->due : nullptr; }
 
 // Apply staged upserts / removes / results on stream `s` (called with the tick guard held).
 // The staging lock is held only for the buffer swap.
@@ -829,7 +844,7 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
   AM_CUDA(h, launch(h, mark_ops, G, B, s, h->marks, d_ops, (uint32_t)n, spec ? h->spec_marks : nullptr));
   if (st->n_state)
     AM_CUDA(h, launch_pdl(h, apply_state_ops_kernel, G, B, s, h->cols, h->marks, d_ops, d_recs, (uint32_t)n,
-                          h->seg_dirty));
+                          h->seg_dirty, due_kept(h), h->due_epoch));
   if (spec) {  // spec updates on top of the upserts: their W after the upserts' W, so a later spec update's wins
     if (st->any_wf && !h->wf_timeout) {
       const int rc = alloc_timeouts(h, s);
@@ -839,7 +854,8 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
       AM_CUDA(h, launch_pdl(h, store_wf_timeout_kernel, G, B, s, h->wf_timeout, h->marks, d_ops, d_recs, (uint32_t)n));
     AM_CUDA(h, launch_pdl(h, apply_spec_ops_kernel, G, B, s, h->cols, h->marks, (const uint32_t*)h->spec_marks, d_ops,
                           d_recs, (uint32_t)n, h->seg_dirty, h->wf_timeout, h->track ? h->chg_bits : nullptr,
-                          h->details ? h->det_applied : nullptr, h->details ? h->det_start : nullptr));
+                          h->details ? h->det_applied : nullptr, h->details ? h->det_start : nullptr, due_kept(h),
+                          h->due_epoch));
   }
   if (st->n_state || spec) {
     // upserts, removes and spec updates may change kinds, zones and masks: rebuild the plane words of the segments
@@ -886,7 +902,8 @@ int drain_staged(am_sweep* h, cudaStream_t s, const int64_t* tick_T = nullptr, b
     auto* apply_now = r ? apply_results_now_kernel<true> : apply_results_now_kernel<false>;
     AM_CUDA(h, launch_pdl(h, apply_now, G, B, s, h->cols, h->marks, d_ops, (uint32_t)n, *tick_T, ts.acc,
                           r ? h->since : nullptr, r ? h->deadline : nullptr,
-                          r ? (const int32_t*)h->wf_timeout : nullptr, r ? h->seg_deadline : nullptr));
+                          r ? (const int32_t*)h->wf_timeout : nullptr, r ? h->seg_deadline : nullptr, due_kept(h),
+                          h->due_epoch));
   } else if (st->n_result) {
     AM_CUDA(h, launch_pdl(h, apply_result_ops_kernel, G, B, s, h->cols.flags, h->marks, d_ops, (uint32_t)n));
   }
@@ -1011,13 +1028,13 @@ int plan_window(am_sweep* h, int64_t T, uint32_t mode, WindowPlan* w) {
 }
 
 // The sweep variant of a tick: a row per loop mode, a column per way the masks are read (not at all, the planes of
-// T's minute, the canonical masks against a catch-up window's boxes).  These are the 18 instantiations of
-// sweep_tick_kernel there are.  Two combinations have none and never get here: closed loop with the hold on (refused
-// before the drain, and run_ticks refuses the hold) and a window with the planes (launch_tick sets `masks` only
-// without a window).
+// T's minute, the canonical masks against a catch-up window's boxes).  These are the 22 instantiations of
+// sweep_tick_kernel there are.  Three combinations have none and never get here: closed loop with the hold on (refused
+// before the drain, and run_ticks refuses the hold), a window with the planes (launch_tick sets `masks` only
+// without a window) and the due words with a window (due_tick takes them only without one).
 using SweepFn = void (*)(const SweepParams);
-SweepFn sweep_variant(bool closed, bool masks, bool window, bool hold, bool timeout, bool remedy) {
-  static constexpr SweepFn kVariants[6][3] = {
+SweepFn sweep_variant(bool closed, bool masks, bool window, bool hold, bool timeout, bool remedy, int due) {
+  static constexpr SweepFn kVariants[8][3] = {
       // open loop
       {sweep_tick_kernel<false, false>, sweep_tick_kernel<false, true>, sweep_tick_kernel<false, false, true>},
       // closed loop
@@ -1033,8 +1050,37 @@ SweepFn sweep_variant(bool closed, bool masks, bool window, bool hold, bool time
        sweep_tick_kernel<false, false, true, true, false, true>},
       // ... and workflow timeouts
       {sweep_tick_kernel<false, false, false, true, true, true>, sweep_tick_kernel<false, true, false, true, true, true>,
-       sweep_tick_kernel<false, false, true, true, true, true>}};
-  return kVariants[hold ? 2 + timeout + 2 * remedy : closed][window ? 2 : masks];
+       sweep_tick_kernel<false, false, true, true, true, true>},
+      // open loop from the due words, and open loop building them (no window, no hold: due_tick)
+      {sweep_tick_kernel<false, false, false, false, false, false, kDueRead>,
+       sweep_tick_kernel<false, true, false, false, false, false, kDueRead>, nullptr},
+      {sweep_tick_kernel<false, false, false, false, false, false, kDueBuild>,
+       sweep_tick_kernel<false, true, false, false, false, false, kDueBuild>, nullptr}};
+  return kVariants[due ? 5 + due : hold ? 2 + timeout + 2 * remedy : closed][window ? 2 : masks];
+}
+
+// The DUE of a tick's sweep variant.  An open-loop tick without a window or the hold, on a handle that has not handed
+// out ras or finishedAt, reads the due words when they are exact for every slot it sweeps and T lies in their epoch's
+// window; otherwise it builds them (kDueBuild, epoch T - 2^31: the tick reads ras and finishedAt as without the words and
+// writes every swept slot's word, so a rebuild costs no launch).  Any other tick runs a variant that may write
+// finishedAt without its word: the words are dropped.
+int due_tick(am_sweep* h, int64_t T, bool plain, uint32_t n_tiles, cudaStream_t s, int* due) {
+  *due = kDueOff;
+  if (!plain || h->due_exposed.load(std::memory_order_relaxed)) {
+    h->due_valid = false;
+    return AM_OK;
+  }
+  const uint64_t end = (uint64_t)n_tiles * kTile;
+  if (h->due_valid && T >= h->due_epoch && T - h->due_epoch < kDueSpan && end <= h->due_end) {
+    *due = kDueRead;
+    return AM_OK;
+  }
+  if (!h->due) AM_CUDA(h, dev_array(h, &h->due, h->cap_padded * 4, s, false));
+  h->due_epoch = T - kDueEpochLead;
+  h->due_end = end;
+  h->due_valid = true;  // (from this tick's sweep on)
+  *due = kDueBuild;
+  return AM_OK;
 }
 
 int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStream_t s, const WindowPlan* win = nullptr) {
@@ -1090,6 +1136,9 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
     p.pl.dow = plane(kPlaneDow + ct.dow);
     p.pl.star = plane(kPlaneStar);
   }
+  const bool closed = (mode & AM_SWEEP_CLOSED_LOOP) != 0;
+  int due = kDueOff;
+  if (int rc = due_tick(h, T, !closed && !window && !h->hold, p.n_tiles, s, &due)) return rc;
   if (h->profiling) AM_CUDA(h, cudaEventRecord(h->evp[0], s));
   const bool timeout = h->hold && h->wf_timeout;
   if (h->hold) p.since = h->since;  // hold in flight: the variants that read and write since
@@ -1098,7 +1147,12 @@ int launch_tick(am_sweep* h, int64_t T, uint32_t mode, const ListOut& o, cudaStr
     p.deadline = h->deadline;
     p.seg_deadline = h->seg_deadline;
   }
-  const SweepFn sweep = sweep_variant((mode & AM_SWEEP_CLOSED_LOOP) != 0, masks, window, h->hold, timeout, h->remedy);
+  if (due) {
+    p.due = h->due;
+    p.due_t = (uint32_t)(T - h->due_epoch);
+    p.due_epoch = h->due_epoch;
+  }
+  const SweepFn sweep = sweep_variant(closed, masks, window, h->hold, timeout, h->remedy, due);
   // A single-stream tick's sweep launches early and hides behind its predecessor (the previous tick's publish, the
   // drain).  am_sweep_tick_shard's is a plain launch: an early-launched sweep could park its CTAs on every SM ahead
   // of the previous tick's exchange on the other stream; measured at two GPUs it made no difference to the step, so
@@ -1275,6 +1329,7 @@ uint64_t block_ticks() {
 template <class P, class Launch>
 int run_blocks(am_sweep* h, int64_t T0, uint64_t n, am_tick_stats_t* stats, P b, Launch&& launch_block) {
   const uint64_t per_block = block_ticks();
+  h->due_valid = false;  // (the blocked kernels write finishedAt without the due words)
   const unsigned grid = (unsigned)((h->n_records + kBlockRecords - 1) / kBlockRecords);
   for (uint64_t k = 0; k < n;) {
     const int64_t T = T0 + (int64_t)k;
@@ -1466,7 +1521,9 @@ int am_sweep_device(const am_sweep_t* h) { return h ? h->device : -1; }
 double am_sweep_last_kernel_ms(const am_sweep_t* h) { return h ? h->last_ms : -1.0; }
 uint64_t am_sweep_launch_count(const am_sweep_t* h) { return h ? h->launches.load(std::memory_order_relaxed) : 0; }
 void* am_sweep_column_ptr(am_sweep_t* h, int column) {
-  return (h && column >= 0 && column < 16) ? *col_slot(h->cols, column) : nullptr;
+  if (!h || column < 0 || column >= 16) return nullptr;
+  if (column == 5 || column == 7) h->due_exposed.store(true, std::memory_order_relaxed);  // ras, finished_at
+  return *col_slot(h->cols, column);
 }
 int am_sweep_set_profiling(am_sweep_t* h, int on) {
   if (!h) return AM_E_INVAL;
@@ -3086,7 +3143,8 @@ int am_sweep_restore_delta(am_sweep_t* h, const void* buf, uint64_t len) {
   }
   if (m) {
     AM_CUDA(h, launch(h, delta_scatter_kernel, (unsigned)((m + 255) / 256), 256, h->stream, ckpt_state(h),
-                      ckd_blob(h, L, m), (const uint32_t*)h->ckd_off, first, lut, h->seg_dirty));
+                      ckd_blob(h, L, m), (const uint32_t*)h->ckd_off, first, lut, h->seg_dirty, due_kept(h),
+                      h->due_epoch));
     AM_CUDA(h, launch(h, delta_planes_kernel, (unsigned)((m + kWarps - 1) / kWarps), kBlock, h->stream, h->cols,
                       h->planes, h->seg_dirty, (const uint32_t*)h->ckd_off, first, (uint32_t)m));
   }

@@ -29,8 +29,9 @@
 //     (five ANDs, no loop) — on the minute evaluated 32 records per word from
 //     the six bit planes (MaskPlanes) those words select;
 //   * remedy/counter columns are touched only by lanes whose record has a
-//     posted result (or is due, in closed-loop mode): 16 B/record otherwise, plus
-//     0.75 B of mask planes on the minute;
+//     posted result (or is due, in closed-loop mode): 16 B/record otherwise (8 B in the open-loop
+//     variants that read the due words instead of ras and finishedAt, DUE), plus 0.75 B of mask
+//     planes on the minute;
 //   * the emitted set leaves the kernel as a BITMAP (one bit per record: the four
 //     warp ballots the kernel takes anyway, interleaved into four 32-record words
 //     per warp, one 128-B line per tile) plus a per-tile list of EXCEPTIONS — the
@@ -278,6 +279,25 @@ __device__ __forceinline__ bool interval_due(uint32_t f, int32_t ras, int64_t fa
   return !((elapsed < (int64_t)ras) & armed);
 }
 
+// The due word of a record against the handle's epoch E: its repeat deadline D = finishedAt + ras as an offset from
+// E, clamped to [0, 0xFFFFFFFF].  For every T in [E, E + 0xFFFFFFFF) an armed record without a posted workflow phase is
+// due (interval_due) exactly when T - E >= the word: D <= E gives 0 and T >= E >= D; D - E >= 0xFFFFFFFF gives the
+// top word, which no T - E of the window reaches, and T < D.  Exact in the column domain (|time| < 2^55, i32 ras),
+// where neither T - finishedAt nor finishedAt + ras overflows.  The DUE variants of the sweep read this word instead
+// of ras and finishedAt; every writer of either column keeps it or the handle stops using it (sweep.cu, due_valid).
+AM_HD uint32_t due_word(int32_t ras, int64_t fa, int64_t E) {
+  const int64_t D = (int64_t)((uint64_t)fa + (uint64_t)(int64_t)ras);
+  if (D <= E) return 0u;
+  const uint64_t d = (uint64_t)D - (uint64_t)E;
+  return d >= 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)d;
+}
+// The handle's epoch window: the seconds T whose T - E a due word decides.
+constexpr int64_t kDueSpan = 0xFFFFFFFFll;
+constexpr int64_t kDueEpochLead = 1ll << 31;  // a build at T takes E = T - 2^31: T sits in the middle of its window
+// The sweep's use of the due words (sweep_tick_kernel's DUE): none, decide from them, or decide from ras and finishedAt
+// as without them and write every swept record's word (the build, fused into an open-loop tick).
+constexpr int kDueOff = 0, kDueRead = 1, kDueBuild = 2;
+
 // The hold rule: the run in a since word is still in flight — it started no earlier than the record's finishedAt and
 // no workflow phase is pending.  finishedAt and the flags are callables, read only when the terms before them hold.
 template <typename FinishedAt, typename Flags>
@@ -372,7 +392,13 @@ __global__ void tz_words_kernel(const int32_t* __restrict__ tz_off, TickWords* _
 // per warp lowers the segment's bound (p.seg_deadline) that expire_runs_kernel reads.
 // REMEDY = remedy hold (HOLD only, am_sweep_set_hold_remedy): a record whose posted result this sweep applies and which
 // gains AM_ACT_RUN_REMEDY without a remedy outcome merged starts a remedy run (start_remedy_run): it is not submitted.
-template <bool CLOSED, bool MASKS, bool WINDOW = false, bool HOLD = false, bool TIMEOUT = false, bool REMEDY = false>
+// DUE = kDueRead: the interval rule from the due words (open loop only, no window, no hold): phase A reads the 4-B word
+// p.due instead of 4 B of ras and 8 B of finishedAt.  The few records whose decision or finishedAt needs more — a posted
+// workflow phase (due iff ras <= 0, finishedAt = T) or STOPPED reported now (finishedAt = T) — load their ras on their
+// own and store finishedAt and the new word one record at a time.  DUE = kDueBuild: the tick of DUE = kDueOff, which
+// also writes every record's word from ras and the finishedAt the tick leaves.
+template <bool CLOSED, bool MASKS, bool WINDOW = false, bool HOLD = false, bool TIMEOUT = false, bool REMEDY = false,
+          int DUE = kDueOff>
 __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN_BLOCKS : AM_MIN_BLOCKS + 1)
     sweep_tick_kernel(const SweepParams p) {
   // one row per warp, written unconditionally: no zero-initialisation, no shared
@@ -398,12 +424,17 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
   longlong2 fa[2];
   int2 ras[2];
   uint2 fl[2];
+  uint2 dw[2];  // DUE: the due words
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     r0[h] = tile_base + (uint32_t)(warp * kRecPerWarp + h * 64 + lane * 2);
     fl[h] = ld_stream(reinterpret_cast<const uint2*>(p.c.flags + r0[h]));
-    ras[h] = ld_stream(reinterpret_cast<const int2*>(p.c.ras + r0[h]));
-    fa[h] = ld_stream(reinterpret_cast<const longlong2*>(p.c.finished_at + r0[h]));
+    if (DUE == kDueRead) {
+      dw[h] = ld_stream(reinterpret_cast<const uint2*>(p.due + r0[h]));
+    } else {
+      ras[h] = ld_stream(reinterpret_cast<const int2*>(p.c.ras + r0[h]));
+      fa[h] = ld_stream(reinterpret_cast<const longlong2*>(p.c.finished_at + r0[h]));
+    }
   }
   // The masks come from the six bit planes T tests (MaskPlanes): the warp's 128 records are 4 words of
   // each, one 16-B load per plane that every lane of the warp makes at the same address.  Nothing about
@@ -511,6 +542,7 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
   int64_t nfa[2][2];
   bool dirty[2] = {false, false};
   uint32_t needy = 0, due_bits = 0;  // bit (2h+j): record needs the remedy/counter columns / is due
+  uint32_t fix = 0;                  // DUE, bit (2h+j): the tick sets the record's finishedAt to T
 
   // ---- schedule decision for the lane's four records ------------------------
 #pragma unroll
@@ -518,7 +550,7 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const uint32_t f = j ? fl[h].y : fl[h].x;
-      const int64_t fav = j ? fa[h].y : fa[h].x;
+      const int64_t fav = DUE == kDueRead ? 0 : (j ? fa[h].y : fa[h].x);
       const bool live = is_live(f);
       const bool pending = (f & kPendBits) != 0;
       // (an if, not `MASKS && ...`: with the latter ptxas hoisted this loop's arithmetic above the
@@ -526,7 +558,11 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
       bool due_cron = false;
       if (MASKS || WINDOW) due_cron = ((cron_bits >> (2 * h + j)) & 1u) != 0;
       const uint32_t kind = f & AM_KIND_MASK;
-      const bool due_iv = interval_due(f, j ? ras[h].y : ras[h].x, fav, T);
+      bool due_iv;
+      if (DUE == kDueRead)  // (a posted workflow phase: decided from ras below)
+        due_iv = !(f & kHcBits) && (!(f & AM_F_TIMER_ARMED) || p.due_t >= (j ? dw[h].y : dw[h].x));
+      else
+        due_iv = interval_due(f, j ? ras[h].y : ras[h].x, fav, T);
       const bool is_iv = is_interval_kind(kind);
       // (the rest of the ladder is written out here and in block_record: behind a function, ptxas turned
       // these `live && ...` into branch-free code that spilled more in the closed-loop on-minute variant)
@@ -543,6 +579,33 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
       }
       if (live && (pending || (CLOSED && due))) needy |= 1u << (2 * h + j);
       if (due) due_bits |= 1u << (2 * h + j);
+      if (DUE && live && (stopped_now || (f & kHcBits))) fix |= 1u << (2 * h + j);
+    }
+  }
+
+  // ---- kDueBuild: every record's word, from its finishedAt after this tick (T where `fix` says so)
+  if (DUE == kDueBuild) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t a0 = (fix >> (2 * h)) & 1u ? T : fa[h].x, a1 = (fix >> (2 * h + 1)) & 1u ? T : fa[h].y;
+      st_stream(reinterpret_cast<uint2*>(p.due + r0[h]),
+                make_uint2(due_word(ras[h].x, a0, p.due_epoch), due_word(ras[h].y, a1, p.due_epoch)));
+    }
+  }
+  // ---- kDueRead: the records whose finishedAt this tick sets to T (apply_result does for a workflow phase, and the
+  //      pause rule for STOPPED; both when the two meet).  Rare: their ras one record at a time, which also decides a
+  //      posted phase's interval rule (elapsed 0: due iff ras <= 0), then finishedAt and the new due word.
+  if (DUE == kDueRead && __any_sync(kFull, fix != 0)) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if ((fix >> q) & 1u) {
+        const uint32_t i = r0[q >> 1] + (uint32_t)(q & 1);
+        const uint32_t f = (q & 1) ? fl[q >> 1].y : fl[q >> 1].x;
+        const int32_t rv = ld_stream(p.c.ras + i);
+        if ((f & kHcBits) && is_interval_kind(f & AM_KIND_MASK) && rv <= 0) act[q >> 1][q & 1] |= AM_ACT_SUBMIT_HC;
+        st_stream(p.c.finished_at + i, T);
+        st_stream(p.due + i, due_word(rv, T, p.due_epoch));
+      }
     }
   }
 
@@ -713,7 +776,8 @@ __global__ void __launch_bounds__(kBlock, ((CLOSED && MASKS) || WINDOW) ? AM_MIN
   for (int h = 0; h < 2; ++h) {
     if (dirty[h]) {
       st_stream(reinterpret_cast<uint2*>(p.c.flags + r0[h]), make_uint2(nfl[h][0], nfl[h][1]));
-      st_stream(reinterpret_cast<longlong2*>(p.c.finished_at + r0[h]), make_longlong2(nfa[h][0], nfa[h][1]));
+      if (DUE != kDueRead)  // (kDueRead: stored above, per record)
+        st_stream(reinterpret_cast<longlong2*>(p.c.finished_at + r0[h]), make_longlong2(nfa[h][0], nfa[h][1]));
     }
   }
 
@@ -1185,7 +1249,8 @@ __global__ void mark_ops_kernel(uint32_t* marks, const uint2* __restrict__ ops, 
 // upserts (hcc.go:170-188 Reconcile) and removes (hcc.go:175-186).  Both may change the slot's kind or
 // masks: its segment is marked for build_planes_dirty_kernel.
 __global__ void apply_state_ops_kernel(DevCols c, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops,
-                                       const am_record_t* __restrict__ recs, uint32_t n, uint32_t* seg_dirty) {
+                                       const am_record_t* __restrict__ recs, uint32_t n, uint32_t* seg_dirty,
+                                       uint32_t* due, int64_t due_epoch) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
@@ -1202,6 +1267,7 @@ __global__ void apply_state_ops_kernel(DevCols c, const uint32_t* __restrict__ m
   c.success[i] = r.success; c.failed[i] = r.failed; c.remedy_success[i] = r.remedy_success;
   c.remedy_failed[i] = r.remedy_failed; c.remedy_total[i] = r.remedy_total;
   c.remedy_finished_at[i] = r.remedy_finished_at;
+  if (due) due[i] = due_word(r.ras, r.finished_at, due_epoch);
 }
 
 // ---- the mask bit planes (MaskPlanes) --------------------------------------
@@ -1302,7 +1368,8 @@ __global__ void apply_result_ops_kernel(uint32_t* flags, const uint32_t* __restr
 template <bool REMEDY>
 __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__ marks, const uint2* __restrict__ ops, uint32_t n,
                                          int64_t T, unsigned long long* acc, int64_t* since, int64_t* deadline,
-                                         const int32_t* __restrict__ wf_timeout, unsigned long long* seg_deadline) {
+                                         const int32_t* __restrict__ wf_timeout, unsigned long long* seg_deadline,
+                                         uint32_t* due, int64_t due_epoch) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   uint32_t res = 0;
@@ -1341,7 +1408,10 @@ __global__ void apply_results_now_kernel(DevCols c, const uint32_t* __restrict__
         }
         const RecState b = s;
         const uint32_t a = apply_result(s, T, res);
-        if (r_ok || r_fail) c.finished_at[i] = s.fa;
+        if (r_ok || r_fail) {
+          c.finished_at[i] = s.fa;
+          if (due) due[i] = due_word(c.ras[i], s.fa, due_epoch);
+        }
         if (s.s != b.s) c.success[i] = s.s;
         if (s.f != b.f) c.failed[i] = s.f;
         if (s.rs != b.rs) c.remedy_success[i] = s.rs;
@@ -1869,7 +1939,7 @@ __global__ void capture_superseded_kernel(int64_t* start, const uint32_t* __rest
 __global__ void apply_spec_ops_kernel(DevCols c, const uint32_t* __restrict__ marks, const uint32_t* __restrict__ spec_marks,
                                       const uint2* __restrict__ ops, const am_record_t* __restrict__ recs, uint32_t n,
                                       uint32_t* seg_dirty, int32_t* wf, uint32_t* chg, uint8_t* det_applied,
-                                      int64_t* det_start) {
+                                      int64_t* det_start, uint32_t* due, int64_t due_epoch) {
   pdl_wait();  // (launched with programmatic stream serialisation: nothing of the predecessor is touched before this)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
@@ -1888,7 +1958,10 @@ __global__ void apply_spec_ops_kernel(DevCols c, const uint32_t* __restrict__ ma
 #pragma unroll
   for (int x = 0; x < 5; ++x)
     if (col[x][i] != m[x]) { col[x][i] = m[x]; planes = true; }
-  if (c.ras[i] != r.ras) c.ras[i] = r.ras;
+  if (c.ras[i] != r.ras) {
+    c.ras[i] = r.ras;
+    if (due) due[i] = due_word(r.ras, c.finished_at[i], due_epoch);
+  }
   if (c.runs_limit[i] != r.runs_limit) c.runs_limit[i] = r.runs_limit;
   if (c.reset_interval[i] != r.reset_interval) c.reset_interval[i] = r.reset_interval;
   if (wf && wf[i] != r.wf_timeout) wf[i] = r.wf_timeout;

@@ -133,6 +133,11 @@ struct SweepParams {
   const int32_t* wf_timeout;           // [cap] the slot's workflow timeout in seconds, 0 = none (the latest upsert's)
   int64_t* deadline;                   // [cap] the running workflow's deadline, kNoDeadline when none
   unsigned long long* seg_deadline;    // [cap / kRecPerWarp] per warp segment a lower bound of its deadlines (biased key)
+  // DUE variants (open loop, no window, no hold): the due words (due_word, sweep_kernels.cuh) instead of ras and
+  // finishedAt, and T - E of the handle's epoch E; NULL / 0 otherwise
+  uint32_t* due;
+  uint32_t due_t;
+  int64_t due_epoch;
 };
 constexpr int64_t kNotInFlight = INT64_MIN;
 constexpr int64_t kNoDeadline = INT64_MAX;

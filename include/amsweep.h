@@ -861,7 +861,11 @@ uint64_t am_sweep_launch_count(const am_sweep_t*);
  * column (AM_KIND_MASK, AM_F_TZ_MASK) must not be written through this
  * pointer: the on-minute sweep reads the masks as bit planes (one bitmap over the
  * shard per value a field can take) that only am_sweep_load_range, upserts and
- * removes keep up to date.  The other flag bits and the other columns may be. */
+ * removes keep up to date.  The other flag bits and the other columns may be.
+ * Handing out ras (5) or finished_at (7) switches the handle, for good, from the
+ * 4-B due word per record the open-loop tick otherwise decides interval checks
+ * from back to reading both columns (16 B per record): the library cannot see a
+ * write through the pointer, so it stops relying on a word derived from them. */
 void* am_sweep_column_ptr(am_sweep_t*, int column);
 int am_sweep_set_seed(am_sweep_t*, uint64_t seed);
 /* The handle's own non-blocking stream (cudaStream_t as void*). */
