@@ -73,6 +73,16 @@ template <class T>
 __device__ __forceinline__ uint64_t ck_term(const CkptBlob& b, int s, uint64_t j, T v) {
   return ckpt_mix((b.off[s] + j * sizeof(T)) * 8, ck_bits(v));
 }
+// Bit j of the bit section s of the blob.
+__device__ __forceinline__ uint32_t ck_blob_bit(const CkptBlob& b, int s, uint64_t j) {
+  return (ck_blob_get<uint32_t>(b, s, j >> 5) >> (j & 31)) & 1u;
+}
+// Element j of section s of the blob := v; returns its checksum term.
+template <class T>
+__device__ __forceinline__ uint64_t ck_put(const CkptBlob& b, int s, uint64_t j, T v) {
+  reinterpret_cast<T*>(b.p + b.off[s])[j] = v;
+  return ck_term(b, s, j, v);
+}
 
 // Zone ids belong to 5-field schedules only (the other kinds' bits 24..31 are carried as they are).
 __device__ __forceinline__ bool zone_bound(uint32_t flags) {
@@ -91,7 +101,47 @@ __device__ __forceinline__ void ck_reduce(uint64_t acc, uint32_t* s_zones, unsig
   if (threadIdx.x < 8 && s_zones[threadIdx.x]) atomicOr(&zones[threadIdx.x], s_zones[threadIdx.x]);
 }
 
-// am_sweep_checkpoint: element j = slot first + j, one thread each (a warp's 32 slots make one word of the bit section).
+// The section rules of a pack, per slot: slot i of the handle to element k of every section of the blob but the bit
+// section; returns the elements' checksum terms and marks the slot's zone in s_zones.
+__device__ __forceinline__ uint64_t ck_pack_slot(const CkptState& s, const CkptBlob& b, uint64_t i, uint64_t k,
+                                                 uint32_t* s_zones) {
+  uint64_t acc = 0;
+#pragma unroll
+  for (int q = 0; q < 16; ++q) {
+    if (ck_elem(q) == 8) {
+      acc += ck_put(b, q, k, reinterpret_cast<const uint64_t*>(s.col[q])[i]);
+    } else {
+      const uint32_t v = reinterpret_cast<const uint32_t*>(s.col[q])[i];
+      acc += ck_put(b, q, k, v);
+      if (q == 6) mark_zone(s_zones, v);
+    }
+  }
+  if (b.off[kCkSecWfTimeout]) {  // (both loads before the stores: the compiler cannot tell that they do not alias)
+    const int32_t w = s.wf_timeout[i];
+    const int64_t d = s.deadline[i];
+    acc += ck_put(b, kCkSecWfTimeout, k, w) + ck_put(b, kCkSecDeadline, k, d);
+  }
+  if (b.off[kCkSecSince]) acc += ck_put(b, kCkSecSince, k, s.since[i]);
+  if (b.off[kCkSecDetApplied]) {
+    const uint8_t a = s.det_applied[i];
+    const int64_t t = s.det_start[i];
+    acc += ck_put(b, kCkSecDetApplied, k, a) + ck_put(b, kCkSecDetStart, k, t);
+  }
+  if (b.off[kCkSecWait]) acc += ck_put(b, kCkSecWait, k, s.wait[i]);
+  return acc;
+}
+
+// ... and of the bit section, warp-collective (every lane calls it; `in`: k is one of the blob's elements): the change
+// bit of slot i to bit k, a warp's 32 elements one word; returns the bit's checksum term.
+__device__ __forceinline__ uint64_t ck_pack_changed(const CkptState& s, const CkptBlob& b, bool in, uint64_t i,
+                                                    uint64_t k) {
+  const uint32_t bit = in ? (s.changed[i >> 5] >> (i & 31)) & 1u : 0u;
+  const uint32_t word = __ballot_sync(kFull, bit);
+  if ((threadIdx.x & 31) == 0 && in) reinterpret_cast<uint32_t*>(b.p + b.off[kCkSecChanged])[k >> 5] = word;
+  return in ? ckpt_mix(b.off[kCkSecChanged] * 8 + k, bit) : 0;
+}
+
+// am_sweep_checkpoint: element j = slot first + j, one thread each.
 __global__ void __launch_bounds__(256) checkpoint_pack_kernel(const CkptState s, const CkptBlob b, uint64_t first,
                                                              unsigned long long* sum, uint32_t* zones) {
   __shared__ uint32_t s_zones[8];
@@ -99,53 +149,8 @@ __global__ void __launch_bounds__(256) checkpoint_pack_kernel(const CkptState s,
   __syncthreads();
   const uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   const bool in = j < b.n;
-  const uint64_t i = first + j;
-  uint64_t acc = 0;
-  if (in) {
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
-      if (ck_elem(k) == 8) {
-        const uint64_t v = reinterpret_cast<const uint64_t*>(s.col[k])[i];
-        reinterpret_cast<uint64_t*>(b.p + b.off[k])[j] = v;
-        acc += ck_term(b, k, j, v);
-      } else {
-        const uint32_t v = reinterpret_cast<const uint32_t*>(s.col[k])[i];
-        reinterpret_cast<uint32_t*>(b.p + b.off[k])[j] = v;
-        acc += ck_term(b, k, j, v);
-        if (k == 6) mark_zone(s_zones, v);
-      }
-    }
-    if (b.off[kCkSecWfTimeout]) {
-      const int32_t w = s.wf_timeout[i];
-      const int64_t d = s.deadline[i];
-      reinterpret_cast<int32_t*>(b.p + b.off[kCkSecWfTimeout])[j] = w;
-      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecDeadline])[j] = d;
-      acc += ck_term(b, kCkSecWfTimeout, j, w) + ck_term(b, kCkSecDeadline, j, d);
-    }
-    if (b.off[kCkSecSince]) {
-      const int64_t v = s.since[i];
-      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecSince])[j] = v;
-      acc += ck_term(b, kCkSecSince, j, v);
-    }
-    if (b.off[kCkSecDetApplied]) {
-      const uint8_t a = s.det_applied[i];
-      const int64_t t = s.det_start[i];
-      reinterpret_cast<uint8_t*>(b.p + b.off[kCkSecDetApplied])[j] = a;
-      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecDetStart])[j] = t;
-      acc += ckpt_mix((b.off[kCkSecDetApplied] + j) * 8, a) + ck_term(b, kCkSecDetStart, j, t);
-    }
-    if (b.off[kCkSecWait]) {
-      const int64_t v = s.wait[i];
-      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecWait])[j] = v;
-      acc += ck_term(b, kCkSecWait, j, v);
-    }
-  }
-  if (b.off[kCkSecChanged]) {  // (warp-uniform)
-    const uint32_t bit = in ? (s.changed[i >> 5] >> (i & 31)) & 1u : 0u;
-    const uint32_t word = __ballot_sync(kFull, bit);
-    if ((threadIdx.x & 31) == 0 && j < b.n) reinterpret_cast<uint32_t*>(b.p + b.off[kCkSecChanged])[j >> 5] = word;
-    if (in) acc += ckpt_mix(b.off[kCkSecChanged] * 8 + j, bit);
-  }
+  uint64_t acc = in ? ck_pack_slot(s, b, first + j, j, s_zones) : 0;
+  if (b.off[kCkSecChanged]) acc += ck_pack_changed(s, b, in, first + j, j);  // (warp-uniform)
   ck_reduce(acc, s_zones, sum, zones);
 }
 
@@ -167,8 +172,8 @@ __global__ void __launch_bounds__(256) checkpoint_verify_kernel(const CkptBlob b
           if (k == 6) mark_zone(s_zones, v);
           break;
         }
-        case 1: acc += ckpt_mix((b.off[k] + j) * 8, ck_blob_get<uint8_t>(b, k, j)); break;
-        default: acc += ckpt_mix(b.off[k] * 8 + j, (ck_blob_get<uint32_t>(b, k, j >> 5) >> (j & 31)) & 1u);
+        case 1: acc += ck_term(b, k, j, ck_blob_get<uint8_t>(b, k, j)); break;
+        default: acc += ckpt_mix(b.off[k] * 8 + j, ck_blob_bit(b, k, j));
       }
     }
   }
@@ -180,41 +185,46 @@ struct ZoneLut {
   uint8_t id[256];
 };
 
-// am_sweep_restore: element j to slot first + j, every section the handle has; zone ids rewritten through `lut`.  A
-// handle with the timeout state restoring a blob without it gets no timeout and no deadline for the slots.
-__global__ void __launch_bounds__(256) checkpoint_scatter_kernel(const CkptState s, const CkptBlob b, uint64_t first,
-                                                                const ZoneLut lut) {
-  const uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (j >= b.n) return;
-  const uint64_t i = first + j;
+// The section rules of a restore, per slot: element k of the blob to slot i, every section the handle has; zone ids
+// rewritten through `lut`.  A handle with the timeout state restoring a blob without it gets no timeout and no
+// deadline for the slot.
+__device__ __forceinline__ void ck_scatter_slot(const CkptState& s, const CkptBlob& b, uint64_t i, uint64_t k,
+                                                const ZoneLut& lut) {
 #pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    if (ck_elem(k) == 8) {
-      reinterpret_cast<uint64_t*>(s.col[k])[i] = ck_blob_get<uint64_t>(b, k, j);
+  for (int q = 0; q < 16; ++q) {
+    if (ck_elem(q) == 8) {
+      reinterpret_cast<uint64_t*>(s.col[q])[i] = ck_blob_get<uint64_t>(b, q, k);
     } else {
-      uint32_t v = ck_blob_get<uint32_t>(b, k, j);
-      if (k == 6 && zone_bound(v)) v = (v & ~AM_F_TZ_MASK) | ((uint32_t)lut.id[v >> AM_F_TZ_SHIFT] << AM_F_TZ_SHIFT);
-      reinterpret_cast<uint32_t*>(s.col[k])[i] = v;
+      uint32_t v = ck_blob_get<uint32_t>(b, q, k);
+      if (q == 6 && zone_bound(v)) v = (v & ~AM_F_TZ_MASK) | ((uint32_t)lut.id[v >> AM_F_TZ_SHIFT] << AM_F_TZ_SHIFT);
+      reinterpret_cast<uint32_t*>(s.col[q])[i] = v;
     }
   }
   if (s.wf_timeout) {
     const bool has = b.off[kCkSecWfTimeout] != 0;
-    const int64_t d = has ? ck_blob_get<int64_t>(b, kCkSecDeadline, j) : kNoDeadline;
-    s.wf_timeout[i] = has ? ck_blob_get<int32_t>(b, kCkSecWfTimeout, j) : 0;
+    const int64_t d = has ? ck_blob_get<int64_t>(b, kCkSecDeadline, k) : kNoDeadline;
+    s.wf_timeout[i] = has ? ck_blob_get<int32_t>(b, kCkSecWfTimeout, k) : 0;
     s.deadline[i] = d;
     if (d != kNoDeadline) atomicMin(&s.seg_deadline[i / kRecPerWarp], biased_key(d));
   }
-  if (s.since) s.since[i] = ck_blob_get<int64_t>(b, kCkSecSince, j);
+  if (s.since) s.since[i] = ck_blob_get<int64_t>(b, kCkSecSince, k);
   if (s.changed) {
     const uint32_t m = 1u << (i & 31);
-    if ((ck_blob_get<uint32_t>(b, kCkSecChanged, j >> 5) >> (j & 31)) & 1u) atomicOr(&s.changed[i >> 5], m);
+    if (ck_blob_bit(b, kCkSecChanged, k)) atomicOr(&s.changed[i >> 5], m);
     else atomicAnd(&s.changed[i >> 5], ~m);
   }
   if (s.det_applied) {
-    s.det_applied[i] = ck_blob_get<uint8_t>(b, kCkSecDetApplied, j);
-    s.det_start[i] = ck_blob_get<int64_t>(b, kCkSecDetStart, j);
+    s.det_applied[i] = ck_blob_get<uint8_t>(b, kCkSecDetApplied, k);
+    s.det_start[i] = ck_blob_get<int64_t>(b, kCkSecDetStart, k);
   }
-  if (s.wait) s.wait[i] = ck_blob_get<int64_t>(b, kCkSecWait, j);
+  if (s.wait) s.wait[i] = ck_blob_get<int64_t>(b, kCkSecWait, k);
+}
+
+// am_sweep_restore: element j to slot first + j.
+__global__ void __launch_bounds__(256) checkpoint_scatter_kernel(const CkptState s, const CkptBlob b, uint64_t first,
+                                                                const ZoneLut lut) {
+  const uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (j < b.n) ck_scatter_slot(s, b, first + j, j, lut);
 }
 
 // ---- delta checkpoints (am_sweep_checkpoint_delta / am_sweep_restore_delta, DESIGN.md "Delta format") ----------------
@@ -260,8 +270,7 @@ __global__ void __launch_bounds__(256) delta_diff_kernel(const CkptState s, cons
       d |= s.wf_timeout[i] != ck_blob_get<int32_t>(b, kCkSecWfTimeout, j) ||
            s.deadline[i] != ck_blob_get<int64_t>(b, kCkSecDeadline, j);
     if (b.off[kCkSecSince]) d |= s.since[i] != ck_blob_get<int64_t>(b, kCkSecSince, j);
-    if (b.off[kCkSecChanged])
-      d |= ((s.changed[i >> 5] >> (i & 31)) & 1u) != ((ck_blob_get<uint32_t>(b, kCkSecChanged, j >> 5) >> (j & 31)) & 1u);
+    if (b.off[kCkSecChanged]) d |= ((s.changed[i >> 5] >> (i & 31)) & 1u) != ck_blob_bit(b, kCkSecChanged, j);
     if (b.off[kCkSecDetApplied])
       d |= s.det_applied[i] != ck_blob_get<uint8_t>(b, kCkSecDetApplied, j) ||
            s.det_start[i] != ck_blob_get<int64_t>(b, kCkSecDetStart, j);
@@ -298,53 +307,9 @@ __global__ void __launch_bounds__(256) delta_pack_kernel(const CkptState s, char
   const bool in = k < m;
   const uint64_t j = in ? offs[k] : 0;
   const uint64_t i = first + j;
-  uint64_t acc = 0;
-  if (in) {
-    acc += ckpt_mix((kCkHeaderBytes + k * 4) * 8, j);
-#pragma unroll
-    for (int q = 0; q < 16; ++q) {
-      if (ck_elem(q) == 8) {
-        const uint64_t v = reinterpret_cast<const uint64_t*>(s.col[q])[i];
-        reinterpret_cast<uint64_t*>(b.p + b.off[q])[k] = v;
-        acc += ck_term(b, q, k, v);
-      } else {
-        const uint32_t v = reinterpret_cast<const uint32_t*>(s.col[q])[i];
-        reinterpret_cast<uint32_t*>(b.p + b.off[q])[k] = v;
-        acc += ck_term(b, q, k, v);
-        if (q == 6) mark_zone(s_zones, v);
-      }
-    }
-    if (b.off[kCkSecWfTimeout]) {
-      const int32_t w = s.wf_timeout[i];
-      const int64_t d = s.deadline[i];
-      reinterpret_cast<int32_t*>(b.p + b.off[kCkSecWfTimeout])[k] = w;
-      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecDeadline])[k] = d;
-      acc += ck_term(b, kCkSecWfTimeout, k, w) + ck_term(b, kCkSecDeadline, k, d);
-    }
-    if (b.off[kCkSecSince]) {
-      const int64_t v = s.since[i];
-      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecSince])[k] = v;
-      acc += ck_term(b, kCkSecSince, k, v);
-    }
-    if (b.off[kCkSecDetApplied]) {
-      const uint8_t a = s.det_applied[i];
-      const int64_t t = s.det_start[i];
-      reinterpret_cast<uint8_t*>(b.p + b.off[kCkSecDetApplied])[k] = a;
-      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecDetStart])[k] = t;
-      acc += ckpt_mix((b.off[kCkSecDetApplied] + k) * 8, a) + ck_term(b, kCkSecDetStart, k, t);
-    }
-    if (b.off[kCkSecWait]) {
-      const int64_t v = s.wait[i];
-      reinterpret_cast<int64_t*>(b.p + b.off[kCkSecWait])[k] = v;
-      acc += ck_term(b, kCkSecWait, k, v);
-    }
-  }
-  if (b.off[kCkSecChanged]) {  // (block-uniform)
-    const uint32_t bit = in ? (s.changed[i >> 5] >> (i & 31)) & 1u : 0u;
-    const uint32_t word = __ballot_sync(kFull, bit);
-    if ((threadIdx.x & 31) == 0 && in) reinterpret_cast<uint32_t*>(b.p + b.off[kCkSecChanged])[k >> 5] = word;
-    if (in) acc += ckpt_mix(b.off[kCkSecChanged] * 8 + k, bit);
-  }
+  uint64_t acc = in ? ckpt_mix((kCkHeaderBytes + k * 4) * 8, j) : 0;
+  if (in) acc += ck_pack_slot(s, b, i, k, s_zones);
+  if (b.off[kCkSecChanged]) acc += ck_pack_changed(s, b, in, i, k);  // (block-uniform)
   ck_reduce(acc, s_zones, sum, zones);
 }
 
@@ -364,7 +329,7 @@ __global__ void __launch_bounds__(256) delta_commit_kernel(const CkptBlob b, con
       default: {
         uint32_t* w = reinterpret_cast<uint32_t*>(b.p + b.off[q]) + (j >> 5);
         const uint32_t bit = 1u << (j & 31);
-        if ((ck_blob_get<uint32_t>(d, q, k >> 5) >> (k & 31)) & 1u) atomicOr(w, bit);
+        if (ck_blob_bit(d, q, k)) atomicOr(w, bit);
         else atomicAnd(w, ~bit);
       }
     }
@@ -389,9 +354,8 @@ __global__ void __launch_bounds__(256) delta_offsets_verify_kernel(const uint32_
   ck_reduce(acc, s_zones, sum, nullptr);  // (no zone marks: ck_reduce touches `zones` only for marked ids)
 }
 
-// am_sweep_restore_delta: element k of the delta to slot first + offs[k], by the rules of checkpoint_scatter_kernel,
-// and the slot's segment marked for delta_planes_kernel; the slot's due word as well while the handle keeps them (`due`
-// NULL otherwise).
+// am_sweep_restore_delta: element k of the delta to slot first + offs[k], and the slot's segment marked for
+// delta_planes_kernel; the slot's due word as well while the handle keeps them (`due` NULL otherwise).
 __global__ void __launch_bounds__(256) delta_scatter_kernel(const CkptState s, const CkptBlob b,
                                                            const uint32_t* __restrict__ offs, uint64_t first,
                                                            const ZoneLut lut, uint32_t* seg_dirty, uint32_t* due,
@@ -399,34 +363,7 @@ __global__ void __launch_bounds__(256) delta_scatter_kernel(const CkptState s, c
   const uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (k >= b.n) return;
   const uint64_t i = first + offs[k];
-#pragma unroll
-  for (int q = 0; q < 16; ++q) {
-    if (ck_elem(q) == 8) {
-      reinterpret_cast<uint64_t*>(s.col[q])[i] = ck_blob_get<uint64_t>(b, q, k);
-    } else {
-      uint32_t v = ck_blob_get<uint32_t>(b, q, k);
-      if (q == 6 && zone_bound(v)) v = (v & ~AM_F_TZ_MASK) | ((uint32_t)lut.id[v >> AM_F_TZ_SHIFT] << AM_F_TZ_SHIFT);
-      reinterpret_cast<uint32_t*>(s.col[q])[i] = v;
-    }
-  }
-  if (s.wf_timeout) {
-    const bool has = b.off[kCkSecWfTimeout] != 0;
-    const int64_t d = has ? ck_blob_get<int64_t>(b, kCkSecDeadline, k) : kNoDeadline;
-    s.wf_timeout[i] = has ? ck_blob_get<int32_t>(b, kCkSecWfTimeout, k) : 0;
-    s.deadline[i] = d;
-    if (d != kNoDeadline) atomicMin(&s.seg_deadline[i / kRecPerWarp], biased_key(d));
-  }
-  if (s.since) s.since[i] = ck_blob_get<int64_t>(b, kCkSecSince, k);
-  if (s.changed) {
-    const uint32_t m = 1u << (i & 31);
-    if ((ck_blob_get<uint32_t>(b, kCkSecChanged, k >> 5) >> (k & 31)) & 1u) atomicOr(&s.changed[i >> 5], m);
-    else atomicAnd(&s.changed[i >> 5], ~m);
-  }
-  if (s.det_applied) {
-    s.det_applied[i] = ck_blob_get<uint8_t>(b, kCkSecDetApplied, k);
-    s.det_start[i] = ck_blob_get<int64_t>(b, kCkSecDetStart, k);
-  }
-  if (s.wait) s.wait[i] = ck_blob_get<int64_t>(b, kCkSecWait, k);
+  ck_scatter_slot(s, b, i, k, lut);
   if (due) due[i] = due_word(ck_blob_get<int32_t>(b, 5, k), ck_blob_get<int64_t>(b, 7, k), due_epoch);
   seg_dirty[i / kRecPerWarp] = 1u;
 }

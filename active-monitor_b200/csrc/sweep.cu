@@ -2441,20 +2441,10 @@ constexpr uint32_t kCkAllSwitches =
     AM_CKPT_HOLD | AM_CKPT_REMEDY | AM_CKPT_TRACK | AM_CKPT_DETAILS | AM_CKPT_TIMEOUTS | AM_CKPT_ADMISSION;
 constexpr size_t kCkChunk = 32u << 20;  // bytes per pinned chunk of a restore's upload
 
-struct CkptHeader {
-  uint64_t magic;
-  uint32_t version, switches;
-  uint64_t bytes, checksum, first_global, n, swept_end;
-  int64_t prev_tick;
-  uint64_t seed;
-  uint32_t n_zones, reserved32;
-  uint64_t reserved[6];
-};
-static_assert(sizeof(CkptHeader) == kCkHeader && kCkHeader == kCkHeaderBytes, "checkpoint header: 16 words");
-
-// A delta: the full header's words, the link's in its reserved words.
 constexpr uint64_t kCkdMagic = 0x4C444B4357534D41ull;  // "AMSWCKDL"
-struct CkptDeltaHeader {
+
+// The header of a full blob and of a delta.  Words 10..13 are a delta's link; a full blob leaves them zero.
+struct CkptHeader {
   uint64_t magic;
   uint32_t version, switches;
   uint64_t bytes, checksum, first_global, n, swept_end;
@@ -2466,26 +2456,18 @@ struct CkptDeltaHeader {
   uint64_t parent_checksum;
   uint64_t reserved[2];
 };
-static_assert(sizeof(CkptDeltaHeader) == kCkHeader &&
-                  offsetof(CkptDeltaHeader, checksum) == offsetof(CkptHeader, checksum) &&
-                  offsetof(CkptDeltaHeader, n_zones) == offsetof(CkptHeader, n_zones),
-              "delta header: the full header's words first");
+static_assert(sizeof(CkptHeader) == kCkHeader && kCkHeader == kCkHeaderBytes, "checkpoint header: 16 words");
 
 struct CkptLayout {
   uint64_t off[kCkSections] = {};
   uint64_t sections_end = kCkHeader;
 };
 
-// The sections a blob of n slots with `switches` has, in order, each at an 8-B aligned offset.
-CkptLayout ckpt_layout(uint64_t n, uint32_t switches) {
+// The sections a blob of n slots with `switches` has, in order, each at an 8-B aligned offset from `start` on (a
+// delta of n slots: ckd_start(n), after the offset section).
+CkptLayout ckpt_layout(uint64_t n, uint32_t switches, uint64_t start = kCkHeader) {
   CkptLayout L;
-  L.sections_end = ck_layout(n, switches, kCkHeader, L.off);
-  return L;
-}
-// ... and of a delta of m slots (its sections after the offset section)
-CkptLayout ckd_layout(uint64_t m, uint32_t switches) {
-  CkptLayout L;
-  L.sections_end = ck_layout(m, switches, ckd_start(m), L.off);
+  L.sections_end = ck_layout(n, switches, start, L.off);
   return L;
 }
 
@@ -2519,51 +2501,38 @@ struct CkptZone {
   std::string name;
 };
 
-// The header words a full blob and a delta share, and the zone table from the end of the sections to `bytes`, checked
-// for consistency (not the checksum: that is a device pass).
-template <class Header>
-int ckpt_parse_common(const char* p, uint64_t len, const Header& hd, uint64_t sections_end,
-                      std::vector<CkptZone>* zones) {
-  if (hd.version != AM_CHECKPOINT_VERSION) return AM_E_INVAL;
-  if ((hd.switches & ~kCkAllSwitches) || ((hd.switches & AM_CKPT_REMEDY) && !(hd.switches & AM_CKPT_HOLD)) ||
-      ((hd.switches & AM_CKPT_DETAILS) && !(hd.switches & AM_CKPT_TRACK)) ||
-      ((hd.switches & AM_CKPT_ADMISSION) && !(hd.switches & AM_CKPT_HOLD)))
+// A full blob's or, with `delta`, a delta's header, layout and zone table (from the end of the sections to `bytes`),
+// checked for consistency (not the checksum: that is a device pass).
+int ckpt_parse(const void* buf, uint64_t len, bool delta, CkptHeader* hd, CkptLayout* L,
+               std::vector<CkptZone>* zones) {
+  if (!buf || len < kCkHeader) return AM_E_INVAL;
+  memcpy(hd, buf, kCkHeader);
+  if (hd->magic != (delta ? kCkdMagic : kCkMagic) || hd->version != AM_CHECKPOINT_VERSION) return AM_E_INVAL;
+  if (delta && (hd->n_changed > hd->n || hd->seq == 0)) return AM_E_INVAL;
+  if ((hd->switches & ~kCkAllSwitches) || ((hd->switches & AM_CKPT_REMEDY) && !(hd->switches & AM_CKPT_HOLD)) ||
+      ((hd->switches & AM_CKPT_DETAILS) && !(hd->switches & AM_CKPT_TRACK)) ||
+      ((hd->switches & AM_CKPT_ADMISSION) && !(hd->switches & AM_CKPT_HOLD)))
     return AM_E_INVAL;
-  if (hd.bytes > len || hd.bytes % 8 || hd.n > 0xFFFFFFFFull || hd.first_global + hd.n < hd.first_global ||
-      hd.swept_end < hd.first_global || hd.swept_end > hd.first_global + hd.n || hd.n_zones > 255)
+  if (hd->bytes > len || hd->bytes % 8 || hd->n > 0xFFFFFFFFull || hd->first_global + hd->n < hd->first_global ||
+      hd->swept_end < hd->first_global || hd->swept_end > hd->first_global + hd->n || hd->n_zones > 255)
     return AM_E_INVAL;
-  uint64_t at = sections_end;
+  *L = delta ? ckpt_layout(hd->n_changed, hd->switches, ckd_start(hd->n_changed)) : ckpt_layout(hd->n, hd->switches);
+  const char* p = (const char*)buf;
+  uint64_t at = L->sections_end;  // (past `bytes` when a delta's n_changed is out of range: refused below)
   bool seen[256] = {};
   zones->clear();
-  for (uint32_t k = 0; k < hd.n_zones; ++k) {
-    if (at + 8 > hd.bytes) return AM_E_INVAL;
+  for (uint32_t k = 0; k < hd->n_zones; ++k) {
+    if (at + 8 > hd->bytes) return AM_E_INVAL;
     uint32_t id, nl;
     memcpy(&id, p + at, 4);
     memcpy(&nl, p + at + 4, 4);
-    if (id < 1 || id > 255 || seen[id] || nl < 1 || nl > 255 || at + ckpt_zone_entry_bytes(nl) > hd.bytes)
+    if (id < 1 || id > 255 || seen[id] || nl < 1 || nl > 255 || at + ckpt_zone_entry_bytes(nl) > hd->bytes)
       return AM_E_INVAL;
     seen[id] = true;
     zones->push_back({id, std::string(p + at + 8, nl)});
     at += ckpt_zone_entry_bytes(nl);
   }
-  return at == hd.bytes ? AM_OK : AM_E_INVAL;
-}
-
-// A blob's header, layout and zone table.
-int ckpt_parse(const void* buf, uint64_t len, CkptHeader* hd, CkptLayout* L, std::vector<CkptZone>* zones) {
-  if (!buf || len < kCkHeader) return AM_E_INVAL;
-  memcpy(hd, buf, kCkHeader);
-  if (hd->magic != kCkMagic) return AM_E_INVAL;
-  *L = ckpt_layout(hd->n, hd->switches);
-  return ckpt_parse_common((const char*)buf, len, *hd, L->sections_end, zones);
-}
-// ... a delta's (its sections end past `bytes` when n_changed is out of range: refused there)
-int ckd_parse(const void* buf, uint64_t len, CkptDeltaHeader* hd, CkptLayout* L, std::vector<CkptZone>* zones) {
-  if (!buf || len < kCkHeader) return AM_E_INVAL;
-  memcpy(hd, buf, kCkHeader);
-  if (hd->magic != kCkdMagic || hd->n_changed > hd->n || hd->n > 0xFFFFFFFFull || hd->seq == 0) return AM_E_INVAL;
-  *L = ckd_layout(hd->n_changed, hd->switches);
-  return ckpt_parse_common((const char*)buf, len, *hd, L->sections_end, zones);
+  return at == hd->bytes ? AM_OK : AM_E_INVAL;
 }
 
 // The zones a pass marked (8 words of marks, one bit per id) with their names.  AM_E_DEVICE: an id that is not
@@ -2650,9 +2619,11 @@ CkptState ckpt_state(am_sweep* h) {
   return s;
 }
 
+// A blob of n elements per section (layout L) in the staging area: its sections from byte 128 of ck_dev on (a delta's
+// offsets are in ckd_off).
 CkptBlob ckpt_blob(const am_sweep* h, const CkptLayout& L, uint64_t n) {
   CkptBlob b{};
-  b.p = h->ck_dev;
+  b.p = h->ck_dev + kCkHeader - L.off[0];
   memcpy(b.off, L.off, sizeof b.off);
   b.n = n;
   return b;
@@ -2661,12 +2632,6 @@ CkptBlob ckpt_blob(const am_sweep* h, const CkptLayout& L, uint64_t n) {
 CkptBlob ckd_base_blob(const am_sweep* h, uint64_t n, uint32_t switches) {
   CkptBlob b = ckpt_blob(h, ckpt_layout(n, switches), n);
   b.p = h->ckd_base;
-  return b;
-}
-// A delta of m slots in the staging area: its offsets in ckd_off, its sections from byte 128 of ck_dev on.
-CkptBlob ckd_blob(const am_sweep* h, const CkptLayout& L, uint64_t m) {
-  CkptBlob b = ckpt_blob(h, L, m);
-  b.p = h->ck_dev + kCkHeader - ckd_start(m);
   return b;
 }
 
@@ -2715,40 +2680,169 @@ int ckpt_restore_switches(am_sweep* h, uint32_t switches, const char* who) {
   return AM_OK;
 }
 
-// The end of a restore after its scatter (tick guard held): the high-water mark, the admission order, P and the seed;
-// the previous tick's lists are not carried: empty until the next tick.
-int ckpt_restore_finish(am_sweep* h, uint64_t swept_end, int64_t prev_tick, uint64_t seed) {
-  AM_CUDA(h, cudaStreamSynchronize(h->stream));
-  const uint64_t hwm = swept_end - h->shard_base;
-  if (hwm > h->n_records) set_hwm(h, hwm);
-  if (admission_on(h)) {  // the admission order of every waiting slot of the handle, from the waits as they now stand
-    const int rc = rebuild_admission_fifo(h);
+// A blob a restore has checked and staged: its header, its layout, its zone ids here, and its first slot in the handle.
+struct CkptRestore {
+  bool delta;
+  CkptHeader hd;
+  CkptLayout L;
+  ZoneLut lut;
+  uint64_t first;
+  uint64_t m;  // elements per section: n, or a delta's n_changed
+};
+
+// A restore's steps before anything of the handle changes (ck_mu held): the blob `buf` (a delta with `delta`) parsed,
+// its range checked against the shard and its zone table resolved; its sections (and a delta's offsets) up in chunks,
+// then the device passes that verify the checksum (and that the offsets ascend inside the range) and the zone ids its
+// records use.
+int ckpt_restore_check(am_sweep* h, const void* buf, uint64_t len, bool delta, CkptRestore* r) {
+  const char* who = delta ? "am_sweep_restore_delta" : "am_sweep_restore";
+  const std::string what = delta ? "delta" : "blob";
+  const CkptHeader& hd = r->hd;
+  std::vector<CkptZone> zones;
+  r->delta = delta;
+  int rc = ckpt_parse(buf, len, delta, &r->hd, &r->L, &zones);
+  if (rc != AM_OK) {
+    h->last_error = std::string(who) + ": not a " + (delta ? "delta" : "checkpoint") +
+                    " of this format version, or truncated";
+    return rc;
+  }
+  if (hd.first_global < h->shard_base || hd.first_global - h->shard_base + hd.n > h->capacity) {
+    h->last_error = std::string(who) + ": the " + what + "'s slots are not all inside this shard";
+    return AM_E_RANGE;
+  }
+  r->first = hd.first_global - h->shard_base;
+  r->m = delta ? hd.n_changed : hd.n;
+  rc = ckpt_zone_lut(h, zones, who, &r->lut);
+  if (rc != AM_OK) return rc;
+  rc = ckpt_alloc(h);
+  if (rc == AM_OK && delta) rc = ckd_alloc(h, false);
+  if (rc != AM_OK) return rc;
+  const char* p = (const char*)buf;
+  const uint64_t m = r->m, start = r->L.off[0];
+  if (delta) rc = ckpt_upload(h, (char*)h->ckd_off, p + kCkHeader, m * 4);
+  if (rc == AM_OK) rc = ckpt_upload(h, h->ck_dev + kCkHeader, p + start, r->L.sections_end - start);
+  if (rc != AM_OK) return rc;
+  AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->ck_stream));
+  if (delta) AM_CUDA(h, cudaMemsetAsync(h->ckd_acc, 0, 4 * 8, h->ck_stream));
+  if (m) {
+    const unsigned grid = (unsigned)((m + 255) / 256);
+    if (delta)
+      AM_CUDA(h, launch(h, delta_offsets_verify_kernel, grid, 256, h->ck_stream, (const uint32_t*)h->ckd_off, m, hd.n,
+                        h->ck_meta, (uint32_t*)(h->ckd_acc + 2)));
+    AM_CUDA(h, launch(h, checkpoint_verify_kernel, grid, 256, h->ck_stream, ckpt_blob(h, r->L, m), h->ck_meta,
+                      (uint32_t*)(h->ck_meta + 1)));
+  }
+  AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
+  if (delta) AM_CUDA(h, cudaMemcpyAsync(h->ckd_acc_h, h->ckd_acc, 4 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  h->ck_pin_pending[0] = h->ck_pin_pending[1] = false;
+  const uint64_t sum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, r->L.sections_end, hd.bytes);
+  if (sum != hd.checksum) {
+    h->last_error = std::string(who) + ": checksum mismatch";
+    return AM_E_INVAL;
+  }
+  if (delta && h->ckd_acc_h[2]) {
+    h->last_error = std::string(who) + ": the slot offsets are not strictly ascending inside the range";
+    return AM_E_INVAL;
+  }
+  const uint32_t* marks = (const uint32_t*)(h->ck_meta_h + 1);
+  for (uint32_t id = 1; id < 256; ++id)
+    if (((marks[id >> 5] >> (id & 31)) & 1u) && !r->lut.id[id]) {
+      h->last_error = std::string(who) + ": a record names a zone the " + what + "'s table does not";
+      return AM_E_INVAL;
+    }
+  return AM_OK;
+}
+
+// The rest of a restore once its entry point's own preconditions hold (tick guard held).  A restore is a call in the
+// per-slot order: the calls staged before it are applied first, and it replaces them.  Then the timeout state the
+// blob carries, the scatter and the planes of its slots (a full restore's rebuild_planes drops the due words, a
+// delta's scatter keeps them exact), the high-water mark, the admission order, P and the seed; the previous tick's
+// lists are not carried: empty until the next tick.
+int ckpt_restore_apply(am_sweep* h, const CkptRestore& r) {
+  const CkptHeader& hd = r.hd;
+  int rc = begin_call(h);
+  if (rc != AM_OK) return rc;
+  if ((hd.switches & AM_CKPT_TIMEOUTS) && !h->wf_timeout) {
+    rc = alloc_timeouts(h, h->stream);
     if (rc != AM_OK) return rc;
   }
-  if (prev_tick != INT64_MIN) {
-    h->has_prev = true;
-    h->prev_T = prev_tick;
+  if (r.m && r.delta) {
+    AM_CUDA(h, launch(h, delta_scatter_kernel, (unsigned)((r.m + 255) / 256), 256, h->stream, ckpt_state(h),
+                      ckpt_blob(h, r.L, r.m), (const uint32_t*)h->ckd_off, r.first, r.lut, h->seg_dirty, due_kept(h),
+                      h->due_epoch));
+    AM_CUDA(h, launch(h, delta_planes_kernel, (unsigned)((r.m + kWarps - 1) / kWarps), kBlock, h->stream, h->cols,
+                      h->planes, h->seg_dirty, (const uint32_t*)h->ckd_off, r.first, (uint32_t)r.m));
+  } else if (r.m) {
+    AM_CUDA(h, launch(h, checkpoint_scatter_kernel, (unsigned)((r.m + 255) / 256), 256, h->stream, ckpt_state(h),
+                      ckpt_blob(h, r.L, r.m), r.first, r.lut));
+    rc = rebuild_planes(h, r.first, r.m);
+    if (rc != AM_OK) return rc;
   }
-  h->seed = seed;
+  AM_CUDA(h, cudaStreamSynchronize(h->stream));
+  const uint64_t hwm = hd.swept_end - h->shard_base;
+  if (hwm > h->n_records) set_hwm(h, hwm);
+  if (admission_on(h)) {  // the admission order of every waiting slot of the handle, from the waits as they now stand
+    rc = rebuild_admission_fifo(h);
+    if (rc != AM_OK) return rc;
+  }
+  if (hd.prev_tick != INT64_MIN) {
+    h->has_prev = true;
+    h->prev_T = hd.prev_tick;
+  }
+  h->seed = hd.seed;
   h->host_n = 0;
   h->to_ran = h->to_fetched = false;
   h->chg_listed = h->chg_fetched = false;
   return AM_OK;
 }
 
-// A full checkpoint (am_sweep_checkpoint, ck_mu held); *hd_out and *L_out = its header and layout.
-int checkpoint_locked(am_sweep* h, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out,
-                      CkptHeader* hd_out, CkptLayout* L_out) {
+// The header words every blob of the slots [first, first + n) carries: the handle's switches, P and seed (tick guard
+// held).  The producer fills in the rest at its seal.
+CkptHeader ckpt_header(const am_sweep* h, uint64_t magic, uint64_t first, uint64_t n) {
   CkptHeader hd{};
-  CkptLayout L;
+  hd.magic = magic;
+  hd.version = AM_CHECKPOINT_VERSION;
+  hd.switches = ckpt_switches(h);
+  hd.first_global = h->shard_base + first;
+  hd.n = n;
+  hd.swept_end = h->shard_base + std::min(std::max(h->n_records, first), first + n);
+  hd.prev_tick = h->has_prev ? h->prev_T : INT64_MIN;
+  hd.seed = h->seed;
+  return hd;
+}
+
+// The end of a producer, after its pass (ck_ev) and once the caller's buffer `p` has room for the blob: the zone table
+// of the pass's marks (`zones`), the header, the sections of the staging area (n elements each, layout L), their
+// padding and the checksum word; *len_out = the blob's length.
+int ckpt_seal(am_sweep* h, char* p, CkptHeader* hd, const CkptLayout& L, uint64_t n,
+              const std::vector<CkptZone>& zones, uint64_t* len_out) {
+  hd->n_zones = (uint32_t)zones.size();
+  hd->bytes = ckpt_put_zones(p, L.sections_end, zones);
+  memcpy(p, hd, kCkHeader);
+  AM_CUDA(h, cudaStreamWaitEvent(h->ck_stream, h->ck_ev, 0));
+  if (L.sections_end > L.off[0])  // (the sections start at L.off[0]: the header's end, or a delta's offsets' end)
+    AM_CUDA(h, cudaMemcpyAsync(p + L.off[0], h->ck_dev + kCkHeader, L.sections_end - L.off[0], cudaMemcpyDeviceToHost,
+                               h->ck_stream));
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  ckpt_zero_padding(p, L, n);
+  hd->checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, hd->bytes);
+  memcpy(p + offsetof(CkptHeader, checksum), &hd->checksum, 8);
+  *len_out = hd->bytes;
+  return AM_OK;
+}
+
+// A full checkpoint (am_sweep_checkpoint, ck_mu held); *hd and *L = its header and layout.
+int checkpoint_locked(am_sweep* h, uint64_t first, uint64_t n, void* buf, uint64_t cap, uint64_t* len_out,
+                      CkptHeader* hd, CkptLayout* L) {
   {  // the pass, with the tick guard held: the drain, then one kernel over the range on the handle's stream
     TickGuard g(h);
     if (!g.ok) return AM_E_BUSY;
     int rc = begin_call(h);  // (first: the drain may allocate the timeout state, a section of the blob)
     if (rc != AM_OK) return rc;
-    hd.switches = ckpt_switches(h);
-    L = ckpt_layout(n, hd.switches);
-    uint64_t bound = L.sections_end;  // (room for the names of every registered zone)
+    *hd = ckpt_header(h, kCkMagic, first, n);
+    *L = ckpt_layout(n, hd->switches);
+    uint64_t bound = L->sections_end;  // (room for the names of every registered zone)
     std::string name;
     for (int32_t id = 1; amsweep_tz::name_of(id, &name); ++id) bound += ckpt_zone_entry_bytes(name.size());
     if (cap < bound) {
@@ -2757,42 +2851,19 @@ int checkpoint_locked(am_sweep* h, uint64_t first, uint64_t n, void* buf, uint64
     }
     rc = ckpt_alloc(h);
     if (rc != AM_OK) return rc;
-    hd.magic = kCkMagic;
-    hd.version = AM_CHECKPOINT_VERSION;
-    hd.first_global = h->shard_base + first;
-    hd.n = n;
-    hd.swept_end = h->shard_base + std::min(std::max(h->n_records, first), first + n);
-    hd.prev_tick = h->has_prev ? h->prev_T : INT64_MIN;
-    hd.seed = h->seed;
     AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->stream));
     if (n)
       AM_CUDA(h, launch(h, checkpoint_pack_kernel, (unsigned)((n + 255) / 256), 256, h->stream, ckpt_state(h),
-                        ckpt_blob(h, L, n), first, h->ck_meta, (uint32_t*)(h->ck_meta + 1)));
+                        ckpt_blob(h, *L, n), first, h->ck_meta, (uint32_t*)(h->ck_meta + 1)));
     AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->stream));
     AM_CUDA(h, cudaEventRecord(h->ck_ev, h->stream));
   }
   // Ticks may run from here on: the copy to the caller waits for the pass only, on the checkpoint stream.
   AM_CUDA(h, cudaEventSynchronize(h->ck_ev));
-  char* p = (char*)buf;
   std::vector<CkptZone> zones;
   const int rc = ckpt_marked_zones(h, (const uint32_t*)(h->ck_meta_h + 1), "am_sweep_checkpoint", &zones);
   if (rc != AM_OK) return rc;
-  const uint64_t at = ckpt_put_zones(p, L.sections_end, zones);
-  hd.n_zones = (uint32_t)zones.size();
-  hd.bytes = at;
-  memcpy(p, &hd, kCkHeader);
-  AM_CUDA(h, cudaStreamWaitEvent(h->ck_stream, h->ck_ev, 0));
-  if (L.sections_end > kCkHeader)
-    AM_CUDA(h, cudaMemcpyAsync(p + kCkHeader, h->ck_dev + kCkHeader, L.sections_end - kCkHeader, cudaMemcpyDeviceToHost,
-                               h->ck_stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
-  ckpt_zero_padding(p, L, n);
-  hd.checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, at);
-  memcpy(p + offsetof(CkptHeader, checksum), &hd.checksum, 8);
-  *len_out = at;
-  *hd_out = hd;
-  *L_out = L;
-  return AM_OK;
+  return ckpt_seal(h, (char*)buf, hd, *L, n, zones, len_out);
 }
 
 // A restored full blob starts the handle's link entry for its range, replacing every entry that overlaps it.
@@ -2825,7 +2896,7 @@ int am_checkpoint_info(const void* buf, uint64_t len, am_checkpoint_info_t* info
   CkptHeader hd;
   CkptLayout L;
   std::vector<CkptZone> zones;
-  const int rc = ckpt_parse(buf, len, &hd, &L, &zones);
+  const int rc = ckpt_parse(buf, len, false, &hd, &L, &zones);
   if (rc != AM_OK) return rc;
   *info = am_checkpoint_info_t{};
   info->first_global = hd.first_global;
@@ -2842,71 +2913,21 @@ int am_checkpoint_info(const void* buf, uint64_t len, am_checkpoint_info_t* info
 
 int am_sweep_restore(am_sweep_t* h, const void* buf, uint64_t len) {
   if (!h || !buf) return AM_E_INVAL;
-  CkptHeader hd;
-  CkptLayout L;
-  std::vector<CkptZone> zones;
-  int rc = ckpt_parse(buf, len, &hd, &L, &zones);
-  if (rc != AM_OK) {
-    h->last_error = "am_sweep_restore: not a checkpoint of this format version, or truncated";
-    return rc;
-  }
-  if (hd.first_global < h->shard_base || hd.first_global - h->shard_base + hd.n > h->capacity) {
-    h->last_error = "am_sweep_restore: the blob's slots are not all inside this shard";
-    return AM_E_RANGE;
-  }
-  const uint64_t first = hd.first_global - h->shard_base;
-  ZoneLut lut;
-  rc = ckpt_zone_lut(h, zones, "am_sweep_restore", &lut);
-  if (rc != AM_OK) return rc;
   std::lock_guard<std::mutex> ck(h->ck_mu);
-  rc = ckpt_alloc(h);
+  CkptRestore r;
+  int rc = ckpt_restore_check(h, buf, len, false, &r);
   if (rc != AM_OK) return rc;
-  // Up in chunks, then the device pass that verifies the checksum: all before anything of the handle changes.
-  const char* p = (const char*)buf;
-  rc = ckpt_upload(h, h->ck_dev + kCkHeader, p + kCkHeader, L.sections_end - kCkHeader);
-  if (rc != AM_OK) return rc;
-  AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->ck_stream));
-  if (hd.n)
-    AM_CUDA(h, launch(h, checkpoint_verify_kernel, (unsigned)((hd.n + 255) / 256), 256, h->ck_stream,
-                      ckpt_blob(h, L, hd.n), h->ck_meta, (uint32_t*)(h->ck_meta + 1)));
-  AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
-  h->ck_pin_pending[0] = h->ck_pin_pending[1] = false;
-  const uint64_t sum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, hd.bytes);
-  if (sum != hd.checksum) {
-    h->last_error = "am_sweep_restore: checksum mismatch";
-    return AM_E_INVAL;
-  }
-  const uint32_t* marks = (const uint32_t*)(h->ck_meta_h + 1);
-  for (uint32_t id = 1; id < 256; ++id)
-    if (((marks[id >> 5] >> (id & 31)) & 1u) && !lut.id[id]) {
-      h->last_error = "am_sweep_restore: a record names a zone the blob's table does not";
-      return AM_E_INVAL;
-    }
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
-  rc = ckpt_restore_switches(h, hd.switches, "am_sweep_restore");
+  rc = ckpt_restore_switches(h, r.hd.switches, "am_sweep_restore");
   if (rc != AM_OK) return rc;
-  if (h->has_prev && (hd.prev_tick == INT64_MIN || hd.prev_tick != h->prev_T)) {
+  if (h->has_prev && (r.hd.prev_tick == INT64_MIN || r.hd.prev_tick != h->prev_T)) {
     h->last_error = "am_sweep_restore: the handle's previous tick differs from the blob's";
     return AM_E_INVAL;
   }
-  // a restore is a call in the per-slot order: the calls staged before it are applied first, and it replaces them
-  rc = begin_call(h);
+  rc = ckpt_restore_apply(h, r);
   if (rc != AM_OK) return rc;
-  if ((hd.switches & AM_CKPT_TIMEOUTS) && !h->wf_timeout) {
-    rc = alloc_timeouts(h, h->stream);
-    if (rc != AM_OK) return rc;
-  }
-  if (hd.n) {
-    AM_CUDA(h, launch(h, checkpoint_scatter_kernel, (unsigned)((hd.n + 255) / 256), 256, h->stream, ckpt_state(h),
-                      ckpt_blob(h, L, hd.n), first, lut));
-    rc = rebuild_planes(h, first, hd.n);
-    if (rc != AM_OK) return rc;
-  }
-  rc = ckpt_restore_finish(h, hd.swept_end, hd.prev_tick, hd.seed);
-  if (rc != AM_OK) return rc;
-  ckpt_start_link(h, hd.first_global, hd.n, hd.checksum);
+  ckpt_start_link(h, r.hd.first_global, r.hd.n, r.hd.checksum);
   return AM_OK;
 }
 
@@ -2944,7 +2965,7 @@ int am_sweep_checkpoint_delta(am_sweep_t* h, void* buf, uint64_t cap, uint64_t* 
     return AM_E_INVAL;
   }
   const uint64_t first = h->chain_first, n = h->chain_n;
-  CkptDeltaHeader hd{};
+  CkptHeader hd;
   {  // the passes, with the tick guard held: the drain, then the diff, its compaction and the pack on the handle's stream
     TickGuard g(h);
     if (!g.ok) return AM_E_BUSY;
@@ -2954,14 +2975,7 @@ int am_sweep_checkpoint_delta(am_sweep_t* h, void* buf, uint64_t cap, uint64_t* 
       h->last_error = "am_sweep_checkpoint_delta: the switches differ from the chain root's: start a new chain";
       return AM_E_INVAL;
     }
-    hd.magic = kCkdMagic;
-    hd.version = AM_CHECKPOINT_VERSION;
-    hd.switches = h->chain_switches;
-    hd.first_global = h->shard_base + first;
-    hd.n = n;
-    hd.swept_end = h->shard_base + std::min(std::max(h->n_records, first), first + n);
-    hd.prev_tick = h->has_prev ? h->prev_T : INT64_MIN;
-    hd.seed = h->seed;
+    hd = ckpt_header(h, kCkdMagic, first, n);
     hd.seq = h->chain_seq + 1;
     hd.parent_prev_tick = h->chain_prev_tick;
     hd.parent_checksum = h->chain_checksum;
@@ -2990,7 +3004,7 @@ int am_sweep_checkpoint_delta(am_sweep_t* h, void* buf, uint64_t cap, uint64_t* 
   // Ticks may run from here on: the copy to the caller and the commit wait for the passes only, on the checkpoint stream.
   AM_CUDA(h, cudaEventSynchronize(h->ck_ev));
   const uint64_t m = n ? h->ckd_acc_h[1] : 0;
-  const CkptLayout L = ckd_layout(m, hd.switches);
+  const CkptLayout L = ckpt_layout(m, hd.switches, ckd_start(m));
   std::vector<CkptZone> zones;
   int rc = ckpt_marked_zones(h, (const uint32_t*)(h->ck_meta_h + 1), "am_sweep_checkpoint_delta", &zones);
   if (rc != AM_OK) return rc;
@@ -3001,43 +3015,31 @@ int am_sweep_checkpoint_delta(am_sweep_t* h, void* buf, uint64_t cap, uint64_t* 
     return AM_E_NOSPACE;
   }
   char* p = (char*)buf;
-  ckpt_put_zones(p, L.sections_end, zones);
   hd.n_changed = m;
-  hd.n_zones = (uint32_t)zones.size();
-  hd.bytes = need;
-  memcpy(p, &hd, kCkHeader);
-  const uint64_t start = ckd_start(m);
-  memset(p + kCkHeader + m * 4, 0, start - kCkHeader - m * 4);  // (the offset section's padding)
-  AM_CUDA(h, cudaStreamWaitEvent(h->ck_stream, h->ck_ev, 0));
+  rc = ckpt_seal(h, p, &hd, L, m, zones, len_out);
+  if (rc != AM_OK) return rc;
+  // the offset section (its checksum terms are the pack's) and its padding; then the blob is the caller's: the base
+  // image advances to it
+  memset(p + kCkHeader + m * 4, 0, L.off[0] - kCkHeader - m * 4);
   if (m) {
     AM_CUDA(h, cudaMemcpyAsync(p + kCkHeader, h->ckd_off, m * 4, cudaMemcpyDeviceToHost, h->ck_stream));
-    AM_CUDA(h, cudaMemcpyAsync(p + start, h->ck_dev + kCkHeader, L.sections_end - start, cudaMemcpyDeviceToHost,
-                               h->ck_stream));
-  }
-  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
-  ckpt_zero_padding(p, L, m);
-  hd.checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, need);
-  memcpy(p + offsetof(CkptDeltaHeader, checksum), &hd.checksum, 8);
-  // the blob is the caller's: the base image advances to it
-  if (m) {
     AM_CUDA(h, launch(h, delta_commit_kernel, (unsigned)((m + 255) / 256), 256, h->ck_stream,
-                      ckd_base_blob(h, n, hd.switches), ckd_blob(h, L, m), (const uint32_t*)h->ckd_off));
+                      ckd_base_blob(h, n, hd.switches), ckpt_blob(h, L, m), (const uint32_t*)h->ckd_off));
     AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
   }
   h->chain_checksum = hd.checksum;
   h->chain_seq = hd.seq;
   h->chain_prev_tick = hd.prev_tick;
-  *len_out = need;
   *n_changed = m;
   return AM_OK;
 }
 
 int am_checkpoint_delta_info(const void* buf, uint64_t len, am_checkpoint_delta_info_t* info) {
   if (!info) return AM_E_INVAL;
-  CkptDeltaHeader hd;
+  CkptHeader hd;
   CkptLayout L;
   std::vector<CkptZone> zones;
-  const int rc = ckd_parse(buf, len, &hd, &L, &zones);
+  const int rc = ckpt_parse(buf, len, true, &hd, &L, &zones);
   if (rc != AM_OK) return rc;
   *info = am_checkpoint_delta_info_t{};
   info->first_global = hd.first_global;
@@ -3059,61 +3061,11 @@ int am_checkpoint_delta_info(const void* buf, uint64_t len, am_checkpoint_delta_
 
 int am_sweep_restore_delta(am_sweep_t* h, const void* buf, uint64_t len) {
   if (!h || !buf) return AM_E_INVAL;
-  CkptDeltaHeader hd;
-  CkptLayout L;
-  std::vector<CkptZone> zones;
-  int rc = ckd_parse(buf, len, &hd, &L, &zones);
-  if (rc != AM_OK) {
-    h->last_error = "am_sweep_restore_delta: not a delta of this format version, or truncated";
-    return rc;
-  }
-  if (hd.first_global < h->shard_base || hd.first_global - h->shard_base + hd.n > h->capacity) {
-    h->last_error = "am_sweep_restore_delta: the delta's slots are not all inside this shard";
-    return AM_E_RANGE;
-  }
-  const uint64_t first = hd.first_global - h->shard_base, m = hd.n_changed;
-  ZoneLut lut;
-  rc = ckpt_zone_lut(h, zones, "am_sweep_restore_delta", &lut);
-  if (rc != AM_OK) return rc;
   std::lock_guard<std::mutex> ck(h->ck_mu);
-  rc = ckpt_alloc(h);
-  if (rc == AM_OK) rc = ckd_alloc(h, false);
+  CkptRestore r;
+  int rc = ckpt_restore_check(h, buf, len, true, &r);
   if (rc != AM_OK) return rc;
-  // Up in chunks (the offsets to ckd_off, the sections to the staging area), then the device passes that verify the
-  // checksum and the offsets: all before anything of the handle changes.
-  const char* p = (const char*)buf;
-  const uint64_t start = ckd_start(m);
-  rc = ckpt_upload(h, (char*)h->ckd_off, p + kCkHeader, m * 4);
-  if (rc == AM_OK) rc = ckpt_upload(h, h->ck_dev + kCkHeader, p + start, L.sections_end - start);
-  if (rc != AM_OK) return rc;
-  AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->ck_stream));
-  AM_CUDA(h, cudaMemsetAsync(h->ckd_acc, 0, 4 * 8, h->ck_stream));
-  if (m) {
-    const unsigned grid = (unsigned)((m + 255) / 256);
-    AM_CUDA(h, launch(h, delta_offsets_verify_kernel, grid, 256, h->ck_stream, (const uint32_t*)h->ckd_off, m, hd.n,
-                      h->ck_meta, (uint32_t*)(h->ckd_acc + 2)));
-    AM_CUDA(h, launch(h, checkpoint_verify_kernel, grid, 256, h->ck_stream, ckd_blob(h, L, m), h->ck_meta,
-                      (uint32_t*)(h->ck_meta + 1)));
-  }
-  AM_CUDA(h, cudaMemcpyAsync(h->ck_meta_h, h->ck_meta, 5 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
-  AM_CUDA(h, cudaMemcpyAsync(h->ckd_acc_h, h->ckd_acc, 4 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
-  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
-  h->ck_pin_pending[0] = h->ck_pin_pending[1] = false;
-  const uint64_t sum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, hd.bytes);
-  if (sum != hd.checksum) {
-    h->last_error = "am_sweep_restore_delta: checksum mismatch";
-    return AM_E_INVAL;
-  }
-  if (h->ckd_acc_h[2]) {
-    h->last_error = "am_sweep_restore_delta: the slot offsets are not strictly ascending inside the range";
-    return AM_E_INVAL;
-  }
-  const uint32_t* marks = (const uint32_t*)(h->ck_meta_h + 1);
-  for (uint32_t id = 1; id < 256; ++id)
-    if (((marks[id >> 5] >> (id & 31)) & 1u) && !lut.id[id]) {
-      h->last_error = "am_sweep_restore_delta: a record names a zone the delta's table does not";
-      return AM_E_INVAL;
-    }
+  const CkptHeader& hd = r.hd;
   TickGuard g(h);
   if (!g.ok) return AM_E_BUSY;
   CkptLink* link = nullptr;
@@ -3134,21 +3086,7 @@ int am_sweep_restore_delta(am_sweep_t* h, const void* buf, uint64_t len) {
     h->last_error = "am_sweep_restore_delta: the handle's previous tick is neither the delta's nor its parent's";
     return AM_E_INVAL;
   }
-  // a call in the per-slot order: the calls staged before it are applied first
-  rc = begin_call(h);
-  if (rc != AM_OK) return rc;
-  if ((hd.switches & AM_CKPT_TIMEOUTS) && !h->wf_timeout) {
-    rc = alloc_timeouts(h, h->stream);
-    if (rc != AM_OK) return rc;
-  }
-  if (m) {
-    AM_CUDA(h, launch(h, delta_scatter_kernel, (unsigned)((m + 255) / 256), 256, h->stream, ckpt_state(h),
-                      ckd_blob(h, L, m), (const uint32_t*)h->ckd_off, first, lut, h->seg_dirty, due_kept(h),
-                      h->due_epoch));
-    AM_CUDA(h, launch(h, delta_planes_kernel, (unsigned)((m + kWarps - 1) / kWarps), kBlock, h->stream, h->cols,
-                      h->planes, h->seg_dirty, (const uint32_t*)h->ckd_off, first, (uint32_t)m));
-  }
-  rc = ckpt_restore_finish(h, hd.swept_end, hd.prev_tick, hd.seed);
+  rc = ckpt_restore_apply(h, r);
   if (rc != AM_OK) return rc;
   link->checksum = hd.checksum;
   link->ticks = h->ticks;
