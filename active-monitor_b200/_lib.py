@@ -205,6 +205,7 @@ SYMBOLS = {
     "am_sweep_set_change_details": (C.c_int, [C.c_void_p, C.c_int]),
     "am_sweep_last_change_details": (C.c_int, [C.c_void_p, u64, C.c_void_p, C.c_void_p, u64, P(u64)]),
     "am_sweep_checkpoint": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, u64, P(u64)]),
+    "am_sweep_set_checkpoint_packing": (C.c_int, [C.c_void_p, C.c_int]),
     "am_checkpoint_info": (C.c_int, [C.c_void_p, u64, P(AmCheckpointInfo)]),
     "am_sweep_restore": (C.c_int, [C.c_void_p, C.c_void_p, u64]),
     "am_sweep_checkpoint_chain": (C.c_int, [C.c_void_p, u64, u64, C.c_void_p, u64, P(u64)]),

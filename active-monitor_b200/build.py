@@ -22,7 +22,7 @@ AMGEN = os.path.join(ROOT, "tools", "amgen", "libamgen.so")
 ORACLE = os.path.join(ROOT, "oracle", "_build", "libamsweep_oracle.so")
 
 SOURCES = ("sweep.cu", "gather.cu", "cron_parse.cpp", "handoff.cpp", "host_loops.cpp", "tz.cpp", "ingest_json.cpp")
-HEADERS = ("sweep_kernels.cuh", "admission_kernels.cuh", "checkpoint_kernels.cuh", "sweep_block.cuh", "sweep_types.h", "sweep_internal.h", "gather_kernels.cuh", "civil.h", "tz.h", "tz_eval.h")
+HEADERS = ("sweep_kernels.cuh", "admission_kernels.cuh", "checkpoint_kernels.cuh", "checkpoint_pack_kernels.cuh", "sweep_block.cuh", "sweep_types.h", "sweep_internal.h", "gather_kernels.cuh", "civil.h", "tz.h", "tz_eval.h")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]

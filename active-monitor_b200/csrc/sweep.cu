@@ -44,6 +44,7 @@
 
 #include "admission_kernels.cuh"
 #include "checkpoint_kernels.cuh"
+#include "checkpoint_pack_kernels.cuh"
 #include "sweep_internal.h"
 #include "sweep_kernels.cuh"
 #include "tz.h"
@@ -281,6 +282,17 @@ struct am_sweep {
   uint32_t* ckd_off = nullptr;
   unsigned long long* ckd_acc = nullptr;
   unsigned long long* ckd_acc_h = nullptr;
+  // packed checkpoints (am_sweep_set_checkpoint_packing), also under ck_mu: whether producers pack, and, at the first
+  // packed checkpoint or restore, the packed staging area (a directory and payload as large as a delta with every slot
+  // of capacity changed and every section), the encode's per-block sizes, their scan and base values, and the
+  // accumulators ([1] the payload's words, [2] a refused directory or block), device and pinned.
+  bool ck_packing = false;
+  char* ckp_dev = nullptr;
+  uint32_t* ckp_words = nullptr;
+  uint32_t* ckp_prefix = nullptr;
+  int64_t* ckp_base = nullptr;
+  unsigned long long* ckp_acc = nullptr;
+  unsigned long long* ckp_acc_h = nullptr;
   // the producer's chain: its range, the root's switches, the last link's checksum, sequence number and P
   bool chain = false;
   uint64_t chain_first = 0, chain_n = 0, chain_checksum = 0, chain_seq = 0;
@@ -2443,7 +2455,8 @@ constexpr size_t kCkChunk = 32u << 20;  // bytes per pinned chunk of a restore's
 
 constexpr uint64_t kCkdMagic = 0x4C444B4357534D41ull;  // "AMSWCKDL"
 
-// The header of a full blob and of a delta.  Words 10..13 are a delta's link; a full blob leaves them zero.
+// The header of a full blob and of a delta.  Words 10..13 are a delta's link; a full blob leaves them zero.  Word 14 is
+// a packed blob's length once decoded (version 2; zero in version 1).
 struct CkptHeader {
   uint64_t magic;
   uint32_t version, switches;
@@ -2454,20 +2467,25 @@ struct CkptHeader {
   uint64_t n_changed, seq;
   int64_t parent_prev_tick;
   uint64_t parent_checksum;
-  uint64_t reserved[2];
+  uint64_t raw_bytes;
+  uint64_t reserved;
 };
 static_assert(sizeof(CkptHeader) == kCkHeader && kCkHeader == kCkHeaderBytes, "checkpoint header: 16 words");
 
+// A blob's layout: the version-1 sections' offsets and end; where its zone table starts (the sections' end in version
+// 1) and, packed, its blocks and the payload's bytes.
 struct CkptLayout {
   uint64_t off[kCkSections] = {};
   uint64_t sections_end = kCkHeader;
+  uint64_t zones_at = kCkHeader;
+  uint64_t blocks = 0, payload = 0;
 };
 
 // The sections a blob of n slots with `switches` has, in order, each at an 8-B aligned offset from `start` on (a
 // delta of n slots: ckd_start(n), after the offset section).
 CkptLayout ckpt_layout(uint64_t n, uint32_t switches, uint64_t start = kCkHeader) {
   CkptLayout L;
-  L.sections_end = ck_layout(n, switches, start, L.off);
+  L.sections_end = L.zones_at = ck_layout(n, switches, start, L.off);
   return L;
 }
 
@@ -2484,16 +2502,54 @@ void ckpt_zero_padding(char* p, const CkptLayout& L, uint64_t n) {
   }
 }
 
-// The checksum's terms of the words in [a, b) of a blob (the header, whose checksum word counts as 0, and the zone table).
-uint64_t ckpt_host_sum(const char* buf, uint64_t a, uint64_t b) {
+// The checksum's terms of `len` bytes of words at `w`, which stand at byte `at` of the version-1 blob (the header, whose
+// checksum word counts as 0, and the zone table).
+uint64_t ckpt_host_sum(const void* w, uint64_t at, uint64_t len) {
   uint64_t s = 0;
-  for (uint64_t o = a; o < b; o += 8) {
-    uint64_t w;
-    memcpy(&w, buf + o, 8);
-    if (o == offsetof(CkptHeader, checksum)) w = 0;
-    s += ckpt_mix(o * 8, w);
+  for (uint64_t o = 0; o < len; o += 8) {
+    uint64_t v;
+    memcpy(&v, (const char*)w + o, 8);
+    if (at + o == offsetof(CkptHeader, checksum)) v = 0;
+    s += ckpt_mix((at + o) * 8, v);
   }
   return s;
+}
+
+// The header of the version-1 blob a packed one decodes to: the checksum covers that one.
+CkptHeader ckpt_v1_header(const CkptHeader& hd) {
+  CkptHeader v = hd;
+  if (v.version == AM_CHECKPOINT_VERSION_PACKED) {
+    v.version = AM_CHECKPOINT_VERSION;
+    v.bytes = hd.raw_bytes;
+    v.raw_bytes = 0;
+  }
+  return v;
+}
+
+// The sections a packed blob of layout L (m elements per section; a delta's offsets first) encodes, at `blob` (the
+// version-1 blob's byte 0) and `offs`; NULL for the geometry alone.
+CkpSecs ckp_secs(const CkptLayout& L, uint64_t m, bool delta, char* blob, uint32_t* offs) {
+  CkpSecs S{};
+  uint64_t blk = 0;
+  auto add = [&](char* p, uint64_t cnt, uint32_t esize, int64_t none) {
+    S.p[S.n] = p;
+    S.cnt[S.n] = cnt;
+    S.esize[S.n] = esize;
+    S.none[S.n] = none;
+    S.blk0[S.n++] = blk;
+    blk += (cnt + kCkpBlock - 1) / kCkpBlock;
+  };
+  if (delta) add((char*)offs, m, 4, 0);
+  for (int q = 0; q < kCkSections; ++q) {
+    if (!L.off[q]) continue;
+    const bool bits = q == kCkSecChanged;
+    add(blob ? blob + L.off[q] : nullptr, bits ? (m + 31) / 32 : m, bits ? 4 : ck_elem(q),
+        q == kCkSecSince || q == kCkSecDetStart || q == kCkSecWait ? INT64_MIN
+        : q == kCkSecDeadline                                      ? INT64_MAX
+                                                                   : 0);
+  }
+  S.blk0[S.n] = blk;
+  return S;
 }
 
 struct CkptZone {
@@ -2507,7 +2563,9 @@ int ckpt_parse(const void* buf, uint64_t len, bool delta, CkptHeader* hd, CkptLa
                std::vector<CkptZone>* zones) {
   if (!buf || len < kCkHeader) return AM_E_INVAL;
   memcpy(hd, buf, kCkHeader);
-  if (hd->magic != (delta ? kCkdMagic : kCkMagic) || hd->version != AM_CHECKPOINT_VERSION) return AM_E_INVAL;
+  const bool packed = hd->version == AM_CHECKPOINT_VERSION_PACKED;
+  if (hd->magic != (delta ? kCkdMagic : kCkMagic) || (hd->version != AM_CHECKPOINT_VERSION && !packed))
+    return AM_E_INVAL;
   if (delta && (hd->n_changed > hd->n || hd->seq == 0)) return AM_E_INVAL;
   if ((hd->switches & ~kCkAllSwitches) || ((hd->switches & AM_CKPT_REMEDY) && !(hd->switches & AM_CKPT_HOLD)) ||
       ((hd->switches & AM_CKPT_DETAILS) && !(hd->switches & AM_CKPT_TRACK)) ||
@@ -2516,9 +2574,27 @@ int ckpt_parse(const void* buf, uint64_t len, bool delta, CkptHeader* hd, CkptLa
   if (hd->bytes > len || hd->bytes % 8 || hd->n > 0xFFFFFFFFull || hd->first_global + hd->n < hd->first_global ||
       hd->swept_end < hd->first_global || hd->swept_end > hd->first_global + hd->n || hd->n_zones > 255)
     return AM_E_INVAL;
-  *L = delta ? ckpt_layout(hd->n_changed, hd->switches, ckd_start(hd->n_changed)) : ckpt_layout(hd->n, hd->switches);
+  const uint64_t m = delta ? hd->n_changed : hd->n;
+  *L = delta ? ckpt_layout(m, hd->switches, ckd_start(m)) : ckpt_layout(hd->n, hd->switches);
   const char* p = (const char*)buf;
-  uint64_t at = L->sections_end;  // (past `bytes` when a delta's n_changed is out of range: refused below)
+  if (packed) {  // the directory, then the payload up to the end of the last block's, then the zone table
+    const CkpSecs S = ckp_secs(*L, m, delta, nullptr, nullptr);
+    L->blocks = S.blk0[S.n];
+    const uint64_t dir_end = kCkHeader + L->blocks * sizeof(CkpEntry);
+    if (L->blocks > hd->bytes / sizeof(CkpEntry) || dir_end > hd->bytes) return AM_E_INVAL;
+    if (L->blocks) {
+      CkpEntry e;
+      memcpy(&e, p + dir_end - sizeof(CkpEntry), sizeof e);
+      const int s = S.n - 1;  // (the last section has the last block: m > 0)
+      const uint64_t cnt = S.cnt[s] - (L->blocks - 1 - S.blk0[s]) * kCkpBlock;
+      if (!ckp_entry_ok(e, cnt, S.esize[s]) || e.off > hd->bytes) return AM_E_INVAL;
+      L->payload = e.off + ckp_bytes(e.mode, e.width, e.aux, cnt, S.esize[s]);
+    }
+    // (no block is larger than its elements verbatim: the encoder falls back to RAW)
+    if (L->payload > L->sections_end - kCkHeader || dir_end + L->payload > hd->bytes) return AM_E_INVAL;
+    L->zones_at = dir_end + L->payload;
+  }
+  uint64_t at = L->zones_at;  // (past `bytes` when a delta's n_changed is out of range: refused below)
   bool seen[256] = {};
   zones->clear();
   for (uint32_t k = 0; k < hd->n_zones; ++k) {
@@ -2532,6 +2608,7 @@ int ckpt_parse(const void* buf, uint64_t len, bool delta, CkptHeader* hd, CkptLa
     zones->push_back({id, std::string(p + at + 8, nl)});
     at += ckpt_zone_entry_bytes(nl);
   }
+  if (packed && hd->raw_bytes != L->sections_end + (hd->bytes - L->zones_at)) return AM_E_INVAL;
   return at == hd->bytes ? AM_OK : AM_E_INVAL;
 }
 
@@ -2655,6 +2732,28 @@ int ckd_alloc(am_sweep* h, bool producer) {
   return AM_OK;
 }
 
+// The packed staging area of a handle, at its first packed checkpoint or restore (ck_mu held, after ckpt_alloc).
+// AM_E_UNSUPPORTED: a capacity whose payload would not fit the scan's u32 word counts.
+int ckp_alloc(am_sweep* h) {
+  if (h->ckp_dev) return AM_OK;
+  const CkptLayout L = ckpt_layout(h->cap_padded, kCkAllSwitches, ckd_start(h->cap_padded));
+  const CkpSecs S = ckp_secs(L, h->cap_padded, true, nullptr, nullptr);
+  const uint64_t nb = S.blk0[S.n];
+  const uint64_t payload = L.sections_end - kCkHeader;
+  if (payload / 8 > 0xFFFFFFFFull) {
+    h->last_error = "packed checkpoints: the capacity is too large for the encoder's 32-bit payload word counts";
+    return AM_E_UNSUPPORTED;
+  }
+  AM_CUDA(h, dev_array(h, &h->ckp_words, nb * 4, h->ck_stream, false));
+  AM_CUDA(h, dev_array(h, &h->ckp_prefix, (nb + 1) * 4, h->ck_stream, false));
+  AM_CUDA(h, dev_array(h, &h->ckp_base, nb * 8, h->ck_stream, false));
+  AM_CUDA(h, dev_array(h, &h->ckp_acc, 4 * 8, h->ck_stream));
+  AM_CUDA(h, host_array(h, &h->ckp_acc_h, 4 * 8));
+  AM_CUDA(h, dev_array(h, &h->ckp_dev, nb * sizeof(CkpEntry) + payload, h->ck_stream, false));  // (the last)
+  AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+  return AM_OK;
+}
+
 // `bytes` at `src` (host) to `dst` (device) on the checkpoint stream, in chunks through the two pinned buffers (the
 // host fills one while the other crosses).
 int ckpt_upload(am_sweep* h, char* dst, const char* src, uint64_t bytes) {
@@ -2719,9 +2818,27 @@ int ckpt_restore_check(am_sweep* h, const void* buf, uint64_t len, bool delta, C
   if (rc != AM_OK) return rc;
   const char* p = (const char*)buf;
   const uint64_t m = r->m, start = r->L.off[0];
-  if (delta) rc = ckpt_upload(h, (char*)h->ckd_off, p + kCkHeader, m * 4);
-  if (rc == AM_OK) rc = ckpt_upload(h, h->ck_dev + kCkHeader, p + start, r->L.sections_end - start);
-  if (rc != AM_OK) return rc;
+  const bool packed = hd.version == AM_CHECKPOINT_VERSION_PACKED;
+  if (packed) {  // the directory and payload up; the directory validated, then decoded into the version-1 places
+    rc = ckp_alloc(h);
+    if (rc == AM_OK) rc = ckpt_upload(h, h->ckp_dev, p + kCkHeader, r->L.zones_at - kCkHeader);
+    if (rc != AM_OK) return rc;
+    AM_CUDA(h, cudaMemsetAsync(h->ckp_acc, 0, 4 * 8, h->ck_stream));
+    const CkpSecs S = ckp_secs(r->L, m, delta, ckpt_blob(h, r->L, m).p, h->ckd_off);
+    const uint64_t nb = r->L.blocks;
+    const CkpEntry* dir = (const CkpEntry*)h->ckp_dev;
+    if (nb) {
+      AM_CUDA(h, launch(h, ckp_validate_kernel, (unsigned)((nb + 255) / 256), 256, h->ck_stream, S, dir,
+                        r->L.payload, (uint32_t*)(h->ckp_acc + 2)));
+      AM_CUDA(h, launch(h, ckp_decode_kernel, (unsigned)nb, kCkpThreads, h->ck_stream, S, dir,
+                        (const char*)(dir + nb), (uint32_t*)(h->ckp_acc + 2)));
+    }
+    AM_CUDA(h, cudaMemcpyAsync(h->ckp_acc_h, h->ckp_acc, 4 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
+  } else {
+    if (delta) rc = ckpt_upload(h, (char*)h->ckd_off, p + kCkHeader, m * 4);
+    if (rc == AM_OK) rc = ckpt_upload(h, h->ck_dev + kCkHeader, p + start, r->L.sections_end - start);
+    if (rc != AM_OK) return rc;
+  }
   AM_CUDA(h, cudaMemsetAsync(h->ck_meta, 0, 5 * 8, h->ck_stream));
   if (delta) AM_CUDA(h, cudaMemsetAsync(h->ckd_acc, 0, 4 * 8, h->ck_stream));
   if (m) {
@@ -2736,7 +2853,13 @@ int ckpt_restore_check(am_sweep* h, const void* buf, uint64_t len, bool delta, C
   if (delta) AM_CUDA(h, cudaMemcpyAsync(h->ckd_acc_h, h->ckd_acc, 4 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
   AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
   h->ck_pin_pending[0] = h->ck_pin_pending[1] = false;
-  const uint64_t sum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, r->L.sections_end, hd.bytes);
+  if (packed && h->ckp_acc_h[2]) {
+    h->last_error = std::string(who) + ": a packed block or its directory entry is malformed";
+    return AM_E_INVAL;
+  }
+  const CkptHeader v1 = ckpt_v1_header(hd);
+  const uint64_t sum = h->ck_meta_h[0] + ckpt_host_sum(&v1, 0, kCkHeader) +
+                       ckpt_host_sum(p + r->L.zones_at, r->L.sections_end, hd.bytes - r->L.zones_at);
   if (sum != hd.checksum) {
     h->last_error = std::string(who) + ": checksum mismatch";
     return AM_E_INVAL;
@@ -2812,21 +2935,74 @@ CkptHeader ckpt_header(const am_sweep* h, uint64_t magic, uint64_t first, uint64
   return hd;
 }
 
-// The end of a producer, after its pass (ck_ev) and once the caller's buffer `p` has room for the blob: the zone table
-// of the pass's marks (`zones`), the header, the sections of the staging area (n elements each, layout L), their
-// padding and the checksum word; *len_out = the blob's length.
-int ckpt_seal(am_sweep* h, char* p, CkptHeader* hd, const CkptLayout& L, uint64_t n,
+// The end of a producer, after its pass (ck_ev): the blob of the staging area's sections (n elements each, layout L;
+// with `delta` the offsets in ckd_off first) and the zone table of the pass's marks (`zones`) into the caller's
+// buffer `p`, with the header *hd and the checksum word; *len_out = the blob's length.  AM_E_NOSPACE (*len_out = the
+// length) when cap is below it.  While the handle packs, the encode runs first on the checkpoint stream and the blob
+// is packed (DESIGN.md "Packed format"); its checksum is that of the version-1 blob it decodes to.
+int ckpt_seal(am_sweep* h, char* p, uint64_t cap, CkptHeader* hd, const CkptLayout& L, uint64_t n, bool delta,
               const std::vector<CkptZone>& zones, uint64_t* len_out) {
+  uint64_t zone_bytes = 0;
+  for (const CkptZone& z : zones) zone_bytes += ckpt_zone_entry_bytes(z.name.size());
   hd->n_zones = (uint32_t)zones.size();
-  hd->bytes = ckpt_put_zones(p, L.sections_end, zones);
-  memcpy(p, hd, kCkHeader);
+  hd->bytes = L.sections_end + zone_bytes;
   AM_CUDA(h, cudaStreamWaitEvent(h->ck_stream, h->ck_ev, 0));
+  if (h->ck_packing) {
+    int rc = ckp_alloc(h);
+    if (rc != AM_OK) return rc;
+    const CkpSecs S = ckp_secs(L, n, delta, ckpt_blob(h, L, n).p, h->ckd_off);
+    const uint64_t nb = S.blk0[S.n];
+    CkpEntry* dir = (CkpEntry*)h->ckp_dev;
+    uint64_t payload = 0;
+    if (nb) {  // sizes, their scan into word offsets, the payloads; one synchronisation for the packed length
+      AM_CUDA(h, launch(h, ckp_size_kernel, (unsigned)nb, kCkpThreads, h->ck_stream, S, dir, h->ckp_words,
+                        h->ckp_base));
+      ScanParams sc{};
+      sc.group_count = h->ckp_words;
+      sc.group_prefix = h->ckp_prefix;
+      sc.acc = h->ckp_acc;
+      sc.n_groups = (uint32_t)nb;
+      sc.cap = 0xFFFFFFFFu;
+      AM_CUDA(h, launch(h, scan_groups_kernel, 1, 1024, h->ck_stream, sc));
+      AM_CUDA(h, launch(h, ckp_write_kernel, (unsigned)nb, kCkpThreads, h->ck_stream, S, dir,
+                        (const uint32_t*)h->ckp_prefix, (const int64_t*)h->ckp_base, (char*)(dir + nb)));
+      AM_CUDA(h, cudaMemcpyAsync(h->ckp_acc_h, h->ckp_acc, 4 * 8, cudaMemcpyDeviceToHost, h->ck_stream));
+      AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+      payload = h->ckp_acc_h[1] * 8;
+    }
+    const uint64_t at = kCkHeader + nb * sizeof(CkpEntry) + payload;
+    if (cap < at + zone_bytes) {
+      *len_out = at + zone_bytes;
+      return AM_E_NOSPACE;
+    }
+    ckpt_put_zones(p, at, zones);
+    hd->checksum = h->ck_meta_h[0] + ckpt_host_sum(hd, 0, kCkHeader) + ckpt_host_sum(p + at, L.sections_end, zone_bytes);
+    hd->version = AM_CHECKPOINT_VERSION_PACKED;
+    hd->raw_bytes = hd->bytes;
+    hd->bytes = at + zone_bytes;
+    memcpy(p, hd, kCkHeader);
+    if (at > kCkHeader)
+      AM_CUDA(h, cudaMemcpyAsync(p + kCkHeader, h->ckp_dev, at - kCkHeader, cudaMemcpyDeviceToHost, h->ck_stream));
+    AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
+    *len_out = hd->bytes;
+    return AM_OK;
+  }
+  if (cap < hd->bytes) {  // (a full blob's room was checked before its pass, for every registered zone)
+    *len_out = hd->bytes;
+    return AM_E_NOSPACE;
+  }
+  ckpt_put_zones(p, L.sections_end, zones);
+  memcpy(p, hd, kCkHeader);
   if (L.sections_end > L.off[0])  // (the sections start at L.off[0]: the header's end, or a delta's offsets' end)
     AM_CUDA(h, cudaMemcpyAsync(p + L.off[0], h->ck_dev + kCkHeader, L.sections_end - L.off[0], cudaMemcpyDeviceToHost,
                                h->ck_stream));
+  if (delta && n)  // the offset section (its checksum terms are the pack's)
+    AM_CUDA(h, cudaMemcpyAsync(p + kCkHeader, h->ckd_off, n * 4, cudaMemcpyDeviceToHost, h->ck_stream));
   AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));
   ckpt_zero_padding(p, L, n);
-  hd->checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) + ckpt_host_sum(p, L.sections_end, hd->bytes);
+  if (delta) memset(p + kCkHeader + n * 4, 0, L.off[0] - kCkHeader - n * 4);
+  hd->checksum = h->ck_meta_h[0] + ckpt_host_sum(p, 0, kCkHeader) +
+                 ckpt_host_sum(p + L.sections_end, L.sections_end, hd->bytes - L.sections_end);
   memcpy(p + offsetof(CkptHeader, checksum), &hd->checksum, 8);
   *len_out = hd->bytes;
   return AM_OK;
@@ -2842,10 +3018,10 @@ int checkpoint_locked(am_sweep* h, uint64_t first, uint64_t n, void* buf, uint64
     if (rc != AM_OK) return rc;
     *hd = ckpt_header(h, kCkMagic, first, n);
     *L = ckpt_layout(n, hd->switches);
-    uint64_t bound = L->sections_end;  // (room for the names of every registered zone)
+    uint64_t bound = L->sections_end;  // (room for the names of every registered zone; a packed blob's after its encode)
     std::string name;
     for (int32_t id = 1; amsweep_tz::name_of(id, &name); ++id) bound += ckpt_zone_entry_bytes(name.size());
-    if (cap < bound) {
+    if (cap < bound && !h->ck_packing) {
       *len_out = bound;
       return AM_E_NOSPACE;
     }
@@ -2863,7 +3039,7 @@ int checkpoint_locked(am_sweep* h, uint64_t first, uint64_t n, void* buf, uint64
   std::vector<CkptZone> zones;
   const int rc = ckpt_marked_zones(h, (const uint32_t*)(h->ck_meta_h + 1), "am_sweep_checkpoint", &zones);
   if (rc != AM_OK) return rc;
-  return ckpt_seal(h, (char*)buf, hd, *L, n, zones, len_out);
+  return ckpt_seal(h, (char*)buf, cap, hd, *L, n, false, zones, len_out);
 }
 
 // A restored full blob starts the handle's link entry for its range, replacing every entry that overlaps it.
@@ -2889,6 +3065,13 @@ int am_sweep_checkpoint(am_sweep_t* h, uint64_t first, uint64_t n, void* buf, ui
   CkptHeader hd;
   CkptLayout L;
   return checkpoint_locked(h, first, n, buf, cap, len_out, &hd, &L);
+}
+
+int am_sweep_set_checkpoint_packing(am_sweep_t* h, int on) {
+  if (!h) return AM_E_INVAL;
+  std::lock_guard<std::mutex> ck(h->ck_mu);
+  h->ck_packing = on != 0;
+  return AM_OK;
 }
 
 int am_checkpoint_info(const void* buf, uint64_t len, am_checkpoint_info_t* info) {
@@ -3008,21 +3191,11 @@ int am_sweep_checkpoint_delta(am_sweep_t* h, void* buf, uint64_t cap, uint64_t* 
   std::vector<CkptZone> zones;
   int rc = ckpt_marked_zones(h, (const uint32_t*)(h->ck_meta_h + 1), "am_sweep_checkpoint_delta", &zones);
   if (rc != AM_OK) return rc;
-  uint64_t need = L.sections_end;
-  for (const CkptZone& z : zones) need += ckpt_zone_entry_bytes(z.name.size());
-  if (cap < need) {  // (nothing committed: the next delta carries these slots again)
-    *len_out = need;
-    return AM_E_NOSPACE;
-  }
-  char* p = (char*)buf;
   hd.n_changed = m;
-  rc = ckpt_seal(h, p, &hd, L, m, zones, len_out);
-  if (rc != AM_OK) return rc;
-  // the offset section (its checksum terms are the pack's) and its padding; then the blob is the caller's: the base
-  // image advances to it
-  memset(p + kCkHeader + m * 4, 0, L.off[0] - kCkHeader - m * 4);
+  rc = ckpt_seal(h, (char*)buf, cap, &hd, L, m, true, zones, len_out);
+  if (rc != AM_OK) return rc;  // (AM_E_NOSPACE: nothing committed, the next delta carries these slots again)
+  // the blob is the caller's: the base image advances to it
   if (m) {
-    AM_CUDA(h, cudaMemcpyAsync(p + kCkHeader, h->ckd_off, m * 4, cudaMemcpyDeviceToHost, h->ck_stream));
     AM_CUDA(h, launch(h, delta_commit_kernel, (unsigned)((m + 255) / 256), 256, h->ck_stream,
                       ckd_base_blob(h, n, hd.switches), ckpt_blob(h, L, m), (const uint32_t*)h->ckd_off));
     AM_CUDA(h, cudaStreamSynchronize(h->ck_stream));

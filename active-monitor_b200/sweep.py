@@ -212,7 +212,7 @@ class Sweep:
         if getattr(self, "_h", None):
             self._lib.am_sweep_destroy(self._h)
             self._h = None
-        self._delta_buf = None
+        self._delta_buf = self._packed_buf = None
 
     def __enter__(self):
         return self
@@ -381,16 +381,33 @@ class Sweep:
         (am_sweep_checkpoint_chain): the same blob checkpoint() returns"""
         return self._checkpoint("am_sweep_checkpoint_chain", first, n)
 
+    def set_checkpoint_packing(self, on: bool):
+        """write packed blobs (format version 2) from the next checkpoint, chain root or delta on
+        (am_sweep_set_checkpoint_packing); restores and checkpoint_info take both versions.  While packing is on,
+        checkpoint() and checkpoint_chain() write into a host buffer this object keeps, grown to 1.25 times the
+        largest packed blob, because a packed length is known only after the encode: a call into a buffer that is too
+        small runs its pass and encode again.  Switch packing through this method: a switch made through the C-ABI
+        directly leaves these calls on the raw sizing, so every packed call would run twice."""
+        self._check(self._lib.am_sweep_set_checkpoint_packing(self._h, int(bool(on))),
+                    "am_sweep_set_checkpoint_packing")
+        self._packing = bool(on)
+
     def _checkpoint(self, fn: str, first: int, n: int | None) -> bytes:
         n = self.capacity - first if n is None else n
         need = L.u64(0)
         buf = np.zeros(0, np.uint8)
+        if getattr(self, "_packing", False):  # (a packed length is known after the encode: a kept buffer, as deltas)
+            buf = getattr(self, "_packed_buf", None)
+            buf = np.zeros(0, np.uint8) if buf is None else buf
         while True:  # (a zone registered between the calls can make the first size too small)
             rc = getattr(self._lib, fn)(self._h, first, n, buf.ctypes.data if len(buf) else None, len(buf),
                                         C.byref(need))
             if rc != L.AM_E_NOSPACE:
                 break
-            buf = np.zeros(need.value, np.uint8)
+            if getattr(self, "_packing", False):
+                buf = self._packed_buf = np.zeros(need.value + need.value // 4, np.uint8)
+            else:
+                buf = np.zeros(need.value, np.uint8)
         self._check(rc, fn)
         return buf[:need.value].tobytes()
 

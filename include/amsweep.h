@@ -717,6 +717,7 @@ int am_sweep_last_change_details(am_sweep_t*, uint64_t offset, uint64_t* idx, am
  * in_flight, remedy_in_flight, select, repeat_after_sec, next_due; the timed-out lists, the changes and the details).
  * With one handle of the same shard that includes n_records. */
 #define AM_CHECKPOINT_VERSION 1
+#define AM_CHECKPOINT_VERSION_PACKED 2 /* a packed blob (am_sweep_set_checkpoint_packing) */
 #define AM_CKPT_HOLD 0x1u     /* the hold in flight was on                   */
 #define AM_CKPT_REMEDY 0x2u   /* ... and the remedy hold                      */
 #define AM_CKPT_TRACK 0x4u    /* status changes were tracked                  */
@@ -749,6 +750,25 @@ int am_sweep_checkpoint(am_sweep_t*, uint64_t first, uint64_t n, void* buf, uint
 /* The header of a blob, checked for consistency (format version, sizes, zone table); no handle, no GPU.  The checksum
  * is verified by am_sweep_restore.  AM_E_INVAL: not a blob of this format version, or truncated. */
 int am_checkpoint_info(const void* buf, uint64_t len, am_checkpoint_info_t* info);
+/* Packed checkpoints (DESIGN.md section 6 item 23, "Packed format"): while `on`, am_sweep_checkpoint,
+ * am_sweep_checkpoint_chain and am_sweep_checkpoint_delta write packed blobs (format version 2, the same magics): the
+ * version-1 blob's sections cut into blocks of 1024 elements, each encoded on the device in the smallest of five
+ * modes (verbatim, one value, frame of reference, sparse, dictionary), with a directory of 16 B per block.  A packed
+ * blob is never longer than the version-1 blob plus its directory.  Its header is the version-1 header with version 2,
+ * `bytes` its own length, word 14 the version-1 length, and the checksum of the version-1 blob it decodes to, so
+ * chains link by content: a raw root may be followed by packed links and the reverse.  While off (the default) they
+ * write exactly what they wrote before.  The setting is not handle state: no AM_CKPT_* switch, a restore never needs
+ * it, and it may change between the links of a chain.  am_sweep_restore, am_sweep_restore_delta, am_checkpoint_info
+ * and am_checkpoint_delta_info take both versions (info.version 1 or 2, info.bytes the blob's own length).
+ * A packed blob's length is known only after its encode: a packed checkpoint returns AM_E_NOSPACE (*len_out = the
+ * packed length) after its passes, and a refused delta commits nothing.  The encode adds 3 launches to a checkpoint
+ * over a non-empty range (sizes, their scan, payloads) on the checkpoint stream after the tick guard is released, and
+ * the decode 2 to a restore of a packed blob (directory check, decode).  The packed staging area (about 134 B per slot
+ * of capacity) is allocated at the first packed checkpoint or restore and kept until am_sweep_destroy; a handle that
+ * never packs allocates and launches nothing for it.  A restore refuses a malformed directory or block (AM_E_INVAL)
+ * before anything changes.  Serialised with the handle's checkpoints and restores. */
+int am_sweep_set_checkpoint_packing(am_sweep_t*, int on);
+
 /* Restore a blob into this handle: slot g of the blob goes to local slot g - shard_base.  A call in the per-slot order:
  * the calls staged before it are drained first and it replaces them for its slots.  The blob is copied up in chunks,
  * verified on the device (checksum) and its zone names resolved with am_tz_lookup before anything changes; then one
